@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Benchmark of the HyperReel per-ray rendering hot path on B200 (contract: see the task prompt / DESIGN.md section 5).
+"""Benchmark of the HyperReel per-ray rendering hot path on H100 (DESIGN.md section 5).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path (sample net -> intersect -> VM gather -> decode -> composite) over one
 synthetic batch of 65 536 rays x 32 samples per GPU, Technicolor-shape model (technicolor_z_plane: C_in=8,
@@ -11,7 +11,8 @@ defaults (tensor-core sample net).  Weak scaling: every rank renders its own 65 
 in every rank's gather buffer (ray_shard.render_sharded: peer-memory epilogue, else one NCCL all_gather), inside the timed
 region.  Rank 0 prints ONE JSON line; extra keys carry the other BASELINE configurations (DoNeRF shape S=16, Neural-3D
 shape S=64), strong-scaling points and the stated baselines (reference's op sequence on the host CPUs and, eagerly, on
-the same B200).
+the same GPU).  --dump-outputs DIR writes what the last timed step returned (DIR/<key>.npy, float32); the inputs
+are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -36,6 +37,7 @@ PARAM_SEED = 11
 CPU_SAMPLE_RAYS = int(os.environ.get("HR_BENCH_CPU_RAYS", "8192"))  # bounded CPU sample (the env override is for the CPU test)
 L2_FLUSH_BYTES = 512 << 20
 METRIC = "Mrays/s at 65k-ray x 32-sample batch"
+DUMP_BYTES = 64 << 20  # cap of --dump-outputs
 
 # the other single-GPU BASELINE configurations, reported as extra keys (rays per GPU: one 800x800 DoNeRF frame; one eighth
 # of a 2704x2028 Neural-3D frame = the per-GPU share of BASELINE config 4)
@@ -75,18 +77,18 @@ def measured_peaks():
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (NVIDIA H100 SXM data sheet, HBM3)"
 
 
 def measured_tensor_peak():
-    """Dense bf16 TFLOP/s: burst figure of MEASURED_PEAKS.json (cuBLAS 8192^3), else the profiling recipe's fallback."""
+    """Dense bf16 TFLOP/s: burst figure of MEASURED_PEAKS.json (cuBLAS 8192^3), else the data-sheet figure."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
         if "bf16_tflops" in d:
             return float(d["bf16_tflops"]), float(d.get("bf16_tflops_sustained", 0.0)), "measured (MEASURED_PEAKS.json bf16_tflops, cuBLAS burst)"
-    return 1590.0, 1400.0, "fallback (B200_PROFILING.md)"
+    return 989.0, None, "fallback (NVIDIA H100 SXM data sheet, dense BF16)"
 
 
 def usable_cpus() -> int:
@@ -124,7 +126,7 @@ def cpu_model() -> str:
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         super().__init__(daemon=True)
@@ -178,7 +180,7 @@ def workload_config(sig, n: int, world: int) -> dict:
 def time_oracle(cfg, ds, sd, sig, hb, steps: int, warmup: int, rays_n: int, device: str = "cpu"):
     """The reference's op sequence restated (oracle port, same torch ops as the reference: F.grid_sample gathers, boolean-
     mask compaction, cumprod), eager PyTorch.  device='cpu': all usable host threads.  device='cuda': the same eager ops on
-    the B200 -- the "beat eager PyTorch on the same GPU" baseline of SURVEY.md 2.3.  Returns (Mrays/s from the median step,
+    the GPU -- the "beat eager PyTorch on the same GPU" baseline of SURVEY.md 2.3.  Returns (Mrays/s from the median step,
     median ms, threads)."""
     import torch
     from oracle.hyperreel_oracle import HyperReelOracle
@@ -230,7 +232,7 @@ def run_reference(args):
 
 
 def ncu_summary():
-    """Numbers of the committed ncu --set full capture of the render kernel (profiles/render_kernel_traffic.json)."""
+    """Numbers of an ncu --set full capture of the render kernel, when one is stored in profiles/render_kernel_traffic.json."""
     p = os.path.join(ROOT, "profiles", "render_kernel_traffic.json")
     if os.path.exists(p):
         with open(p) as f:
@@ -362,6 +364,21 @@ def run_train_step(torch, hb, dev, steps):
     return out
 
 
+def dump_outputs(out_dir, outputs):
+    """The arrays of the last timed step as out_dir/<key>.npy (float32); a seeded sample of rows when they exceed 64 MiB."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    budget = DUMP_BYTES // max(1, len(outputs))
+    for key, t in outputs.items():
+        rows_max = max(1, budget // max(1, t[0].numel() * 4)) if t.dim() > 0 else 1
+        if t.dim() > 0 and t.shape[0] > rows_max:
+            idx = torch.randperm(t.shape[0], generator=torch.Generator().manual_seed(0))[:rows_max].sort().values
+            t = t[idx]
+        np.save(os.path.join(out_dir, key + ".npy"), t.numpy().astype(np.float32))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -390,10 +407,14 @@ def run_ours(args):
     flush = torch.empty(L2_FLUSH_BYTES // 4, dtype=torch.float32, device=dev)
     gather_mode = "single GPU"
 
+    last = {}
+
     def step():
         if world > 1:
-            return render_sharded(rays_all, render)  # the product path: each rank renders its shard, tiles land everywhere
-        return render(rays)["rgb"]
+            last["rgb"] = render_sharded(rays_all, render)  # the product path: each rank renders its shard, tiles land everywhere
+        else:
+            last.update(render(rays))
+        return last["rgb"]
 
     sampler = ClockSampler(local)
     sampler.start()
@@ -415,6 +436,7 @@ def run_ours(args):
             dist.barrier()
         torch.cuda.synchronize()
         total_ms = timed_steps(torch, step, args.steps, flush)
+        outputs = {k: v.detach().float().cpu() for k, v in last.items() if torch.is_tensor(v)}
         if world > 1:
             dist.barrier()
         launches = model.launch_count() - launches0
@@ -426,6 +448,8 @@ def run_ours(args):
             break
         remeasured = True
         time.sleep(2.0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, outputs)
     # per-kernel durations for the roofline: a second pass with the library's CUDA events around each kernel (kept out of
     # the headline loop so the event records do not sit between the two kernels of a step)
     tm = kernel_times(torch, model, step, args.steps, flush)
@@ -524,13 +548,13 @@ def run_ours(args):
         except Exception as e:  # the render line must survive a failure of the next-tier row
             extras["train_step"] = {"unavailable": repr(e)[:300]}
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
-        try:  # the reference's op sequence, eager PyTorch, on this same B200 (full 65 536-ray batch)
+        try:  # the reference's op sequence, eager PyTorch, on this same GPU (full 65 536-ray batch)
             mr, ms, _ = time_oracle(cfg, ds, sd, sig, hb, 5, 2, n, device=f"cuda:{local}")
-            baselines["torch_eager_b200"] = {"value": mr, "unit": "Mrays/s", "ms_per_step": ms, "rays": n,
+            baselines["torch_eager_gpu"] = {"value": mr, "unit": "Mrays/s", "ms_per_step": ms, "rays": n,
                                              "what": "oracle port (the reference's torch op sequence: grid_sample gathers, mask compaction, cumprod) "
                                                      "run eagerly on cuda:0, fp32, median of 5 after 2 warm-ups; a stated baseline"}
         except Exception as e:  # never let a baseline break the bench line
-            baselines["torch_eager_b200"] = {"unavailable": repr(e)[:200]}
+            baselines["torch_eager_gpu"] = {"unavailable": repr(e)[:200]}
         torch.cuda.empty_cache()
 
     if rank == 0:
@@ -547,12 +571,12 @@ def run_ours(args):
         tach = (2.0 * products * macs * n / (tm["mlp_ms"] * 1e-3) / 1e12) if tm["mlp_ms"] > 0 else 0.0
         cfg_obj = workload_config(sig, n, world)
         cfg_obj["gather"] = gather_mode
-        cfg_obj["sample_net"] = "bf16x3 on tcgen05 (registry default)" if tc else "fp32 CUDA cores"
+        cfg_obj["sample_net"] = "bf16x3 on wgmma (registry default)" if tc else "fp32 CUDA cores"
         line = {
             "metric": METRIC, "value": value, "unit": "Mrays/s", "n_gpus": world,
             "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms_per_step, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None,
-            "dtype": "f32 (sample net bf16x3 split on tcgen05, fp32 accumulate)" if tc else "f32",
+            "dtype": "f32 (sample net bf16x3 split on wgmma, fp32 accumulate)" if tc else "f32",
             "data": "synthetic", "config": cfg_obj,
             "e2e": {"value": e2e_val, "unit": "Mrays/s", "h2d_bytes_per_step": n * sig.c_in * 4, "d2h_bytes_per_step": n * 12,
                     "ms_per_step": float(t2.item()),
@@ -565,7 +589,7 @@ def run_ours(args):
             "roofline_sample_net": {"bound": "tensor" if tc else "fp32 simt", "achieved": tach, "peak": tpeak,
                                     "unit": "TFLOP/s", "frac": tach / tpeak if tpeak else None, "peak_sustained": tsust,
                                     "useful_frac": (tach / products) / tpeak if tpeak else None,
-                                    "kernel": "mlp_tc2_kernel (bf16 hi/lo split, 3 tcgen05.mma per k-step)" if tc else "mlp_simt_kernel",
+                                    "kernel": "mlp_tc2_kernel (bf16 hi/lo split, 3 wgmma per k-step)" if tc else "mlp_simt_kernel",
                                     "algorithmic_macs_per_ray": macs, "executed_flop_per_ray": 2 * products * macs,
                                     "kernel_ms": tm["mlp_ms"], "peak_source": tsrc},
         }
@@ -596,7 +620,10 @@ def main():
     ap.add_argument("--rays", type=int, default=RAYS_PER_GPU)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the arrays the last timed step returned to DIR/<key>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,9 +1,9 @@
-"""hyperreel_b200 -- B200-native drop-in for HyperReel's per-ray rendering hot path.
+"""hyperreel_b200 -- H100-native drop-in for HyperReel's per-ray rendering hot path.
 
 Operator surface (same names as the reference's ``nlf`` package, SURVEY.md section 8b):
 ``render_fn_dict`` / ``RenderLightfield`` / ``render_chunked`` (rendering.py), ``model_dict`` /
 ``LightfieldModel`` (models.py), ``INRSystem`` (system.py).  All compute is in
-``libhyperreel_b200.so`` (csrc/, sm_100a CUDA behind the C-ABI of include/hyperreel_b200.h).
+``libhyperreel_b200.so`` (csrc/, sm_90a CUDA behind the C-ABI of include/hyperreel_b200.h).
 """
 from . import camera, configs, rays  # noqa: F401
 from .camera import Camera, generate_rays  # noqa: F401

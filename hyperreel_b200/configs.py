@@ -1,8 +1,7 @@
 """Built-in model configs in the reference's own schema (the keys ``conf/experiment/model/*.yaml`` uses).
 
-The GPU box has no reference checkout, so the BASELINE.json configurations are generated here from a few
-parametric builders instead of shipping copies of the YAML files; ``tests/test_configs_vs_reference.py``
-asserts (when ``/root/reference`` is present) that each built-in equals ``yaml.safe_load`` of the
+The package ships no copies of the reference's YAML files, so the BASELINE.json configurations are generated here from a few
+parametric builders; ``tests/test_oracle_vs_reference.py`` asserts that each built-in equals ``yaml.safe_load`` of the
 reference file it names.  A user of the reference passes their own YAML through
 ``hyperreel_b200.config.load_model_yaml`` instead.
 

@@ -260,7 +260,7 @@ __global__ void unblend_time_lines(const float* __restrict__ src, float* __restr
 
 int grid_for(long long total) {
   long long g = (total + 255) / 256;
-  if (g > 148 * 32) g = 148 * 32;
+  if (g > 132 * 32) g = 132 * 32;
   if (g < 1) g = 1;
   return (int)g;
 }
@@ -402,7 +402,8 @@ int hr_create(const hr_config* cfg, int device, hr_handle** out) {
   if (device < 0 || device >= ndev) return fail("hr_create: device %d out of range (%d devices)", device, ndev);
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return fail("hr_create: device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0)
+    return fail("hr_create: device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
   DeviceGuard guard(device);
   hr_handle* h = new (std::nothrow) hr_handle();
   if (!h) return fail("hr_create: out of memory");
@@ -619,8 +620,7 @@ static int64_t heads_bytes(const hr_handle* h, int64_t n_rays) {
 
 // hr_render walks a large batch in sub-batches (sample net, then render kernel, per sub-batch) so that the heads scratch
 // stays bounded (0.58 GB at S*15 = 480) instead of growing to 8-21 GB for 4 M-ray batches / full Neural-3D frames.
-// Measured (profiles/r2_notes.md): wave-sized sub-batches that would keep the scratch in L2 cost more in launch ramps than
-// the HBM round trip they save (0.341 vs 0.288 ms per 65 536 rays); 16 tile waves per sub-batch cost ~1.5 % at 1 M rays.
+// Wave-sized sub-batches that would keep the scratch in L2 pay more in launch ramps than the HBM round trip they save.
 static int64_t sub_batch_rays(const hr_handle* h) {
   if (h->sub_rays > 0) return h->sub_rays;
   return (int64_t)h->num_sms * 128 * 16;
@@ -673,7 +673,7 @@ static int launch_net(hr_handle* h, const hr_config& nc, const hr::MlpSimtPack& 
   }
   if (nc.mlp_mode == HR_MLP_BF16X3_TC) {
     if (!tc_ready) return fail("hr_render: tensor-core pack missing");
-    e = hr::launch_mlp_tc2(nc, tc, h->tma_encode, in, out, rows, h->num_sms, st);
+    e = hr::launch_mlp_tc2(nc, tc, in, out, rows, h->num_sms, st);
   } else {
     e = hr::launch_mlp_simt(nc, simt, in, out, rows, h->num_sms, st);
   }
@@ -1014,7 +1014,7 @@ int hr_render_host(hr_handle* h, const float* rays_host, int64_t n_rays, float* 
     float* d_rays = P.d_rays[0];
     float* d_rgb = P.d_rgb[0];
     float* heads = (float*)P.d_ws[0];
-    cudaError_t e = hr::launch_mlp_tc2(c, h->tc, h->tma_encode, rays_dev_view, heads, n_rays, h->num_sms, s0, d_rays);
+    cudaError_t e = hr::launch_mlp_tc2(c, h->tc, rays_dev_view, heads, n_rays, h->num_sms, s0, d_rays);
     if (e != cudaSuccess) return fail("sample-net launch failed: %s", cudaGetErrorString(e));
     h->launches += 1;
     if (rgb_dev_view != nullptr) {

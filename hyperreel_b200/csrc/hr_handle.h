@@ -52,7 +52,6 @@ struct hr_handle {
   bool tc_pre_ready = false;
   size_t tc_pre_alloc_bytes = 0;
   int tc_pre_alloc_bias = 0;
-  void* tma_encode = nullptr; // cuTensorMapEncodeTiled, from cudaGetDriverEntryPoint
   // gradient tables of the backward pass (hr_render_backward), packed like the forward tables; allocated on first use
   float* g_sig_space[3] = {nullptr, nullptr, nullptr};
   float* g_sig_second[3] = {nullptr, nullptr, nullptr};

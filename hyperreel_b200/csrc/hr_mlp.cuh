@@ -20,12 +20,12 @@ struct MlpSimtPack {
   int skip;
 };
 
-// tcgen05 path (HR_MLP_BF16X3_TC): see hr_mlp_tc2.cu.  A "pass" is one accumulator's worth of output columns
+// wgmma path (HR_MLP_BF16X3_TC): see hr_mlp_tc2.cu.  A "pass" is one accumulator's worth of output columns
 // (128 columns of a hidden layer or of the last layer); its weights are stored as n_chunks*2 k-step images.
 #define HR_TC_MAX_PASSES 40  // 10 hidden half passes + 28 last-layer parts (S = 256 x 14 channels)
 struct TcPass {
   int layer;        // Linear layer index
-  int n;            // output columns of this pass (multiple of 16, <= 256)
+  int n;            // output columns of this pass (128; a partial last-layer pass is zero padded)
   int first_chunk;  // first A chunk consumed (0 = encoded input, in_chunks = first hidden chunk)
   int n_chunks;     // chunks of 32 k
   int bias_off;     // offset into the bias table
@@ -34,7 +34,7 @@ struct TcPass {
   int wait_a;       // the issuer must wait for the A chunks (first pass of a layer)
 };
 struct MlpTcPack {
-  const void* wpack;   // bf16 hi/lo weight images, UMMA K-major no-swizzle layout, consumption order
+  const void* wpack;   // bf16 hi/lo weight images, K-major no-swizzle layout, consumption order
   const float* bias;   // [bias_count]
   long long wpack_bytes;
   int n_passes;
@@ -47,10 +47,9 @@ size_t mlp_simt_smem_bytes(const MlpSimtPack& pk, int W);
 cudaError_t launch_mlp_simt(const hr_config& cfg, const MlpSimtPack& pk, const float* rays, float* heads,
                             long long n, int num_sms, cudaStream_t stream);
 
-// rays may point to pinned host memory (read once, by the encoder warps); rays_copy (optional) receives a device copy;
-// tma_encode = the driver's cuTensorMapEncodeTiled (hr_handle::tma_encode)
-cudaError_t launch_mlp_tc2(const hr_config& cfg, const MlpTcPack& pk, void* tma_encode, const float* rays, float* heads,
-                           long long n, int num_sms, cudaStream_t stream, float* rays_copy = nullptr);
+// rays may point to pinned host memory (read once, by the encoding threads); rays_copy (optional) receives a device copy
+cudaError_t launch_mlp_tc2(const hr_config& cfg, const MlpTcPack& pk, const float* rays, float* heads, long long n,
+                           int num_sms, cudaStream_t stream, float* rays_copy = nullptr);
 }  // namespace hr
 
 struct hr_handle;

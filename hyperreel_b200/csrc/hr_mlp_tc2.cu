@@ -1,35 +1,24 @@
-// Sample-prediction network on the 5th-generation tensor cores (HR_MLP_BF16X3_TC).
+// Sample-prediction network on the Hopper tensor cores (HR_MLP_BF16X3_TC), wgmma.
 //
 // Math (reference: nlf/nets/mlp.py:159-172 behind nlf/embedding/ray.py:320-326): every fp32 operand x is split into
 // bf16 hi = rn(x) and lo = rn(x - hi) and each Linear layer is
-//     D = A_hi*B_hi + A_lo*B_hi + A_hi*B_lo          (three tcgen05.mma kind::f16 per k-step, fp32 accumulation in TMEM);
+//     D = A_hi*B_hi + A_lo*B_hi + A_hi*B_lo          (three wgmma m64n128k16 per k-step, fp32 accumulation in registers);
 // the dropped A_lo*B_lo term and the split residuals are O(2^-16) relative per product (DESIGN.md).
 // Hidden width 128 or 256, encoded input up to 64 features (one or two 32-wide input chunks).
 //
-// Where the activation operand lives, so that the tensor pipe never waits for an epilogue:
-//   * every Linear layer is issued as two half passes of N = 128 output columns (the last layer as ceil(out/128) parts),
-//     alternating between two 128-column TMEM accumulators D0 / D1;
-//   * the activation operand is double buffered across layers: layer l reads A(l) from buffer l&1 while the epilogue
-//     of layer l writes A(l+1) into buffer (l+1)&1 -- there is no in-place hazard, so the epilogue of half 0 runs under
-//     the MMAs of half 1, and the next layer's first half starts as soon as its first k-steps exist;
-//   * A_hi (used by two of the three products) lives in TMEM (2 x 128 columns of packed bf16 pairs, written with
-//     tcgen05.st, consumed as the TMEM A operand), A_lo (used once) in shared memory (2 x 64 KB, UMMA K-major
-//     no-swizzle).  Per k-step the tensor pipe reads 4 KB (A_lo) + 3 x 4 KB (weights) of shared memory instead of
-//     3 x 4 KB + 3 x 8 KB of an all-in-shared-memory layout (the measured limiter of the first version, profiles/r1_notes.md).
-//   TMEM map (512 columns): [0,128) A_hi buffer 0 | [128,256) A_hi buffer 1 | [256,384) D0 | [384,512) D1.
-//
-// Warp roles (384 threads, one persistent CTA per SM, one 128-ray tile at a time):
-//   warps 0-7   epilogue, thread = ray (two groups of four warps; group g takes k-step 2j+g of chunk j): TMEM -> bias,
-//               LeakyReLU, bf16 split -> A_hi by tcgen05.st, A_lo by st.shared.  Last layer: 32 x 16 boxes staged in the
-//               idle A_lo buffer and written with TMA tensor stores.
-//   warp 8      weight producer: cp.async.bulk ring, one stage = one 32-k chunk of one pass (two k-step images).
-//   warp 9      MMA issuer: the whole warp runs the loop, the tcgen05 instructions are guarded by elect.sync (ptxas then
-//               keeps all operands in uniform registers; inside `if (lane == 0)` it wraps every UTCHMMA in an ELECT/branch
-//               loop and the issue rate, not the tensor pipe, bounds an N = 128 layout).
-//   warps 10-11 ray encoders: RayParam + WindowedPE of the NEXT tile into the other encoded-input buffer (inputs wider than
-//               32 features have one buffer, released after the skip layer so the encode still hides under layers 4..).
-// Measured on B200 (profiles/r1_notes.md): 51 K cycles per tile in steady state (14 passes x 3.3-3.7 K) against 81 K for
-// the first layout; the kernel now runs power-limited (~1.68 GHz SM clock under this tensor load).
+// Layout (one persistent CTA per SM, one 128-ray tile at a time):
+//   * warpgroups 0 and 1 each own 64 rays of the tile (wgmma M = 64) and everything about them: they encode their rays
+//     into the input operand, issue the wgmmas of every layer, and run the epilogues.  A warpgroup's operand rows are
+//     read by its own wgmmas only, so the two warpgroups never wait for each other, and one's epilogue runs under the
+//     other's MMAs;
+//   * every Linear layer is issued as passes of N = 128 output columns (a 256-wide hidden layer as two passes held in
+//     two register accumulators, the last layer as ceil(out / 128) passes);
+//   * the activation operand A (hi and lo, 2 x 64 KB, K-major no-swizzle) is rewritten in place by the epilogue of the
+//     layer that reads it: the warpgroup's wgmmas of that layer have all retired by then (wgmma.wait_group 0);
+//   * warp 8 streams the weight images (bf16 hi + lo, consumption order, hr_tc_pack.cu) through a 4-stage
+//     cp.async.bulk ring guarded by mbarriers; each consumer warpgroup releases a stage once the wgmmas that read it
+//     have retired.
+// The last layer's columns go from the accumulators (+ bias) straight to the heads scratch in global memory.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -46,434 +35,232 @@ namespace hr {
 namespace tc2 {
 using namespace tc;
 
-constexpr int NSTAGE = 3;           // weight ring depth
-constexpr int STAGE_BYTES = 16384;  // one 32-k chunk of a pass: two k-step images of N<=128 rows x 16 k x (hi+lo) bf16
-constexpr int KSTEP_BYTES = 4096;   // 128 rays x 16 k bf16
-constexpr int NKSTEP = 16;          // hidden width 256 / 16
-constexpr int EPI_GROUPS = 2;
-constexpr int EPI_WARPS = 4 * EPI_GROUPS;
-constexpr int ENC_WARPS = 2;         // ray encoders: each thread encodes rows t, t + 64 of the next tile
-constexpr int NTHREADS = (EPI_WARPS + 2 + ENC_WARPS) * 32;
-constexpr int BIAS_FLOATS = 2560;
-constexpr int STG_BOXES = 4;         // 32 x 16 fp32 TMA-store boxes per epilogue warp, carved from the idle A_lo buffer
+constexpr int PASS_N = 128;          // output columns of one pass (wgmma N)
+constexpr int NSTAGE = 4;            // weight ring depth
+constexpr int STAGE_BYTES = 16384;   // one 32-k chunk of a pass: two k-step images of 128 rows x 16 k x (hi+lo) bf16
+constexpr int KSTEP_BYTES = 4096;    // 128 rays x 16 k bf16
+constexpr int NKSTEP = 16;           // hidden width 256 / 16
+constexpr int CONSUMERS = 2;         // warpgroups of 64 rays
+constexpr int NTHREADS = CONSUMERS * 128 + 32;
 
 // shared memory map (bytes)
-constexpr int ALO_BUF_BYTES = NKSTEP * KSTEP_BYTES;          // 64 KB per A_lo buffer
-constexpr int OFF_ALO = 0;                                   // [2 buffers][16 k-steps][4 KB]
-constexpr int X_BUF_BYTES = 4 * KSTEP_BYTES;                 // encoded input of one tile: 2 k-steps (32 k) x (hi, lo); a 64-wide
-                                                             // input uses both buffers as one: 4 k-steps x (hi, lo)
-constexpr int OFF_X = OFF_ALO + 2 * ALO_BUF_BYTES;           // 131072: [2 tiles][hi 8 KB | lo 8 KB]
-constexpr int OFF_B = OFF_X + 2 * X_BUF_BYTES;               // 163840
-constexpr int OFF_BIAS = OFF_B + NSTAGE * STAGE_BYTES;       // 212992
-constexpr int OFF_BAR = OFF_BIAS + BIAS_FLOATS * 4;          // 223232
-constexpr int SMEM_BYTES = OFF_BAR + 512;                    // 223744 (of 232448 available)
+constexpr int A_BYTES = NKSTEP * KSTEP_BYTES;                // 64 KB: one half (hi or lo) of the activation operand
+constexpr int OFF_AHI = 0;
+constexpr int OFF_ALO = OFF_AHI + A_BYTES;
+constexpr int X_BYTES = 4 * KSTEP_BYTES;                     // encoded input: up to 4 k-steps (64 k) hi, then as many lo
+constexpr int OFF_X = OFF_ALO + A_BYTES;                     // 131072
+constexpr int OFF_B = OFF_X + 2 * X_BYTES;                   // 163840
+constexpr int OFF_BAR = OFF_B + NSTAGE * STAGE_BYTES;        // 229376
+constexpr int SMEM_BYTES = OFF_BAR + 128;                    // 229504 (of 232448 available)
 static_assert(SMEM_BYTES <= 232448, "shared memory budget");
-static_assert(EPI_WARPS * STG_BOXES * 2048 <= ALO_BUF_BYTES, "staging boxes fit the idle A_lo buffer");
-
-// TMEM columns
-constexpr int TM_AHI = 0;   // + buffer * 128
-constexpr int TM_D = 256;   // + accumulator * 128
 
 // barrier slots (8 bytes each) inside OFF_BAR
-constexpr int BAR_FULL = 0;                        // [NSTAGE]
-constexpr int BAR_EMPTY = BAR_FULL + NSTAGE;       // [NSTAGE]
-constexpr int NCHUNK = 8;                          // hidden width 256 / 32
-constexpr int BAR_AREADY = BAR_EMPTY + NSTAGE;     // [1 + NCHUNK]: 0 = encoded input, 1+j = hidden chunk j (k-steps 2j, 2j+1)
-constexpr int BAR_DFULL = BAR_AREADY + 1 + NCHUNK; // [2]
-constexpr int BAR_DEMPTY = BAR_DFULL + 2;          // [2]
-constexpr int BAR_XFREE = BAR_DEMPTY + 2;          // [2]: encoded-input buffer b may be overwritten
-constexpr int BAR_TMEMPTR = BAR_XFREE + 2;         // 4-byte TMEM base address lives in this slot
-static_assert((BAR_TMEMPTR + 1) * 8 <= 512, "barrier block");
-
-// Offset (bytes) of the 16-byte slot holding k-group kg (0/1) of row `row` inside a 128-row x 16-k k-step image.
-__device__ __forceinline__ uint32_t ks_slot(int row, int kg) { return (uint32_t)((kg * 16 + (row >> 3)) * 128 + (row & 7) * 16); }
+constexpr int BAR_FULL = 0;                   // [NSTAGE]
+constexpr int BAR_EMPTY = BAR_FULL + NSTAGE;  // [NSTAGE]
+static_assert((BAR_EMPTY + NSTAGE) * 8 <= 128, "barrier block");
 
 }  // namespace tc2
 
 __global__ void __launch_bounds__(tc2::NTHREADS, 1)
 mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ MlpTcPack pk, const float* __restrict__ rays,
-               float* __restrict__ heads, long long n_rays, unsigned long long* trace,
-               const __grid_constant__ CUtensorMap heads_map, float* __restrict__ rays_copy, int trace_iter) {
+               float* __restrict__ heads, long long n_rays, float* __restrict__ rays_copy) {
   using namespace tc2;
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t sbase = smem_u32(smem);
-  const bool tracing0 = (trace != nullptr) && (blockIdx.x == 0);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  float* s_bias = reinterpret_cast<float*>(smem + OFF_BIAS);
   auto bar = [&](int slot) -> uint32_t { return sbase + OFF_BAR + slot * 8; };
-  volatile uint32_t* s_tmem = reinterpret_cast<volatile uint32_t*>(smem + OFF_BAR + BAR_TMEMPTR * 8);
 
   // ---- one-time setup ----
   {
-    // pull the weight stream into L2 once (every CTA walks the same 1.5 MB per tile; after a cold start the first walk
+    // pull the weight stream into L2 once (every CTA walks the same weights per tile; after a cold start the first walk
     // would otherwise pay DRAM latency on every ring stage)
     const char* w = reinterpret_cast<const char*>(pk.wpack);
     const long long lines = pk.wpack_bytes >> 7;
     for (long long i = (long long)blockIdx.x * NTHREADS + tid; i < lines; i += (long long)gridDim.x * NTHREADS)
       asm volatile("prefetch.global.L2 [%0];" ::"l"(w + i * 128));
   }
-  for (int i = tid; i < min(pk.bias_count, BIAS_FLOATS); i += NTHREADS) s_bias[i] = pk.bias[i];
-  for (int i = tid; i < (2 * X_BUF_BYTES) / 16; i += NTHREADS)  // encoded-input operands: columns >= mlp_in stay zero
+  for (int i = tid; i < (2 * X_BYTES) / 16; i += NTHREADS)  // encoded-input operand: columns >= mlp_in stay zero
     reinterpret_cast<uint4*>(smem + OFF_X)[i] = make_uint4(0u, 0u, 0u, 0u);
-  fence_async_smem();
-  if (tracing0 && tid == 0) trace[240] = clock64();
-  if (trace != nullptr && tid == 0) {  // per-CTA wall-clock record: [256 + 3*cta] = {start ns, end ns, cycles}
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    trace[256 + 3 * blockIdx.x] = t;
-    trace[256 + 3 * blockIdx.x + 2] = clock64();
-  }
   if (tid == 0) {
-    for (int s = 0; s < NSTAGE; ++s) { mbar_init(bar(BAR_FULL + s), 1); mbar_init(bar(BAR_EMPTY + s), 1); }
-    mbar_init(bar(BAR_AREADY + 0), 32 * ENC_WARPS);                                       // encoded input: the encoder warps
-    for (int c = 1; c <= NCHUNK; ++c) mbar_init(bar(BAR_AREADY + c), 128 * EPI_GROUPS);  // every group writes a part of each chunk
-    for (int b = 0; b < 2; ++b) mbar_init(bar(BAR_XFREE + b), 1);
-    for (int d = 0; d < 2; ++d) { mbar_init(bar(BAR_DFULL + d), 1); mbar_init(bar(BAR_DEMPTY + d), 128 * EPI_GROUPS); }
+    for (int s = 0; s < NSTAGE; ++s) { mbar_init(bar(BAR_FULL + s), 1); mbar_init(bar(BAR_EMPTY + s), CONSUMERS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == EPI_WARPS + 1) {
-    uint32_t dst = sbase + OFF_BAR + BAR_TMEMPTR * 8;
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(dst) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *s_tmem;
 
   const long long n_tiles = (n_rays + BM - 1) / BM;
   const int n_passes = pk.n_passes;
   // tiles blockIdx.x, blockIdx.x + gridDim.x, ... : every role of this CTA runs exactly this many iterations
   const long long n_iters = ((long long)blockIdx.x < n_tiles) ? (n_tiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
-  // diagnostic timeline (HR_TC_TRACE): CTA 0, second tile; slot = pass * 8 + event
-  const bool tracing = (trace != nullptr) && (blockIdx.x == 0);
-  auto TR = [&](long long iter, int pass, int ev) {
-    if (tracing && iter == trace_iter && (threadIdx.x & 31) == 0) trace[pass * 8 + ev] = clock64();
-  };
 
-  if (warp == EPI_WARPS) {
+  if (warp == CONSUMERS * 4) {
     // =========================== producer: weight images, in consumption order ===========================
-    // One ring stage = one 32-k chunk of one pass = two consecutive k-step images (hi+lo each).
     if (lane == 0) {
       uint32_t stage = 0, phase = 0;
       for (long long iter = 0; iter < n_iters; ++iter) {
         const uint8_t* src = reinterpret_cast<const uint8_t*>(pk.wpack);
         for (int p = 0; p < n_passes; ++p) {
-          const uint32_t bytes = (uint32_t)pk.passes[p].n * 128u;
-          const int n_ch = pk.passes[p].n_chunks;
-          for (int i = 0; i < n_ch; ++i) {
+          for (int i = 0; i < pk.passes[p].n_chunks; ++i) {
             mbar_wait(bar(BAR_EMPTY + stage), phase ^ 1);
-            mbar_expect_tx(bar(BAR_FULL + stage), bytes);
-            bulk_g2s(sbase + OFF_B + stage * STAGE_BYTES, src, bytes, bar(BAR_FULL + stage));
-            src += bytes;
+            mbar_expect_tx(bar(BAR_FULL + stage), STAGE_BYTES);
+            bulk_g2s(sbase + OFF_B + stage * STAGE_BYTES, src, STAGE_BYTES, bar(BAR_FULL + stage));
+            src += STAGE_BYTES;
             if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
           }
         }
       }
     }
-  } else if (warp == EPI_WARPS + 1) {
-    // =========================== MMA issuer ===========================
-    // The issuer's own instruction stream is the critical path (measured: with N = 128 the MMAs retire faster than a
-    // naive loop can issue them).  So: the whole warp runs this loop in uniform control flow and only the tcgen05
-    // instructions are guarded by elect.sync -- ptxas then keeps every operand in uniform registers and emits bare UTCHMMA
-    // (inside an `if (lane == 0)` region it wraps each one in an ELECT/branch loop and R2UR moves); a whole 32-k chunk -- six
-    // MMAs and the stage-release commit -- goes out per barrier wait; the pass descriptor is read once per pass.
-    {
-      uint32_t stage = 0, phase = 0, gp = 0, titer = 0;
-      const uint32_t n_hidden = (uint32_t)cfg.mlp_layers - 1u;
-      const int in_chunks = pk.in_chunks;            // 32-wide chunks of the encoded input: 1 or 2
-      const bool x_double = (in_chunks == 1);        // two encoded-input buffers (tile parity) or one
-      const uint64_t xdesc_hi0 = umma_desc(sbase + OFF_X, 2048, 128);
-      const uint64_t xdesc_lo0 = umma_desc(sbase + OFF_X + 2 * in_chunks * KSTEP_BYTES, 2048, 128);
-      const uint32_t full0 = bar(BAR_FULL), empty0 = bar(BAR_EMPTY), aready0 = bar(BAR_AREADY);
-      // Pass after which the encoders may write the next tile's input.  Two buffers: the last pass of the first layer
-      // (everything that read the *other* buffer -- the previous tile's first and skip layers -- was issued before it).
-      // One buffer: the last pass that reads the input at all (skip layer, else first layer).
-      int p_x = 0;
-      for (int p = 0; p < n_passes; ++p)
-        if (pk.passes[p].first_chunk == 0 && (pk.passes[p].layer == 0 || !x_double)) p_x = p;
-      for (long long iter = 0; iter < n_iters; ++iter, ++titer) {
-        for (int p = 0; p < n_passes; ++p, ++gp) {
-          const int Pn = pk.passes[p].n, Player = pk.passes[p].layer, Pfirst = pk.passes[p].first_chunk;
-          const int Pchunks = pk.passes[p].n_chunks, Pwait = pk.passes[p].wait_a;
-          const uint32_t db = gp & 1, use = gp >> 1;
-          const uint32_t d_tmem = tmem_base + TM_D + db * 128;
-          const uint32_t idesc = umma_idesc(Pn);
-          const uint64_t img = (uint64_t)((Pn * 64) >> 4);  // descriptor units between the two k-step images of a stage
-          const uint64_t wdesc_hi0 = umma_desc(sbase + OFF_B, (uint32_t)Pn * 16, 128);
-          const uint64_t wdesc_lo0 = umma_desc(sbase + OFF_B + (uint32_t)Pn * 32, (uint32_t)Pn * 16, 128);
-          const uint32_t abuf = (uint32_t)Player & 1u;  // A(l) lives in buffer l & 1
-          uint32_t a_hi = tmem_base + TM_AHI + abuf * 128;
-          uint64_t a_lo = umma_desc(sbase + OFF_ALO + abuf * ALO_BUF_BYTES, 2048, 128);
-          mbar_wait(bar(BAR_DEMPTY + db), (use & 1) ^ 1);  // accumulator drained by its previous reader
-          TR(iter, p, 0);
-          uint32_t acc = 0;
-          int n_h = Pchunks;
-          if (Pfirst == 0) {
-            // ---- encoded input (32 k per chunk): both halves of the split come from shared memory ----
-            n_h -= in_chunks;
-            // written once per tile (during the previous tile); only the first layer has to wait for it
-            if (Player == 0 && Pwait) mbar_wait(aready0, titer & 1);
-            const uint64_t xoff = x_double ? (uint64_t)(((titer & 1u) * X_BUF_BYTES) >> 4) : 0ull;
-            for (int ic = 0; ic < in_chunks; ++ic) {
-              const uint64_t coff = xoff + (uint64_t)((ic * 2 * KSTEP_BYTES) >> 4);
-              const uint64_t xdesc_hi = xdesc_hi0 + coff, xdesc_lo = xdesc_lo0 + coff;
-              mbar_wait(full0 + stage * 8, phase);
-              tc_fence_after();
-              const uint64_t woff = (uint64_t)((stage * STAGE_BYTES) >> 4);
-              asm volatile(
-                  "{\n\t"
-                  ".reg .pred e, p, q;\n\t"
-                  ".reg .b64 xh1, xl1, wh1, wl1;\n\t"
-                  "elect.sync _|e, 0xffffffff;\n\t"
-                  "setp.ne.b32 p, %8, 0;\n\t"
-                  "setp.eq.b32 q, %5, %5;\n\t"
-                  "add.s64 xh1, %1, 256;\n\t"
-                  "add.s64 xl1, %2, 256;\n\t"
-                  "add.s64 wh1, %3, %7;\n\t"
-                  "add.s64 wl1, %4, %7;\n\t"
-                  "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %3, %5, p;\n\t"
-                  "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %2, %3, %5, q;\n\t"
-                  "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %4, %5, q;\n\t"
-                  "@e tcgen05.mma.cta_group::1.kind::f16 [%0], xh1, wh1, %5, q;\n\t"
-                  "@e tcgen05.mma.cta_group::1.kind::f16 [%0], xl1, wh1, %5, q;\n\t"
-                  "@e tcgen05.mma.cta_group::1.kind::f16 [%0], xh1, wl1, %5, q;\n\t"
-                  "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%6];\n\t"
-                  "}" ::"r"(d_tmem),
-                  "l"(xdesc_hi), "l"(xdesc_lo), "l"(wdesc_hi0 + woff), "l"(wdesc_lo0 + woff), "r"(idesc), "r"(empty0 + stage * 8),
-                  "l"(img), "r"(acc)
-                  : "memory");
-              acc = 1;
-              if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
-            }
-          }
-          // ---- hidden activations: A_hi from TMEM (8 packed columns per k-step), A_lo from shared memory ----
-          const uint32_t a_par = (titer * n_hidden + (uint32_t)(Player - 1)) & 1u;
-          uint32_t abar = aready0 + 8;
-          for (int j = 0; j < n_h; ++j) {
-            if (Pwait) {
-              mbar_wait(abar, a_par);
-              abar += 8;
-              if (j == 0) TR(iter, p, 1);
-              if (j == n_h - 1) TR(iter, p, 2);
-            }
-            mbar_wait(full0 + stage * 8, phase);
-            tc_fence_after();
-            const uint64_t woff = (uint64_t)((stage * STAGE_BYTES) >> 4);
-            asm volatile(
-                "{\n\t"
-                ".reg .pred e, p, q;\n\t"
-                ".reg .b64 al1, wh1, wl1;\n\t"
-                ".reg .b32 ah1;\n\t"
-                "elect.sync _|e, 0xffffffff;\n\t"
-                "setp.ne.b32 p, %6, 0;\n\t"
-                "setp.eq.b32 q, %6, %6;\n\t"
-                "add.s32 ah1, %1, 8;\n\t"
-                "add.s64 al1, %2, 256;\n\t"
-                "add.s64 wh1, %3, %8;\n\t"
-                "add.s64 wl1, %4, %8;\n\t"
-                "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %3, %5, p;\n\t"
-                "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %2, %3, %5, q;\n\t"
-                "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %4, %5, q;\n\t"
-                "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [ah1], wh1, %5, q;\n\t"
-                "@e tcgen05.mma.cta_group::1.kind::f16 [%0], al1, wh1, %5, q;\n\t"
-                "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [ah1], wl1, %5, q;\n\t"
-                "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%7];\n\t"
-                "}" ::"r"(d_tmem),
-                "r"(a_hi), "l"(a_lo), "l"(wdesc_hi0 + woff), "l"(wdesc_lo0 + woff), "r"(idesc), "r"(acc), "r"(empty0 + stage * 8),
-                "l"(img)
-                : "memory");
-            acc = 1;
-            a_hi += 16;
-            a_lo += (uint64_t)((2 * KSTEP_BYTES) >> 4);
-            if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
-          }
-          asm volatile(
-              "{\n\t.reg .pred e;\n\telect.sync _|e, 0xffffffff;\n\t"
-              "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(bar(BAR_DFULL + db))
-              : "memory");  // accumulator complete -> epilogue
-          if (p == p_x) {
-            // see p_x above: the encoders may now fill the next tile's input buffer
-            asm volatile(
-                "{\n\t.reg .pred e;\n\telect.sync _|e, 0xffffffff;\n\t"
-                "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(bar(BAR_XFREE + (x_double ? ((titer + 1u) & 1u) : 0u)))
-                : "memory");
-          }
-          TR(iter, p, 3);
-        }
-      }
-    }
-  } else if (warp >= EPI_WARPS + 2) {
-    // =========================== ray encoders ===========================
-    // RayParam + WindowedPE (encode_ray_features) of tile j into encoded-input buffer j & 1, every feature straight to its
-    // bf16 hi / lo slot of the UMMA-layout operand.  Runs one tile ahead of the tensor pipe: buffer b is released by the
-    // issuer (BAR_XFREE) once the previous tile's readers have retired.
-    const int et = (warp - (EPI_WARPS + 2)) * 32 + lane;  // 0 .. 63
-    const bool vec_ok = ((reinterpret_cast<uintptr_t>(rays) | reinterpret_cast<uintptr_t>(rays_copy)) & 15) == 0;
-    const bool x_double = (pk.in_chunks == 1);
-    const uint32_t x_lo_off = (uint32_t)(2 * pk.in_chunks * KSTEP_BYTES);  // lo half follows the hi k-steps
-    for (long long j = 0; j < n_iters; ++j) {
-      const uint32_t xb = x_double ? (uint32_t)(j & 1) : 0u;
-      // buffer xb was released once per two tiles (two buffers) / once per tile (one buffer)
-      if (j >= 1) mbar_wait(bar(BAR_XFREE + xb), x_double ? (uint32_t)(((j - 1) >> 1) & 1) : (uint32_t)((j - 1) & 1));
-      uint8_t* xhi = smem + OFF_X + xb * X_BUF_BYTES;
-      const long long tile = j * gridDim.x + blockIdx.x;
-      for (int r = et; r < BM; r += 32 * ENC_WARPS) {
-        auto put = [&](int k, float val) {
-          const __nv_bfloat16 hi = __float2bfloat16_rn(val);
-          const __nv_bfloat16 lo = __float2bfloat16_rn(val - __bfloat162float(hi));
-          const uint32_t off = (uint32_t)(k >> 4) * KSTEP_BYTES + ks_slot(r, (k >> 3) & 1) + (uint32_t)(k & 7) * 2u;
-          *reinterpret_cast<__nv_bfloat16*>(xhi + off) = hi;
-          *reinterpret_cast<__nv_bfloat16*>(xhi + x_lo_off + off) = lo;
-        };
-        const long long ray = tile * BM + r;
-        if (ray < n_rays) {
-          // The ray is read exactly once, with vector loads: `rays` may be pinned host memory (zero-copy input of
-          // hr_render_host), in which case this warp's loads are the host->device transfer, one tile ahead of the math,
-          // and `rays_copy` receives the device copy the render kernel reads.
-          float rbuf[16];
-          const float* src = rays + ray * cfg.c_in;
-          if (cfg.c_in == 8 && vec_ok) {
-            const float4 a = *reinterpret_cast<const float4*>(src), b = *reinterpret_cast<const float4*>(src + 4);
-            rbuf[0] = a.x; rbuf[1] = a.y; rbuf[2] = a.z; rbuf[3] = a.w; rbuf[4] = b.x; rbuf[5] = b.y; rbuf[6] = b.z; rbuf[7] = b.w;
-            if (rays_copy != nullptr) {
-              float4* dst = reinterpret_cast<float4*>(rays_copy + ray * 8);
-              dst[0] = a; dst[1] = b;
-            }
-          } else {
-            for (int i = 0; i < cfg.c_in; ++i) rbuf[i] = src[i];
-            if (rays_copy != nullptr)
-              for (int i = 0; i < cfg.c_in; ++i) rays_copy[ray * cfg.c_in + i] = rbuf[i];
-          }
-          encode_ray_features(cfg, rbuf, 0, 1, put);
-        } else {
-          for (int k = 0; k < cfg.mlp_in; ++k) put(k, 0.0f);  // masked row: defined (never stored) values
-        }
-      }
-      fence_async_smem();
-      mbar_arrive(bar(BAR_AREADY + 0));
-    }
-  } else {
-    // =========================== epilogue warps: thread = ray ===========================
-    const int grp = warp >> 2;               // 0 .. EPI_GROUPS-1
-    const int row = (warp & 3) * 32 + lane;  // TMEM lane == ray within the tile
-    const uint32_t lane_base = ((uint32_t)((warp & 3) * 32)) << 16;
-    uint32_t gp = 0, box = 0;
-    // TMA-store staging: the A_lo buffer the last layer does not read (its parity is mlp_layers & 1) is idle from the
-    // moment the last layer's first accumulator is complete until the next tile's second layer is written.
-    const uint32_t stg_off = OFF_ALO + (uint32_t)(cfg.mlp_layers & 1) * ALO_BUF_BYTES + (uint32_t)warp * (STG_BOXES * 2048);
-    for (long long iter = 0; iter < n_iters; ++iter) {
-      const long long tile = iter * gridDim.x + blockIdx.x;  // may be >= n_tiles: fully masked
-      const long long ray = tile * BM + row;
-      // The first tile is encoded here; every later tile is encoded under the previous tile's last layer.
-      if (tracing0 && tid == 0 && iter < 16) trace[224 + iter] = clock64();
-      for (int p = 0; p < n_passes; ++p, ++gp) {
-        const TcPass& P = pk.passes[p];
-        const uint32_t db = gp & 1, use = gp >> 1;
-        mbar_wait(bar(BAR_DFULL + db), use & 1);
-        if (tid == 0) TR(iter, p, 4);
-        tc_fence_after();
-        const uint32_t t_addr = tmem_base + lane_base + TM_D + db * 128;
-        const float* bias = s_bias + P.bias_off;  // hidden layers always fit the table (pack_mlp_tc2 checks)
-        if (!P.is_final) {
-          // Hidden half pass: columns [out_col0, out_col0 + 128) of layer l = k-steps 8h .. 8h+7 of A(l+1).  Group g
-          // takes the 16 columns of k-step 8h + 2jj + g in sweep jj, so k-steps become ready in consumption order.
-          const uint32_t nb = (uint32_t)(P.layer + 1) & 1u;
-          const uint32_t ahi_t = tmem_base + lane_base + TM_AHI + nb * 128;
-          uint8_t* alo = smem + OFF_ALO + nb * ALO_BUF_BYTES;
-          const int kk0 = (P.out_col0 >> 4);
-#pragma unroll 1
-          for (int jj = 0; jj < 4; ++jj) {
-            const int sub = jj * 2 + grp;  // 16-column slice of this half pass
-            uint32_t v[16];
-            tmem_ld16(t_addr + sub * 16, v);
-            if (jj == 3) { tc_fence_before(); mbar_arrive(bar(BAR_DEMPTY + db)); }
-            const float4* b4 = reinterpret_cast<const float4*>(bias + sub * 16);
-            uint32_t hi_regs[8];
-            const int kk = kk0 + sub;
-#pragma unroll
-            for (int kg = 0; kg < 2; ++kg) {
-              const float4 ba = b4[kg * 2], bb = b4[kg * 2 + 1];
-              const float bv[8] = {ba.x, ba.y, ba.z, ba.w, bb.x, bb.y, bb.z, bb.w};
-              float x[8];
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float t = __uint_as_float(v[kg * 8 + i]) + bv[i];
-                x[i] = fmaxf(t, t * cfg.leaky_slope);  // LeakyReLU, slope in (0,1)
-              }
-              uint4 hi, lo;
-              split8(x, hi, lo);
-              hi_regs[kg * 4 + 0] = hi.x; hi_regs[kg * 4 + 1] = hi.y; hi_regs[kg * 4 + 2] = hi.z; hi_regs[kg * 4 + 3] = hi.w;
-              *reinterpret_cast<uint4*>(alo + kk * KSTEP_BYTES + ks_slot(row, kg)) = lo;
-            }
-            tmem_st8(ahi_t + (uint32_t)kk * 8u, hi_regs);
-            tmem_st_wait();
-            tc_fence_before();
-            fence_async_smem();
-            mbar_arrive(bar(BAR_AREADY + 1 + (kk >> 1)));
-            if (tid == 0 && jj == 0) TR(iter, p, 5);
-            if (tid == 0 && jj == 3) TR(iter, p, 6);
-          }
-        } else {
-          // Last layer: 16-column slices go TMEM -> registers -> 32 x 16 box in shared memory (row = lane) -> one TMA tensor
-          // store per box (rows past n_rays / columns past mlp_out are clipped by the tensor map).  Two boxes per warp.
-          // biases past the shared-memory table (very wide last layers: S = 256) are read from global memory
-          if (P.bias_off + P.n > BIAS_FLOATS) bias = pk.bias + P.bias_off;
-          const int nslice = (P.n + 15) / 16;
-          const int last_h = (grp < nslice) ? ((nslice - 1 - grp) / EPI_GROUPS) * EPI_GROUPS + grp : -1;
-          if (last_h < 0) { tc_fence_before(); mbar_arrive(bar(BAR_DEMPTY + db)); }
-          for (int h = grp; h < nslice; h += EPI_GROUPS) {
-            uint32_t v[16];
-            tmem_ld16(t_addr + h * 16, v);
-            if (h == last_h) { tc_fence_before(); mbar_arrive(bar(BAR_DEMPTY + db)); }
-            const float4* b4 = reinterpret_cast<const float4*>(bias + h * 16);
-            const uint32_t stg_s = sbase + stg_off + box * 2048;
-            box = (box + 1) & (STG_BOXES - 1);
-            // the store issued STG_BOXES boxes ago must have been read out of this box
-            if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 3;" ::: "memory");
-            __syncwarp();
-#pragma unroll
-            for (int i4 = 0; i4 < 4; ++i4) {
-              const float4 b = b4[i4];
-              float4 o;
-              o.x = __uint_as_float(v[i4 * 4 + 0]) + b.x;
-              o.y = __uint_as_float(v[i4 * 4 + 1]) + b.y;
-              o.z = __uint_as_float(v[i4 * 4 + 2]) + b.z;
-              o.w = __uint_as_float(v[i4 * 4 + 3]) + b.w;
-              asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(stg_s + lane * 64 + i4 * 16), "f"(o.x), "f"(o.y),
-                           "f"(o.z), "f"(o.w)
-                           : "memory");
-            }
-            fence_async_smem();
-            __syncwarp();
-            if (lane == 0) {
-              const int x = P.out_col0 + h * 16;
-              const int y = (int)(tile * BM + (warp & 3) * 32);
-              asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];" ::"l"(
-                               reinterpret_cast<uint64_t>(&heads_map)),
-                           "r"(x), "r"(y), "r"(stg_s)
-                           : "memory");
-              asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            }
-          }
-        }
-      }
-    }
+    return;
   }
 
-  // ---- teardown ----
-  if (tracing0 && tid == 0) trace[241] = clock64();
-  if (trace != nullptr && tid == 0) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    trace[256 + 3 * blockIdx.x + 1] = t;
-    trace[256 + 3 * blockIdx.x + 2] = clock64() - trace[256 + 3 * blockIdx.x + 2];
-  }
-  if (warp < EPI_WARPS && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // TMA stores landed
-  tc_fence_before();
-  __syncthreads();
-  if (warp == EPI_WARPS + 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
+  // =========================== consumer warpgroups: 64 rays each ===========================
+  const int wg = warp >> 2;                 // 0 .. CONSUMERS-1
+  const int wt = tid & 127;                 // thread within the warpgroup
+  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // tile rows of accumulator elements (i / 2) % 2 == 0; +8 for 1
+  const int q2 = (lane & 3) * 2;            // first of the two columns of an accumulator pair
+  const int in_chunks = pk.in_chunks;
+  const int W = cfg.mlp_width;
+  const int L = cfg.mlp_layers;
+  const uint32_t x_lo_off = (uint32_t)(2 * in_chunks * KSTEP_BYTES);  // lo half follows the hi k-steps
+  const uint32_t rows_off = (uint32_t)wg * 1024u;                     // this warpgroup's 8 row groups of a k-step image
+  const uint32_t full0 = bar(BAR_FULL), empty0 = bar(BAR_EMPTY);
+  const bool vec_ok = ((reinterpret_cast<uintptr_t>(rays) | reinterpret_cast<uintptr_t>(rays_copy)) & 15) == 0;
+  uint32_t stage = 0, phase = 0;
+  int pend = -1;  // ring stage whose wgmmas were committed but not yet waited for
+
+  float acc0[64], acc1[64];
+
+  // one pass: acc = A(chunks of P) * B(P)^T, 3 wgmmas per k-step; the ring stage of each chunk is released one chunk later
+  auto run_pass = [&](float (&acc)[64], const TcPass& P) {
+    for (int c = P.first_chunk; c < P.first_chunk + P.n_chunks; ++c) {
+      uint32_t a_hi, a_lo;
+      if (c < in_chunks) {
+        a_hi = sbase + OFF_X + (uint32_t)(2 * c) * KSTEP_BYTES + rows_off;
+        a_lo = a_hi + x_lo_off;
+      } else {
+        a_hi = sbase + OFF_AHI + (uint32_t)(2 * (c - in_chunks)) * KSTEP_BYTES + rows_off;
+        a_lo = a_hi + (OFF_ALO - OFF_AHI);
+      }
+      mbar_wait(full0 + stage * 8, phase);
+      const uint32_t b0 = sbase + OFF_B + stage * STAGE_BYTES;
+      wgmma_fence();
+      acc_fence(acc);
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) {
+        const uint64_t ah = gmma_desc(a_hi + ks * KSTEP_BYTES, 2048, 128);
+        const uint64_t al = gmma_desc(a_lo + ks * KSTEP_BYTES, 2048, 128);
+        const uint64_t bh = gmma_desc(b0 + ks * (PASS_N * 64), PASS_N * 16, 128);
+        const uint64_t bl = gmma_desc(b0 + ks * (PASS_N * 64) + PASS_N * 32, PASS_N * 16, 128);
+        wgmma_128(acc, ah, bh, (c != P.first_chunk || ks != 0) ? 1u : 0u);
+        wgmma_128(acc, al, bh, 1u);
+        wgmma_128(acc, ah, bl, 1u);
+      }
+      wgmma_commit();
+      acc_fence(acc);
+      wgmma_wait<1>();
+      if (pend >= 0 && wt == 0) mbar_arrive(empty0 + pend * 8);
+      pend = (int)stage;
+      if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
+    }
+  };
+  auto drain = [&]() {
+    wgmma_wait<0>();
+    acc_fence(acc0);
+    acc_fence(acc1);
+    if (pend >= 0 && wt == 0) mbar_arrive(empty0 + pend * 8);
+    pend = -1;
+  };
+  // hidden epilogue: columns [col0, col0 + 128) of A(l+1) = LeakyReLU(acc + bias), split into hi / lo
+  auto store_hidden = [&](const float (&acc)[64], int col0, const float* bias) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int k = col0 + 8 * j + q2;
+      const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + q2));
+      const uint32_t off = (uint32_t)(k >> 4) * KSTEP_BYTES + (uint32_t)(k & 7) * 2u;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float t0 = acc[4 * j + 2 * h] + b.x, t1 = acc[4 * j + 2 * h + 1] + b.y;
+        t0 = fmaxf(t0, t0 * cfg.leaky_slope);  // LeakyReLU, slope in (0,1)
+        t1 = fmaxf(t1, t1 * cfg.leaky_slope);
+        uint32_t hi, lo;
+        split2(t0, t1, hi, lo);
+        const uint32_t o = off + ks_slot(row0 + 8 * h, (k >> 3) & 1);
+        *reinterpret_cast<uint32_t*>(smem + OFF_AHI + o) = hi;
+        *reinterpret_cast<uint32_t*>(smem + OFF_ALO + o) = lo;
+      }
+    }
+  };
+
+  for (long long iter = 0; iter < n_iters; ++iter) {
+    const long long tile = iter * gridDim.x + blockIdx.x;
+    // ---- RayParam + WindowedPE of this warpgroup's 64 rays, two threads per ray, straight into the bf16 hi / lo slots ----
+    {
+      const int r = wg * 64 + (wt & 63), part = wt >> 6;
+      auto put = [&](int k, float val) {
+        const __nv_bfloat16 hi = __float2bfloat16_rn(val);
+        const __nv_bfloat16 lo = __float2bfloat16_rn(val - __bfloat162float(hi));
+        const uint32_t off = (uint32_t)(k >> 4) * KSTEP_BYTES + ks_slot(r, (k >> 3) & 1) + (uint32_t)(k & 7) * 2u;
+        *reinterpret_cast<__nv_bfloat16*>(smem + OFF_X + off) = hi;
+        *reinterpret_cast<__nv_bfloat16*>(smem + OFF_X + x_lo_off + off) = lo;
+      };
+      const long long ray = tile * BM + r;
+      if (ray < n_rays) {
+        // `rays` may be pinned host memory (zero-copy input of hr_render_host): each ray is read once per thread, with
+        // vector loads, and `rays_copy` receives the device copy the render kernel reads.
+        float rbuf[16];
+        const float* src = rays + ray * cfg.c_in;
+        if (cfg.c_in == 8 && vec_ok) {
+          const float4 a = *reinterpret_cast<const float4*>(src), b = *reinterpret_cast<const float4*>(src + 4);
+          rbuf[0] = a.x; rbuf[1] = a.y; rbuf[2] = a.z; rbuf[3] = a.w; rbuf[4] = b.x; rbuf[5] = b.y; rbuf[6] = b.z; rbuf[7] = b.w;
+          if (rays_copy != nullptr && part == 0) {
+            float4* dst = reinterpret_cast<float4*>(rays_copy + ray * 8);
+            dst[0] = a; dst[1] = b;
+          }
+        } else {
+          for (int i = 0; i < cfg.c_in; ++i) rbuf[i] = src[i];
+          if (rays_copy != nullptr && part == 0)
+            for (int i = 0; i < cfg.c_in; ++i) rays_copy[ray * cfg.c_in + i] = rbuf[i];
+        }
+        encode_ray_features(cfg, rbuf, part, 2, put);
+      } else if (part == 0) {
+        for (int k = 0; k < cfg.mlp_in; ++k) put(k, 0.0f);  // masked row: defined (never stored) values
+      }
+      fence_async_smem();
+      wg_sync(1 + wg);
+    }
+    // ---- the layers ----
+    int p = 0;
+    for (int l = 0; l < L - 1; ++l) {
+      run_pass(acc0, pk.passes[p]);
+      if (W == 256) run_pass(acc1, pk.passes[p + 1]);
+      drain();
+      wg_sync(1 + wg);  // every warp's wgmmas that read A(l) have retired before A(l+1) overwrites it
+      store_hidden(acc0, 0, pk.bias + pk.passes[p].bias_off);
+      if (W == 256) store_hidden(acc1, PASS_N, pk.bias + pk.passes[p + 1].bias_off);
+      fence_async_smem();
+      wg_sync(1 + wg);
+      p += W / PASS_N;
+    }
+    // ---- last layer: accumulators + bias -> heads scratch (rows past n_rays / columns past mlp_out are dropped) ----
+    for (; p < n_passes; ++p) {
+      const TcPass& P = pk.passes[p];
+      run_pass(acc0, P);
+      drain();
+      const float* bias = pk.bias + P.bias_off;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const long long ray = tile * BM + row0 + 8 * h;
+        if (ray >= n_rays) continue;
+        float* dst = heads + ray * cfg.mlp_out + P.out_col0;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int c = 8 * j + q2;
+          if (P.out_col0 + c < cfg.mlp_out) {  // mlp_out is a multiple of 4: the pair is in or out as a whole
+            const float2 b = __ldg(reinterpret_cast<const float2*>(bias + c));
+            *reinterpret_cast<float2*>(dst + c) = make_float2(acc0[4 * j + 2 * h] + b.x, acc0[4 * j + 2 * h + 1] + b.y);
+          }
+        }
+      }
+    }
   }
 }
 
@@ -494,25 +281,23 @@ int pack_mlp_tc2(hr_handle* h, const hr_config& c, MlpTcPack& pk, size_t& alloc_
   for (int l = 0; l < L; ++l) {
     const bool last = (l == L - 1);
     const int out = last ? c.mlp_out : W;
-    const int n_parts = (out + 127) / 128;
+    const int n_parts = (out + tc2::PASS_N - 1) / tc2::PASS_N;
     for (int part = 0; part < n_parts; ++part) {
       if (np >= HR_TC_MAX_PASSES) return hr_fail("tensor-core sample net: too many passes (%d output columns)", c.mlp_out);
       TcPass& P = np_.passes[np++];
-      const int rem = out - part * 128;
       const bool reads_input = (l == 0 || l == c.mlp_skip);
       P.layer = l;
-      P.n = rem >= 128 ? 128 : (rem + 15) / 16 * 16;
+      P.n = tc2::PASS_N;  // a partial last pass is zero padded
       P.first_chunk = reads_input ? 0 : in_chunks;
       P.n_chunks = (l == 0) ? in_chunks : (W / 32 + (reads_input ? in_chunks : 0));
       P.bias_off = bias_off;
       P.is_final = last ? 1 : 0;
-      P.out_col0 = part * 128;
+      P.out_col0 = part * tc2::PASS_N;
       P.wait_a = (part == 0) ? 1 : 0;
       bias_off += P.n;
       bytes += (size_t)P.n_chunks * 2 * P.n * 64;
     }
   }
-  if ((L - 1) * W > tc2::BIAS_FLOATS) return hr_fail("tensor-core sample net: hidden bias table too large");
   np_.n_passes = np;
   np_.bias_count = bias_off;
   np_.wpack_bytes = (long long)bytes;
@@ -528,16 +313,9 @@ int pack_mlp_tc2(hr_handle* h, const hr_config& c, MlpTcPack& pk, size_t& alloc_
     if (e != cudaSuccess) { cudaFree(wp); return hr_fail("cudaMalloc(tc bias): %s", cudaGetErrorString(e)); }
     np_.wpack = wp; np_.bias = bp;
     alloc_bytes = bytes; alloc_bias = bias_off;
-    // opt in to the 219 KB of dynamic shared memory once per (handle, device)
+    // opt in to the 224 KB of dynamic shared memory once per (handle, device)
     e = cudaFuncSetAttribute(mlp_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::SMEM_BYTES);
     if (e != cudaSuccess) return hr_fail("cudaFuncSetAttribute(mlp_tc2_kernel): %s", cudaGetErrorString(e));
-    // the TMA descriptor encoder comes from the driver through the runtime (no link-time libcuda dependency)
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      h->tma_encode = fn;
-    if (!h->tma_encode) return hr_fail("cuTensorMapEncodeTiled is not available from this driver");
   } else {
     np_.wpack = pk.wpack; np_.bias = pk.bias;
   }
@@ -570,56 +348,15 @@ void free_mlp_tc2(hr_handle* h) {
   h->tc_pre_alloc_bytes = 0; h->tc_pre_alloc_bias = 0;
 }
 
-cudaError_t launch_mlp_tc2(const hr_config& cfg, const MlpTcPack& pk, void* tma_encode, const float* rays, float* heads,
-                           long long n, int num_sms, cudaStream_t stream, float* rays_copy) {
-  unsigned long long* trace = nullptr;
-  int trace_iter = 1;
-#ifdef HR_DIAG
-  const bool want_trace = getenv("HR_TC_TRACE") != nullptr;
-  if (want_trace) {
-    cudaMalloc((void**)&trace, 1024 * sizeof(unsigned long long));
-    cudaMemset(trace, 0, 1024 * sizeof(unsigned long long));
-    if (getenv("HR_TC_TRACE_ITER")) trace_iter = atoi(getenv("HR_TC_TRACE_ITER"));
-  }
-#endif
+cudaError_t launch_mlp_tc2(const hr_config& cfg, const MlpTcPack& pk, const float* rays, float* heads, long long n, int num_sms,
+                           cudaStream_t stream, float* rays_copy) {
+  // the epilogue stores column pairs and drops a pair past mlp_out as a whole
+  if ((cfg.mlp_out % 4) != 0 || ((uintptr_t)heads % 16) != 0) return cudaErrorInvalidValue;
   long long tiles = (n + tc::BM - 1) / tc::BM;
   int grid = (int)(tiles < num_sms ? tiles : num_sms);
   if (grid < 1) grid = 1;
-  CUtensorMap hmap;
-  if (!make_heads_map(&hmap, tma_encode, heads, cfg.mlp_out, n, 16)) return cudaErrorInvalidValue;
-  mlp_tc2_kernel<<<grid, tc2::NTHREADS, tc2::SMEM_BYTES, stream>>>(cfg, pk, rays, heads, n, trace, hmap, rays_copy, trace_iter);
-  cudaError_t le = cudaGetLastError();
-#ifdef HR_DIAG
-  if (want_trace) {
-    unsigned long long hbuf[1024];
-    cudaStreamSynchronize(stream);
-    cudaMemcpy(hbuf, trace, sizeof(hbuf), cudaMemcpyDeviceToHost);
-    cudaFree(trace);
-    unsigned long long t0 = hbuf[0];
-    fprintf(stderr, "[tc2-trace] pass: demp_ok a_first a_last commit | dfull_seen first_kstep last_kstep (cycles rel. to pass 0)\n");
-    for (int p = 0; p < pk.n_passes; ++p) {
-      fprintf(stderr, "[tc2-trace] %2d:", p);
-      for (int e = 0; e < 7; ++e) fprintf(stderr, " %8lld", hbuf[p * 8 + e] ? (long long)(hbuf[p * 8 + e] - t0) : -1LL);
-      fprintf(stderr, "\n");
-    }
-    fprintf(stderr, "[tc2-trace] CTA 0: setup %lld cycles; tile starts (rel. to setup end):", (long long)(hbuf[224] - hbuf[240]));
-    for (int i = 0; i < 16 && hbuf[224 + i]; ++i) fprintf(stderr, " %lld", (long long)(hbuf[224 + i] - hbuf[224]));
-    fprintf(stderr, "; end %lld\n", (long long)(hbuf[241] - hbuf[224]));
-    unsigned long long s0 = ~0ull, s1 = 0, e0 = ~0ull, e1 = 0;
-    double mhz = 0;
-    for (int b = 0; b < grid && b < 256; ++b) {
-      const unsigned long long* r = hbuf + 256 + 3 * b;
-      if (r[0] < s0) s0 = r[0];
-      if (r[0] > s1) s1 = r[0];
-      if (r[1] < e0) e0 = r[1];
-      if (r[1] > e1) e1 = r[1];
-      mhz += (double)r[2] / (double)(r[1] - r[0]) * 1e3 / grid;
-    }
-    fprintf(stderr, "[tc2-trace] CTAs: first start 0, last start %lld ns, first end %lld ns, last end %lld ns; CTA0 %lld..%lld ns; mean SM clock %.0f MHz\n",
-            (long long)(s1 - s0), (long long)(e0 - s0), (long long)(e1 - s0), (long long)(hbuf[256] - s0), (long long)(hbuf[257] - s0), mhz);
-  }
-#endif
-  return le;
+  mlp_tc2_kernel<<<grid, tc2::NTHREADS, tc2::SMEM_BYTES, stream>>>(cfg, pk, rays, heads, n, rays_copy);
+  return cudaGetLastError();
 }
 
 }  // namespace hr

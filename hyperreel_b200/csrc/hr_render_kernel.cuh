@@ -196,7 +196,7 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
   for (int i = 0; i < N1; ++i) lcol[N0 + i] = C0 + ((C1 == 8) ? alt * 4 : 0) + i;
 #pragma unroll
   for (int i = 0; i < N2; ++i) lcol[N0 + N1 + i] = C0 + C1 + ((C2 == 8) ? alt * 4 : 0) + i;
-  // Two ways to finish a sample (measured, profiles/r2_notes.md):
+  // Two ways to finish a sample:
   //   FOLD  (several groups, [8,4,4] / [8,8,8]): every lane accumulates partial sums of all three colours and of the density
   //         over its own taps / channels (G = all three colour rows of its slots), one transposing reduction per sample;
   //   !FOLD (one group, [8,0,0]): complete features f[NT] in every lane, each lane computes its own colour (G = one row).

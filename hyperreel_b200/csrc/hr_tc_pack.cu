@@ -1,14 +1,11 @@
-// Host helpers of the tensor-core sample net (hr_mlp_tc2.cu): weight images and the TMA tensor map of the heads scratch.
+// Host helper of the tensor-core sample net (hr_mlp_tc2.cu): weight images.
 //
 // Weight images: every fp32 weight w of the reference's nn.Linear (nlf/nets/mlp.py:127-154) is split into bf16
-// hi = rn(w), lo = rn(w - hi) and laid out the way tcgen05.mma reads its B operand from shared memory: UMMA K-major,
+// hi = rn(w), lo = rn(w - hi) and laid out the way wgmma reads its B operand from shared memory: K-major,
 // no swizzle, core matrices of 8 rows x 16 bytes (LBO = N * 16 B between the two 8-wide k-groups of a 16-wide k-step,
 // SBO = 128 B between 8-row groups).  One image = one k-step of one pass = N x 16 bf16 hi followed by N x 16 bf16 lo;
 // images are concatenated in consumption order so the producer warp streams them with cp.async.bulk.
-#include <cuda.h>  // CUtensorMap (types only; the encoder is fetched through cudaGetDriverEntryPoint)
 #include <cuda_bf16.h>
-
-#include <cstring>
 
 #include "hr_tc_prims.cuh"
 
@@ -68,30 +65,9 @@ void launch_pack_tc_pass(const float* W, const float* b, uint8_t* dst, float* bi
                          int out_col0, cudaStream_t st) {
   long long total = (long long)n_chunks * 2 * n * 16 + n;
   int grid = (int)((total + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > 4096) grid = 4096;
   pack_tc_pass<<<grid, 256, 0, st>>>(W, b, dst, bias_dst, n, first_chunk, n_chunks, in_src, mlp_in, is_skip, in_chunks, out_rows,
                                      perm_S, perm_stride, out_col0);
-}
-
-// Tensor map of the heads scratch [n rays][mlp_out] fp32, box = box_cols columns x 32 rows (one epilogue warp's slice).
-// encode_fn = cuTensorMapEncodeTiled, fetched once per handle through cudaGetDriverEntryPoint (no link-time libcuda
-// dependency).  False = the map could not be built.
-bool make_heads_map(CUtensorMap* hmap, void* encode_fn, const float* heads, int mlp_out, long long n, int box_cols) {
-  memset(hmap, 0, sizeof(*hmap));
-  if ((mlp_out % 4) != 0 || ((uintptr_t)heads % 16) != 0) return false;
-  typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  if (encode_fn == nullptr) return false;
-  EncodeFn encode = (EncodeFn)encode_fn;
-  cuuint64_t gdim[2] = {(cuuint64_t)mlp_out, (cuuint64_t)n};
-  cuuint64_t gstride[1] = {(cuuint64_t)mlp_out * sizeof(float)};
-  cuuint32_t box[2] = {(cuuint32_t)box_cols, 32};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = encode(hmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)heads, gdim, gstride, box, estr,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS;
 }
 
 }  // namespace hr

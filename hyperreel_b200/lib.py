@@ -173,7 +173,7 @@ class HyperReelLibraryError(RuntimeError):
 
 
 def build(verbose: bool = False) -> str:
-    """Compile the CUDA sources for sm_100a into ``libhyperreel_b200.so`` (in-tree)."""
+    """Compile the CUDA sources for sm_90a into ``libhyperreel_b200.so`` (in-tree)."""
     cmd = ["make", "-C", CSRC_DIR, "-j", str(min(8, os.cpu_count() or 1))]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if verbose or res.returncode != 0:

@@ -1,4 +1,4 @@
-"""``model_dict['lightfield']`` of the drop-in: the fused B200 light-field model.
+"""``model_dict['lightfield']`` of the drop-in: the fused H100 light-field model.
 
 Mirrors the surface of the reference's ``LightfieldModel`` (nlf/models/models.py:104-143):
 ``cls(cfg.model, system=...)``, ``forward(rays, render_kwargs) -> {'rgb': [N,3], ...}``,
@@ -44,7 +44,7 @@ def _dataset_facts(system) -> dict:
 
 
 def resolve_mlp_mode(name: str) -> int:
-    """'auto' (default) and 'bf16x3' select the tcgen05 sample net -- every pipeline the fused path accepts runs on it
+    """'auto' (default) and 'bf16x3' select the wgmma sample net -- every pipeline the fused path accepts runs on it
     (hidden width 128 / 256, encoded input <= 64 features); 'fp32' selects the CUDA-core kernel, the parity anchor."""
     try:
         return {"auto": L.MLP_BF16X3_TC, "bf16x3": L.MLP_BF16X3_TC, "fp32": L.MLP_FP32_SIMT}[name]
@@ -408,7 +408,7 @@ class LightfieldModel(nn.Module):
 
     def _check_rays(self, rays):
         if not rays.is_cuda:
-            raise RuntimeError("hyperreel_b200 renders on a B200 only: rays must be a CUDA tensor (no CPU fallback)")
+            raise RuntimeError("hyperreel_b200 renders on an H100 only: rays must be a CUDA tensor (no CPU fallback)")
         rays = rays.reshape(-1, rays.shape[-1])
         if rays.shape[-1] != self.sig.c_in:
             raise ValueError(f"rays must have {self.sig.c_in} channels, got {rays.shape[-1]}")

@@ -7,7 +7,7 @@ cross the fabric; nothing else does (SURVEY.md section 8e).
 
 Two ways to assemble ``[N,3]`` on every rank:
 
-* **peer-memory epilogue** (B200 / NVSwitch, the default on CUDA): a gather buffer ``[N,3]`` lives in symmetric memory on
+* **peer-memory epilogue** (NVSwitch, the default on CUDA): a gather buffer ``[N,3]`` lives in symmetric memory on
   every GPU (``torch.distributed._symmetric_memory``: one allocation per rank, peer-mapped over NVLink).  The render
   kernel's epilogue stores each finished pixel into *every* rank's buffer (``hr_render_scatter``): the gather is fused
   into the kernel, no collective kernel follows -- only a signal-pad barrier so that nobody reads before all tiles landed.

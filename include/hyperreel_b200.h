@@ -1,5 +1,5 @@
 /*
- * hyperreel_b200 -- C-ABI of the B200-native HyperReel per-ray rendering hot path.
+ * hyperreel_b200 -- C-ABI of the H100-native HyperReel per-ray rendering hot path.
  *
  * This is the drop-in boundary: plain pointers and sizes, no torch types.  The reference has no
  * FFI (it is pure PyTorch); every entry point below names the reference interface it replaces
@@ -14,7 +14,7 @@
  *     torch's current stream (nlf/__init__.py:486-502); no hidden synchronisation except in
  *     hr_render_host, which is synchronous by contract;
  *   - a handle is re-entrant per handle, no global state except the thread-local error string;
- *   - there is NO CPU fallback: if no sm_100 device is present hr_create fails.
+ *   - there is NO CPU fallback: if no sm_90 device is present hr_create fails.
  */
 #ifndef HYPERREEL_B200_H
 #define HYPERREEL_B200_H
@@ -63,8 +63,8 @@ enum { HR_SHADE_SH = 0, HR_SHADE_RGB = 1 };
 enum { HR_DENSE_RELU = 0, HR_DENSE_SOFTPLUS = 1, HR_DENSE_RELU_ABS = 2 };
 
 /* Sample-net arithmetic.  FP32_SIMT: fp32 FMA on CUDA cores (bit-level closest to the reference's
- * cuBLAS SGEMM).  BF16X3_TC: tcgen05 tensor cores, every fp32 operand split into bf16 hi+lo and the
- * three leading cross products accumulated in fp32 TMEM (error ~2^-16 per product, see DESIGN.md). */
+ * cuBLAS SGEMM).  BF16X3_TC: wgmma tensor cores, every fp32 operand split into bf16 hi+lo and the
+ * three leading cross products accumulated in fp32 registers (error ~2^-16 per product, see DESIGN.md). */
 enum { HR_MLP_FP32_SIMT = 0, HR_MLP_BF16X3_TC = 1,
        HR_MLP_ZERO = 2 /* `net: {type: zero}` (ZeroMLP, nlf/nets/mlp.py:14-33): every head is 0, no network runs */ };
 
@@ -222,7 +222,7 @@ const char* hr_last_error(void);
 
 /* Replaces: model_dict['lightfield'](cfg.model, system) + render_fn_dict['lightfield'](...)
  * construction (nlf/__init__.py:351-364, nlf/models/models.py:104-129, nlf/rendering.py:59-70).
- * `device` is the CUDA ordinal.  Fails if the device is not sm_100 or the signature is unsupported. */
+ * `device` is the CUDA ordinal.  Fails if the device is not sm_90 or the signature is unsupported. */
 int hr_create(const hr_config* cfg, int device, hr_handle** out);
 
 /* Replaces: INRSystem.load_state_dict (nlf/__init__.py:433-479) for the render path: ingest a

@@ -1,9 +1,9 @@
 """Reference-through-shim runner (TEST INFRASTRUCTURE ONLY -- never imported by the product).
 
-Imports the *unmodified* HyperReel hot-path modules from ``/root/reference`` on CPU so that their
+Imports the *unmodified* HyperReel hot-path modules from a reference checkout (``$HYPERREEL_REFERENCE``) on CPU so that their
 outputs can pin the oracle (``oracle/hyperreel_oracle.py``) and generate the golden vectors under
-``tests/golden/``.  It only works where ``/root/reference`` exists (this container); the GPU box has
-no reference checkout, so nothing executed there may import this file.
+``tests/golden/``.  It only works where that checkout exists; the tests read the recorded vectors and
+never call into it.
 
 What the shim does (SURVEY.md Appendix D):
   * registers an empty namespace package ``nlf`` whose ``__path__`` points at the reference, so the
@@ -27,7 +27,7 @@ from types import SimpleNamespace
 
 import torch
 
-REFERENCE_ROOT = os.environ.get("HYPERREEL_REFERENCE", "/root/reference")
+REFERENCE_ROOT = os.environ.get("HYPERREEL_REFERENCE", "")
 
 
 def reference_available() -> bool:

@@ -1,8 +1,7 @@
 """Generate the golden vectors under tests/golden/ by running the *reference itself* (unmodified modules
-from /root/reference, on CPU, through oracle/ref_shim.py) on seeded inputs.
+from a reference checkout, on CPU, through oracle/ref_shim.py) on seeded inputs.
 
-Only runnable where /root/reference exists (the build container).  The fixtures travel to the GPU box;
-the reference does not.  Each fixture stores: the case description, the rays, a SHA-256 of the seeded
+Only runnable with HYPERREEL_REFERENCE set to a reference checkout; the tests that read the fixtures need none.  Each fixture stores: the case description, the rays, a SHA-256 of the seeded
 parameters (parameters are regenerated from the seed by ``tests/cases.py`` -- torch's CPU generators are
 deterministic -- and the hash guards against drift), and the reference outputs:
 ``rgb``, ``points``/``distances`` from ``render_fn.embed`` (nlf/rendering.py:79-84) and every other key that call returns

@@ -1,6 +1,6 @@
 """Golden vectors for the model YAMLs the reference SHIPS (conf/experiment/model/*.yaml) and the fused path accepts.
 
-For each such YAML: the configuration as JSON (the GPU box has no reference checkout, hence no YAML files), the dataset
+For each such YAML: the configuration as JSON (the tests need no reference checkout, hence no YAML files), the dataset
 facts, seeded rays, and the rgb the *unmodified reference* renders for seeded parameters (grid shrunk to 24^3 so that the
 fixtures stay small; parameters are regenerated from the seed by hyperreel_b200.state.seeded_state_dict).
 

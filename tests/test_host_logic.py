@@ -159,19 +159,22 @@ def test_lowering_of_the_f3_families():
     assert c.isect_type == L.ISECT_SPHERE and c.dynamic == 1 and c.contract_type == L.CONTRACT_MIPNERF
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/conf/experiment/model"), reason="reference checkout not present")
 def test_shipped_model_yamls_that_lower_to_the_fused_path():
-    """Coverage ledger over the reference's 51 shipped model YAMLs: these must lower (DESIGN.md section 7 lists why the
-    rest are rejected)."""
-    import glob
+    """Coverage ledger over the reference's 51 shipped model YAMLs (tests/golden/reference/model_yamls.npz): these must lower
+    (DESIGN.md section 7 lists why the rest are rejected)."""
+    from tests.test_oracle_vs_reference import shipped_yamls
     ds = {"num_keyframes": 12, "num_frames": 50, "near": 0.5, "far": 10.0, "depth_range": [0.5, 10.0], "name": "x", "collection": "y",
           "bbox_min": [-1.5, -1.25, -1.0], "bbox_max": [1.5, 1.25, 1.0], "total_images_per_frame": 5, "val_all": True}
+    yamls = shipped_yamls()
+    assert len(yamls) == 52
     ok = set()
-    for f in sorted(glob.glob("/root/reference/conf/experiment/model/*.yaml")):
+    for name, plain in yamls.items():
+        if plain is None:  # bom_z_plane.yaml is an empty file
+            continue
         try:
-            lower(hb.load_model_yaml(f), ds)
-            ok.add(os.path.basename(f)[:-5])
-        except (UnsupportedPipeline, TypeError):  # bom_z_plane.yaml is an empty file
+            lower(hb.to_cfg(plain), ds)
+            ok.add(name)
+        except UnsupportedPipeline:
             pass
     expected = {
         "donerf_sphere", "donerf_cylinder", "donerf_cylinder_no_point", "donerf_cylinder_small", "llff_z_plane", "llff_z_plane_small",
@@ -188,7 +191,7 @@ def test_shipped_model_yamls_that_lower_to_the_fused_path():
         # cascaded pipelines (point_prediction): a second net at the points of a first, coarse intersection
         "shiny_z_plane_cascaded", "shiny_z_plane_feedback", "technicolor_cascaded", "shiny_z_tensorf_cascaded",
     }
-    assert len(ok) == 45  # every shipped YAML the unmodified reference itself can run (test_oracle_vs_reference.py holds the other 6; bom_z_plane.yaml is empty)
+    assert len(ok) == 45  # every shipped YAML the unmodified reference itself can run (the other 6 fail inside the reference; bom_z_plane.yaml is empty)
     assert expected <= ok, sorted(expected - ok)
 
 
@@ -247,34 +250,32 @@ def test_system_loads_shrunk_grid_checkpoint_shapes():
 
 def test_lowering_of_the_round_2_families():
     """Voxel grids (per-axis sample tables, interleaved), plane grids, 256 samples per ray, the per-camera colour transform and
-    cascaded (point_prediction) pipelines, lowered from the reference's own YAML files."""
-    ref = "/root/reference/conf/experiment/model"
-    if not os.path.isdir(ref):
-        pytest.skip("reference checkout not present")
+    cascaded (point_prediction) pipelines, lowered from the reference's own YAML files (tests/golden/reference/model_yamls.npz)."""
+    from tests.test_oracle_vs_reference import shipped_cfg
     ds = {"num_keyframes": 12, "num_frames": 50, "near": 0.5, "far": 10.0, "depth_range": [0.5, 10.0], "name": "x", "collection": "y",
           "bbox_min": [-1.5, -1.25, -1.0], "bbox_max": [1.5, 1.25, 1.0], "total_images_per_frame": 5, "val_all": True}
-    c = lower(hb.load_model_yaml(f"{ref}/donerf_voxel.yaml"), ds).cfg
+    c = lower(shipped_cfg("donerf_voxel"), ds).cfg
     assert c.isect_type == L.ISECT_VOXEL and c.n_samples == 48 and c.isect_axes == 3 and c.n_z == 1
     # sample s = plane s // 3 of axis s % 3: first / last plane of every axis are the (contracted) dataset bounds
     assert c.samples[0] < 0 < c.samples[45] and c.samples[1] < 0 < c.samples[46] and c.samples[2] < 0 < c.samples[47]
     assert all(abs(c.z_scale3[a] - abs(c.samples[3 + a] - c.samples[a])) < 1e-6 for a in range(3))
-    c = lower(hb.load_model_yaml(f"{ref}/shiny_z_deformable.yaml"), ds).cfg
+    c = lower(shipped_cfg("shiny_z_deformable"), ds).cfg
     assert c.isect_type == L.ISECT_PLANE and c.n_z == 4 and c.isect_axes == 1 and list(c.plane_normal)[:3] == [0.0, 0.0, 1.0]
     assert c.plane_normal_scale == 1.0
-    sig = lower(hb.load_model_yaml(f"{ref}/neural_3d_z_plane_static.yaml"), ds)
+    sig = lower(shipped_cfg("neural_3d_z_plane_static"), ds)
     assert sig.n_samples == 256 and sig.cfg.mlp_out == 256 * 14 and sig.cfg.dynamic == 0
-    sig = lower(hb.load_model_yaml(f"{ref}/immersive_z_plane.yaml"), ds)
+    sig = lower(shipped_cfg("immersive_z_plane"), ds)
     assert sig.cfg.n_color_views == 5 and sig.cfg.c_in == 8 and sig.color_views == 5 and sig.color_embedding_index > 0
     assert abs(sig.cfg.act_ctransform.inner_fac - 0.1) < 1e-7
     off = dict(ds, val_all=False)
-    assert lower(hb.load_model_yaml(f"{ref}/immersive_z_plane.yaml"), off).cfg.n_color_views == 0  # ColorTransformEmbedding is a no-op then
-    sig = lower(hb.load_model_yaml(f"{ref}/technicolor_cascaded.yaml"), ds)
+    assert lower(shipped_cfg("immersive_z_plane"), off).cfg.n_color_views == 0  # ColorTransformEmbedding is a no-op then
+    sig = lower(shipped_cfg("technicolor_cascaded"), ds)
     c = sig.cfg
     assert c.cascade == 1 and c.pre_samples == 8 and c.n_samples == 32 and sig.net_index == 2
     assert sig.pre_layer_shapes[-1] == (8, 256) and sig.mlp_layer_shapes[-1] == (c.mlp_out // 8, 256)
     assert list(c.pt_src) == [0, 1, 2, 3, 4, 5, 9, -1]  # points, viewdirs, times
     assert c.pre_mlp_mode == c.mlp_mode and c.pre_near == float("-inf")  # mask.stop_iters: -1 -> nothing masked
-    c = lower(hb.load_model_yaml(f"{ref}/shiny_z_plane_cascaded.yaml"), ds).cfg
+    c = lower(shipped_cfg("shiny_z_plane_cascaded"), ds).cfg
     assert c.cascade == 1 and c.pre_mlp_mode == L.MLP_ZERO  # zero ray net: the first stage is the bare z-planes
     sd = seeded_state_dict(sig, seed=1)
     assert sd["model.embedding_model.embeddings.2.net.layers.0.0.weight"].shape == (256, 24)

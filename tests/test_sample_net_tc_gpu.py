@@ -1,4 +1,4 @@
-"""The tcgen05 (bf16x3 split) sample net against the reference golden vectors and the fp32 CUDA-core path."""
+"""The wgmma (bf16x3 split) sample net against the reference golden vectors and the fp32 CUDA-core path."""
 import os
 
 import numpy as np
@@ -38,7 +38,7 @@ def test_tc_matches_fp32_path_on_many_tiles(name):
 
 
 def test_default_mode_is_the_tensor_core_net():
-    """The registry path (no mlp_mode argument, like the reference constructor) must run the tcgen05 kernel."""
+    """The registry path (no mlp_mode argument, like the reference constructor) must run the wgmma kernel."""
     from hyperreel_b200 import lib as L
 
     case = build_case("technicolor_trained")

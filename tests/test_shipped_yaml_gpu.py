@@ -1,7 +1,7 @@
 """CUDA path vs the unmodified reference for every model YAML the reference ships and the fused path accepts
 (tests/golden/shipped/*.npz, see tests/test_shipped_yaml_golden.py for the fixture format and the CPU half).
 
-All 34 passed on B200 in round 1's driver run (63 XPASS); the marker is gone, a regression fails the suite.  The tensor-core
+A regression fails the suite.  The tensor-core
 sample net covers every one of them (hidden width 128 / 256, encoded inputs up to 64 features): no skips."""
 import os
 
