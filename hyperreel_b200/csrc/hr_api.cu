@@ -23,8 +23,8 @@ cudaError_t launch_render(const hr_config& cfg, const Derived& dv, const RenderT
                           cudaStream_t stream, unsigned char* rgb8);
 cudaError_t launch_render_bwd(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs, float* const* g_sig_space,
                               float* const* g_sig_second, float* const* g_app_space, float* const* g_app_second, float* g_basis,
-                              const float* rays, const float* heads, const float* d_rgb, float* d_heads, long long n, int clamp_output,
-                              int white_bg, int num_sms, cudaStream_t stream);
+                              float* g_color_embedding, const float* rays, const float* heads, const float* d_rgb, float* d_heads,
+                              long long n, int clamp_output, int white_bg, int num_sms, cudaStream_t stream);
 cudaError_t launch_generate_rays(const hr_camera& cam, int c_in, long long first, long long n, float* out, cudaStream_t st);
 }  // namespace hr
 
@@ -1086,10 +1086,8 @@ static int train_supported(const hr_config& c) {
   if (c.mlp_mode == HR_MLP_ZERO) { /* no sample net: d heads is simply unused by the caller */ }
   if ((c.isect_type == HR_ISECT_SPHERE || c.isect_type == HR_ISECT_CYLINDER) && c.sphere_origin_scale != 0.0f)
     return fail("backward: learned primitive origins (origin_scale_factor != 0) are not supported yet");
-  if (c.contract_type == HR_CONTRACT_AFFINE) return fail("backward: bbox / z_depth contraction is not supported yet");
-  if (c.off_cscale_global >= 0) return fail("backward: per-ray colour heads are not supported yet");
-  if (c.isect_type == HR_ISECT_VOXEL || c.isect_type == HR_ISECT_PLANE) return fail("backward: voxel-grid primitives are not supported yet");
-  if (c.n_color_views > 0) return fail("backward: the per-camera colour transform is not supported yet");
+  // the colour transform's gradient is summed per CTA in shared memory
+  if (c.n_color_views > 512) return fail("backward: more than 512 colour-transform views are not supported");
   if (c.n_samples > 64) return fail("backward: more than 64 samples per ray are not supported yet");
   if (c.cascade) return fail("backward: cascaded (point_prediction) pipelines are not supported yet");
   return 0;
@@ -1097,17 +1095,18 @@ static int train_supported(const hr_config& c) {
 
 static int ensure_grad_tables(hr_handle* h, cudaStream_t st) {
   const hr_config& c = h->cfg;
-  size_t want[13];
+  size_t want[14];
   for (int i = 0; i < 3; ++i) {
     const hr::PlaneTab& t = h->tabs.sig[i];
     const size_t sp = (size_t)t.C * t.H * t.W, se = (size_t)t.C * t.H2 * t.L;
     want[i] = sp; want[3 + i] = se; want[6 + i] = sp; want[9 + i] = se;
   }
   want[12] = (size_t)c.app_dim * h->tabs.n_app_total;
-  float** bufs[13] = {&h->g_sig_space[0], &h->g_sig_space[1], &h->g_sig_space[2], &h->g_sig_second[0], &h->g_sig_second[1],
+  want[13] = (size_t)c.n_color_views * 12;
+  float** bufs[14] = {&h->g_sig_space[0], &h->g_sig_space[1], &h->g_sig_space[2], &h->g_sig_second[0], &h->g_sig_second[1],
                       &h->g_sig_second[2], &h->g_app_space[0], &h->g_app_space[1], &h->g_app_space[2], &h->g_app_second[0],
-                      &h->g_app_second[1], &h->g_app_second[2], &h->g_basis};
-  for (int i = 0; i < 13; ++i) {
+                      &h->g_app_second[1], &h->g_app_second[2], &h->g_basis, &h->g_color_embedding};
+  for (int i = 0; i < 14; ++i) {
     if (h->g_sizes[i] == want[i] && (*bufs[i] || want[i] == 0)) continue;
     if (*bufs[i]) cudaFree(*bufs[i]);
     *bufs[i] = nullptr;
@@ -1173,7 +1172,7 @@ int hr_render_backward(hr_handle* h, const float* rays, const float* heads, int6
   const bool timing = h->timing && h->ev_bwd.size() < 8192;
   if (timing) { CK(cudaEventCreate(&eb.a)); CK(cudaEventCreate(&eb.b)); CK(cudaEventRecord(eb.a, st)); }
   cudaError_t e = hr::launch_render_bwd(c, h->dv, h->tabs, h->g_sig_space, h->g_sig_second, h->g_app_space, h->g_app_second, h->g_basis,
-                                        rays, hcm, d_rgb, gcm, n, opts->clamp_output ? 1 : 0, white, h->num_sms, st);
+                                        h->g_color_embedding, rays, hcm, d_rgb, gcm, n, opts->clamp_output ? 1 : 0, white, h->num_sms, st);
   if (e != cudaSuccess) return fail("hr_render_backward: %s", cudaGetErrorString(e));
   if (timing) { CK(cudaEventRecord(eb.b, st)); h->ev_bwd.push_back(eb); }
   unpermute_heads<<<grid_for(n * (long long)c.mlp_out), 256, 0, st>>>(gcm, d_heads, n, c.n_samples, c.head_stride);
@@ -1189,10 +1188,10 @@ int hr_grad_zero(hr_handle* h, void* stream) {
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   if (ensure_grad_tables(h, st)) return 1;
-  float* bufs[13] = {h->g_sig_space[0], h->g_sig_space[1], h->g_sig_space[2], h->g_sig_second[0], h->g_sig_second[1], h->g_sig_second[2],
+  float* bufs[14] = {h->g_sig_space[0], h->g_sig_space[1], h->g_sig_space[2], h->g_sig_second[0], h->g_sig_second[1], h->g_sig_second[2],
                      h->g_app_space[0], h->g_app_space[1], h->g_app_space[2], h->g_app_second[0], h->g_app_second[1], h->g_app_second[2],
-                     h->g_basis};
-  for (int i = 0; i < 13; ++i)
+                     h->g_basis, h->g_color_embedding};
+  for (int i = 0; i < 14; ++i)
     if (bufs[i]) CK(cudaMemsetAsync(bufs[i], 0, h->g_sizes[i] * sizeof(float), st));
   return 0;
 }
@@ -1223,6 +1222,8 @@ int hr_grad_read(hr_handle* h, const hr_grads* out, void* stream) {
     }
   }
   if (out->basis_mat) CK(cudaMemcpyAsync(out->basis_mat, h->g_basis, h->g_sizes[12] * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (out->color_embedding && h->g_sizes[13])
+    CK(cudaMemcpyAsync(out->color_embedding, h->g_color_embedding, h->g_sizes[13] * sizeof(float), cudaMemcpyDeviceToDevice, st));
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail("hr_grad_read: %s", cudaGetErrorString(e));
   return 0;
@@ -1290,6 +1291,7 @@ int hr_destroy(hr_handle* h) {
     cudaFree(h->g_sig_space[i]); cudaFree(h->g_sig_second[i]); cudaFree(h->g_app_space[i]); cudaFree(h->g_app_second[i]);
   }
   cudaFree(h->g_basis);
+  cudaFree(h->g_color_embedding);
   hr::free_mlp_tc2(h);
   drop_events(h->ev_render);
   drop_events(h->ev_mlp);

@@ -58,7 +58,8 @@ struct hr_handle {
   float* g_app_space[3] = {nullptr, nullptr, nullptr};
   float* g_app_second[3] = {nullptr, nullptr, nullptr};
   float* g_basis = nullptr;
-  size_t g_sizes[13] = {0};   // element counts of the 13 buffers above (to notice a resized grid)
+  float* g_color_embedding = nullptr;  // [n_color_views][12], the colour transform's table (none without one)
+  size_t g_sizes[14] = {0};   // element counts of the 14 buffers above (to notice a resized grid)
   int64_t launches = 0;
   bool timing = false;
   size_t timed_calls = 0;      // hr_render calls covered by ev_render / ev_mlp (a call may run several sub-batches)

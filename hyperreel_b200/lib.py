@@ -11,7 +11,7 @@ import os
 import subprocess
 import threading
 
-HR_ABI_VERSION = 10
+HR_ABI_VERSION = 11
 HR_MAX_GROUPS = 4
 HR_MAX_LAYERS = 10
 HR_MAX_SAMPLES = 256
@@ -117,7 +117,7 @@ class hr_train_opts(C.Structure):
 
 class hr_grads(C.Structure):
     _fields_ = [("sigma_plane", C.c_void_p * 3), ("app_plane", C.c_void_p * 3), ("sigma_second", C.c_void_p * 3),
-                ("app_second", C.c_void_p * 3), ("basis_mat", C.c_void_p)]
+                ("app_second", C.c_void_p * 3), ("basis_mat", C.c_void_p), ("color_embedding", C.c_void_p)]
 
 
 class hr_camera(C.Structure):

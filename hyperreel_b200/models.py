@@ -221,6 +221,8 @@ class LightfieldModel(nn.Module):
         tn = self.color_model.net
         dplane, dsecond, aplane, asecond = tn.tables()
         params = [t for t in list(dplane) + list(aplane) + list(dsecond) + list(asecond) if t.numel() > 0] + [tn.basis_mat.weight]
+        if c.n_color_views > 0:  # ColorTransformEmbedding (point.py:558-605): its table acts on the pixel inside the fused op
+            params.append(self.embedding_model.embeddings[self.sig.color_embedding_index].color_embedding)
         rgb = _RenderHeads.apply(self, rays, x, clamp_output, white_bg, *params)
         return (rgb, x) if return_heads else rgb  # x: the sample-net output [N, S*stride] (gradient bisecting)
 
@@ -267,8 +269,13 @@ class LightfieldModel(nn.Module):
                     slot[i] = g.data_ptr()
         gb = torch.empty(tn.basis_mat.weight.shape, device=rays.device, dtype=torch.float32)
         G.basis_mat = gb.data_ptr()
-        L.check(self._lib.hr_grad_read(self._handle, C.byref(G), stream))
         order = [outs[(nm, i)] for nm in ("dp", "ap", "d2", "a2") for i in range(3) if (nm, i) in outs] + [gb]
+        if self.sig.cfg.n_color_views > 0:
+            emb = self.embedding_model.embeddings[self.sig.color_embedding_index].color_embedding
+            ge = torch.empty(emb.shape, device=rays.device, dtype=torch.float32)
+            G.color_embedding = ge.data_ptr()
+            order.append(ge)
+        L.check(self._lib.hr_grad_read(self._handle, C.byref(G), stream))
         return d_heads, order
 
     # ------------------------------------------------------------------ the dict `x` of the reference, by name

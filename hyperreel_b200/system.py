@@ -116,16 +116,23 @@ class INRSystem(nn.Module):
         return render_chunked(coords, fn, render_kwargs, chunk=chunk)
 
     # ---- nlf/__init__.py:504-523 + utils/__init__.py:49-76 (get_optimizer): one Adam(betas=(0.9, 0.99), eps=1e-8) per group
-    OPT_DEFAULTS = {"color": 0.02, "color_impl": 0.001, "embedding_impl": 0.00075}  # conf/experiment/training/*_tensorf.yaml
+    OPT_DEFAULTS = {"color": 0.02, "color_impl": 0.001, "embedding_impl": 0.00075,  # conf/experiment/training/*_tensorf.yaml
+                    "embedding": 0.01}
 
     def optimizer_groups(self):
         """Parameters by the reference's `opt_group` names: the VM tables ('color'), basis_mat ('color_impl'), the sample
-        net ('embedding_impl') (nlf/nets/tensorf_base.py opt_group dict, nlf/embedding/ray.py net group)."""
+        net ('embedding_impl') (nlf/nets/tensorf_base.py opt_group dict, nlf/embedding/ray.py net group) and, when the
+        pipeline has a per-camera colour transform, its table ('embedding', ColorTransformEmbedding, point.py:567)."""
         model = self.render_fn.model
         net = model.color_model.net
         tables = [p for n, p in net.named_parameters() if "plane" in n or "line" in n]
         impl = [p for n, p in net.named_parameters() if "basis_mat" in n]
-        return {"color": tables, "color_impl": impl, "embedding_impl": list(model.embedding_model.parameters())}
+        emb = [p for n, p in model.embedding_model.named_parameters() if n.endswith("color_embedding")]
+        groups = {"color": tables, "color_impl": impl,
+                  "embedding_impl": [p for n, p in model.embedding_model.named_parameters() if not n.endswith("color_embedding")]}
+        if emb:
+            groups["embedding"] = emb
+        return groups
 
     def configure_optimizers(self):
         training = self.cfg.get("training", Cfg())

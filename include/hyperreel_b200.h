@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define HR_ABI_VERSION 10
+#define HR_ABI_VERSION 11
 
 #define HR_MAX_GROUPS 4   /* ray-parameterisation groups feeding the sample net (ray.py:235-263) */
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
@@ -352,8 +352,10 @@ int hr_render_frame_to8b_host(hr_handle* h, const hr_camera* cam, uint8_t* rgb8_
  *   hr_render_heads     sample-net output -> rgb, the forward of everything after the net (training or eval semantics)
  *   hr_render_backward  d rgb -> d (sample-net output); gradients of the VM tables and basis_mat accumulate in the handle
  *   hr_grad_zero / hr_grad_read   clear / export the accumulated parameter gradients in the reference's tensor layouts
- * Supported: z_plane / sphere / cylinder primitives with origin_scale_factor == 0, no or mipnerf contraction, per-sample
- * colour heads; other pipelines are rejected (hr_last_error). */
+ * Supported: z_plane / sphere / cylinder (origin_scale_factor == 0) / euclidean-distance / voxel-grid / deformable-plane
+ * primitives, no / mipnerf / bbox / z_depth contraction, per-sample and per-ray colour heads, the per-camera colour transform
+ * with at most 512 views (its gradient is summed per CTA in shared memory), at most 64 samples per ray; sphere_new, cascaded (point_prediction) pipelines and learned primitive origins are rejected
+ * (hr_last_error). */
 typedef struct hr_train_opts {
   int32_t clamp_output; /* 1: eval() forward, clamp(0,1) (tensorf_dynamic.py:805-806); 0: training forward            */
   int32_t white_bg;     /* rgb_map += 1 - acc_map: cfg.white_bg, or the training coin flip of :795-796 drawn by the caller */
@@ -365,6 +367,7 @@ typedef struct hr_grads {  /* device buffers in the reference's layouts (hr_para
   float* sigma_second[3];
   float* app_second[3];
   float* basis_mat;
+  float* color_embedding;  /* [n_color_views, 12]; ignored when n_color_views == 0 */
 } hr_grads;
 
 /* enc [n, mlp_in] fp32 device */
