@@ -21,8 +21,9 @@ struct MlpSimtPack {
 };
 
 // wgmma path (HR_MLP_BF16X3_TC): see hr_mlp_tc2.cu.  A "pass" is one accumulator's worth of output columns
-// (128 columns of a hidden layer or of the last layer); its weights are stored as n_chunks*2 k-step images.
-#define HR_TC_MAX_PASSES 40  // 10 hidden half passes + 28 last-layer parts (S = 256 x 14 channels)
+// (W = hidden width: a whole hidden layer, or W columns of the last layer); its weights are stored as n_chunks*2 k-step
+// images.
+#define HR_TC_MAX_PASSES 40  // 9 hidden layers + 28 last-layer parts (W = 128, S = 256 x 14 channels)
 struct TcPass {
   int layer;        // Linear layer index
   int n;            // output columns of this pass (128; a partial last-layer pass is zero padded)

@@ -2,22 +2,24 @@
 //
 // Math (reference: nlf/nets/mlp.py:159-172 behind nlf/embedding/ray.py:320-326): every fp32 operand x is split into
 // bf16 hi = rn(x) and lo = rn(x - hi) and each Linear layer is
-//     D = A_hi*B_hi + A_lo*B_hi + A_hi*B_lo          (three wgmma m64n128k16 per k-step, fp32 accumulation in registers);
+//     D = A_hi*B_hi + A_lo*B_hi + A_hi*B_lo          (three wgmma m64nWk16 per k-step, in this order, k-steps ascending,
+//                                                      fp32 accumulation in registers);
 // the dropped A_lo*B_lo term and the split residuals are O(2^-16) relative per product (DESIGN.md).
-// Hidden width 128 or 256, encoded input up to 64 features (one or two 32-wide input chunks).
+// Hidden width W = 128 or 256 (a template parameter), encoded input up to 64 features (one or two 32-wide input chunks).
 //
 // Layout (one persistent CTA per SM, one 128-ray tile at a time):
 //   * warpgroups 0 and 1 each own 64 rays of the tile (wgmma M = 64) and everything about them: they encode their rays
 //     into the input operand, issue the wgmmas of every layer, and run the epilogues.  A warpgroup's operand rows are
 //     read by its own wgmmas only, so the two warpgroups never wait for each other, and one's epilogue runs under the
 //     other's MMAs;
-//   * every Linear layer is issued as passes of N = 128 output columns (a 256-wide hidden layer as two passes held in
-//     two register accumulators, the last layer as ceil(out / 128) passes);
-//   * the activation operand A (hi and lo, 2 x 64 KB, K-major no-swizzle) is rewritten in place by the epilogue of the
-//     layer that reads it: the warpgroup's wgmmas of that layer have all retired by then (wgmma.wait_group 0);
-//   * warp 8 streams the weight images (bf16 hi + lo, consumption order, hr_tc_pack.cu) through a 4-stage
-//     cp.async.bulk ring guarded by mbarriers; each consumer warpgroup releases a stage once the wgmmas that read it
-//     have retired.
+//   * every Linear layer is issued as passes of N = W output columns: a hidden layer is one pass held in one register
+//     accumulator (128 registers at W = 256), the last layer is ceil(out / W) zero-padded passes;
+//   * the activation operand A (hi and lo, 2 x 64 KB at W = 256, K-major no-swizzle) is rewritten in place by the
+//     epilogue of the layer that reads it: the warpgroup's wgmmas of that layer have all retired by then
+//     (wgmma.wait_group 0);
+//   * warpgroup 2 streams the weight images (bf16 hi + lo, consumption order, hr_tc_pack.cu) through a 4-stage
+//     cp.async.bulk ring of 16 KB stages (one k-step at W = 256) guarded by mbarriers; each consumer warpgroup releases a
+//     stage once the wgmmas that read it have retired, so every stage is loaded once per tile for both.
 // The last layer's columns go from the accumulators (+ bias) straight to the heads scratch in global memory.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -35,16 +37,19 @@ namespace hr {
 namespace tc2 {
 using namespace tc;
 
-constexpr int PASS_N = 128;          // output columns of one pass (wgmma N)
 constexpr int NSTAGE = 4;            // weight ring depth
-constexpr int STAGE_BYTES = 16384;   // one 32-k chunk of a pass: two k-step images of 128 rows x 16 k x (hi+lo) bf16
-constexpr int KSTEP_BYTES = 4096;    // 128 rays x 16 k bf16
-constexpr int NKSTEP = 16;           // hidden width 256 / 16
+constexpr int STAGE_BYTES = 16384;   // one ring stage: k-step images of W x 16 k x (hi + lo) bf16, 1 (W = 256) or 2 (W = 128)
+constexpr int KSTEP_BYTES = 4096;    // activation k-step image: 128 rays x 16 k bf16
 constexpr int CONSUMERS = 2;         // warpgroups of 64 rays
-constexpr int NTHREADS = CONSUMERS * 128 + 32;
+constexpr int NTHREADS = (CONSUMERS + 1) * 128;  // + the producer warpgroup (one thread of it issues the copies)
+// register split of the 64 K registers (setmaxnreg): the producer warpgroup gives up what the consumers need beside their
+// 128 accumulator registers at W = 256
+constexpr int PRODUCER_REGS = 40;
+constexpr int CONSUMER_REGS = 232;
+static_assert(128 * PRODUCER_REGS + CONSUMERS * 128 * CONSUMER_REGS <= 65536, "register file");
 
 // shared memory map (bytes)
-constexpr int A_BYTES = NKSTEP * KSTEP_BYTES;                // 64 KB: one half (hi or lo) of the activation operand
+constexpr int A_BYTES = 16 * KSTEP_BYTES;                    // 64 KB: one half (hi or lo) of the activation operand
 constexpr int OFF_AHI = 0;
 constexpr int OFF_ALO = OFF_AHI + A_BYTES;
 constexpr int X_BYTES = 4 * KSTEP_BYTES;                     // encoded input: up to 4 k-steps (64 k) hi, then as many lo
@@ -61,10 +66,16 @@ static_assert((BAR_EMPTY + NSTAGE) * 8 <= 128, "barrier block");
 
 }  // namespace tc2
 
+template <int W>
 __global__ void __launch_bounds__(tc2::NTHREADS, 1)
 mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ MlpTcPack pk, const float* __restrict__ rays,
                float* __restrict__ heads, long long n_rays, float* __restrict__ rays_copy) {
   using namespace tc2;
+  constexpr int NACC = W / 2;                        // accumulator registers of one W-column pass
+  constexpr int NK = W / 16;                         // k-steps of the hidden activation operand
+  constexpr int IMG_BYTES = W * 64;                  // weight image of one k-step: W x 16 k, hi then lo
+  constexpr int KPS = STAGE_BYTES / IMG_BYTES;       // k-steps per ring stage
+  static_assert(KPS * IMG_BYTES == STAGE_BYTES && NK * KSTEP_BYTES <= A_BYTES, "pass width");
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t sbase = smem_u32(smem);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -92,20 +103,20 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
   // tiles blockIdx.x, blockIdx.x + gridDim.x, ... : every role of this CTA runs exactly this many iterations
   const long long n_iters = ((long long)blockIdx.x < n_tiles) ? (n_tiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
 
-  if (warp == CONSUMERS * 4) {
+  if (warp >= CONSUMERS * 4) {
     // =========================== producer: weight images, in consumption order ===========================
-    if (lane == 0) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == CONSUMERS * 4 && lane == 0) {
+      const int n_stages = (int)(pk.wpack_bytes / STAGE_BYTES);  // every pass is a whole number of stages
       uint32_t stage = 0, phase = 0;
       for (long long iter = 0; iter < n_iters; ++iter) {
         const uint8_t* src = reinterpret_cast<const uint8_t*>(pk.wpack);
-        for (int p = 0; p < n_passes; ++p) {
-          for (int i = 0; i < pk.passes[p].n_chunks; ++i) {
-            mbar_wait(bar(BAR_EMPTY + stage), phase ^ 1);
-            mbar_expect_tx(bar(BAR_FULL + stage), STAGE_BYTES);
-            bulk_g2s(sbase + OFF_B + stage * STAGE_BYTES, src, STAGE_BYTES, bar(BAR_FULL + stage));
-            src += STAGE_BYTES;
-            if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
-          }
+        for (int i = 0; i < n_stages; ++i) {
+          mbar_wait(bar(BAR_EMPTY + stage), phase ^ 1);
+          mbar_expect_tx(bar(BAR_FULL + stage), STAGE_BYTES);
+          bulk_g2s(sbase + OFF_B + stage * STAGE_BYTES, src, STAGE_BYTES, bar(BAR_FULL + stage));
+          src += STAGE_BYTES;
+          if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
         }
       }
     }
@@ -113,12 +124,12 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
   }
 
   // =========================== consumer warpgroups: 64 rays each ===========================
+  setmaxnreg_inc<CONSUMER_REGS>();
   const int wg = warp >> 2;                 // 0 .. CONSUMERS-1
   const int wt = tid & 127;                 // thread within the warpgroup
   const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // tile rows of accumulator elements (i / 2) % 2 == 0; +8 for 1
   const int q2 = (lane & 3) * 2;            // first of the two columns of an accumulator pair
   const int in_chunks = pk.in_chunks;
-  const int W = cfg.mlp_width;
   const int L = cfg.mlp_layers;
   const uint32_t x_lo_off = (uint32_t)(2 * in_chunks * KSTEP_BYTES);  // lo half follows the hi k-steps
   const uint32_t rows_off = (uint32_t)wg * 1024u;                     // this warpgroup's 8 row groups of a k-step image
@@ -127,54 +138,68 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
   uint32_t stage = 0, phase = 0;
   int pend = -1;  // ring stage whose wgmmas were committed but not yet waited for
 
-  float acc0[64], acc1[64];
+  float acc[NACC];
 
-  // one pass: acc = A(chunks of P) * B(P)^T, 3 wgmmas per k-step; the ring stage of each chunk is released one chunk later
-  auto run_pass = [&](float (&acc)[64], const TcPass& P) {
-    for (int c = P.first_chunk; c < P.first_chunk + P.n_chunks; ++c) {
-      uint32_t a_hi, a_lo;
-      if (c < in_chunks) {
-        a_hi = sbase + OFF_X + (uint32_t)(2 * c) * KSTEP_BYTES + rows_off;
-        a_lo = a_hi + x_lo_off;
-      } else {
-        a_hi = sbase + OFF_AHI + (uint32_t)(2 * (c - in_chunks)) * KSTEP_BYTES + rows_off;
-        a_lo = a_hi + (OFF_ALO - OFF_AHI);
-      }
-      mbar_wait(full0 + stage * 8, phase);
-      const uint32_t b0 = sbase + OFF_B + stage * STAGE_BYTES;
-      wgmma_fence();
-      acc_fence(acc);
+  auto stage_begin = [&]() {
+    mbar_wait(full0 + stage * 8, phase);
+    wgmma_fence();
+    acc_fence(acc);
+  };
+  // the ring stage of each k-step group is released one stage later, once its wgmmas have retired
+  auto stage_end = [&]() {
+    wgmma_commit();
+    acc_fence(acc);
+    wgmma_wait<1>();
+    if (pend >= 0 && wt == 0) mbar_arrive(empty0 + pend * 8);
+    pend = (int)stage;
+    if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
+  };
+  auto b_img = [&](int sub) -> uint32_t { return sbase + OFF_B + stage * STAGE_BYTES + (uint32_t)sub * IMG_BYTES; };
+  // one pass: acc = A(chunks of P) * B(P)^T, 3 wgmmas per k-step
+  auto run_pass = [&](const TcPass& P) {
+    int ki = 0;  // k-steps issued in this pass; the input's count (2 per chunk) is even, so a stage never straddles
+    if (P.first_chunk == 0) {  // encoded input: hi and lo from shared memory
+      for (; ki < 2 * in_chunks; ki += KPS) {
+        stage_begin();
 #pragma unroll
-      for (int ks = 0; ks < 2; ++ks) {
-        const uint64_t ah = gmma_desc(a_hi + ks * KSTEP_BYTES, 2048, 128);
-        const uint64_t al = gmma_desc(a_lo + ks * KSTEP_BYTES, 2048, 128);
-        const uint64_t bh = gmma_desc(b0 + ks * (PASS_N * 64), PASS_N * 16, 128);
-        const uint64_t bl = gmma_desc(b0 + ks * (PASS_N * 64) + PASS_N * 32, PASS_N * 16, 128);
-        wgmma_128(acc, ah, bh, (c != P.first_chunk || ks != 0) ? 1u : 0u);
-        wgmma_128(acc, al, bh, 1u);
-        wgmma_128(acc, ah, bl, 1u);
+        for (int sub = 0; sub < KPS; ++sub) {
+          const uint32_t a_hi = sbase + OFF_X + (uint32_t)(ki + sub) * KSTEP_BYTES + rows_off, b = b_img(sub);
+          const uint64_t ah = gmma_desc(a_hi, 2048, 128), al = gmma_desc(a_hi + x_lo_off, 2048, 128);
+          const uint64_t bh = gmma_desc(b, W * 16, 128), bl = gmma_desc(b + W * 32, W * 16, 128);
+          wgmma_ss(acc, ah, bh, (ki + sub) != 0 ? 1u : 0u);
+          wgmma_ss(acc, al, bh, 1u);
+          wgmma_ss(acc, ah, bl, 1u);
+        }
+        stage_end();
       }
-      wgmma_commit();
-      acc_fence(acc);
-      wgmma_wait<1>();
-      if (pend >= 0 && wt == 0) mbar_arrive(empty0 + pend * 8);
-      pend = (int)stage;
-      if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
+    }
+    if (P.first_chunk + P.n_chunks > in_chunks) {  // hidden activation
+      const uint32_t scale0 = ki != 0 ? 1u : 0u;
+#pragma unroll
+      for (int kk = 0; kk < NK; ++kk) {
+        if (kk % KPS == 0) stage_begin();
+        const uint32_t a_hi = sbase + OFF_AHI + (uint32_t)kk * KSTEP_BYTES + rows_off, b = b_img(kk % KPS);
+        const uint64_t ah = gmma_desc(a_hi, 2048, 128), al = gmma_desc(a_hi + (OFF_ALO - OFF_AHI), 2048, 128);
+        const uint64_t bh = gmma_desc(b, W * 16, 128), bl = gmma_desc(b + W * 32, W * 16, 128);
+        wgmma_ss(acc, ah, bh, kk != 0 ? 1u : scale0);
+        wgmma_ss(acc, al, bh, 1u);
+        wgmma_ss(acc, ah, bl, 1u);
+        if (kk % KPS == KPS - 1) stage_end();
+      }
     }
   };
   auto drain = [&]() {
     wgmma_wait<0>();
-    acc_fence(acc0);
-    acc_fence(acc1);
+    acc_fence(acc);
     if (pend >= 0 && wt == 0) mbar_arrive(empty0 + pend * 8);
     pend = -1;
   };
-  // hidden epilogue: columns [col0, col0 + 128) of A(l+1) = LeakyReLU(acc + bias), split into hi / lo
-  auto store_hidden = [&](const float (&acc)[64], int col0, const float* bias) {
+  // hidden epilogue: A(l+1) = LeakyReLU(acc + bias), split into hi / lo
+  auto store_hidden = [&](const float* bias) {
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int k = col0 + 8 * j + q2;
-      const float2 b = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + q2));
+    for (int j = 0; j < W / 8; ++j) {
+      const int k = 8 * j + q2;
+      const float2 b = __ldg(reinterpret_cast<const float2*>(bias + k));
       const uint32_t off = (uint32_t)(k >> 4) * KSTEP_BYTES + (uint32_t)(k & 7) * 2u;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -227,23 +252,19 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
       fence_async_smem();
       wg_sync(1 + wg);
     }
-    // ---- the layers ----
-    int p = 0;
+    // ---- the hidden layers: one pass each (passes[l] is layer l) ----
     for (int l = 0; l < L - 1; ++l) {
-      run_pass(acc0, pk.passes[p]);
-      if (W == 256) run_pass(acc1, pk.passes[p + 1]);
+      run_pass(pk.passes[l]);
       drain();
       wg_sync(1 + wg);  // every warp's wgmmas that read A(l) have retired before A(l+1) overwrites it
-      store_hidden(acc0, 0, pk.bias + pk.passes[p].bias_off);
-      if (W == 256) store_hidden(acc1, PASS_N, pk.bias + pk.passes[p + 1].bias_off);
+      store_hidden(pk.bias + pk.passes[l].bias_off);
       fence_async_smem();
       wg_sync(1 + wg);
-      p += W / PASS_N;
     }
     // ---- last layer: accumulators + bias -> heads scratch (rows past n_rays / columns past mlp_out are dropped) ----
-    for (; p < n_passes; ++p) {
+    for (int p = L - 1; p < n_passes; ++p) {
       const TcPass& P = pk.passes[p];
-      run_pass(acc0, P);
+      run_pass(P);
       drain();
       const float* bias = pk.bias + P.bias_off;
 #pragma unroll
@@ -252,11 +273,11 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
         if (ray >= n_rays) continue;
         float* dst = heads + ray * cfg.mlp_out + P.out_col0;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
+        for (int j = 0; j < W / 8; ++j) {
           const int c = 8 * j + q2;
           if (P.out_col0 + c < cfg.mlp_out) {  // mlp_out is a multiple of 4: the pair is in or out as a whole
             const float2 b = __ldg(reinterpret_cast<const float2*>(bias + c));
-            *reinterpret_cast<float2*>(dst + c) = make_float2(acc0[4 * j + 2 * h] + b.x, acc0[4 * j + 2 * h + 1] + b.y);
+            *reinterpret_cast<float2*>(dst + c) = make_float2(acc[4 * j + 2 * h] + b.x, acc[4 * j + 2 * h + 1] + b.y);
           }
         }
       }
@@ -281,18 +302,18 @@ int pack_mlp_tc2(hr_handle* h, const hr_config& c, MlpTcPack& pk, size_t& alloc_
   for (int l = 0; l < L; ++l) {
     const bool last = (l == L - 1);
     const int out = last ? c.mlp_out : W;
-    const int n_parts = (out + tc2::PASS_N - 1) / tc2::PASS_N;
+    const int n_parts = (out + W - 1) / W;  // one pass per hidden layer
     for (int part = 0; part < n_parts; ++part) {
       if (np >= HR_TC_MAX_PASSES) return hr_fail("tensor-core sample net: too many passes (%d output columns)", c.mlp_out);
       TcPass& P = np_.passes[np++];
       const bool reads_input = (l == 0 || l == c.mlp_skip);
       P.layer = l;
-      P.n = tc2::PASS_N;  // a partial last pass is zero padded
+      P.n = W;  // a partial last pass is zero padded
       P.first_chunk = reads_input ? 0 : in_chunks;
       P.n_chunks = (l == 0) ? in_chunks : (W / 32 + (reads_input ? in_chunks : 0));
       P.bias_off = bias_off;
       P.is_final = last ? 1 : 0;
-      P.out_col0 = part * tc2::PASS_N;
+      P.out_col0 = part * W;
       P.wait_a = (part == 0) ? 1 : 0;
       bias_off += P.n;
       bytes += (size_t)P.n_chunks * 2 * P.n * 64;
@@ -314,7 +335,8 @@ int pack_mlp_tc2(hr_handle* h, const hr_config& c, MlpTcPack& pk, size_t& alloc_
     np_.wpack = wp; np_.bias = bp;
     alloc_bytes = bytes; alloc_bias = bias_off;
     // opt in to the 224 KB of dynamic shared memory once per (handle, device)
-    e = cudaFuncSetAttribute(mlp_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::SMEM_BYTES);
+    e = (W == 256) ? cudaFuncSetAttribute(mlp_tc2_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::SMEM_BYTES)
+                   : cudaFuncSetAttribute(mlp_tc2_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::SMEM_BYTES);
     if (e != cudaSuccess) return hr_fail("cudaFuncSetAttribute(mlp_tc2_kernel): %s", cudaGetErrorString(e));
   } else {
     np_.wpack = pk.wpack; np_.bias = pk.bias;
@@ -355,7 +377,12 @@ cudaError_t launch_mlp_tc2(const hr_config& cfg, const MlpTcPack& pk, const floa
   long long tiles = (n + tc::BM - 1) / tc::BM;
   int grid = (int)(tiles < num_sms ? tiles : num_sms);
   if (grid < 1) grid = 1;
-  mlp_tc2_kernel<<<grid, tc2::NTHREADS, tc2::SMEM_BYTES, stream>>>(cfg, pk, rays, heads, n, rays_copy);
+  if (cfg.mlp_width == 256)
+    mlp_tc2_kernel<256><<<grid, tc2::NTHREADS, tc2::SMEM_BYTES, stream>>>(cfg, pk, rays, heads, n, rays_copy);
+  else if (cfg.mlp_width == 128)
+    mlp_tc2_kernel<128><<<grid, tc2::NTHREADS, tc2::SMEM_BYTES, stream>>>(cfg, pk, rays, heads, n, rays_copy);
+  else
+    return cudaErrorInvalidValue;
   return cudaGetLastError();
 }
 
