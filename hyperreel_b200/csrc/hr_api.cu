@@ -1229,6 +1229,67 @@ int hr_grad_read(hr_handle* h, const hr_grads* out, void* stream) {
   return 0;
 }
 
+// ---- the sample net's training forward / backward on the tensor cores (hr_mlp_tc2.cu, hr_mlp_train.cu) ----
+static int train_net_supported(const hr_handle* h, const char* fn) {
+  const hr_config& c = h->cfg;
+  if (c.cascade) return fail("%s: cascaded (point_prediction) pipelines have two sample nets; only single-net pipelines train on the tensor cores", fn);
+  if (c.mlp_mode == HR_MLP_ZERO) return fail("%s: a zero sample net has no layers to train", fn);
+  if (c.mlp_mode != HR_MLP_BF16X3_TC) return fail("%s: the training forward is the wgmma sample net: create the handle with mlp_mode HR_MLP_BF16X3_TC", fn);
+  if (!h->uploaded || !h->tc_ready) return fail("%s: parameters not uploaded", fn);
+  return 0;
+}
+
+int64_t hr_train_net_workspace_bytes(const hr_handle* h, int64_t n_rays) {
+  if (!h || n_rays < 0) return -1;
+  return (int64_t)hr::train_net_layout(h->cfg, n_rays, h->num_sms).total;
+}
+
+int hr_train_net_forward(hr_handle* h, const float* rays, int64_t n, float* heads, void* workspace, int64_t workspace_bytes,
+                         void* stream) {
+  if (!h || !rays || !heads || !workspace) return fail("hr_train_net_forward: null argument");
+  if (train_net_supported(h, "hr_train_net_forward")) return 1;
+  if (n == 0) return 0;
+  const hr::TrainNetLayout t = hr::train_net_layout(h->cfg, n, h->num_sms);
+  if (workspace_bytes < (int64_t)t.total) return fail("hr_train_net_forward: workspace too small (hr_train_net_workspace_bytes)");
+  if (((uintptr_t)workspace & 255) != 0) return fail("hr_train_net_forward: workspace must be 256-byte aligned");
+  DeviceGuard guard(h->device);
+  uint8_t* ws = (uint8_t*)workspace;
+  const hr::TrainSave sv{(float*)(ws + t.enc), (float*)(ws + t.act), (long long)t.act_stride, t.ld_enc};
+  cudaError_t e = hr::launch_mlp_tc2_train(h->cfg, h->tc, rays, heads, n, h->num_sms, (cudaStream_t)stream, sv);
+  if (e != cudaSuccess) return fail("hr_train_net_forward: %s", cudaGetErrorString(e));
+  h->launches += 1;
+  return 0;
+}
+
+int hr_train_net_backward(hr_handle* h, const float* d_heads, int64_t n, const hr_net_grads* out, void* workspace,
+                          int64_t workspace_bytes, void* stream) {
+  if (!h || !d_heads || !out || !workspace) return fail("hr_train_net_backward: null argument");
+  if (train_net_supported(h, "hr_train_net_backward")) return 1;
+  const hr_config& c = h->cfg;
+  const int L = c.mlp_layers, W = c.mlp_width;
+  for (int l = 0; l < L; ++l)
+    if (!out->weight[l] || !out->bias[l]) return fail("hr_train_net_backward: gradient buffers of layer %d missing", l);
+  DeviceGuard guard(h->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n == 0) {  // no rays: every gradient is zero
+    for (int l = 0; l < L; ++l) {
+      const int out_l = l == L - 1 ? c.mlp_out : W, in_l = l == 0 ? c.mlp_in : (l == c.mlp_skip ? c.mlp_in + W : W);
+      CK(cudaMemsetAsync(out->weight[l], 0, (size_t)out_l * in_l * sizeof(float), st));
+      CK(cudaMemsetAsync(out->bias[l], 0, (size_t)out_l * sizeof(float), st));
+    }
+    return 0;
+  }
+  const hr::TrainNetLayout t = hr::train_net_layout(c, n, h->num_sms);
+  if (workspace_bytes < (int64_t)t.total) return fail("hr_train_net_backward: workspace too small (hr_train_net_workspace_bytes)");
+  if (((uintptr_t)workspace & 255) != 0) return fail("hr_train_net_backward: workspace must be 256-byte aligned");
+  uint8_t* ws = (uint8_t*)workspace;
+  permute_heads<<<grid_for(n * (long long)c.mlp_out), 256, 0, st>>>(d_heads, (float*)(ws + t.dlast), n, c.n_samples, c.head_stride);
+  cudaError_t e = hr::train_net_backward(c, h->simt, n, out->weight, out->bias, ws, h->num_sms, st);
+  if (e != cudaSuccess) return fail("hr_train_net_backward: %s", cudaGetErrorString(e));
+  h->launches += 1 + 3 * L;
+  return 0;
+}
+
 int64_t hr_launch_count(const hr_handle* h) { return h ? h->launches : -1; }
 
 int hr_timing_enable(hr_handle* h, int enable) {

@@ -51,6 +51,30 @@ cudaError_t launch_mlp_simt(const hr_config& cfg, const MlpSimtPack& pk, const f
 // rays may point to pinned host memory (read once, by the encoding threads); rays_copy (optional) receives a device copy
 cudaError_t launch_mlp_tc2(const hr_config& cfg, const MlpTcPack& pk, const float* rays, float* heads, long long n,
                            int num_sms, cudaStream_t stream, float* rays_copy = nullptr);
+
+// Training net on the tensor cores (hr_mlp_train.cu).  The forward is mlp_tc2_kernel<W, SAVE = true>: it also writes the
+// encoded input enc [n][ld_enc] (zero padded past mlp_in) and hidden layer l's LeakyReLU output at act + l * act_stride,
+// [n][W], all fp32, and stores the heads in the reference's order.
+struct TrainSave {
+  float* enc;
+  float* act;
+  long long act_stride;  // floats between two layers' activations
+  int ld_enc;
+};
+cudaError_t launch_mlp_tc2_train(const hr_config& cfg, const MlpTcPack& pk, const float* rays, float* heads, long long n,
+                                 int num_sms, cudaStream_t stream, const TrainSave& sv);
+
+// Workspace of one training step of the net over n rays (byte offsets, each 256-byte aligned): the forward's saved
+// activations, the channel-major d heads, two [n][W] buffers for the hidden layers' dY, the dW GEMM's split-K partials.
+struct TrainNetLayout {
+  size_t enc, act, act_stride, dlast, dy[2], part, dbpart, total;
+  int ld_enc;
+};
+TrainNetLayout train_net_layout(const hr_config& c, long long n, int num_sms);
+// d_heads_cm [n][mlp_out] channel-major (inside the workspace at dlast) -> every layer's dW / db into weight[l] / bias[l]
+// ([out, in] / [out] of the uploaded weights).  W_t: the fp32 CUDA-core pack (MlpSimtPack), read as the transposed weights.
+cudaError_t train_net_backward(const hr_config& c, const MlpSimtPack& simt, long long n, float* const* weight,
+                               float* const* bias, uint8_t* ws, int num_sms, cudaStream_t st);
 }  // namespace hr
 
 struct hr_handle;

@@ -21,6 +21,10 @@
 //     cp.async.bulk ring of 16 KB stages (one k-step at W = 256) guarded by mbarriers; each consumer warpgroup releases a
 //     stage once the wgmmas that read it have retired, so every stage is loaded once per tile for both.
 // The last layer's columns go from the accumulators (+ bias) straight to the heads scratch in global memory.
+//
+// SAVE (the training forward, hr_mlp_train.cu): the same arithmetic, plus every fp32 value the epilogues split goes to global
+// memory as well -- the encoded input (sv.enc) and each hidden layer's LeakyReLU output (sv.act) -- and the heads are stored
+// in the reference's sample-major column order instead of channel-major.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -66,10 +70,10 @@ static_assert((BAR_EMPTY + NSTAGE) * 8 <= 128, "barrier block");
 
 }  // namespace tc2
 
-template <int W>
+template <int W, bool SAVE>
 __global__ void __launch_bounds__(tc2::NTHREADS, 1)
 mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ MlpTcPack pk, const float* __restrict__ rays,
-               float* __restrict__ heads, long long n_rays, float* __restrict__ rays_copy) {
+               float* __restrict__ heads, long long n_rays, float* __restrict__ rays_copy, const TrainSave sv) {
   using namespace tc2;
   constexpr int NACC = W / 2;                        // accumulator registers of one W-column pass
   constexpr int NK = W / 16;                         // k-steps of the hidden activation operand
@@ -195,7 +199,7 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
     pend = -1;
   };
   // hidden epilogue: A(l+1) = LeakyReLU(acc + bias), split into hi / lo
-  auto store_hidden = [&](const float* bias) {
+  auto store_hidden = [&](const float* bias, int layer, long long tile) {
 #pragma unroll
     for (int j = 0; j < W / 8; ++j) {
       const int k = 8 * j + q2;
@@ -208,6 +212,10 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
         t1 = fmaxf(t1, t1 * cfg.leaky_slope);
         uint32_t hi, lo;
         split2(t0, t1, hi, lo);
+        if constexpr (SAVE) {
+          const long long ray = tile * BM + row0 + 8 * h;
+          if (ray < n_rays) *reinterpret_cast<float2*>(sv.act + layer * sv.act_stride + ray * W + k) = make_float2(t0, t1);
+        }
         const uint32_t o = off + ks_slot(row0 + 8 * h, (k >> 3) & 1);
         *reinterpret_cast<uint32_t*>(smem + OFF_AHI + o) = hi;
         *reinterpret_cast<uint32_t*>(smem + OFF_ALO + o) = lo;
@@ -220,14 +228,17 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
     // ---- RayParam + WindowedPE of this warpgroup's 64 rays, two threads per ray, straight into the bf16 hi / lo slots ----
     {
       const int r = wg * 64 + (wt & 63), part = wt >> 6;
+      const long long ray = tile * BM + r;
       auto put = [&](int k, float val) {
+        if constexpr (SAVE) {
+          if (ray < n_rays) sv.enc[ray * sv.ld_enc + k] = val;
+        }
         const __nv_bfloat16 hi = __float2bfloat16_rn(val);
         const __nv_bfloat16 lo = __float2bfloat16_rn(val - __bfloat162float(hi));
         const uint32_t off = (uint32_t)(k >> 4) * KSTEP_BYTES + ks_slot(r, (k >> 3) & 1) + (uint32_t)(k & 7) * 2u;
         *reinterpret_cast<__nv_bfloat16*>(smem + OFF_X + off) = hi;
         *reinterpret_cast<__nv_bfloat16*>(smem + OFF_X + x_lo_off + off) = lo;
       };
-      const long long ray = tile * BM + r;
       if (ray < n_rays) {
         // `rays` may be pinned host memory (zero-copy input of hr_render_host): each ray is read once per thread, with
         // vector loads, and `rays_copy` receives the device copy the render kernel reads.
@@ -246,6 +257,10 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
             for (int i = 0; i < cfg.c_in; ++i) rays_copy[ray * cfg.c_in + i] = rbuf[i];
         }
         encode_ray_features(cfg, rbuf, part, 2, put);
+        if constexpr (SAVE) {
+          if (part == 0)
+            for (int k = cfg.mlp_in; k < sv.ld_enc; ++k) sv.enc[ray * sv.ld_enc + k] = 0.0f;  // the padding the dW GEMM reads
+        }
       } else if (part == 0) {
         for (int k = 0; k < cfg.mlp_in; ++k) put(k, 0.0f);  // masked row: defined (never stored) values
       }
@@ -257,7 +272,7 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
       run_pass(pk.passes[l]);
       drain();
       wg_sync(1 + wg);  // every warp's wgmmas that read A(l) have retired before A(l+1) overwrites it
-      store_hidden(pk.bias + pk.passes[l].bias_off);
+      store_hidden(pk.bias + pk.passes[l].bias_off, l, tile);
       fence_async_smem();
       wg_sync(1 + wg);
     }
@@ -277,7 +292,14 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
           const int c = 8 * j + q2;
           if (P.out_col0 + c < cfg.mlp_out) {  // mlp_out is a multiple of 4: the pair is in or out as a whole
             const float2 b = __ldg(reinterpret_cast<const float2*>(bias + c));
-            *reinterpret_cast<float2*>(dst + c) = make_float2(acc[4 * j + 2 * h] + b.x, acc[4 * j + 2 * h + 1] + b.y);
+            if constexpr (SAVE) {  // channel-major column c*S+s -> the reference's s*stride+c
+              float* row = heads + ray * cfg.mlp_out;
+              const int c0 = P.out_col0 + c, c1 = c0 + 1, S = cfg.n_samples;
+              row[(c0 % S) * cfg.head_stride + c0 / S] = acc[4 * j + 2 * h] + b.x;
+              row[(c1 % S) * cfg.head_stride + c1 / S] = acc[4 * j + 2 * h + 1] + b.y;
+            } else {
+              *reinterpret_cast<float2*>(dst + c) = make_float2(acc[4 * j + 2 * h] + b.x, acc[4 * j + 2 * h + 1] + b.y);
+            }
           }
         }
       }
@@ -335,8 +357,8 @@ int pack_mlp_tc2(hr_handle* h, const hr_config& c, MlpTcPack& pk, size_t& alloc_
     np_.wpack = wp; np_.bias = bp;
     alloc_bytes = bytes; alloc_bias = bias_off;
     // opt in to the 224 KB of dynamic shared memory once per (handle, device)
-    e = (W == 256) ? cudaFuncSetAttribute(mlp_tc2_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::SMEM_BYTES)
-                   : cudaFuncSetAttribute(mlp_tc2_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::SMEM_BYTES);
+    e = (W == 256) ? cudaFuncSetAttribute(mlp_tc2_kernel<256, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::SMEM_BYTES)
+                   : cudaFuncSetAttribute(mlp_tc2_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::SMEM_BYTES);
     if (e != cudaSuccess) return hr_fail("cudaFuncSetAttribute(mlp_tc2_kernel): %s", cudaGetErrorString(e));
   } else {
     np_.wpack = pk.wpack; np_.bias = pk.bias;
@@ -378,11 +400,25 @@ cudaError_t launch_mlp_tc2(const hr_config& cfg, const MlpTcPack& pk, const floa
   int grid = (int)(tiles < num_sms ? tiles : num_sms);
   if (grid < 1) grid = 1;
   if (cfg.mlp_width == 256)
-    mlp_tc2_kernel<256><<<grid, tc2::NTHREADS, tc2::SMEM_BYTES, stream>>>(cfg, pk, rays, heads, n, rays_copy);
+    mlp_tc2_kernel<256, false><<<grid, tc2::NTHREADS, tc2::SMEM_BYTES, stream>>>(cfg, pk, rays, heads, n, rays_copy, TrainSave{});
   else if (cfg.mlp_width == 128)
-    mlp_tc2_kernel<128><<<grid, tc2::NTHREADS, tc2::SMEM_BYTES, stream>>>(cfg, pk, rays, heads, n, rays_copy);
+    mlp_tc2_kernel<128, false><<<grid, tc2::NTHREADS, tc2::SMEM_BYTES, stream>>>(cfg, pk, rays, heads, n, rays_copy, TrainSave{});
   else
     return cudaErrorInvalidValue;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_mlp_tc2_train(const hr_config& cfg, const MlpTcPack& pk, const float* rays, float* heads, long long n,
+                                 int num_sms, cudaStream_t stream, const TrainSave& sv) {
+  if ((cfg.mlp_out % 4) != 0) return cudaErrorInvalidValue;
+  long long tiles = (n + tc::BM - 1) / tc::BM;
+  int grid = (int)(tiles < num_sms ? tiles : num_sms);
+  if (grid < 1) grid = 1;
+  auto kern = cfg.mlp_width == 256 ? mlp_tc2_kernel<256, true> : mlp_tc2_kernel<128, true>;
+  if (cfg.mlp_width != 256 && cfg.mlp_width != 128) return cudaErrorInvalidValue;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::SMEM_BYTES);
+  if (e != cudaSuccess) return e;
+  kern<<<grid, tc2::NTHREADS, tc2::SMEM_BYTES, stream>>>(cfg, pk, rays, heads, n, nullptr, sv);
   return cudaGetLastError();
 }
 

@@ -11,7 +11,7 @@ import os
 import subprocess
 import threading
 
-HR_ABI_VERSION = 11
+HR_ABI_VERSION = 12
 HR_MAX_GROUPS = 4
 HR_MAX_LAYERS = 10
 HR_MAX_SAMPLES = 256
@@ -120,6 +120,10 @@ class hr_grads(C.Structure):
                 ("app_second", C.c_void_p * 3), ("basis_mat", C.c_void_p), ("color_embedding", C.c_void_p)]
 
 
+class hr_net_grads(C.Structure):
+    _fields_ = [("weight", C.c_void_p * HR_MAX_LAYERS), ("bias", C.c_void_p * HR_MAX_LAYERS)]
+
+
 class hr_camera(C.Structure):
     _fields_ = [
         ("c2w", C.c_float * 12), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float),
@@ -156,6 +160,10 @@ EXPORTS = {
                                       C.c_void_p, C.c_int64, C.c_void_p]),
     "hr_grad_zero": (C.c_int, [C.c_void_p, C.c_void_p]),
     "hr_grad_read": (C.c_int, [C.c_void_p, C.POINTER(hr_grads), C.c_void_p]),
+    "hr_train_net_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int64]),
+    "hr_train_net_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "hr_train_net_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(hr_net_grads), C.c_void_p, C.c_int64,
+                                         C.c_void_p]),
     "hr_launch_count": (C.c_int64, [C.c_void_p]),
     "hr_timing_enable": (C.c_int, [C.c_void_p, C.c_int]),
     "hr_timing_reset": (C.c_int, [C.c_void_p]),

@@ -71,6 +71,24 @@ class _RenderHeads(torch.autograd.Function):
         return (None, None, d_heads, None, None) + tuple(grads)
 
 
+class _TrainNet(torch.autograd.Function):
+    """The sample net's Linear layers as one differentiable op on the tensor cores: (rays, weights, biases) -> heads
+    [N, S*stride].  forward = hr_train_net_forward (the wgmma render net, saving its activations in a workspace kept for
+    backward); backward = hr_train_net_backward (bf16x3 wgmma dX / dW GEMMs) -> every layer's weight and bias gradient."""
+
+    @staticmethod
+    def forward(ctx, model, rays, *params):
+        heads, ws = model._train_net_forward(rays)
+        ctx.model, ctx.ws, ctx.n = model, ws, rays.shape[0]
+        return heads
+
+    @staticmethod
+    def backward(ctx, d_heads):
+        grads = ctx.model._train_net_backward(ctx.ws, d_heads.contiguous().float(), ctx.n)
+        ctx.ws = None
+        return (None, None) + tuple(grads)
+
+
 class LightfieldModel(nn.Module):
     def __init__(self, cfg, **kwargs):
         super().__init__()
@@ -79,6 +97,12 @@ class LightfieldModel(nn.Module):
         dataset.setdefault("far", 1.0)
         dataset.setdefault("depth_range", [dataset["near"], dataset["far"]])
         self._mlp_mode = resolve_mlp_mode(kwargs.get("mlp_mode", "auto"))
+        # how render_differentiable trains the sample net: "torch" (its Linear layers as torch ops) or "tc" (hr_train_net_*)
+        self._train_net = kwargs.get("train_net", "torch")
+        if self._train_net not in ("torch", "tc"):
+            raise ValueError(f"train_net must be 'torch' or 'tc', got {self._train_net!r}")
+        if self._train_net == "tc" and self._mlp_mode != L.MLP_BF16X3_TC:
+            raise ValueError("train_net='tc' trains the wgmma sample net: mlp_mode must be 'auto' or 'bf16x3'")
         self._iters_per_epoch = kwargs.get("iters_per_epoch")
         self.cfg = cfg
         self.sig: Signature = lower(cfg, dataset, cur_iter=RENDER_ITER,
@@ -182,9 +206,10 @@ class LightfieldModel(nn.Module):
                               return_heads: bool = False):
         """rgb [N,3] with an autograd graph back to every parameter -- what ``training_step`` (nlf/__init__.py:634-709) needs.
         Defaults follow the module mode like the reference: training -> no clamp, white background by coin flip
-        (tensorf_dynamic.py:795-806); eval -> clamp, configured background.  The sample net's Linear layers run as torch
-        ops on the library's encoded input (hr_encode_rays); everything after them is one autograd op around the fused
-        kernels (hr_render_heads / hr_render_backward)."""
+        (tensorf_dynamic.py:795-806); eval -> clamp, configured background.  With train_net="torch" the sample net's
+        Linear layers run as torch ops on the library's encoded input (hr_encode_rays); with "tc" they are one autograd op
+        around the library's tensor-core training net (hr_train_net_forward / hr_train_net_backward).  Everything after them
+        is one autograd op around the fused kernels (hr_render_heads / hr_render_backward)."""
         rays = self._check_rays(rays)
         c = self.sig.cfg
         if self.sig.cascade:
@@ -195,6 +220,21 @@ class LightfieldModel(nn.Module):
             white_bg = bool(c.white_bg) or (self.training and not c.black_bg and bool(torch.rand(()) < 0.5))
         white_bg = bool(white_bg) and not c.black_bg
         self._ensure_uploaded(rays.device)
+        if self._train_net == "tc":
+            x = _TrainNet.apply(self, rays, *self._net_params())
+        else:
+            x = self._torch_net(rays, return_heads)
+        tn = self.color_model.net
+        dplane, dsecond, aplane, asecond = tn.tables()
+        params = [t for t in list(dplane) + list(aplane) + list(dsecond) + list(asecond) if t.numel() > 0] + [tn.basis_mat.weight]
+        if c.n_color_views > 0:  # ColorTransformEmbedding (point.py:558-605): its table acts on the pixel inside the fused op
+            params.append(self.embedding_model.embeddings[self.sig.color_embedding_index].color_embedding)
+        rgb = _RenderHeads.apply(self, rays, x, clamp_output, white_bg, *params)
+        return (rgb, x) if return_heads else rgb  # x: the sample-net output [N, S*stride] (gradient bisecting)
+
+    def _torch_net(self, rays, return_heads):
+        """BaseMLP.forward (mlp.py:159-172) as torch ops on the library's encoded input."""
+        c = self.sig.cfg
         n = rays.shape[0]
         enc = torch.empty((n, c.mlp_in), device=rays.device)
         stream = torch.cuda.current_stream(rays.device).cuda_stream
@@ -218,13 +258,43 @@ class LightfieldModel(nn.Module):
             x = torch.nn.functional.linear(x, lin.weight, lin.bias)
             if i < last:
                 x = torch.nn.functional.leaky_relu(x, c.leaky_slope)
-        tn = self.color_model.net
-        dplane, dsecond, aplane, asecond = tn.tables()
-        params = [t for t in list(dplane) + list(aplane) + list(dsecond) + list(asecond) if t.numel() > 0] + [tn.basis_mat.weight]
-        if c.n_color_views > 0:  # ColorTransformEmbedding (point.py:558-605): its table acts on the pixel inside the fused op
-            params.append(self.embedding_model.embeddings[self.sig.color_embedding_index].color_embedding)
-        rgb = _RenderHeads.apply(self, rays, x, clamp_output, white_bg, *params)
-        return (rgb, x) if return_heads else rgb  # x: the sample-net output [N, S*stride] (gradient bisecting)
+        return x
+
+    def _net_params(self):
+        """[weight, bias] of every Linear layer of the sample net, in order."""
+        out = []
+        for layer in getattr(self.embedding_model.embeddings[0].net, "layers", []):
+            lin = layer[0] if isinstance(layer, nn.Sequential) else layer
+            out += [lin.weight, lin.bias]
+        return out
+
+    def _train_net_forward(self, rays):
+        n, c = rays.shape[0], self.sig.cfg
+        heads = torch.empty((n, c.mlp_out), device=rays.device)
+        # one workspace per step: the backward reads the activations this forward saves in it
+        ws = torch.empty(int(self._lib.hr_train_net_workspace_bytes(self._handle, n)), dtype=torch.uint8, device=rays.device)
+        stream = torch.cuda.current_stream(rays.device).cuda_stream
+        L.check(self._lib.hr_train_net_forward(self._handle, rays.data_ptr(), n, heads.data_ptr(), ws.data_ptr(), ws.numel(), stream))
+        return heads, ws
+
+    def _train_net_backward(self, ws, d_heads, n):
+        params = self._net_params()
+        grads = [torch.empty(p.shape, device=d_heads.device, dtype=torch.float32) for p in params]
+        G = L.hr_net_grads()
+        for i, g in enumerate(grads):
+            (G.weight if i % 2 == 0 else G.bias)[i // 2] = g.data_ptr()
+        stream = torch.cuda.current_stream(d_heads.device).cuda_stream
+        L.check(self._lib.hr_train_net_backward(self._handle, d_heads.data_ptr(), n, C.byref(G), ws.data_ptr(), ws.numel(), stream))
+        perm = list(self.sig.in_perm)
+        if perm != list(range(len(perm))):
+            # BasicPE: the uploaded first / skip layer has its input columns in the kernels' order (_ensure_uploaded), reference
+            # column in_perm[k] = uploaded column k; the hidden part of the skip layer keeps its place
+            for i in {0, self.sig.cfg.mlp_skip} - {-1}:
+                w = grads[2 * i]
+                src = torch.arange(w.shape[1])
+                src[torch.tensor(perm)] = torch.arange(len(perm))
+                grads[2 * i] = w.index_select(1, src.to(w.device))
+        return grads
 
     def _train_workspace(self, n, dev):
         need = int(self._lib.hr_train_workspace_bytes(self._handle, n))

@@ -75,7 +75,7 @@ class TensoRFRegularizer:
 
 
 class INRSystem(nn.Module):
-    def __init__(self, cfg, dm=None, dataset: Optional[dict] = None, mlp_mode: str = "auto"):
+    def __init__(self, cfg, dm=None, dataset: Optional[dict] = None, mlp_mode: str = "auto", train_net: str = "torch"):
         super().__init__()
         self.cfg = to_cfg(cfg)
         self.dm = dm
@@ -87,7 +87,8 @@ class INRSystem(nn.Module):
             d = self.cfg.dataset
             dataset = {k: d[k] for k in ("name", "collection", "num_keyframes", "num_frames", "near", "far", "depth_range") if k in d}
         model = model_dict[self.cfg.model.type](self.cfg.model, system=self if dm is not None else None,
-                                                dataset=dataset, iters_per_epoch=ipe, mlp_mode=mlp_mode)
+                                                dataset=dataset, iters_per_epoch=ipe, mlp_mode=mlp_mode,
+                                                train_net=train_net)
         self.rendering = False
         self.render_fn = render_fn_dict[self.cfg.model.render.type](
             model, None, self.cfg.model.render, net_chunk=training.get("net_chunk", 32768))

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define HR_ABI_VERSION 11
+#define HR_ABI_VERSION 12
 
 #define HR_MAX_GROUPS 4   /* ray-parameterisation groups feeding the sample net (ray.py:235-263) */
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
@@ -381,6 +381,31 @@ int hr_render_backward(hr_handle* h, const float* rays, const float* heads, int6
                        const hr_train_opts* opts, void* workspace, int64_t workspace_bytes, void* stream);
 int hr_grad_zero(hr_handle* h, void* stream);
 int hr_grad_read(hr_handle* h, const hr_grads* out, void* stream);
+
+/* ---- the sample net's training forward / backward on the tensor cores ----
+ * Replaces: the sample net's Linear layers in the training graph (BaseMLP.forward, nlf/nets/mlp.py:159-172, and what
+ * loss.backward() runs for them), as the alternative to keeping them with the caller (hr_encode_rays).  Every GEMM is
+ * bf16x3 on wgmma (hi*hi + lo*hi + hi*lo, fp32 accumulation), like the HR_MLP_BF16X3_TC render net:
+ *   hr_train_net_forward   rays -> heads [n, mlp_out] in the reference's order, bit-identical to the render net's heads;
+ *                          the encoded input and every hidden activation are saved in the workspace
+ *   hr_train_net_backward  d heads [n, mlp_out] (reference order) -> every layer's dW / db, written (not accumulated) into
+ *                          the caller's buffers; the same workspace, untouched since the forward, is read.  The
+ *                          gradients are bit-reproducible (split-K partials summed in a fixed order, no atomics).
+ * The weights are those of the last hr_upload.  Needs a handle with mlp_mode HR_MLP_BF16X3_TC; cascaded pipelines and zero
+ * nets are refused (hr_last_error).
+ * Workspace (hr_train_net_workspace_bytes, 256-byte aligned): fp32 encoded input [n, mlp_in rounded up to 16], fp32
+ * activations [mlp_layers - 1][n, mlp_width], d heads [n, mlp_out], two [n, mlp_width] dY buffers and the split-K partials
+ * (2 x SMs x 128 x 128 floats) -- 0.62 GB at 65,536 rays on the Technicolor
+ * shape (6 layers of width 256, 9 input features, 480 outputs). */
+int64_t hr_train_net_workspace_bytes(const hr_handle* h, int64_t n_rays);
+int hr_train_net_forward(hr_handle* h, const float* rays, int64_t n_rays, float* heads, void* workspace, int64_t workspace_bytes,
+                         void* stream);
+typedef struct hr_net_grads {  /* device buffers in nn.Linear's layouts of the uploaded net (hr_params.mlp_weight / mlp_bias) */
+  float* weight[HR_MAX_LAYERS]; /* [out, in] */
+  float* bias[HR_MAX_LAYERS];   /* [out]     */
+} hr_net_grads;
+int hr_train_net_backward(hr_handle* h, const float* d_heads, int64_t n_rays, const hr_net_grads* out, void* workspace,
+                          int64_t workspace_bytes, void* stream);
 
 /* Number of kernels hr_render launched since creation (bench.py's gpu_launches). */
 int64_t hr_launch_count(const hr_handle* h);
