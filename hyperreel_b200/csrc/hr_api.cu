@@ -188,7 +188,7 @@ __global__ void cascade_points_kernel(const __grid_constant__ hr_config cfg, con
     const int s = act ? lane : 0;
     const float zraw = heads0 ? __ldg(heads0 + ray * out0 + cfg.pre_off_z * S0 + s) : 0.0f;
     const float sraw = (heads0 && cfg.pre_off_sigma >= 0) ? __ldg(heads0 + ray * out0 + cfg.pre_off_sigma * S0 + s) : 0.0f;
-    const float sg = cfg.pre_use_sigma ? hr::apply_act(cfg.pre_act_sigma, sraw) : 0.0f;
+    const float sg = cfg.pre_use_sigma ? hr::apply_act_eased(cfg.pre_act_sigma, sraw) : 0.0f;
     const float zr = __fmul_rn(hr::apply_act(cfg.pre_isect_act, hr::apply_act(cfg.pre_act_z, zraw)), __fsub_rn(1.0f, sg));
     const float z = __fadd_rn(__fmul_rn(zr, cfg.pre_z_scale), cfg.pre_samples_tab[s]);
     const float dzg = (fabsf(dz) < 1e-5f) ? 1e12f : dz;  // intersect_utils.py:135-142
@@ -304,6 +304,7 @@ int stage_in(const float* src, size_t count, int on_device, cudaStream_t st, std
 
 int validate(const hr_config& c) {
   if (c.abi_version != HR_ABI_VERSION) return fail("hr_config.abi_version %d != %d", c.abi_version, HR_ABI_VERSION);
+  if (hr::eases_density(c) && c.n_samples > 64) return fail("eased density heads above 64 samples per ray are not supported");
   if (c.c_in != 6 && c.c_in != 8) return fail("unsupported c_in %d (6: static rays, 8: video rays)", c.c_in);
   if (c.n_groups < 1 || c.n_groups > HR_MAX_GROUPS) return fail("unsupported n_groups %d", c.n_groups);
   if (c.mlp_mode != HR_MLP_FP32_SIMT && c.mlp_mode != HR_MLP_BF16X3_TC && c.mlp_mode != HR_MLP_ZERO) return fail("unsupported mlp_mode");
@@ -1287,6 +1288,35 @@ int hr_train_net_backward(hr_handle* h, const float* d_heads, int64_t n, const h
   cudaError_t e = hr::train_net_backward(c, h->simt, n, out->weight, out->bias, ws, h->num_sms, st);
   if (e != cudaSuccess) return fail("hr_train_net_backward: %s", cudaGetErrorString(e));
   h->launches += 1 + 3 * L;
+  return 0;
+}
+
+// every hr_act member of hr_config (the members hr_set_activations may change)
+static hr_act hr_config::* const kActMembers[] = {
+    &hr_config::act_z, &hr_config::act_flow, &hr_config::act_sigma, &hr_config::act_point_sigma, &hr_config::act_offset,
+    &hr_config::act_cscale, &hr_config::act_cshift, &hr_config::isect_act, &hr_config::flow_act, &hr_config::offset_act,
+    &hr_config::act_cscale_global, &hr_config::act_cshift_global, &hr_config::act_ctransform, &hr_config::act_ctshift,
+    &hr_config::pre_act_z, &hr_config::pre_act_sigma, &hr_config::pre_isect_act};
+
+int hr_set_activations(hr_handle* h, const hr_config* cfg) {
+  if (!h || !cfg) return fail("hr_set_activations: null argument");
+  // everything but the activations must be the handle's configuration (hr_config has no padding: 4-byte members only)
+  hr_config probe = *cfg;
+  for (hr_act hr_config::* m : kActMembers) probe.*m = h->cfg.*m;
+  if (memcmp(&probe, &h->cfg, sizeof(hr_config)) != 0)
+    return fail("hr_set_activations: the configuration differs from the handle's beyond its activations (create a new handle)");
+  for (hr_act hr_config::* m : kActMembers) {
+    const hr_act& a = cfg->*m;
+    if (a.kind != HR_ACT_IDENTITY && a.kind != HR_ACT_SIGMOID && a.kind != HR_ACT_TANH)
+      return fail("hr_set_activations: unknown activation kind %d", a.kind);
+    if (a.eased && m != &hr_config::act_sigma && m != &hr_config::act_point_sigma && m != &hr_config::pre_act_sigma)
+      return fail("hr_set_activations: only act_sigma, act_point_sigma and pre_act_sigma may be eased");
+  }
+  if (hr::eases_density(*cfg) && cfg->n_samples > 64)
+    return fail("hr_set_activations: eased density heads above 64 samples per ray are not supported");
+  // the nets' configurations (cfg_net / cfg_pre) are copies of cfg: keep their activations in step, although no net reads them
+  for (hr_act hr_config::* m : kActMembers) h->cfg.*m = h->cfg_net.*m = h->cfg_pre.*m = cfg->*m;
+  drop_host_graph(h);  // its kernel nodes hold the old configuration by value
   return 0;
 }
 

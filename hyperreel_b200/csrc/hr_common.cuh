@@ -80,4 +80,23 @@ __device__ __forceinline__ float apply_act(const hr_act& a, float x) {
   return __fmul_rn(v, a.outer_fac);
 }
 
+// apply_act of a density head (act_sigma, act_point_sigma, pre_act_sigma: the only members hr_config may ease), with
+// EaseValue.ease_out (activations.py:482-489): w * out + (1 - w) * start_value while the window is open.  `eased` is uniform
+// (a __grid_constant__ config), so a closed window runs exactly apply_act's arithmetic.
+__device__ __forceinline__ float apply_act_eased(const hr_act& a, float x) {
+  const float v = apply_act(a, x);
+  return a.eased ? __fadd_rn(__fmul_rn(v, a.ease_mul), a.ease_add) : v;
+}
+
+// a density head's activation in a render kernel: the EASE variants (launched only while an EaseValue window is open, see
+// eases_density) blend; the others compile exactly apply_act
+template <bool EASE>
+__device__ __forceinline__ float apply_act_head(const hr_act& a, float x) {
+  if constexpr (EASE) return apply_act_eased(a, x);
+  else return apply_act(a, x);
+}
+
+// true while act_sigma or act_point_sigma is eased: the render kernels' EASE variants serve the configuration
+__host__ __device__ inline bool eases_density(const hr_config& c) { return c.act_sigma.eased || c.act_point_sigma.eased; }
+
 }  // namespace hr

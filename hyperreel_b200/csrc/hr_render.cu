@@ -12,11 +12,16 @@ HR_BIG_DECL(launch_render_big_4_1);
 HR_BIG_DECL(launch_render_big_8_0);
 HR_BIG_DECL(launch_render_big_8_1);
 HR_BIG_DECL(launch_render_rare);  // hr_render_rare.cu: S <= 64 with the less common primitives / the colour transform
+HR_BIG_DECL(launch_render_ease);  // hr_render_ease.cu: S <= 64 with an eased density head
 
 // Entry used by hr_api.cu.  Returns cudaErrorInvalidValue for an unsupported component layout.
 cudaError_t launch_render(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs, const float* rays,
                           const float* heads, const RgbDst& rgb, long long n, const ExtraOut* so, int num_sms,
                           cudaStream_t stream, unsigned char* rgb8) {
+  if (eases_density(cfg)) {  // hr_create / hr_set_activations refuse eased heads above 64 samples
+    if (cfg.n_samples > 64) return cudaErrorInvalidValue;
+    return launch_render_ease(cfg, dv, tabs, rays, heads, rgb, n, so, num_sms, stream, rgb8);
+  }
   if (cfg.n_samples > 64) {  // 4 (S <= 128) or 8 (S <= 256) samples per lane
     auto* fn = cfg.n_samples > 128 ? (cfg.dynamic ? launch_render_big_8_1 : launch_render_big_8_0)
                                    : (cfg.dynamic ? launch_render_big_4_1 : launch_render_big_4_0);

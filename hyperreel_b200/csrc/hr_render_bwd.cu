@@ -16,6 +16,7 @@ cudaError_t launch_render_bwd(const hr_config& cfg, const Derived& dv, const Ren
   gt.basis = g_basis;
   gt.color_embedding = g_color_embedding;
   BwdOpts opt{clamp_output, white_bg};
+  if (eases_density(cfg)) return launch_render_bwd_ease(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, stream);
   if (needs_rare_bwd(cfg)) return launch_render_bwd_rare(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, stream);
   return bwd_launch<false>(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, stream);
 }

@@ -45,6 +45,19 @@ __device__ __forceinline__ float act_grad(const hr_act& a, float x) {
   return g * a.inner_fac * a.outer_fac;
 }
 
+// d / d x of apply_act_eased: act_grad times ease_mul while an EaseValue window is open (0 while the head is held at its
+// start value)
+__device__ __forceinline__ float act_grad_eased(const hr_act& a, float x) {
+  const float g = act_grad(a, x);
+  return a.eased ? g * a.ease_mul : g;
+}
+
+template <bool EASE>
+__device__ __forceinline__ float act_grad_head(const hr_act& a, float x) {
+  if constexpr (EASE) return act_grad_eased(a, x);
+  else return act_grad(a, x);
+}
+
 // sort (key, id) pairs ascending by key (ties by id, so the ids stay a permutation); element e = reg*32 + lane
 template <int SPL>
 __device__ __forceinline__ void sort_pairs(float (&k)[SPL], int (&id)[SPL], int lane) {
@@ -231,7 +244,7 @@ struct BwdOpts {
   int white_bg;      // rgb_map += 1 - acc_map (:795-796)
 };
 
-template <int SPL, bool DYN, int C0, int C1, int C2, int SHADE, bool RARE>
+template <int SPL, bool DYN, int C0, int C1, int C2, int SHADE, bool RARE, bool EASE>
 __global__ void __launch_bounds__(kBwdWarps * 32)
 render_bwd_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Derived dv,
                   const __grid_constant__ RenderTabs tabs, const __grid_constant__ GradTabs gt, const float* __restrict__ rays,
@@ -337,8 +350,8 @@ render_bwd_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__
       const float* hp = hrow + (act ? s : 0);
       const float hsg = (cfg.off_sigma >= 0) ? __ldg(hp + cfg.off_sigma * S) : 0.0f;
       const float hsp = (cfg.off_point_sigma >= 0) ? __ldg(hp + cfg.off_point_sigma * S) : 0.0f;
-      sg[j] = (cfg.off_sigma >= 0) ? apply_act(cfg.act_sigma, hsg) : 0.0f;
-      sgp[j] = (cfg.off_point_sigma >= 0) ? apply_act(cfg.act_point_sigma, hsp) : 0.0f;
+      sg[j] = (cfg.off_sigma >= 0) ? apply_act_head<EASE>(cfg.act_sigma, hsg) : 0.0f;
+      sgp[j] = (cfg.off_point_sigma >= 0) ? apply_act_head<EASE>(cfg.act_point_sigma, hsp) : 0.0f;
       const float dens_i = (cfg.isect_density_off < 0) ? 0.0f : ((cfg.isect_density_off == cfg.off_sigma) ? sg[j] : sgp[j]);
       dens_o[j] = (cfg.offset_density_off < 0) ? 0.0f : ((cfg.offset_density_off == cfg.off_sigma) ? sg[j] : sgp[j]);
       one_m[j] = __fsub_rn(1.0f, cfg.isect_use_sigma ? dens_i : 0.0f);
@@ -913,8 +926,9 @@ render_bwd_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__
       if (cfg.use_offset && cfg.offset_density_off >= 0) {
         if (cfg.offset_density_off == cfg.off_sigma) g_sg += g_do; else g_sgp += g_do;
       }
-      if (cfg.off_sigma >= 0) gp[cfg.off_sigma * S] = g_sg * act_grad(cfg.act_sigma, __ldg(hp + cfg.off_sigma * S));
-      if (cfg.off_point_sigma >= 0) gp[cfg.off_point_sigma * S] = g_sgp * act_grad(cfg.act_point_sigma, __ldg(hp + cfg.off_point_sigma * S));
+      if (cfg.off_sigma >= 0) gp[cfg.off_sigma * S] = g_sg * act_grad_head<EASE>(cfg.act_sigma, __ldg(hp + cfg.off_sigma * S));
+      if (cfg.off_point_sigma >= 0)
+        gp[cfg.off_point_sigma * S] = g_sgp * act_grad_head<EASE>(cfg.act_point_sigma, __ldg(hp + cfg.off_point_sigma * S));
     }
     __syncwarp();
   }
@@ -933,7 +947,7 @@ render_bwd_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__
   }
 }
 
-template <int SPL, bool DYN, int C0, int C1, int C2, int SHADE, bool RARE>
+template <int SPL, bool DYN, int C0, int C1, int C2, int SHADE, bool RARE, bool EASE>
 static cudaError_t bwd_launch_one(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs, const GradTabs& gt, const float* rays,
                                   const float* heads, const float* d_rgb, float* d_heads, long long n, BwdOpts opt, int num_sms,
                                   cudaStream_t stream) {
@@ -944,20 +958,20 @@ static cudaError_t bwd_launch_one(const hr_config& cfg, const Derived& dv, const
   const long long cap = (long long)num_sms * 8;
   if (ctas > cap) ctas = cap;
   if (ctas < 1) ctas = 1;
-  render_bwd_kernel<SPL, DYN, C0, C1, C2, SHADE, RARE><<<(unsigned)ctas, kBwdWarps * 32, smem, stream>>>(cfg, dv, tabs, gt, rays, heads,
+  render_bwd_kernel<SPL, DYN, C0, C1, C2, SHADE, RARE, EASE><<<(unsigned)ctas, kBwdWarps * 32, smem, stream>>>(cfg, dv, tabs, gt, rays, heads,
                                                                                                          d_rgb, d_heads, n, opt);
   return cudaGetLastError();
 }
 
-template <int SPL, bool DYN, bool RARE>
+template <int SPL, bool DYN, bool RARE, bool EASE>
 static cudaError_t bwd_launch_comps(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs, const GradTabs& gt, const float* rays,
                                     const float* heads, const float* d_rgb, float* d_heads, long long n, BwdOpts opt, int num_sms,
                                     cudaStream_t st) {
   const int c0 = cfg.n_sigma[0], c1 = cfg.n_sigma[1], c2 = cfg.n_sigma[2];
   const bool sh = cfg.shading == HR_SHADE_SH;
 #define HR_BWD(C0_, C1_, C2_)                                                                                                         \
-  return sh ? bwd_launch_one<SPL, DYN, C0_, C1_, C2_, HR_SHADE_SH, RARE>(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, st) \
-            : bwd_launch_one<SPL, DYN, C0_, C1_, C2_, HR_SHADE_RGB, RARE>(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, st)
+  return sh ? bwd_launch_one<SPL, DYN, C0_, C1_, C2_, HR_SHADE_SH, RARE, EASE>(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, st) \
+            : bwd_launch_one<SPL, DYN, C0_, C1_, C2_, HR_SHADE_RGB, RARE, EASE>(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, st)
   if (c0 == 8 && c1 == 0 && c2 == 0) { HR_BWD(8, 0, 0); }
   if (c0 == 8 && c1 == 4 && c2 == 4) { HR_BWD(8, 4, 4); }
   if (c0 == 8 && c1 == 8 && c2 == 8) { HR_BWD(8, 8, 8); }
@@ -965,16 +979,16 @@ static cudaError_t bwd_launch_comps(const hr_config& cfg, const Derived& dv, con
   return cudaErrorInvalidValue;
 }
 
-template <bool RARE>
+template <bool RARE, bool EASE = false>
 static cudaError_t bwd_launch(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs, const GradTabs& gt, const float* rays,
                               const float* heads, const float* d_rgb, float* d_heads, long long n, BwdOpts opt, int num_sms,
                               cudaStream_t stream) {
   const bool two = cfg.n_samples > 32;
   if (cfg.dynamic)
-    return two ? bwd_launch_comps<2, true, RARE>(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, stream)
-               : bwd_launch_comps<1, true, RARE>(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, stream);
-  return two ? bwd_launch_comps<2, false, RARE>(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, stream)
-             : bwd_launch_comps<1, false, RARE>(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, stream);
+    return two ? bwd_launch_comps<2, true, RARE, EASE>(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, stream)
+               : bwd_launch_comps<1, true, RARE, EASE>(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, stream);
+  return two ? bwd_launch_comps<2, false, RARE, EASE>(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, stream)
+             : bwd_launch_comps<1, false, RARE, EASE>(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, stream);
 }
 
 // pipelines whose backward needs the RARE variants (see render_bwd_kernel)
@@ -984,6 +998,10 @@ static inline bool needs_rare_bwd(const hr_config& cfg) {
 }
 
 cudaError_t launch_render_bwd_rare(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs, const GradTabs& gt, const float* rays,
+                                   const float* heads, const float* d_rgb, float* d_heads, long long n, BwdOpts opt, int num_sms,
+                                   cudaStream_t stream);
+// hr_render_bwd_ease.cu: the RARE variants with eased density heads (eases_density)
+cudaError_t launch_render_bwd_ease(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs, const GradTabs& gt, const float* rays,
                                    const float* heads, const float* d_rgb, float* d_heads, long long n, BwdOpts opt, int num_sms,
                                    cudaStream_t stream);
 

@@ -160,7 +160,7 @@ __device__ __forceinline__ float quad_transpose_reduce(const float (&v)[4], int 
   return (alt ? k1 : k0) + z;                // q = 0: v0, 1: v1, 2: v2, 3: v3
 }
 
-template <int SPL, bool DYN, int C0, int C1, int C2, int SHADE, bool EXTRA, int RPW, bool RARE>
+template <int SPL, bool DYN, int C0, int C1, int C2, int SHADE, bool EXTRA, int RPW, bool RARE, bool EASE>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, SPL > 2 ? 1 : ((C1 + C2 == 0 || SPL == 1) ? 3 : 2))
 render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Derived dv,
               const __grid_constant__ RenderTabs tabs, const float* __restrict__ rays,
@@ -330,8 +330,8 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
     for (int j = 0; j < SPL; ++j) {
       const int s = sl + 32 * j;
       const bool act = s < S;
-      const float sg = (cfg.off_sigma >= 0) ? apply_act(cfg.act_sigma, hsg[j]) : 0.0f;
-      const float sgp = (cfg.off_point_sigma >= 0) ? apply_act(cfg.act_point_sigma, hsp[j]) : 0.0f;
+      const float sg = (cfg.off_sigma >= 0) ? apply_act_head<EASE>(cfg.act_sigma, hsg[j]) : 0.0f;
+      const float sgp = (cfg.off_point_sigma >= 0) ? apply_act_head<EASE>(cfg.act_point_sigma, hsp[j]) : 0.0f;
       const float dens_i = (cfg.isect_density_off < 0) ? 0.0f : ((cfg.isect_density_off == cfg.off_sigma) ? sg : sgp);
       const float dens_o = (cfg.offset_density_off < 0) ? 0.0f : ((cfg.offset_density_off == cfg.off_sigma) ? sg : sgp);
       const float one_m = __fsub_rn(1.0f, cfg.isect_use_sigma ? dens_i : 0.0f);
@@ -673,7 +673,7 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
           for (int c = 0; c < dim; ++c) {
             float v;
             if (hoff >= 0) {
-              v = apply_act(*hact, __ldg(hp + (long long)(hoff + c) * S));
+              v = apply_act_head<EASE>(*hact, __ldg(hp + (long long)(hoff + c) * S));  // eased: sigma / point_sigma only
               // two embeddings write their result back under the head's name:
               //   AdvectPoints: x['spatial_flow'] = spatial_flow_activation(x['spatial_flow'])        (point.py:815-817)
               //   PointOffset : x['point_offset'] = activation(x['point_offset']) * (1 - sigma)        (point.py:383-389)
@@ -791,7 +791,7 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
   }
 }
 
-template <int SPL, bool DYN, int C0, int C1, int C2, int SHADE, bool RARE>
+template <int SPL, bool DYN, int C0, int C1, int C2, int SHADE, bool RARE, bool EASE>
 static cudaError_t launch_one(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs, const float* rays,
                               const float* heads, const RgbDst& rgb, long long n, const ExtraOut* so, int num_sms,
                               cudaStream_t stream, unsigned char* rgb8) {
@@ -806,27 +806,27 @@ static cudaError_t launch_one(const hr_config& cfg, const Derived& dv, const Ren
   if (grid < 1) grid = 1;
   const dim3 g((unsigned)grid), b(kWarpsPerCta * 32);
   if (so) {
-    render_kernel<SPL, DYN, C0, C1, C2, SHADE, true, 1, RARE><<<g, b, smem, stream>>>(cfg, dv, tabs, rays, heads, rgb, n, *so, rgb8);
+    render_kernel<SPL, DYN, C0, C1, C2, SHADE, true, 1, RARE, EASE><<<g, b, smem, stream>>>(cfg, dv, tabs, rays, heads, rgb, n, *so, rgb8);
     return cudaGetLastError();
   }
   ExtraOut none{};
   if constexpr (SPL == 1) {
     if (two_rays) {
-      render_kernel<SPL, DYN, C0, C1, C2, SHADE, false, 2, RARE><<<g, b, smem, stream>>>(cfg, dv, tabs, rays, heads, rgb, n, none, rgb8);
+      render_kernel<SPL, DYN, C0, C1, C2, SHADE, false, 2, RARE, EASE><<<g, b, smem, stream>>>(cfg, dv, tabs, rays, heads, rgb, n, none, rgb8);
       return cudaGetLastError();
     }
   }
-  render_kernel<SPL, DYN, C0, C1, C2, SHADE, false, 1, RARE><<<g, b, smem, stream>>>(cfg, dv, tabs, rays, heads, rgb, n, none, rgb8);
+  render_kernel<SPL, DYN, C0, C1, C2, SHADE, false, 1, RARE, EASE><<<g, b, smem, stream>>>(cfg, dv, tabs, rays, heads, rgb, n, none, rgb8);
   return cudaGetLastError();
 }
 
-template <int SPL, bool DYN, int C0, int C1, int C2, bool RARE>
+template <int SPL, bool DYN, int C0, int C1, int C2, bool RARE, bool EASE>
 static cudaError_t launch_shade(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs, const float* rays,
                                 const float* heads, const RgbDst& rgb, long long n, const ExtraOut* so, int num_sms,
                                 cudaStream_t stream, unsigned char* rgb8) {
   if (cfg.shading == HR_SHADE_SH)
-    return launch_one<SPL, DYN, C0, C1, C2, HR_SHADE_SH, RARE>(cfg, dv, tabs, rays, heads, rgb, n, so, num_sms, stream, rgb8);
-  return launch_one<SPL, DYN, C0, C1, C2, HR_SHADE_RGB, RARE>(cfg, dv, tabs, rays, heads, rgb, n, so, num_sms, stream, rgb8);
+    return launch_one<SPL, DYN, C0, C1, C2, HR_SHADE_SH, RARE, EASE>(cfg, dv, tabs, rays, heads, rgb, n, so, num_sms, stream, rgb8);
+  return launch_one<SPL, DYN, C0, C1, C2, HR_SHADE_RGB, RARE, EASE>(cfg, dv, tabs, rays, heads, rgb, n, so, num_sms, stream, rgb8);
 }
 
 // pipelines served by the RARE variants only (see render_kernel)
@@ -835,17 +835,17 @@ static inline bool needs_rare(const hr_config& cfg) {
          cfg.n_color_views > 0;
 }
 
-template <int SPL, bool DYN, bool RARE>
+template <int SPL, bool DYN, bool RARE, bool EASE = false>
 static cudaError_t launch_comps(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs, const float* rays,
                                 const float* heads, const RgbDst& rgb, long long n, const ExtraOut* so, int num_sms,
                                 cudaStream_t stream, unsigned char* rgb8) {
   const int c0 = cfg.n_sigma[0], c1 = cfg.n_sigma[1], c2 = cfg.n_sigma[2];
   if (c0 == 8 && c1 == 0 && c2 == 0)
-    return launch_shade<SPL, DYN, 8, 0, 0, RARE>(cfg, dv, tabs, rays, heads, rgb, n, so, num_sms, stream, rgb8);
+    return launch_shade<SPL, DYN, 8, 0, 0, RARE, EASE>(cfg, dv, tabs, rays, heads, rgb, n, so, num_sms, stream, rgb8);
   if (c0 == 8 && c1 == 4 && c2 == 4)
-    return launch_shade<SPL, DYN, 8, 4, 4, RARE>(cfg, dv, tabs, rays, heads, rgb, n, so, num_sms, stream, rgb8);
+    return launch_shade<SPL, DYN, 8, 4, 4, RARE, EASE>(cfg, dv, tabs, rays, heads, rgb, n, so, num_sms, stream, rgb8);
   if (c0 == 8 && c1 == 8 && c2 == 8)
-    return launch_shade<SPL, DYN, 8, 8, 8, RARE>(cfg, dv, tabs, rays, heads, rgb, n, so, num_sms, stream, rgb8);
+    return launch_shade<SPL, DYN, 8, 8, 8, RARE, EASE>(cfg, dv, tabs, rays, heads, rgb, n, so, num_sms, stream, rgb8);
   return cudaErrorInvalidValue;
 }
 

@@ -11,7 +11,7 @@ import os
 import subprocess
 import threading
 
-HR_ABI_VERSION = 12
+HR_ABI_VERSION = 13
 HR_MAX_GROUPS = 4
 HR_MAX_LAYERS = 10
 HR_MAX_SAMPLES = 256
@@ -37,7 +37,8 @@ CSRC_DIR = os.path.join(_PKG_DIR, "csrc")
 
 
 class hr_act(C.Structure):
-    _fields_ = [("kind", C.c_int32), ("inner_fac", C.c_float), ("shift", C.c_float), ("outer_fac", C.c_float)]
+    _fields_ = [("kind", C.c_int32), ("inner_fac", C.c_float), ("shift", C.c_float), ("outer_fac", C.c_float),
+                ("eased", C.c_int32), ("ease_mul", C.c_float), ("ease_add", C.c_float), ("ease_pad", C.c_int32)]
 
 
 class hr_encode_group(C.Structure):
@@ -164,6 +165,7 @@ EXPORTS = {
     "hr_train_net_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "hr_train_net_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(hr_net_grads), C.c_void_p, C.c_int64,
                                          C.c_void_p]),
+    "hr_set_activations": (C.c_int, [C.c_void_p, C.POINTER(hr_config)]),
     "hr_launch_count": (C.c_int64, [C.c_void_p]),
     "hr_timing_enable": (C.c_int, [C.c_void_p, C.c_int]),
     "hr_timing_reset": (C.c_int, [C.c_void_p]),

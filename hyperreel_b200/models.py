@@ -19,7 +19,7 @@ import torch
 from torch import nn
 
 from . import lib as L
-from .signature import RENDER_ITER, Signature, UnsupportedPipeline, lower
+from .signature import RENDER_ITER, Signature, UnsupportedPipeline, check_eased, ease_terms, lower, set_ease
 from .state import _Color, _Embedding, default_grid
 
 
@@ -104,9 +104,17 @@ class LightfieldModel(nn.Module):
         if self._train_net == "tc" and self._mlp_mode != L.MLP_BF16X3_TC:
             raise ValueError("train_net='tc' trains the wgmma sample net: mlp_mode must be 'auto' or 'bf16x3'")
         self._iters_per_epoch = kwargs.get("iters_per_epoch")
+        # EaseValue heads (nlf/activations.py:462-496): "elapsed" renders and trains every one at the end of its window at any
+        # iteration (set_iter inside a window raises); "reference" eases them like the reference, set_iter(i) updating them
+        # in place in the native handle
+        self._ease = kwargs.get("ease", "elapsed")
+        if self._ease not in ("elapsed", "reference"):
+            raise ValueError(f"ease must be 'elapsed' or 'reference', got {self._ease!r}")
+        if self._ease == "reference" and self._iters_per_epoch is None:
+            raise ValueError("ease='reference' needs iters_per_epoch: the EaseValue windows are given in epochs")
         self.cfg = cfg
-        self.sig: Signature = lower(cfg, dataset, cur_iter=RENDER_ITER,
-                                    iters_per_epoch=self._iters_per_epoch, mlp_mode=self._mlp_mode)
+        self.sig: Signature = lower(cfg, dataset, cur_iter=RENDER_ITER, iters_per_epoch=self._iters_per_epoch,
+                                    mlp_mode=self._mlp_mode, ease=self._ease == "reference")
         self.num_outputs = 3
         self.cur_iter = RENDER_ITER
         grid = kwargs.get("grid") or default_grid(self.sig)
@@ -120,24 +128,54 @@ class LightfieldModel(nn.Module):
         self._version_tensors = None
         self._device_index: Optional[int] = None
         self._ws: Optional[torch.Tensor] = None
+        self._graph_key = self.sig.graph_key(RENDER_ITER)
 
     # ------------------------------------------------------------------ reference surface
     def set_iter(self, i):
-        """The fused path implements render-time semantics only (all PE windows open, EaseValue elapsed);
-        the reference sets iteration 1e7*iters when rendering (nlf/__init__.py:582-583)."""
+        """The reference's per-iteration hook (nlf/models/models.py:140-143).  With ease="elapsed" the fused path implements
+        render-time semantics only (all PE windows open, EaseValue elapsed; the reference sets iteration 1e7*iters when
+        rendering, nlf/__init__.py:582-583); with ease="reference" open EaseValue windows are eased at iteration i."""
         self.cur_iter = i
-        # Re-lower at iteration i with the same epoch scale and net mode.  Raises UnsupportedPipeline while a PE / EaseValue
-        # window is still open; a different graph at i (an embedding gated by wait/stop_iters, mask.stop_iters) must not be
-        # rendered with the construction-time semantics: adopt it and rebuild the native handle.
-        new = lower(self.cfg, self.sig.dataset, cur_iter=int(i), iters_per_epoch=self._iters_per_epoch, mlp_mode=self._mlp_mode)
+        if self._ease == "reference" and self.sig.graph_key(int(i)) == self._graph_key:
+            self._set_ease_iter(int(i))  # same graph: only the eased activations can differ
+        else:
+            self._relower(int(i))
+        self.color_model.set_iter(i)
+
+    def _relower(self, i):
+        # Re-lower at iteration i with the same epoch scale, net mode and ease mode.  Raises UnsupportedPipeline while a PE
+        # window (or, with ease="elapsed", an EaseValue window) is still open; a different graph at i (an embedding gated by
+        # wait/stop_iters, mask.stop_iters) must not be rendered with the construction-time semantics: adopt it and rebuild the
+        # native handle.  A configuration that differs in its activations alone is updated in place (hr_set_activations).
+        new = lower(self.cfg, self.sig.dataset, cur_iter=i, iters_per_epoch=self._iters_per_epoch, mlp_mode=self._mlp_mode,
+                    ease=self._ease == "reference")
         for k in range(6):
             new.cfg.aabb[k] = self.sig.cfg.aabb[k]  # aabb is checkpoint state, kept in sync by _ensure_uploaded
         if bytes(new.cfg) != bytes(self.sig.cfg):
             if new.mlp_layer_shapes != self.sig.mlp_layer_shapes or list(new.cfg.n_sigma) != list(self.sig.cfg.n_sigma):
                 raise UnsupportedPipeline("set_iter: the pipeline at this iteration has different parameter shapes")
+            same_graph = _without_activations(new.cfg) == _without_activations(self.sig.cfg)
             self.sig = new
-            self._release_handle()
-        self.color_model.set_iter(i)
+            if same_graph and self._handle:
+                L.check(self._lib.hr_set_activations(self._handle, C.byref(self.sig.cfg)))
+            else:
+                self._release_handle()
+        self._graph_key = self.sig.graph_key(i)
+
+    def _set_ease_iter(self, i):
+        """EaseValue.set_iter (activations.py:495-496) of every ease site; the handle's activations are updated in place
+        (hr_set_activations: no re-upload, no device synchronisation) when one of them changed."""
+        # built on a copy, adopted once every check and the native call have passed: sig.cfg always matches the handle
+        c = L.hr_config.from_buffer_copy(bytes(self.sig.cfg))
+        for site in self.sig.ease_sites:
+            a = L.hr_act.from_buffer_copy(bytes(getattr(c, site.field)))
+            set_ease(a, ease_terms(i, site.start_value, site.wait_iters, site.window_iters))
+            setattr(c, site.field, check_eased(a, site.field, c.n_samples))
+        if bytes(c) == bytes(self.sig.cfg):
+            return
+        if self._handle:
+            L.check(self._lib.hr_set_activations(self._handle, C.byref(c)))
+        self.sig.cfg = c
 
     def forward(self, rays: torch.Tensor, render_kwargs: Optional[Dict] = None) -> Dict[str, torch.Tensor]:
         render_kwargs = render_kwargs or {}
@@ -601,6 +639,15 @@ class LightfieldModel(nn.Module):
                 self._handle = None
         except Exception:
             pass
+
+
+def _without_activations(cfg: L.hr_config) -> bytes:
+    """The bytes of an hr_config with every hr_act member cleared: what hr_set_activations requires to be unchanged."""
+    c = L.hr_config.from_buffer_copy(bytes(cfg))
+    for name, typ in L.hr_config._fields_:
+        if typ is L.hr_act:
+            setattr(c, name, L.hr_act())
+    return bytes(c)
 
 
 model_dict = {"lightfield": LightfieldModel}

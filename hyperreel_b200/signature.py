@@ -38,9 +38,52 @@ def _get(cfg, key, default=None):
 RENDER_ITER = 10_000_000  # what the reference sets when rendering (nlf/__init__.py:582-583)
 
 
-def resolve_activation(cfg, cur_iter: int = RENDER_ITER) -> L.hr_act:
-    """get_activation (nlf/activations.py:566-570) lowered to y = f(x*inner+shift)*outer.
-    EaseValue (:462-496) is accepted only once its window has elapsed (then it is its inner activation)."""
+@dataclass
+class EaseSite:
+    """One EaseValue (nlf/activations.py:462-496) that is the outermost activation of an ``hr_config`` member: the member's
+    ``eased`` / ``ease_mul`` / ``ease_add`` follow from these three numbers and the iteration alone (``ease_terms``)."""
+    field: str
+    start_value: float
+    wait_iters: float
+    window_iters: float
+
+
+# the hr_config members whose EaseValue the kernels blend (apply_act_eased): the density heads, the only open windows of the
+# shipped model YAMLs
+EASE_FIELDS = ("act_sigma", "act_point_sigma", "pre_act_sigma")
+
+
+def check_eased(act: L.hr_act, member: str, n_samples: int) -> L.hr_act:
+    """The eased activations the kernels serve: density heads only, at most 64 samples per ray (the render kernels' EASE
+    variants exist for S <= 64 only)."""
+    if act.eased and member not in EASE_FIELDS:
+        raise UnsupportedPipeline(f"an open ease_value window on {member} is not on the fused path (only {', '.join(EASE_FIELDS)})")
+    if act.eased and member != "pre_act_sigma" and n_samples > 64:
+        raise UnsupportedPipeline(f"an open ease_value window with {n_samples} samples per ray is not on the fused path (<= 64)")
+    return act
+
+
+def ease_terms(cur_iter, start_value, wait_iters, window_iters):
+    """EaseValue.set_iter + weight / ease_out (activations.py:473-496) at ``cur_iter``: None once the window has elapsed (the
+    plain activation), else (w, (1 - w) * start_value) in double -- the Python scalars of ``w * out + (1 - w) * start_value``
+    (``window_iters == 0``: w = 0, the start value alone)."""
+    cur = cur_iter - wait_iters
+    if cur >= window_iters:
+        return None
+    w = 0.0 if window_iters == 0 else min(max(float(cur) / window_iters, 0.0), 1.0)
+    return w, (1 - w) * start_value
+
+
+def set_ease(act: L.hr_act, terms) -> None:
+    """Write ``ease_terms`` into an hr_act (each rounded once to fp32); None leaves the struct of the plain activation."""
+    if terms is None:
+        act.eased, act.ease_mul, act.ease_add = 0, 0.0, 0.0
+    else:
+        act.eased, act.ease_mul, act.ease_add = 1, float(terms[0]), float(terms[1])
+
+
+def _resolve(cfg, cur_iter, ease):
+    """-> (hr_act, (start_value, wait_iters, window_iters) of an outermost EaseValue or None)."""
     if cfg is None:
         cfg = {"type": "identity"}
     if isinstance(cfg, str):
@@ -49,16 +92,33 @@ def resolve_activation(cfg, cur_iter: int = RENDER_ITER) -> L.hr_act:
     if t == "ease_value":
         wait = _get(cfg, "wait_iters", 0.0)
         window = _get(cfg, "window_iters", 0.0)
-        if (cur_iter - wait) < window:
+        terms = ease_terms(cur_iter, 1.0, wait, window)
+        if terms is not None and not ease:
             raise UnsupportedPipeline(f"ease_value window still open at iteration {cur_iter} (render-time config expected)")
-        return resolve_activation(cfg["activation"], cur_iter)
+        if not ease:
+            return _resolve(cfg["activation"], cur_iter, False)
+        inner = cfg["activation"]
+        if isinstance(inner, dict) and inner.get("type") == "ease_value":
+            # y * m + a covers one blend of a plain activation; an EaseValue inside another has no such form
+            raise UnsupportedPipeline("an ease_value inside an ease_value is not on the fused path")
+        act, _ = _resolve(inner, cur_iter, False)
+        site = (float(_get(cfg, "start_value", 0.0)), wait, window)
+        set_ease(act, ease_terms(cur_iter, *site))
+        return act, site
     kinds = {"identity": L.ACT_IDENTITY, "sigmoid": L.ACT_SIGMOID, "tanh": L.ACT_TANH}
     if t not in kinds:
         raise UnsupportedPipeline(f"activation '{t}' is not on the fused path")
     outer = _get(cfg, "outer_fac", 1.0)
     if "fac" in cfg:
         outer = cfg["fac"]
-    return L.hr_act(kinds[t], float(_get(cfg, "inner_fac", 1.0)), float(_get(cfg, "shift", 0.0)), float(outer))
+    return L.hr_act(kinds[t], float(_get(cfg, "inner_fac", 1.0)), float(_get(cfg, "shift", 0.0)), float(outer)), None
+
+
+def resolve_activation(cfg, cur_iter: int = RENDER_ITER, ease: bool = False) -> L.hr_act:
+    """get_activation (nlf/activations.py:566-570) lowered to y = f(x*inner+shift)*outer.
+    EaseValue (:462-496): once its window has elapsed it is its inner activation.  An open window raises, unless ``ease``:
+    then it lowers to the eased form y * ease_mul + ease_add (hr_act.eased; an EaseValue must then be the outermost one)."""
+    return _resolve(cfg, cur_iter, ease)[0]
 
 
 # ---- mipnerf distance contraction on the host (nlf/contract.py:160-176), used for the base primitives ----
@@ -100,6 +160,16 @@ class Signature:
     net_index: int = 0
     pre_layer_shapes: List[tuple] = field(default_factory=list)
     pre_in_perm: List[int] = field(default_factory=list)
+    # lower(ease=True): every EaseValue site, to recompute the eased activations at another iteration without lowering again
+    ease_sites: List[EaseSite] = field(default_factory=list)
+    # every iteration threshold a gate of the graph compares against (embedding wait / stop, mask.stop_iters, PE windows):
+    # iterations with the same position relative to all of them lower to the same graph
+    graph_iters: List[float] = field(default_factory=list)
+
+    def graph_key(self, cur_iter) -> tuple:
+        import bisect
+
+        return bisect.bisect_left(self.graph_iters, cur_iter), bisect.bisect_right(self.graph_iters, cur_iter)
 
     @property
     def c_in(self) -> int:
@@ -111,9 +181,19 @@ class Signature:
 
 
 def lower(model_cfg, dataset: dict, cur_iter: int = RENDER_ITER, iters_per_epoch: Optional[int] = None,
-          mlp_mode: int = L.MLP_BF16X3_TC) -> Signature:
-    """model cfg (reference schema) + dataset facts -> Signature / hr_config."""
+          mlp_mode: int = L.MLP_BF16X3_TC, ease: bool = False) -> Signature:
+    """model cfg (reference schema) + dataset facts -> Signature / hr_config.  ``ease``: open EaseValue windows lower to
+    their eased form (resolve_activation) instead of raising; Signature.ease_sites lists every EaseValue site."""
     from .config import epochs_to_iters
+
+    sites: List[EaseSite] = []
+    gates: List[float] = []
+
+    def act_at(acfg, member):
+        a, site = _resolve(acfg, cur_iter, ease)
+        if site is not None:
+            sites.append(EaseSite(member, *site))
+        return check_eased(a, member, c.n_samples)
 
     m = to_cfg(copy.deepcopy(dict(model_cfg)))
     if iters_per_epoch is not None:
@@ -140,6 +220,7 @@ def lower(model_cfg, dataset: dict, cur_iter: int = RENDER_ITER, iters_per_epoch
         e = embs[key]
         wait = _get(e, "wait_iters", 0)
         stop = _get(e, "stop_iters", float("inf"))
+        gates.extend([float(wait), float(stop)])
         if cur_iter >= wait and cur_iter < stop:  # RayPointEmbedding.forward gate (embedding.py:107)
             seq.append(e)
     # ColorTransformEmbedding (point.py:558-612) only adds per-ray keys to the dict: it commutes with the point embeddings
@@ -219,6 +300,7 @@ def lower(model_cfg, dataset: dict, cur_iter: int = RENDER_ITER, iters_per_epoch
                 mfi = float(_get(pe, "max_freq_iter", 0))
                 if "window_iters" in pe:
                     mfi = max(max(w) for w in pe.window_iters)
+                gates.extend([float(_get(pe, "wait_iters", 0)), float(mfi)])
                 if (cur_iter - _get(pe, "wait_iters", 0)) < 0 or (mfi != 0 and not cur_iter > mfi):
                     raise UnsupportedPipeline("windowed PE not fully open at this iteration")
                 if _get(pe, "ceil", False) or _get(pe, "window_identity", False):
@@ -331,17 +413,17 @@ def lower(model_cfg, dataset: dict, cur_iter: int = RENDER_ITER, iters_per_epoch
         if nme in expect_ch and ch != expect_ch[nme]:
             raise UnsupportedPipeline(f"head '{nme}' must have {expect_ch[nme]} channels")
 
-    def act_of(nme):
-        return resolve_activation(_get(pred.outputs[nme], "activation"), cur_iter) if nme in offs else L.hr_act(0, 1.0, 0.0, 1.0)
+    def act_of(nme, member):
+        return act_at(_get(pred.outputs[nme], "activation"), member) if nme in offs else L.hr_act(0, 1.0, 0.0, 1.0)
 
     c.off_z = offs.get("z_vals", -1)
     c.n_z = head_channels[head_names.index("z_vals")] if "z_vals" in offs else 0
     c.off_flow, c.off_sigma = offs.get("spatial_flow", -1), offs.get("sigma", -1)
     c.off_point_sigma, c.off_offset = offs.get("point_sigma", -1), offs.get("point_offset", -1)
     c.off_cscale, c.off_cshift = offs.get("color_scale", -1), offs.get("color_shift", -1)
-    c.act_z, c.act_flow, c.act_sigma = act_of("z_vals"), act_of("spatial_flow"), act_of("sigma")
-    c.act_point_sigma, c.act_offset = act_of("point_sigma"), act_of("point_offset")
-    c.act_cscale, c.act_cshift = act_of("color_scale"), act_of("color_shift")
+    c.act_z, c.act_flow, c.act_sigma = act_of("z_vals", "act_z"), act_of("spatial_flow", "act_flow"), act_of("sigma", "act_sigma")
+    c.act_point_sigma, c.act_offset = act_of("point_sigma", "act_point_sigma"), act_of("point_offset", "act_offset")
+    c.act_cscale, c.act_cshift = act_of("color_scale", "act_cscale"), act_of("color_shift", "act_cshift")
 
     # ------------------------------------------------------------------ first stage of a cascade (ray net -> z-planes -> points)
     c.cascade, c.pre_samples = int(cascade), 0
@@ -358,8 +440,8 @@ def lower(model_cfg, dataset: dict, cur_iter: int = RENDER_ITER, iters_per_epoch
             raise UnsupportedPipeline("per-ray outputs are not on the fused path")
         c.pre_head_stride = len(names0)
         c.pre_off_z, c.pre_off_sigma = names0.index("z_vals"), (names0.index("sigma") if "sigma" in names0 else -1)
-        c.pre_act_z = resolve_activation(_get(pred0.outputs["z_vals"], "activation"), cur_iter)
-        c.pre_act_sigma = (resolve_activation(_get(pred0.outputs["sigma"], "activation"), cur_iter) if "sigma" in names0
+        c.pre_act_z = act_at(_get(pred0.outputs["z_vals"], "activation"), "pre_act_z")
+        c.pre_act_sigma = (act_at(_get(pred0.outputs["sigma"], "activation"), "pre_act_sigma") if "sigma" in names0
                            else L.hr_act(0, 1.0, 0.0, 1.0))
         zero0, c.pre_mlp_width, c.pre_mlp_layers, c.pre_mlp_skip, pre_shapes = net_shape(pred0.net, c.pre_mlp_in, S0 * c.pre_head_stride)
         c.pre_mlp_mode = L.MLP_ZERO if zero0 else int(mlp_mode)
@@ -381,10 +463,12 @@ def lower(model_cfg, dataset: dict, cur_iter: int = RENDER_ITER, iters_per_epoch
         c.pre_z_scale = float(torch.abs(tab0[1] - tab0[0])) if S0 > 1 else 1.0
         c.pre_near = float(_get(it0, "near", ds["near"] if use_ds0 else 0.0))
         c.pre_far = float(_get(it0, "far", float("inf")))
+        if "mask" in it0 and it0.mask is not None:
+            gates.append(float(_get(it0.mask, "stop_iters", float("inf"))))
         if "mask" in it0 and it0.mask is not None and cur_iter > float(_get(it0.mask, "stop_iters", float("inf"))):
             c.pre_near, c.pre_far = float("-inf"), float("inf")  # base.py:104-105,197-198
         c.pre_sort = int(bool(_get(it0, "sort", False)))
-        c.pre_isect_act = resolve_activation(_get(it0, "activation", "identity"), cur_iter)
+        c.pre_isect_act = act_at(_get(it0, "activation", "identity"), "pre_isect_act")
         c.pre_use_sigma = int(bool(_get(it0, "use_sigma", False)) and _get(it0, "in_density_field", "sigma") == "sigma"
                               and "sigma" in names0)
         # the point net's input row (point.py:151-160): the named tensors concatenated in YAML order
@@ -601,11 +685,13 @@ def lower(model_cfg, dataset: dict, cur_iter: int = RENDER_ITER, iters_per_epoch
             c.z_scale3[a_] = c.z_scale
     c.isect_near = float(_get(it, "near", ds["near"] if use_ds else 0.0))
     c.isect_far = float(_get(it, "far", float("inf")))
+    if "mask" in it and it.mask is not None:
+        gates.append(float(_get(it.mask, "stop_iters", float("inf"))))
     if "mask" in it and it.mask is not None and cur_iter > float(_get(it.mask, "stop_iters", float("inf"))):
         # base.py:104-105,197-198: past mask.stop_iters nothing is masked (samples with t == 0 still drop out downstream)
         c.isect_near, c.isect_far = float("-inf"), float("inf")
     c.isect_sort = int(bool(_get(it, "sort", False)))
-    c.isect_act = resolve_activation(_get(it, "activation", "identity"), cur_iter)
+    c.isect_act = act_at(_get(it, "activation", "identity"), "isect_act")
     c.isect_use_sigma = int(bool(_get(it, "use_sigma", False)))
     c.isect_density_off = offs.get(_get(it, "in_density_field", "sigma"), -1)
     if c.isect_density_off not in (-1, c.off_sigma, c.off_point_sigma):
@@ -625,7 +711,7 @@ def lower(model_cfg, dataset: dict, cur_iter: int = RENDER_ITER, iters_per_epoch
             if "spatial_flow" not in offs:
                 raise UnsupportedPipeline("spatial flow without a spatial_flow head")
             c.use_flow = 1
-            c.flow_act = resolve_activation(_get(flow, "spatial_flow_activation", "identity"), cur_iter)
+            c.flow_act = act_at(_get(flow, "spatial_flow_activation", "identity"), "flow_act")
 
     # ------------------------------------------------------------------ point offset (point.py:338-399)
     c.use_offset, c.offset_density_off = 0, -1
@@ -639,7 +725,7 @@ def lower(model_cfg, dataset: dict, cur_iter: int = RENDER_ITER, iters_per_epoch
         c.use_offset = 1
         if _get(offset, "use_sigma", True):
             c.offset_density_off = offs.get(_get(offset, "in_density_field", "sigma"), -1)
-        c.offset_act = resolve_activation(_get(offset, "activation", "identity"), cur_iter)
+        c.offset_act = act_at(_get(offset, "activation", "identity"), "offset_act")
 
     # ------------------------------------------------------------------ outputs to the colour net
     extras = list(addp.extra_outputs)
@@ -659,7 +745,8 @@ def lower(model_cfg, dataset: dict, cur_iter: int = RENDER_ITER, iters_per_epoch
         raise UnsupportedPipeline("color_scale_global and color_shift_global must come together")
     c.off_cscale_global = offs["color_scale_global"] if glob[0] else -1
     c.off_cshift_global = offs["color_shift_global"] if glob[0] else -1
-    c.act_cscale_global, c.act_cshift_global = act_of("color_scale_global"), act_of("color_shift_global")
+    c.act_cscale_global = act_of("color_scale_global", "act_cscale_global")
+    c.act_cshift_global = act_of("color_shift_global", "act_cshift_global")
     # per-camera colour transform (ColorTransformEmbedding point.py:558-612 -> transform_color_one tensorf_utils.py:308-331):
     # active iff the dataset validates on every camera (val_all), the keys pass extract_fields and no color_scale_global exists
     c.n_color_views = 0
@@ -678,8 +765,8 @@ def lower(model_cfg, dataset: dict, cur_iter: int = RENDER_ITER, iters_per_epoch
             if color_views < 1:
                 raise UnsupportedPipeline("color_transform without camera views")
             c.n_color_views = color_views
-            c.act_ctransform = resolve_activation(_get(ctrans, "transform_activation", "identity"), cur_iter)
-            c.act_ctshift = resolve_activation(_get(ctrans, "shift_activation", "identity"), cur_iter)
+            c.act_ctransform = act_at(_get(ctrans, "transform_activation", "identity"), "act_ctransform")
+            c.act_ctshift = act_at(_get(ctrans, "shift_activation", "identity"), "act_ctshift")
             c.c_in = 8  # the camera id is rays[..., -2] (point.py:598)
     c.use_color_scale_shift = int("color_scale" in offs and "color_scale" in fields and "color_shift" in offs and "color_shift" in fields)
     if ("color_scale" in offs and "color_scale" in fields) != ("color_shift" in offs and "color_shift" in fields):
@@ -718,4 +805,4 @@ def lower(model_cfg, dataset: dict, cur_iter: int = RENDER_ITER, iters_per_epoch
     return Signature(cfg=c, model_cfg=m, dataset=ds, head_names=head_names, head_channels=head_channels,
                      mlp_layer_shapes=shapes, dynamic=dynamic, in_perm=in_perm, color_views=color_views,
                      color_embedding_index=ctrans_index, cascade=cascade, net_index=point_index,
-                     pre_layer_shapes=pre_shapes, pre_in_perm=pre_in_perm)
+                     pre_layer_shapes=pre_shapes, pre_in_perm=pre_in_perm, ease_sites=sites, graph_iters=sorted(set(gates)))

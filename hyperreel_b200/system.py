@@ -75,7 +75,8 @@ class TensoRFRegularizer:
 
 
 class INRSystem(nn.Module):
-    def __init__(self, cfg, dm=None, dataset: Optional[dict] = None, mlp_mode: str = "auto", train_net: str = "torch"):
+    def __init__(self, cfg, dm=None, dataset: Optional[dict] = None, mlp_mode: str = "auto", train_net: str = "torch",
+                 ease: str = "elapsed"):
         super().__init__()
         self.cfg = to_cfg(cfg)
         self.dm = dm
@@ -88,7 +89,8 @@ class INRSystem(nn.Module):
             dataset = {k: d[k] for k in ("name", "collection", "num_keyframes", "num_frames", "near", "far", "depth_range") if k in d}
         model = model_dict[self.cfg.model.type](self.cfg.model, system=self if dm is not None else None,
                                                 dataset=dataset, iters_per_epoch=ipe, mlp_mode=mlp_mode,
-                                                train_net=train_net)
+                                                train_net=train_net, ease=ease)
+        self.ease = ease
         self.rendering = False
         self.render_fn = render_fn_dict[self.cfg.model.render.type](
             model, None, self.cfg.model.render, net_chunk=training.get("net_chunk", 32768))
@@ -155,9 +157,13 @@ class INRSystem(nn.Module):
         """The per-iteration hook of the reference's loop (nlf/__init__.py:592-632): the colour net's schedule (grid
         up-sampling, tensorf_base.py:509-553) and the regularisers' (`L1_weight_rest`), then an optimiser rebuild when the
         tables were re-created (`lr_upsample_reset`, nlf/__init__.py:541-578 -- here every group restarts, Adam state of the old
-        Parameter objects is meaningless for the new ones)."""
+        Parameter objects is meaningless for the new ones).  With ease="reference" the whole model's set_iter runs, as in the
+        reference (nlf/__init__.py:608-614), so its EaseValue heads are eased at `train_iter` for this step and later renders."""
         model = self.render_fn.model
-        model.color_model.set_iter(int(train_iter))
+        if self.ease == "reference":
+            model.set_iter(int(train_iter))  # includes the colour net's schedule
+        else:
+            model.color_model.set_iter(int(train_iter))
         for reg in self.regularizers:
             reg.set_iter(int(train_iter))
         net = model.color_model.net

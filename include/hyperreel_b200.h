@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define HR_ABI_VERSION 12
+#define HR_ABI_VERSION 13
 
 #define HR_MAX_GROUPS 4   /* ray-parameterisation groups feeding the sample net (ray.py:235-263) */
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
@@ -33,11 +33,21 @@ extern "C" {
 #define HR_MAX_PEERS 8    /* destination buffers of hr_render_scatter (GPUs of one NVSwitch domain) */
 
 /* Activation y = f(x*inner_fac + shift) * outer_fac  (nlf/activations.py:53-69,121-137,163-178).
- * EaseValue (activations.py:462-496) is resolved on the host at render iteration to its inner act. */
+ * EaseValue (activations.py:462-496) wrapped around it: while its window is open (eased != 0) the result is blended with the
+ * start value, y' = y * ease_mul + ease_add (each op rounded), where the host computes in double ease_mul = w and
+ * ease_add = (1 - w) * start_value from the ease weight w at the current iteration (activations.py:473-489).  A closed window
+ * is eased = 0: the plain activation, ease_mul / ease_add ignored (and zero).  Only the density heads act_sigma,
+ * act_point_sigma and pre_act_sigma may be eased (the only open windows of the shipped model YAMLs); the kernels ignore
+ * `eased` elsewhere, and hr_set_activations refuses it.  `ease_pad` keeps the struct a multiple of 8 bytes, so that every
+ * hr_config member keeps the 8-byte alignment it had before the ease members existed (the render kernels load pairs of
+ * configuration words with 64-bit uniform loads; a shifted alignment changes their register allocation). */
 enum { HR_ACT_IDENTITY = 0, HR_ACT_SIGMOID = 1, HR_ACT_TANH = 2 };
 typedef struct hr_act {
   int32_t kind;
   float inner_fac, shift, outer_fac;
+  int32_t eased;
+  float ease_mul, ease_add;
+  int32_t ease_pad;  /* 0 */
 } hr_act;
 
 /* One `params:` group of RayPredictionEmbedding (nlf/embedding/ray.py:235-263,320-326):
@@ -406,6 +416,14 @@ typedef struct hr_net_grads {  /* device buffers in nn.Linear's layouts of the u
 } hr_net_grads;
 int hr_train_net_backward(hr_handle* h, const float* d_heads, int64_t n_rays, const hr_net_grads* out, void* workspace,
                           int64_t workspace_bytes, void* stream);
+
+/* Replaces: EaseValue.set_iter (activations.py:495-496) reached through LightfieldModel.set_iter each training iteration.
+ * Copies every hr_act member of `cfg` (act_*, isect_act, flow_act, offset_act, pre_act_*, pre_isect_act) into the handle;
+ * every other member must equal the handle's configuration, else the call fails and the handle is unchanged.  No allocation,
+ * no upload, no device synchronisation: launches enqueued after the call returns use the new activations (kernel parameters
+ * are copied at launch), launches already enqueued keep the old ones.  The graph hr_render_host caches is dropped (its kernel
+ * nodes hold the old configuration by value) and captured again by the next hr_render_host call. */
+int hr_set_activations(hr_handle* h, const hr_config* cfg);
 
 /* Number of kernels hr_render launched since creation (bench.py's gpu_launches). */
 int64_t hr_launch_count(const hr_handle* h);
