@@ -5,7 +5,7 @@ Operator surface (same names as the reference's ``nlf`` package, SURVEY.md secti
 ``LightfieldModel`` (models.py), ``INRSystem`` (system.py).  All compute is in
 ``libhyperreel_b200.so`` (csrc/, sm_90a CUDA behind the C-ABI of include/hyperreel_b200.h).
 """
-from . import camera, configs, rays  # noqa: F401
+from . import camera, configs, metrics, rays  # noqa: F401
 from .camera import Camera, generate_rays  # noqa: F401
 from .config import Cfg, epochs_to_iters, load_model_yaml, to_cfg  # noqa: F401
 from .models import LightfieldModel, model_dict  # noqa: F401
@@ -13,6 +13,6 @@ from .rendering import RenderLightfield, render_chunked, render_fn_dict  # noqa:
 from .signature import Signature, UnsupportedPipeline, lower  # noqa: F401
 from .system import INRSystem  # noqa: F401
 
-__all__ = ["camera", "Camera", "generate_rays", "configs", "rays", "Cfg", "to_cfg", "load_model_yaml", "epochs_to_iters", "LightfieldModel", "model_dict",
+__all__ = ["camera", "Camera", "generate_rays", "configs", "metrics", "rays", "Cfg", "to_cfg", "load_model_yaml", "epochs_to_iters", "LightfieldModel", "model_dict",
            "RenderLightfield", "render_chunked", "render_fn_dict", "Signature", "UnsupportedPipeline", "lower",
            "INRSystem"]

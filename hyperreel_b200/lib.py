@@ -11,7 +11,7 @@ import os
 import subprocess
 import threading
 
-HR_ABI_VERSION = 13
+HR_ABI_VERSION = 14
 HR_MAX_GROUPS = 4
 HR_MAX_LAYERS = 10
 HR_MAX_SAMPLES = 256
@@ -166,6 +166,9 @@ EXPORTS = {
     "hr_train_net_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(hr_net_grads), C.c_void_p, C.c_int64,
                                          C.c_void_p]),
     "hr_set_activations": (C.c_int, [C.c_void_p, C.POINTER(hr_config)]),
+    "hr_image_metrics_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32]),
+    "hr_image_metrics": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64,
+                                    C.c_void_p]),
     "hr_launch_count": (C.c_int64, [C.c_void_p]),
     "hr_timing_enable": (C.c_int, [C.c_void_p, C.c_int]),
     "hr_timing_reset": (C.c_int, [C.c_void_p]),

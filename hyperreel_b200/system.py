@@ -199,6 +199,36 @@ class INRSystem(nn.Module):
             psnr = -10.0 * torch.log10(torch.mean((pred.detach() - rgb) ** 2))  # metrics.py:37-45
         return {"train/loss": loss.detach(), "train/psnr": psnr}
 
+    # ---- nlf/__init__.py:895-982, 1015-1030
+    def validation_image(self, batch, batch_idx: int = 0):
+        """Scores one held-out view like the reference's validation_image, without visualisers, image files or logging.
+        batch {'coords' [.., C], 'rgb' [.., 3], 'W', 'H'}: the view is rendered under no_grad in eval() (clamped output, as
+        validation_step runs it, :987-1010) and the previous train / eval mode is restored.  Returns 0-d device tensors, so a
+        loop over views never synchronises: 'val/loss' the unweighted MSE (MSELoss, losses.py:21-28), 'val/psnr' and
+        'val/ssim' metrics.psnr / metrics.ssim of the [H, W, 3] frame (metrics.py:25-34), computed on the device in fp64."""
+        from .metrics import image_metrics
+
+        was_training = self.training
+        self.eval()
+        try:
+            with torch.no_grad():
+                coords = batch["coords"]
+                rgb = batch["rgb"].reshape(-1, 3)
+                W, H = int(batch["W"]), int(batch["H"])
+                pred = self(coords.reshape(-1, coords.shape[-1]))["rgb"]
+                loss = torch.mean((pred - rgb) ** 2)
+                mse, ssim = image_metrics(pred.reshape(H, W, 3), rgb.reshape(H, W, 3))
+                psnr = 10.0 * torch.log10(1.0 / mse[0])
+        finally:
+            self.train(was_training)
+        return {"val/loss": loss, "val/psnr": psnr, "val/ssim": ssim[0]}
+
+    @staticmethod
+    def validation_epoch_end(outputs):
+        """get_mean_outputs(outputs, cpu=True) (metrics.py): the NumPy mean over views of every key, as a Python float (a
+        mean of per-view PSNRs, not the PSNR of the mean MSE).  One device-to-host copy per key."""
+        return {k: float(torch.stack([o[k] for o in outputs]).cpu().numpy().mean()) for k in outputs[0]}
+
     # ---- nlf/__init__.py:433-479
     def load_state_dict(self, state_dict: Dict[str, torch.Tensor], strict: bool = False):
         if "state_dict" in state_dict and isinstance(state_dict["state_dict"], dict):

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define HR_ABI_VERSION 13
+#define HR_ABI_VERSION 14
 
 #define HR_MAX_GROUPS 4   /* ray-parameterisation groups feeding the sample net (ray.py:235-263) */
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
@@ -424,6 +424,23 @@ int hr_train_net_backward(hr_handle* h, const float* d_heads, int64_t n_rays, co
  * are copied at launch), launches already enqueued keep the old ones.  The graph hr_render_host caches is dropped (its kernel
  * nodes hold the old configuration by value) and captured again by the next hr_render_host call. */
 int hr_set_activations(hr_handle* h, const hr_config* cfg);
+
+/* ---- held-out view scoring (handle-free) ----
+ * Replaces: the host-side metrics of INRSystem.validation_image (nlf/__init__.py:976-980), i.e. metrics.psnr / metrics.ssim
+ * (metrics.py:25-34) = scikit-image's peak_signal_noise_ratio(data_range=1) and structural_similarity(win_size=11,
+ * multichannel, gaussian_weights, data_range=1) run on the CPU after a device-to-host copy of the frame.
+ * pred, gt: [n_images, height, width, 3] fp32 device, channel-last.  out: device [n_images][2] fp64 = (mse, ssim) per image:
+ *   mse  = mean over all height*width*3 values of (pred - gt)^2, difference and square in fp32, summed in fp64;
+ *   ssim = per channel, the 11x11 Gaussian window (sigma 1.5, truncate 3.5, SciPy's normalised weights) moments filtered in
+ *          fp64, sample covariance (121/120), C1 = 0.01^2, C2 = 0.03^2, mean of the SSIM map over [5, height-5) x
+ *          [5, width-5), averaged over the 3 channels.
+ * Deterministic: no float atomics, per-tile partials summed in a fixed order, so two calls give identical bits and an image's
+ * result does not depend on the batch it is scored in.  height and width must be >= 11 (the window must fit), n_images in
+ * [1, 65535]; out and workspace 8-byte aligned, the workspace (device) at least hr_image_metrics_workspace_bytes(n_images,
+ * height, width) bytes (-1 for arguments hr_image_metrics refuses).  On error nothing is enqueued and `out` is untouched. */
+int64_t hr_image_metrics_workspace_bytes(int32_t n_images, int32_t height, int32_t width);
+int hr_image_metrics(const float* pred, const float* gt, int32_t n_images, int32_t height, int32_t width, double* out,
+                     void* workspace, int64_t workspace_bytes, void* stream);
 
 /* Number of kernels hr_render launched since creation (bench.py's gpu_launches). */
 int64_t hr_launch_count(const hr_handle* h);
