@@ -84,10 +84,9 @@ __global__ void pack_channel_last(const float* __restrict__ src, float* __restri
 }
 
 // (axis, time) planes -> per-keyframe lines.  The reference samples plane_time[1,C,K,L] bilinearly at (u_c, tau) where
-// tau = normalize_time_coord(base_t) (tensorf_dynamic.py:615-616) and base_t is the ray's keyframe time
-// (utils/flow_utils.py:18-31): tau therefore takes exactly K values, one per keyframe k, and the two rows grid_sample
-// blends (rows it_k, it_k+1 with fraction ft_k, align_corners=True) are a property of k alone.  dst[k][l][c] holds that
-// blend, so the render kernel's second factor is a 2-tap linear lookup instead of 4 taps.
+// base_t is the ray's keyframe time (utils/flow_utils.py:18-31), so the two rows grid_sample blends are a property of the
+// keyframe k alone (keyframe_blend).  dst[k][l][c] holds that blend, so the render kernel's second factor is a 2-tap linear
+// lookup instead of 4 taps.
 __global__ void pack_time_lines(const float* __restrict__ src, float* __restrict__ dst, int C, int K, int L, float inv_fac,
                                 float time_scale, float time_offset) {
   long long total = (long long)K * L * C;
@@ -95,11 +94,8 @@ __global__ void pack_time_lines(const float* __restrict__ src, float* __restrict
     int c = (int)(i % C);
     int l = (int)((i / C) % L);
     int k = (int)(i / ((long long)C * L));
-    float base_t = __fmul_rn((float)k, inv_fac);
-    float tau = __fsub_rn(__fmul_rn(__fadd_rn(__fmul_rn(base_t, time_scale), time_offset), 2.0f), 1.0f);
-    float iy = __fmul_rn(__fmul_rn(__fadd_rn(tau, 1.0f), 0.5f), (float)(K - 1));
-    int it = max(0, min((int)floorf(iy), K - 2));
-    float ft = iy - (float)it;
+    float ft;
+    int it = hr::keyframe_blend(k, K, inv_fac, time_scale, time_offset, ft);
     float a = src[((long long)c * K + it) * L + l];
     float b = src[((long long)c * K + it + 1) * L + l];
     dst[i] = __fmul_rn(1.0f - ft, a) + __fmul_rn(ft, b);
@@ -191,8 +187,7 @@ __global__ void cascade_points_kernel(const __grid_constant__ hr_config cfg, con
     const float sg = cfg.pre_use_sigma ? hr::apply_act_eased(cfg.pre_act_sigma, sraw) : 0.0f;
     const float zr = __fmul_rn(hr::apply_act(cfg.pre_isect_act, hr::apply_act(cfg.pre_act_z, zraw)), __fsub_rn(1.0f, sg));
     const float z = __fadd_rn(__fmul_rn(zr, cfg.pre_z_scale), cfg.pre_samples_tab[s]);
-    const float dzg = (fabsf(dz) < 1e-5f) ? 1e12f : dz;  // intersect_utils.py:135-142
-    float t = __fdiv_rn(__fsub_rn(z, oz), dzg);
+    float t = hr::intersect_axis_plane(z, oz, dz);
     if ((t <= cfg.pre_near) || (t >= cfg.pre_far)) t = 0.0f;
     float key[1] = {act ? t : __int_as_float(0x7f800000)};
     if (cfg.pre_sort) hr::sort_keys<1>(key, lane);
@@ -245,11 +240,8 @@ __global__ void unblend_time_lines(const float* __restrict__ src, float* __restr
     int c = (int)(i / ((long long)K * L));
     float acc = 0.0f;
     for (int k = 0; k < K; ++k) {
-      float base_t = __fmul_rn((float)k, inv_fac);
-      float tau = __fsub_rn(__fmul_rn(__fadd_rn(__fmul_rn(base_t, time_scale), time_offset), 2.0f), 1.0f);
-      float iy = __fmul_rn(__fmul_rn(__fadd_rn(tau, 1.0f), 0.5f), (float)(K - 1));
-      int it = max(0, min((int)floorf(iy), K - 2));
-      float ft = iy - (float)it;
+      float ft;
+      int it = hr::keyframe_blend(k, K, inv_fac, time_scale, time_offset, ft);
       float g = src[((long long)k * L + l) * C + c];
       if (it == r) acc += (1.0f - ft) * g;
       if (it + 1 == r) acc += ft * g;

@@ -99,4 +99,13 @@ __device__ __forceinline__ float apply_act_head(const hr_act& a, float x) {
 // true while act_sigma or act_point_sigma is eased: the render kernels' EASE variants serve the configuration
 __host__ __device__ inline bool eases_density(const hr_config& c) { return c.act_sigma.eased || c.act_point_sigma.eased; }
 
+// intersect_axis_plane (intersect_utils.py:127-150): distance along o + t d to the plane {x_a = z}, with o, d the ray's
+// components along axis a.  axis_plane_dir is the guarded divisor: a component below 1e-5 in magnitude becomes 1e12.
+__device__ __forceinline__ float axis_plane_dir(float d) { return (fabsf(d) < 1e-5f) ? 1e12f : d; }
+
+__device__ __forceinline__ float intersect_axis_plane(float z, float o, float d) {
+  const float dg = axis_plane_dir(d);
+  return __fdiv_rn(__fsub_rn(z, o), dg);
+}
+
 }  // namespace hr

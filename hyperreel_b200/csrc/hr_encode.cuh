@@ -19,9 +19,8 @@ __device__ __forceinline__ void encode_ray_features(const hr_config& cfg, const 
     if (G.fn == HR_PARAM_TWO_PLANE) {
       // TwoPlaneParam (param.py:87-115) + intersect_axis_plane (intersect_utils.py:127-150)
       float oz = r[2], dz = r[5];
-      float dzg = (fabsf(dz) < 1e-5f) ? 1e12f : dz;
-      float t1 = __fdiv_rn(__fsub_rn(G.near, oz), dzg);
-      float t2 = __fdiv_rn(__fsub_rn(G.far, oz), dzg);
+      float t1 = intersect_axis_plane(G.near, oz, dz);
+      float t2 = intersect_axis_plane(G.far, oz, dz);
       v[0] = __fadd_rn(r[0], __fmul_rn(r[3], t1));
       v[1] = __fadd_rn(r[1], __fmul_rn(r[4], t1));
       v[2] = __fadd_rn(r[0], __fmul_rn(r[3], t2));

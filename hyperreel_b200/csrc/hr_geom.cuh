@@ -1,5 +1,6 @@
-// Per-sample geometry shared by the forward and backward render kernels: the sort of the distances, the mipnerf / affine
-// contractions and the SH basis (references cited per function).
+// Per-sample and per-ray arithmetic shared by the forward and backward render kernels (references cited per function).  The
+// backward recomputes the forward from rays and heads, so both kernels must round every step here identically: each step is
+// written once, and a change to it reaches both.
 #pragma once
 #include "hr_common.cuh"
 
@@ -59,6 +60,158 @@ __device__ __forceinline__ void sort_keys_sub(float& k, int e) {
       k = (lower == up) ? fminf(k, other) : fmaxf(k, other);
     }
   }
+}
+
+// Whether a ray's keys need the sort network at all (element e = reg*32 + lane; with two rays per warp, SPL == 1 and e is the
+// lane within the ray's group).  The keys of a trained model are usually in order already (small offsets around increasing
+// base primitives, masked samples at t = 0 in front), so one neighbour exchange and a vote decide.
+template <int SPL>
+__device__ __forceinline__ bool keys_unsorted(const float (&k)[SPL], int e) {
+  bool bad = false;
+#pragma unroll
+  for (int r = 0; r < SPL; ++r) {
+    float prev = __shfl_up_sync(kFull, k[r], 1);
+    if (r > 0) {
+      const float last = __shfl_sync(kFull, k[r > 0 ? r - 1 : 0], 31);
+      if (e == 0) prev = last;
+    }
+    bad = bad || (((r > 0) || (e > 0)) && (prev > k[r]));
+  }
+  return __any_sync(kFull, bad);
+}
+
+// Transmittance of one register row of samples (tensorf_utils.py:242-253): the exclusive product over the LW lanes of a ray
+// (lane sl) of the factors a1 = 1 - alpha + 1e-10, times carryT, the product over the rows before; carryT then moves past
+// this row.
+template <int LW>
+__device__ __forceinline__ float transmittance(float a1, int sl, float& carryT) {
+  float inc = a1;  // inclusive product scan
+#pragma unroll
+  for (int d = 1; d < LW; d <<= 1) {
+    float o = __shfl_up_sync(kFull, inc, d);
+    if (sl >= d) inc *= o;
+  }
+  float exc = __shfl_up_sync(kFull, inc, 1);
+  if (sl == 0) exc = 1.0f;
+  const float T = carryT * exc;
+  carryT = carryT * __shfl_sync(kFull, inc, 31);
+  return T;
+}
+
+// Alpha of sample s = sl + 32 j, register row j of the distances (sl: the lane's position within the ray's group of lanes):
+// delta = dist[s+1] - dist[s], the last 1e10 (tensorf_dynamic.py:663-670); ex = exp(-sigma delta ds), alpha = 1 - ex and
+// a1 = 1 - alpha + 1e-10 (tensorf_utils.py:242-253); samples past S have alpha 0 and a1 1.
+struct SampleAlpha {
+  float delta, ex, alpha, a1;
+};
+
+template <int SPL>
+__device__ __forceinline__ SampleAlpha sample_alpha(const float (&dist)[SPL], int j, float sigma, float ds, int sl, int S) {
+  SampleAlpha a;
+  const int s = sl + 32 * j;
+  float nxt = __shfl_down_sync(kFull, dist[j], 1);
+  if (j + 1 < SPL) {
+    float first_next = __shfl_sync(kFull, dist[(j + 1 < SPL) ? j + 1 : j], 0);
+    if (sl == 31) nxt = first_next;  // SPL >= 2 only (one ray per warp)
+  }
+  a.delta = (s == S - 1) ? 1e10f : __fsub_rn(nxt, dist[j]);
+  a.ex = expf(-__fmul_rn(sigma, __fmul_rn(a.delta, ds)));
+  a.alpha = __fsub_rn(1.0f, a.ex);
+  if (s >= S) a.alpha = 0.0f;
+  a.a1 = __fadd_rn(__fsub_rn(1.0f, a.alpha), 1e-10f);
+  if (s >= S) a.a1 = 1.0f;
+  return a;
+}
+
+// feature2density (tensorf_dynamic.py:373-392; static tensorf_no_sample.py:82-88,187: weights == 1)
+__device__ __forceinline__ float feature2density(const hr_config& cfg, float feat) {
+  if (cfg.fea2dense == HR_DENSE_RELU) return fmaxf(feat, 0.0f);
+  if (cfg.fea2dense == HR_DENSE_RELU_ABS) return fabsf(feat);
+  const float xs = feat + cfg.density_shift;
+  return (xs > 20.0f) ? xs : log1pf(expf(xs));
+}
+
+// Keyframe snap of a ray's time (utils/flow_utils.py:18-31): the keyframe's time base_t, the ray's offset toff from it, and
+// the keyframe's row of the pre-blended second-factor tables (the time coordinate of every sample of the ray depends only on
+// that row).
+struct Keyframe {
+  float base_t, toff;
+  int row;
+};
+
+__device__ __forceinline__ Keyframe keyframe_snap(const Derived& dv, float time) {
+  Keyframe k;
+  float tt = __fmul_rn(time, dv.time_fac);
+  tt = fminf(fmaxf(tt, 0.0f), dv.kf_max);
+  tt = rintf(__fsub_rn(tt, 1e-5f));
+  k.base_t = __fmul_rn(tt, dv.time_inv_fac);
+  k.toff = __fsub_rn(time, k.base_t);
+  k.row = max(0, min((int)tt, dv.kt - 1));
+  return k;
+}
+
+// The two rows of a K-row (axis, time) plane that grid_sample blends (align_corners=True) for keyframe k: it and it + 1 with
+// fraction ft.  The reference samples the plane at tau = normalize_time_coord(base_t) (tensorf_dynamic.py:615-616), which
+// takes one value per keyframe, so the blend is a property of k alone.
+__device__ __forceinline__ int keyframe_blend(int k, int K, float inv_fac, float time_scale, float time_offset, float& ft) {
+  float base_t = __fmul_rn((float)k, inv_fac);
+  float tau = __fsub_rn(__fmul_rn(__fadd_rn(__fmul_rn(base_t, time_scale), time_offset), 2.0f), 1.0f);
+  float iy = __fmul_rn(__fmul_rn(__fadd_rn(tau, 1.0f), 0.5f), (float)(K - 1));
+  int it = max(0, min((int)floorf(iy), K - 2));
+  ft = iy - (float)it;
+  return it;
+}
+
+// Ray-quadric hit of intersect_sphere / intersect_cylinder (intersect_utils.py:45-125) for the ray o + t d given in the
+// quadric's frame (the cylinder uses x and z only): the far root unless it lies behind the origin or the radius is negative,
+// 0 on a miss.  disc, sq and the root taken are what d t / d rad needs.
+struct QuadricHit {
+  float t, disc, sq;
+  bool first;  // t is the root (-b + sq) / 2a
+};
+
+__device__ __forceinline__ QuadricHit intersect_quadric(float ox, float oy, float oz, float dx, float dy, float dz, float rad,
+                                                        bool cylinder) {
+  float oo, dd, od;
+  if (cylinder) {
+    oo = __fadd_rn(__fmul_rn(ox, ox), __fmul_rn(oz, oz));
+    dd = __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dz, dz));
+    od = __fadd_rn(__fmul_rn(ox, dx), __fmul_rn(oz, dz));
+  } else {
+    oo = __fadd_rn(__fadd_rn(__fmul_rn(ox, ox), __fmul_rn(oy, oy)), __fmul_rn(oz, oz));
+    dd = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+    od = __fadd_rn(__fadd_rn(__fmul_rn(ox, dx), __fmul_rn(oy, dy)), __fmul_rn(oz, dz));
+  }
+  QuadricHit h;
+  float a = dd, b = __fmul_rn(2.0f, od), c = __fsub_rn(oo, __fmul_rn(rad, rad));
+  float disc = __fsub_rn(__fmul_rn(b, b), __fmul_rn(__fmul_rn(4.0f, a), c));
+  disc = (disc < 0.0f) ? 0.0f : disc;
+  float sq = sqrtf(__fadd_rn(disc, 1e-8f));
+  float a2 = __fmul_rn(2.0f, a);
+  float t1 = __fdiv_rn(__fadd_rn(-b, sq), a2);
+  float t2 = __fdiv_rn(__fsub_rn(-b, sq), a2);
+  if (disc <= 0.0f) { t1 = 0.0f; t2 = 0.0f; }
+  h.first = (t2 < 0.0f) || (rad < 0.0f);
+  h.t = h.first ? t1 : t2;
+  h.disc = disc;
+  h.sq = sq;
+  return h;
+}
+
+// euclidean_distance_unified (primitive.py:126-180): samples are distances from the ray's point closest to the origin,
+// base = d^ x (o x d^) (pluecker_pos, param.py:297-307); this is the signed distance from o to that point.
+__device__ __forceinline__ float ray_base_distance(float ox, float oy, float oz, float dx, float dy, float dz) {
+  const float nd = fmaxf(sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz))), 1e-12f);
+  const float vx = __fdiv_rn(dx, nd), vy = __fdiv_rn(dy, nd), vz = __fdiv_rn(dz, nd);
+  const float mx = __fsub_rn(__fmul_rn(oy, vz), __fmul_rn(oz, vy));
+  const float my = __fsub_rn(__fmul_rn(oz, vx), __fmul_rn(ox, vz));
+  const float mz = __fsub_rn(__fmul_rn(ox, vy), __fmul_rn(oy, vx));
+  const float ex = __fsub_rn(__fsub_rn(__fmul_rn(vy, mz), __fmul_rn(vz, my)), ox);
+  const float ey = __fsub_rn(__fsub_rn(__fmul_rn(vz, mx), __fmul_rn(vx, mz)), oy);
+  const float ez = __fsub_rn(__fsub_rn(__fmul_rn(vx, my), __fmul_rn(vy, mx)), oz);
+  const float dotde = __fadd_rn(__fadd_rn(__fmul_rn(dx, ex), __fmul_rn(dy, ey)), __fmul_rn(dz, ez));
+  const float sgn = (dotde > 0.0f) ? 1.0f : ((dotde < 0.0f) ? -1.0f : 0.0f);
+  return __fmul_rn(sgn, sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(ez, ez))));
 }
 
 // mipnerf inverse contraction of a scalar distance (reference: nlf/contract.py:143-158).
@@ -127,22 +280,8 @@ static __device__ __noinline__ float intersect_rare(const hr_config& cfg, const 
                                                     float oy, float oz, float dx, float dy, float dz) {
   const float hz[4] = {hz0, hz1, hz2, hz3};
   float t = 0.0f;
-  // ---- euclidean_distance_unified (primitive.py:126-180): samples are distances from the ray's point closest to the
-  // origin, base = d^ x (o x d^) (pluecker_pos, param.py:297-307); per ray: signed distance from o to that point
   float base_distance = 0.0f;
-  if (cfg.isect_type == HR_ISECT_DISTANCE) {
-    const float nd = fmaxf(sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz))), 1e-12f);
-    const float vx = __fdiv_rn(dx, nd), vy = __fdiv_rn(dy, nd), vz = __fdiv_rn(dz, nd);
-    const float mx = __fsub_rn(__fmul_rn(oy, vz), __fmul_rn(oz, vy));
-    const float my = __fsub_rn(__fmul_rn(oz, vx), __fmul_rn(ox, vz));
-    const float mz = __fsub_rn(__fmul_rn(ox, vy), __fmul_rn(oy, vx));
-    const float ex = __fsub_rn(__fsub_rn(__fmul_rn(vy, mz), __fmul_rn(vz, my)), ox);
-    const float ey = __fsub_rn(__fsub_rn(__fmul_rn(vz, mx), __fmul_rn(vx, mz)), oy);
-    const float ez = __fsub_rn(__fsub_rn(__fmul_rn(vx, my), __fmul_rn(vy, mx)), oz);
-    const float dotde = __fadd_rn(__fadd_rn(__fmul_rn(dx, ex), __fmul_rn(dy, ey)), __fmul_rn(dz, ez));
-    const float sgn = (dotde > 0.0f) ? 1.0f : ((dotde < 0.0f) ? -1.0f : 0.0f);
-    base_distance = __fmul_rn(sgn, sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(ez, ez))));
-  }
+  if (cfg.isect_type == HR_ISECT_DISTANCE) base_distance = ray_base_distance(ox, oy, oz, dx, dy, dz);
   if (cfg.isect_type == HR_ISECT_VOXEL) {
     // IntersectVoxelGrid (voxel.py:77-112) + intersect_voxel_grid (intersect_utils.py:152-179): sample s is plane s/3 of
     // axis s%3; process_z_vals scales per axis (base.py:128-130)
@@ -153,8 +292,7 @@ static __device__ __noinline__ float intersect_rare(const hr_config& cfg, const 
     const float da = (ax == 0) ? dx : ((ax == 1) ? dy : dz);
     const float oa = (ax == 0) ? ox : ((ax == 1) ? oy : oz);
     if (cfg.isect_outward) z = __fmul_rn(z, (da > 0.0f) ? 1.0f : ((da < 0.0f) ? -1.0f : 0.0f));
-    const float dg = (fabsf(da) < 1e-5f) ? 1e12f : da;
-    t = __fdiv_rn(__fsub_rn(z, oa), dg);
+    t = intersect_axis_plane(z, oa, da);
     if (cfg.isect_max_axis) {
       const float dmax = fmaxf(fabsf(dx), fmaxf(fabsf(dy), fabsf(dz)));
       if (fabsf(da) < __fsub_rn(dmax, 1e-8f)) t = 0.0f;
@@ -209,22 +347,7 @@ static __device__ __noinline__ float intersect_rare(const hr_config& cfg, const 
     const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(rdx, rdx), __fmul_rn(rdy, rdy)), __fmul_rn(rdz, rdz)));
     const float nd = fmaxf(nrm, 1e-12f);  // F.normalize
     const float ux = __fdiv_rn(rdx, nd), uy = __fdiv_rn(rdy, nd), uz = __fdiv_rn(rdz, nd);
-    // intersect_sphere (intersect_utils.py:45-84)
-    float tq;
-    {
-      const float oo = __fadd_rn(__fadd_rn(__fmul_rn(rox, rox), __fmul_rn(roy, roy)), __fmul_rn(roz, roz));
-      const float dd = __fadd_rn(__fadd_rn(__fmul_rn(ux, ux), __fmul_rn(uy, uy)), __fmul_rn(uz, uz));
-      const float od = __fadd_rn(__fadd_rn(__fmul_rn(rox, ux), __fmul_rn(roy, uy)), __fmul_rn(roz, uz));
-      const float a = dd, b = __fmul_rn(2.0f, od), c = __fsub_rn(oo, __fmul_rn(rad, rad));
-      float disc = __fsub_rn(__fmul_rn(b, b), __fmul_rn(__fmul_rn(4.0f, a), c));
-      disc = (disc < 0.0f) ? 0.0f : disc;
-      const float sq = sqrtf(__fadd_rn(disc, 1e-8f));
-      const float a2 = __fmul_rn(2.0f, a);
-      float t1 = __fdiv_rn(__fadd_rn(-b, sq), a2);
-      float t2 = __fdiv_rn(__fsub_rn(-b, sq), a2);
-      if (disc <= 0.0f) { t1 = 0.0f; t2 = 0.0f; }
-      tq = ((t2 < 0.0f) || (rad < 0.0f)) ? t1 : t2;
-    }
+    float tq = intersect_quadric(rox, roy, roz, ux, uy, uz, rad, false).t;
     // min_sphere_radius (intersect_utils.py:27-33) and pluecker_pos (param.py:297-307) normalise the direction again
     const float n2 = fmaxf(sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(ux, ux), __fmul_rn(uy, uy)), __fmul_rn(uz, uz))), 1e-12f);
     const float vx = __fdiv_rn(ux, n2), vy = __fdiv_rn(uy, n2), vz = __fdiv_rn(uz, n2);

@@ -12,8 +12,9 @@
 //   geometry       p = c(o + t d) + flow * dt + offset * (1 - sigma_p),  t = sorted intersection distances
 //                  -> d t (through the sort permutation), d heads
 // One warp per ray, lane = sample for everything (the forward's quad mapping is not used here: this kernel is bound by the
-// L2 atomics, not by the gathers).  The forward is recomputed from rays + heads with the forward kernel's own arithmetic
-// (same rounding, hence the same masks and the same sort order); nothing per-sample was saved.
+// L2 atomics, not by the gathers).  The forward is recomputed from rays + heads through the per-sample and per-ray functions
+// of hr_geom.cuh that the forward kernel calls (same rounding, hence the same masks and the same sort order); nothing
+// per-sample was saved.
 // Supported for training: z_plane / sphere / cylinder (origin_scale_factor == 0) / euclidean-distance / voxel-grid /
 // deformable-plane primitives, no / mipnerf / bbox / z_depth contraction, per-sample and per-ray colour heads, the per-camera
 // colour transform, S <= 64; hr_render_backward rejects the rest.
@@ -294,12 +295,9 @@ render_bwd_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__
     float toff = 0.0f;
     int krow = 0;
     if (DYN || cfg.use_flow) {
-      float tt = __fmul_rn(time, dv.time_fac);
-      tt = fminf(fmaxf(tt, 0.0f), dv.kf_max);
-      tt = rintf(__fsub_rn(tt, 1e-5f));
-      const float base_t = __fmul_rn(tt, dv.time_inv_fac);
-      toff = __fsub_rn(time, base_t);
-      if (DYN) krow = max(0, min((int)tt, dv.kt - 1));
+      const Keyframe kf = keyframe_snap(dv, time);
+      toff = kf.toff;
+      if (DYN) krow = kf.row;
     }
     __syncwarp();
     if constexpr (SHADE == HR_SHADE_SH) {
@@ -329,20 +327,8 @@ render_bwd_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__
     // the z channel that carries the gradient (the deformable plane's normal channels 0-2 go through dt_dn)
     const int zc_idx = (cfg.isect_type == HR_ISECT_Z_PLANE || cfg.isect_type == HR_ISECT_DISTANCE ||
                         (RARE && cfg.isect_type == HR_ISECT_VOXEL)) ? 0 : 3;
-    float base_distance = 0.0f;  // euclidean_distance_unified: same per-ray term as the forward kernel (no parameter behind it)
-    if (cfg.isect_type == HR_ISECT_DISTANCE) {
-      const float nd = fmaxf(sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz))), 1e-12f);
-      const float vx = __fdiv_rn(dx, nd), vy = __fdiv_rn(dy, nd), vz = __fdiv_rn(dz, nd);
-      const float mx = __fsub_rn(__fmul_rn(oy, vz), __fmul_rn(oz, vy));
-      const float my = __fsub_rn(__fmul_rn(oz, vx), __fmul_rn(ox, vz));
-      const float mz = __fsub_rn(__fmul_rn(ox, vy), __fmul_rn(oy, vx));
-      const float ex = __fsub_rn(__fsub_rn(__fmul_rn(vy, mz), __fmul_rn(vz, my)), ox);
-      const float ey = __fsub_rn(__fsub_rn(__fmul_rn(vz, mx), __fmul_rn(vx, mz)), oy);
-      const float ez = __fsub_rn(__fsub_rn(__fmul_rn(vx, my), __fmul_rn(vy, mx)), oz);
-      const float dotde = __fadd_rn(__fadd_rn(__fmul_rn(dx, ex), __fmul_rn(dy, ey)), __fmul_rn(dz, ez));
-      const float sgn = (dotde > 0.0f) ? 1.0f : ((dotde < 0.0f) ? -1.0f : 0.0f);
-      base_distance = __fmul_rn(sgn, sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(ez, ez))));
-    }
+    float base_distance = 0.0f;  // euclidean_distance_unified: a per-ray term with no parameter behind it
+    if (cfg.isect_type == HR_ISECT_DISTANCE) base_distance = ray_base_distance(ox, oy, oz, dx, dy, dz);
 #pragma unroll
     for (int j = 0; j < SPL; ++j) {
       const int s = lane + 32 * j;
@@ -379,9 +365,8 @@ render_bwd_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__
         const float zpre = __fadd_rn(__fmul_rn(zr, cfg.z_scale), samp);
         float z = zpre, dz_dpre = 1.0f;
         if (cfg.contract_samples) { z = inv_contract_sample(cfg, dv, zpre); dz_dpre = inv_contract_sample_grad<RARE>(cfg, dv, zpre); }
-        const float dzg = (fabsf(dz) < 1e-5f) ? 1e12f : dz;
-        t = __fdiv_rn(__fsub_rn(z, oz), dzg);
-        dtdzr = cfg.z_scale * dz_dpre / dzg;
+        t = intersect_axis_plane(z, oz, dz);
+        dtdzr = cfg.z_scale * dz_dpre / axis_plane_dir(dz);
       } else if (cfg.isect_type == HR_ISECT_DISTANCE) {
         const float zpre = __fadd_rn(__fmul_rn(zr, cfg.z_scale), samp);
         float z = zpre, dz_dpre = 1.0f;
@@ -396,29 +381,10 @@ render_bwd_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__
         if (cfg.contract_samples) { rad = inv_contract_sample(cfg, dv, rpre); drad_dpre = inv_contract_sample_grad<RARE>(cfg, dv, rpre); }
         const float sox = __fmul_rn(ox, gx), soy = __fmul_rn(oy, gy), soz = __fmul_rn(oz, gz);
         const float sdx = __fmul_rn(dx, gx), sdy = __fmul_rn(dy, gy), sdz = __fmul_rn(dz, gz);
-        float oo, dd, od;
-        if (cfg.isect_type == HR_ISECT_CYLINDER) {
-          oo = __fadd_rn(__fmul_rn(sox, sox), __fmul_rn(soz, soz));
-          dd = __fadd_rn(__fmul_rn(sdx, sdx), __fmul_rn(sdz, sdz));
-          od = __fadd_rn(__fmul_rn(sox, sdx), __fmul_rn(soz, sdz));
-        } else {
-          oo = __fadd_rn(__fadd_rn(__fmul_rn(sox, sox), __fmul_rn(soy, soy)), __fmul_rn(soz, soz));
-          dd = __fadd_rn(__fadd_rn(__fmul_rn(sdx, sdx), __fmul_rn(sdy, sdy)), __fmul_rn(sdz, sdz));
-          od = __fadd_rn(__fadd_rn(__fmul_rn(sox, sdx), __fmul_rn(soy, sdy)), __fmul_rn(soz, sdz));
-        }
-        const float a = dd, b = __fmul_rn(2.0f, od), c = __fsub_rn(oo, __fmul_rn(rad, rad));
-        float disc = __fsub_rn(__fmul_rn(b, b), __fmul_rn(__fmul_rn(4.0f, a), c));
-        const bool neg = disc < 0.0f;
-        disc = neg ? 0.0f : disc;
-        const float sq = sqrtf(__fadd_rn(disc, 1e-8f));
-        const float a2 = __fmul_rn(2.0f, a);
-        float t1 = __fdiv_rn(__fadd_rn(-b, sq), a2);
-        float t2 = __fdiv_rn(__fsub_rn(-b, sq), a2);
-        if (disc <= 0.0f) { t1 = 0.0f; t2 = 0.0f; }
-        const bool first = (t2 < 0.0f) || (rad < 0.0f);
-        t = first ? t1 : t2;
+        const QuadricHit h = intersect_quadric(sox, soy, soz, sdx, sdy, sdz, rad, cfg.isect_type == HR_ISECT_CYLINDER);
+        t = h.t;
         // disc = b^2 - 4a(oo - rad^2): d disc / d rad = 8 a rad; d t1,2 / d disc = +-1 / (2 a * 2 sq)
-        float dt_drad = (disc <= 0.0f) ? 0.0f : (first ? 1.0f : -1.0f) * (2.0f * rad) / sq;
+        float dt_drad = (h.disc <= 0.0f) ? 0.0f : (h.first ? 1.0f : -1.0f) * (2.0f * rad) / h.sq;
         dtdzr = dt_drad * drad_dpre * cfg.z_scale;
       }
       if ((t <= cfg.isect_near) || (t >= cfg.isect_far)) {
@@ -438,18 +404,7 @@ render_bwd_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__
       }
     }
     if (cfg.isect_sort) {
-      // keys already in order (the usual case for a trained model): the (key, id) network would return the identity
-      bool bad = false;
-#pragma unroll
-      for (int r = 0; r < SPL; ++r) {
-        float prev = __shfl_up_sync(kFull, tkey[r], 1);
-        if (r > 0) {
-          const float last = __shfl_sync(kFull, tkey[r > 0 ? r - 1 : 0], 31);
-          if (lane == 0) prev = last;
-        }
-        bad = bad || (((r > 0) || (lane > 0)) && (prev > tkey[r]));
-      }
-      if (__any_sync(kFull, bad)) sort_pairs<SPL>(tkey, tid, lane);
+      if (keys_unsorted<SPL>(tkey, lane)) sort_pairs<SPL>(tkey, tid, lane);
     }
 
     // ---- points, validity, texel coordinates (position e = lane + 32 j in sorted order) ----
@@ -548,38 +503,15 @@ render_bwd_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__
     for (int j = 0; j < SPL; ++j) {
       const int s = lane + 32 * j;
       const float* hp = hrow + ((s < S) ? s : 0);
-      float sgm;
-      if (cfg.fea2dense == HR_DENSE_RELU) sgm = fmaxf(feat[j], 0.0f);
-      else if (cfg.fea2dense == HR_DENSE_RELU_ABS) sgm = fabsf(feat[j]);
-      else {
-        const float xs = feat[j] + cfg.density_shift;
-        sgm = (xs > 20.0f) ? xs : log1pf(expf(xs));
-      }
+      float sgm = feature2density(cfg, feat[j]);
       if (!valid[j]) sgm = 0.0f;
       sigma[j] = sgm;
-      float nxt = __shfl_down_sync(kFull, dist[j], 1);
-      if (j + 1 < SPL) {
-        const float first_next = __shfl_sync(kFull, dist[(j + 1 < SPL) ? j + 1 : j], 0);
-        if (lane == 31) nxt = first_next;
-      }
-      delta[j] = (s == S - 1) ? 1e10f : __fsub_rn(nxt, dist[j]);
-      ex[j] = expf(-__fmul_rn(sgm, __fmul_rn(delta[j], cfg.distance_scale)));
-      float alpha = __fsub_rn(1.0f, ex[j]);
-      if (s >= S) alpha = 0.0f;
-      float a1 = __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f);
-      if (s >= S) a1 = 1.0f;
-      a1s[j] = a1;
-      float inc = a1;
-#pragma unroll
-      for (int d = 1; d < 32; d <<= 1) {
-        const float o = __shfl_up_sync(kFull, inc, d);
-        if (lane >= d) inc *= o;
-      }
-      float exc = __shfl_up_sync(kFull, inc, 1);
-      if (lane == 0) exc = 1.0f;
-      Tt[j] = carryT * exc;
-      carryT = carryT * __shfl_sync(kFull, inc, 31);
-      wgt[j] = alpha * Tt[j];
+      const SampleAlpha sa = sample_alpha<SPL>(dist, j, sigma[j], cfg.distance_scale, lane, S);
+      delta[j] = sa.delta;
+      ex[j] = sa.ex;
+      a1s[j] = sa.a1;
+      Tt[j] = transmittance<32>(sa.a1, lane, carryT);
+      wgt[j] = sa.alpha * Tt[j];
       accw += wgt[j];
       const bool app = (s < S) && (wgt[j] > cfg.weight_thre);
 #pragma unroll

@@ -263,16 +263,14 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
       for (int c = 0; c < 3; ++c) hof[j][c] = cfg.use_offset ? __ldg(hp + (cfg.off_offset + c) * S) : 0.0f;
     }
 
-    // ---- per-ray keyframe snap (utils/flow_utils.py:18-31), time coordinate and keyframe row ----
+    // ---- per-ray keyframe snap, time offset and keyframe row ----
     float toff = 0.0f, base_t = 0.0f;
-    int krow = 0;  // keyframe index: the time coordinate of every sample of this ray depends only on it
+    int krow = 0;
     if (DYN || cfg.use_flow) {
-      float tt = __fmul_rn(time, dv.time_fac);
-      tt = fminf(fmaxf(tt, 0.0f), dv.kf_max);
-      tt = rintf(__fsub_rn(tt, 1e-5f));
-      base_t = __fmul_rn(tt, dv.time_inv_fac);
-      toff = __fsub_rn(time, base_t);
-      if (DYN) krow = max(0, min((int)tt, dv.kt - 1));
+      const Keyframe kf = keyframe_snap(dv, time);
+      base_t = kf.base_t;
+      toff = kf.toff;
+      if (DYN) krow = kf.row;
     }
 
     // ---- view-dependent appearance matrix: G[q][i] = sum_k Y_k(dir) * basis[(q*9+k)][i]  (tensorf_utils.py:334-338)
@@ -341,8 +339,7 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
         float zr = __fmul_rn(apply_act(cfg.isect_act, apply_act(cfg.act_z, hz[j][0])), one_m);
         float z = __fadd_rn(__fmul_rn(zr, cfg.z_scale), samp);
         if (cfg.contract_samples) z = inv_contract_sample(cfg, dv, z);
-        float dzg = (fabsf(dz) < 1e-5f) ? 1e12f : dz;  // intersect_utils.py:135-142
-        t = __fdiv_rn(__fsub_rn(z, oz), dzg);
+        t = intersect_axis_plane(z, oz, dz);
       } else if (RARE && cfg.isect_type != HR_ISECT_SPHERE && cfg.isect_type != HR_ISECT_CYLINDER) {
         // the less common primitives (sphere_new, euclidean_distance, voxel grids) live in one out-of-line function and are
         // compiled into the RARE variants only: the z-plane / sphere / cylinder kernels keep their instruction stream and
@@ -358,29 +355,10 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
         float gz = __fadd_rn(__fmul_rn(zc[2], cfg.sphere_origin_scale), cfg.sphere_origin_initial[2]);
         float rad = __fadd_rn(__fmul_rn(zc[3], cfg.z_scale), samp);
         if (cfg.contract_samples) rad = inv_contract_sample(cfg, dv, rad);
-        // primitive.py:420-438 + intersect_utils.py:45-84
+        // primitive.py:420-438; IntersectCylinderOld (primitive.py:181-250) for the cylinder
         float sox = __fmul_rn(ox, gx), soy = __fmul_rn(oy, gy), soz = __fmul_rn(oz, gz);
         float sdx = __fmul_rn(dx, gx), sdy = __fmul_rn(dy, gy), sdz = __fmul_rn(dz, gz);
-        float oo, dd, od;
-        if (cfg.isect_type == HR_ISECT_CYLINDER) {
-          // IntersectCylinderOld (primitive.py:181-250) + intersect_cylinder (intersect_utils.py:86-125): x and z only
-          oo = __fadd_rn(__fmul_rn(sox, sox), __fmul_rn(soz, soz));
-          dd = __fadd_rn(__fmul_rn(sdx, sdx), __fmul_rn(sdz, sdz));
-          od = __fadd_rn(__fmul_rn(sox, sdx), __fmul_rn(soz, sdz));
-        } else {
-          oo = __fadd_rn(__fadd_rn(__fmul_rn(sox, sox), __fmul_rn(soy, soy)), __fmul_rn(soz, soz));
-          dd = __fadd_rn(__fadd_rn(__fmul_rn(sdx, sdx), __fmul_rn(sdy, sdy)), __fmul_rn(sdz, sdz));
-          od = __fadd_rn(__fadd_rn(__fmul_rn(sox, sdx), __fmul_rn(soy, sdy)), __fmul_rn(soz, sdz));
-        }
-        float a = dd, b = __fmul_rn(2.0f, od), c = __fsub_rn(oo, __fmul_rn(rad, rad));
-        float disc = __fsub_rn(__fmul_rn(b, b), __fmul_rn(__fmul_rn(4.0f, a), c));
-        disc = (disc < 0.0f) ? 0.0f : disc;
-        float sq = sqrtf(__fadd_rn(disc, 1e-8f));
-        float a2 = __fmul_rn(2.0f, a);
-        float t1 = __fdiv_rn(__fadd_rn(-b, sq), a2);
-        float t2 = __fdiv_rn(__fsub_rn(-b, sq), a2);
-        if (disc <= 0.0f) { t1 = 0.0f; t2 = 0.0f; }
-        t = ((t2 < 0.0f) || (rad < 0.0f)) ? t1 : t2;
+        t = intersect_quadric(sox, soy, soz, sdx, sdy, sdz, rad, cfg.isect_type == HR_ISECT_CYLINDER).t;
       }
       if ((t <= cfg.isect_near) || (t >= cfg.isect_far)) t = 0.0f;
       tkey[j] = act ? t : __int_as_float(0x7f800000);
@@ -397,20 +375,7 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
 
     // ---- sort distances only (base.py:206-210) ----
     if (cfg.isect_sort) {
-      // the keys of a trained model are usually in order already (small offsets around increasing base primitives, masked
-      // samples at t = 0 in front): one neighbour exchange + vote decides whether the 15-stage network is needed at all
-      bool bad = false;  // element e = r*32 + lane (one ray per warp) or lane within the ray's 16 (two rays per warp)
-#pragma unroll
-      for (int r = 0; r < SPL; ++r) {
-        float prev = __shfl_up_sync(kFull, tkey[r], 1);
-        if (r > 0) {
-          const float last = __shfl_sync(kFull, tkey[r > 0 ? r - 1 : 0], 31);
-          if (lane == 0) prev = last;
-        }
-        bad = bad || (((r > 0) || (sl > 0)) && (prev > tkey[r]));
-      }
-      const bool unsorted = __any_sync(kFull, bad);
-      if (unsorted) {
+      if (keys_unsorted<SPL>(tkey, sl)) {
         if constexpr (RPW == 1) sort_keys<SPL>(tkey, lane);
         else sort_keys_sub<LW>(tkey[0], sl);
       }
@@ -599,37 +564,10 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
         float v = __shfl_sync(kFull, sig_r[4 * j + rr], 4 * (lane & 7) + (FOLD ? 3 : 0));
         if ((lane >> 3) == rr) feat = v;
       }
-      // feature2density (tensorf_dynamic.py:373-392; static tensorf_no_sample.py:82-88,187: weights == 1)
-      float sigma;
-      if (cfg.fea2dense == HR_DENSE_RELU) sigma = fmaxf(feat, 0.0f);
-      else if (cfg.fea2dense == HR_DENSE_RELU_ABS) sigma = fabsf(feat);
-      else {
-        float xs = feat + cfg.density_shift;
-        sigma = (xs > 20.0f) ? xs : log1pf(expf(xs));
-      }
+      float sigma = feature2density(cfg, feat);
       if (!valid[j]) sigma = 0.0f;
-      // deltas: dist[i+1]-dist[i], last = 1e10 (tensorf_dynamic.py:663-670)
-      float nxt = __shfl_down_sync(kFull, dist[j], 1);
-      if (j + 1 < SPL) {
-        float first_next = __shfl_sync(kFull, dist[(j + 1 < SPL) ? j + 1 : j], 0);
-        if (lane == 31) nxt = first_next;  // SPL >= 2 only (one ray per warp)
-      }
-      float delta = (s == S - 1) ? 1e10f : __fsub_rn(nxt, dist[j]);
-      float alpha = __fsub_rn(1.0f, expf(-__fmul_rn(sigma, __fmul_rn(delta, cfg.distance_scale))));
-      if (s >= S) alpha = 0.0f;
-      float a1 = __fadd_rn(__fsub_rn(1.0f, alpha), 1e-10f);
-      if (s >= S) a1 = 1.0f;
-      float inc = a1;  // inclusive product scan
-#pragma unroll
-      for (int d = 1; d < LW; d <<= 1) {
-        float o = __shfl_up_sync(kFull, inc, d);
-        if (sl >= d) inc *= o;
-      }
-      float exc = __shfl_up_sync(kFull, inc, 1);
-      if (sl == 0) exc = 1.0f;
-      const float T = carryT * exc;
-      carryT = carryT * __shfl_sync(kFull, inc, 31);
-      const float w = alpha * T;
+      const SampleAlpha sa = sample_alpha<SPL>(dist, j, sigma, cfg.distance_scale, sl, S);
+      const float w = sa.alpha * transmittance<LW>(sa.a1, sl, carryT);
       wgt[j] = w;
       if (EXTRA && s < S) {
         if (so.sigma) so.sigma[ray * S + s] = sigma;
