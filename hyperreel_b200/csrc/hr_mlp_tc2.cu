@@ -20,7 +20,8 @@
 //   * warpgroup 2 streams the weight images (bf16 hi + lo, consumption order, hr_tc_pack.cu) through a 4-stage
 //     cp.async.bulk ring of 16 KB stages (one k-step at W = 256) guarded by mbarriers; each consumer warpgroup releases a
 //     stage once the wgmmas that read it have retired, so every stage is loaded once per tile for both.
-// The last layer's columns go from the accumulators (+ bias) straight to the heads scratch in global memory.
+// The last layer's columns go from the accumulators (+ bias) straight to the heads scratch in global memory, 4 consecutive
+// columns per 16-byte store; the hidden epilogues write the activation operand with stmatrix.
 //
 // SAVE (the training forward, hr_mlp_train.cu): the same arithmetic, plus every fp32 value the epilogues split goes to global
 // memory as well -- the encoded input (sv.enc) and each hidden layer's LeakyReLU output (sv.act) -- and the heads are stored
@@ -198,28 +199,35 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
     if (pend >= 0 && wt == 0) mbar_arrive(empty0 + pend * 8);
     pend = -1;
   };
-  // hidden epilogue: A(l+1) = LeakyReLU(acc + bias), split into hi / lo
+  // hidden epilogue: A(l+1) = LeakyReLU(acc + bias), split into hi / lo.  The accumulator fragment of columns 8 j .. 8 j + 7
+  // and rows 8 h .. 8 h + 7 of the warp is an 8x8 stmatrix fragment, and its destination rows are 16-byte core-matrix
+  // rows of A, so one stmatrix.x4 writes a whole 16-wide k-step of the warp's 16 rows: matrix i = 2 (j % 2) + h, lane t
+  // addresses row t % 8 of matrix t / 8.
+  const int st_row = wg * 64 + (warp & 3) * 16 + 8 * ((lane >> 3) & 1) + (lane & 7);
+  const uint32_t st_off = ks_slot(st_row, lane >> 4);
   auto store_hidden = [&](const float* bias, int layer, long long tile) {
 #pragma unroll
-    for (int j = 0; j < W / 8; ++j) {
-      const int k = 8 * j + q2;
-      const float2 b = __ldg(reinterpret_cast<const float2*>(bias + k));
-      const uint32_t off = (uint32_t)(k >> 4) * KSTEP_BYTES + (uint32_t)(k & 7) * 2u;
+    for (int m = 0; m < W / 16; ++m) {
+      uint32_t hi[4], lo[4];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float t0 = acc[4 * j + 2 * h] + b.x, t1 = acc[4 * j + 2 * h + 1] + b.y;
-        t0 = fmaxf(t0, t0 * cfg.leaky_slope);  // LeakyReLU, slope in (0,1)
-        t1 = fmaxf(t1, t1 * cfg.leaky_slope);
-        uint32_t hi, lo;
-        split2(t0, t1, hi, lo);
-        if constexpr (SAVE) {
-          const long long ray = tile * BM + row0 + 8 * h;
-          if (ray < n_rays) *reinterpret_cast<float2*>(sv.act + layer * sv.act_stride + ray * W + k) = make_float2(t0, t1);
+      for (int jj = 0; jj < 2; ++jj) {
+        const int j = 2 * m + jj, k = 8 * j + q2;
+        const float2 b = __ldg(reinterpret_cast<const float2*>(bias + k));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float t0 = acc[4 * j + 2 * h] + b.x, t1 = acc[4 * j + 2 * h + 1] + b.y;
+          t0 = fmaxf(t0, t0 * cfg.leaky_slope);  // LeakyReLU, slope in (0,1)
+          t1 = fmaxf(t1, t1 * cfg.leaky_slope);
+          split2(t0, t1, hi[2 * jj + h], lo[2 * jj + h]);
+          if constexpr (SAVE) {
+            const long long ray = tile * BM + row0 + 8 * h;
+            if (ray < n_rays) *reinterpret_cast<float2*>(sv.act + layer * sv.act_stride + ray * W + k) = make_float2(t0, t1);
+          }
         }
-        const uint32_t o = off + ks_slot(row0 + 8 * h, (k >> 3) & 1);
-        *reinterpret_cast<uint32_t*>(smem + OFF_AHI + o) = hi;
-        *reinterpret_cast<uint32_t*>(smem + OFF_ALO + o) = lo;
       }
+      const uint32_t a = sbase + st_off + (uint32_t)m * KSTEP_BYTES;
+      stmatrix_x4(a + OFF_AHI, hi);
+      stmatrix_x4(a + OFF_ALO, lo);
     }
   };
 
@@ -282,24 +290,45 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
       run_pass(P);
       drain();
       const float* bias = pk.bias + P.bias_off;
+      if constexpr (SAVE) {
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const long long ray = tile * BM + row0 + 8 * h;
-        if (ray >= n_rays) continue;
-        float* dst = heads + ray * cfg.mlp_out + P.out_col0;
+        for (int h = 0; h < 2; ++h) {
+          const long long ray = tile * BM + row0 + 8 * h;
+          if (ray >= n_rays) continue;
+          float* row = heads + ray * cfg.mlp_out;
 #pragma unroll
-        for (int j = 0; j < W / 8; ++j) {
-          const int c = 8 * j + q2;
-          if (P.out_col0 + c < cfg.mlp_out) {  // mlp_out is a multiple of 4: the pair is in or out as a whole
-            const float2 b = __ldg(reinterpret_cast<const float2*>(bias + c));
-            if constexpr (SAVE) {  // channel-major column c*S+s -> the reference's s*stride+c
-              float* row = heads + ray * cfg.mlp_out;
+          for (int j = 0; j < W / 8; ++j) {
+            const int c = 8 * j + q2;
+            if (P.out_col0 + c < cfg.mlp_out) {  // mlp_out is a multiple of 4: the pair is in or out as a whole
+              const float2 b = __ldg(reinterpret_cast<const float2*>(bias + c));
+              // channel-major column c*S+s -> the reference's s*stride+c
               const int c0 = P.out_col0 + c, c1 = c0 + 1, S = cfg.n_samples;
               row[(c0 % S) * cfg.head_stride + c0 / S] = acc[4 * j + 2 * h] + b.x;
               row[(c1 % S) * cfg.head_stride + c1 / S] = acc[4 * j + 2 * h + 1] + b.y;
-            } else {
-              *reinterpret_cast<float2*>(dst + c) = make_float2(acc[4 * j + 2 * h] + b.x, acc[4 * j + 2 * h + 1] + b.y);
             }
+          }
+        }
+      } else {
+        // Lanes 2i and 2i + 1 hold 4 consecutive columns of the same row in column groups j and j + 1: they swap one pair
+        // so that each stores 4 consecutive columns with one 16-byte store (the even lane in group j, the odd one in
+        // group j + 1).  mlp_out is a multiple of 4, so the 4 columns are in or out as a whole.
+        const bool odd = (lane & 1) != 0;
+#pragma unroll
+        for (int jp = 0; jp < W / 16; ++jp) {
+          const int j = 2 * jp, c = 8 * j + q2;
+          const float2 b0 = __ldg(reinterpret_cast<const float2*>(bias + c));
+          const float2 b1 = __ldg(reinterpret_cast<const float2*>(bias + c + 8));
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const float2 v0 = make_float2(acc[4 * j + 2 * h] + b0.x, acc[4 * j + 2 * h + 1] + b0.y);
+            const float2 v1 = make_float2(acc[4 * j + 4 + 2 * h] + b1.x, acc[4 * j + 4 + 2 * h + 1] + b1.y);
+            const float2 send = odd ? v0 : v1;
+            const float2 recv = make_float2(__shfl_xor_sync(0xffffffffu, send.x, 1), __shfl_xor_sync(0xffffffffu, send.y, 1));
+            const int c4 = odd ? c + 6 : c;  // first of the lane's 4 columns
+            const long long ray = tile * BM + row0 + 8 * h;
+            if (ray < n_rays && P.out_col0 + c4 < cfg.mlp_out)
+              *reinterpret_cast<float4*>(heads + ray * cfg.mlp_out + P.out_col0 + c4) =
+                  odd ? make_float4(recv.x, recv.y, v1.x, v1.y) : make_float4(v0.x, v0.y, recv.x, recv.y);
           }
         }
       }

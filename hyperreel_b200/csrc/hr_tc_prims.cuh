@@ -133,6 +133,14 @@ __device__ __forceinline__ void wgmma_ss(float (&d)[128], uint64_t adesc, uint64
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
+// Four 8x8 b16 matrices from their mma fragments (r[i]: row t / 4, columns 2 (t % 4) and + 1 of matrix i) to shared memory;
+// lane t gives the address of row t % 8 of matrix t / 8 (16 contiguous bytes).
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]),
+               "r"(r[3])
+               : "memory");
+}
+
 // Offset (bytes) of the 16-byte slot holding k-group kg (0/1) of row `row` inside a 128-row x 16-k k-step image.
 __device__ __forceinline__ uint32_t ks_slot(int row, int kg) { return (uint32_t)((kg * 16 + (row >> 3)) * 128 + (row & 7) * 16); }
 
