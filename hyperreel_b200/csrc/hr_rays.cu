@@ -1,64 +1,28 @@
 // Camera -> rays on the device (the step before the hot path).
-// Reference: get_ray_directions_from_pixels_K / get_rays / get_ndc_rays_fx_fy (utils/ray_utils.py:98-164) as driven
-// by get_coords_from_camera (datasets/base.py:485-518).  One thread per pixel, rays written as [n, c_in] fp32.
-#include "hr_common.cuh"
+// Reference: get_coords_from_camera (datasets/base.py:485-518).  One thread per pixel, rays written as [n, c_in] fp32; the
+// per-pixel arithmetic is camera_ray (hr_rays.cuh).
+#include "hr_rays.cuh"
 
 namespace hr {
 
 __global__ void generate_rays_kernel(const __grid_constant__ hr_camera cam, int c_in, long long first, long long n,
-                                     float ndc_sx, float ndc_sy, float* __restrict__ out) {
+                                     NdcScale ndc, float* __restrict__ out) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const long long p = first + i;
-    const float px = (float)(p % cam.width), py = (float)(p / cam.width);
-    const float off = cam.centered_pixels ? 0.5f : 0.0f;
-    // get_ray_directions_from_pixels_K (ray_utils.py:98-115)
-    const float dcx = __fdiv_rn(__fadd_rn(__fsub_rn(px, cam.cx), off), cam.fx);
-    float dcy = __fdiv_rn(__fadd_rn(__fsub_rn(py, cam.cy), off), cam.fy);
-    if (!cam.flipped) dcy = -dcy;
-    const float dcz = -1.0f;
-    // get_rays (ray_utils.py:121-135): rays_d = directions @ c2w[:, :3].T ; rays_o = c2w[:, 3]
-    float d[3], o[3];
-#pragma unroll
-    for (int r = 0; r < 3; ++r) {
-      d[r] = fmaf(dcz, cam.c2w[r * 4 + 2], fmaf(dcy, cam.c2w[r * 4 + 1], __fmul_rn(dcx, cam.c2w[r * 4 + 0])));
-      o[r] = cam.c2w[r * 4 + 3];
-    }
-    if (cam.normalize) {
-      float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])), __fmul_rn(d[2], d[2])));
-      nrm = fmaxf(nrm, 1e-12f);
-#pragma unroll
-      for (int r = 0; r < 3; ++r) d[r] = __fdiv_rn(d[r], nrm);
-    }
-    if (cam.use_ndc) {
-      // get_ndc_rays_fx_fy (ray_utils.py:137-164); ndc_sx = -1/(W/(2 fx)), ndc_sy = -1/(H/(2 fy)) computed in fp32 on the host
-      const float t = __fdiv_rn(-__fadd_rn(cam.ndc_near, o[2]), d[2]);
-#pragma unroll
-      for (int r = 0; r < 3; ++r) o[r] = __fadd_rn(o[r], __fmul_rn(t, d[r]));
-      const float ox_oz = __fdiv_rn(o[0], o[2]), oy_oz = __fdiv_rn(o[1], o[2]);
-      const float o0 = __fmul_rn(ndc_sx, ox_oz);
-      const float o1 = __fmul_rn(ndc_sy, oy_oz);
-      const float o2 = __fadd_rn(1.0f, __fdiv_rn(__fmul_rn(2.0f, cam.ndc_near), o[2]));
-      const float d0 = __fmul_rn(ndc_sx, __fsub_rn(__fdiv_rn(d[0], d[2]), ox_oz));
-      const float d1 = __fmul_rn(ndc_sy, __fsub_rn(__fdiv_rn(d[1], d[2]), oy_oz));
-      const float d2 = __fsub_rn(1.0f, o2);
-      o[0] = o0; o[1] = o1; o[2] = o2;
-      d[0] = d0; d[1] = d1; d[2] = d2;
-    }
+    float row[8];
+    camera_ray(cam, (int)(p % cam.width), (int)(p / cam.width), ndc, row);
     float* r = out + i * c_in;
-    r[0] = o[0]; r[1] = o[1]; r[2] = o[2];
-    r[3] = d[0]; r[4] = d[1]; r[5] = d[2];
-    if (c_in >= 8) { r[6] = cam.cam_idx; r[7] = cam.time; }
+    r[0] = row[0]; r[1] = row[1]; r[2] = row[2];
+    r[3] = row[3]; r[4] = row[4]; r[5] = row[5];
+    if (c_in >= 8) { r[6] = row[6]; r[7] = row[7]; }
   }
 }
 
 cudaError_t launch_generate_rays(const hr_camera& cam, int c_in, long long first, long long n, float* out, cudaStream_t st) {
   if (n <= 0) return cudaSuccess;
-  // fp32 evaluation order of the reference: -1./(W/(2.*fx)) with fx an fp32 tensor element
-  const float sx = -1.0f / ((float)cam.width / (2.0f * cam.fx));
-  const float sy = -1.0f / ((float)cam.height / (2.0f * cam.fy));
   long long g = (n + 255) / 256;
   if (g > 148 * 16) g = 148 * 16;
-  generate_rays_kernel<<<(unsigned)g, 256, 0, st>>>(cam, c_in, first, n, sx, sy, out);
+  generate_rays_kernel<<<(unsigned)g, 256, 0, st>>>(cam, c_in, first, n, ndc_scale(cam), out);
   return cudaGetLastError();
 }
 

@@ -11,7 +11,7 @@ import os
 import subprocess
 import threading
 
-HR_ABI_VERSION = 14
+HR_ABI_VERSION = 15
 HR_MAX_GROUPS = 4
 HR_MAX_LAYERS = 10
 HR_MAX_SAMPLES = 256
@@ -152,6 +152,9 @@ EXPORTS = {
                                     C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]),
     "hr_render_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]),
     "hr_generate_rays": (C.c_int, [C.POINTER(hr_camera), C.c_int32, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
+    "hr_sample_train_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_uint64, C.c_int64,
+                                         C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.POINTER(C.c_int64), C.c_void_p]),
     "hr_render_to8b": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "hr_render_frame_to8b_host": (C.c_int, [C.c_void_p, C.POINTER(hr_camera), C.c_void_p, C.c_int64]),
     "hr_encode_rays": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define HR_ABI_VERSION 14
+#define HR_ABI_VERSION 15
 
 #define HR_MAX_GROUPS 4   /* ray-parameterisation groups feeding the sample net (ray.py:235-263) */
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
@@ -340,6 +340,27 @@ typedef struct hr_camera {
 /* rays_out [n_pixels, c_in] fp32 device, for pixels first_pixel .. first_pixel + n_pixels - 1; c_in is 6 or 8. */
 int hr_generate_rays(const hr_camera* cam, int32_t c_in, int64_t first_pixel, int64_t n_pixels, float* rays_out,
                      void* stream);
+
+/* ---- training batches from images on the device (SURVEY.md section 2 row 23) ----
+ * Replaces: the training split of the reference's datasets in its default mode (datasets/base.py:111-143,202-227,254-289): the
+ * host table all_inputs = cat([all_coords, all_rgb, all_weights]) of every training ray, re-permuted every epoch
+ * (np.random.permutation) and handed out in consecutive slices that format_batch splits and the loop copies to the GPU.
+ * Handle-free.  cameras: device array of n_views records, each of width `width` and height `height`; images: device uint8
+ * [n_views, height, width, 3].  Pixel p in [0, N), N = n_views*height*width, is view p / (height*width), then row-major within
+ * the view like hr_generate_rays.  Row r of the batch is pixel
+ *   order[r]                                        when order (device int64, batch_size entries) is given;
+ *   element batch_index*batch_size + r of epoch's permutation of [0, N), keyed by (seed, epoch)   otherwise
+ * (a Feistel network over the next power of two >= N with cycle-walking, so an epoch visits every pixel exactly once;
+ * csrc/hr_train_batch.cu states it).  Without order, batch_index must lie in [0, ceil(N / batch_size)) and the last batch of an
+ * epoch is short: *n_rows (host, may be NULL) receives the row count, batch_size or fewer.  Outputs (device, n_rows rows):
+ *   coords [n, c_in] fp32, bit-identical to the row hr_generate_rays writes for that pixel of that view's camera; c_in 6 or 8;
+ *   rgb [n, 3] fp32, u8 / 255 (T.ToTensor());  weight [n, 1] fp32, 1;  pixel_ids [n] int64 (may be NULL), the pixel of each row.
+ * An order entry outside [0, N) gives a zero row of weight 0 and pixel id -1.  coords, order and pixel_ids 8-byte aligned, the
+ * rest 4.  No float atomics, no host synchronisation: two calls with the same arguments write the same bits. */
+int hr_sample_train_batch(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height, int32_t width,
+                          int32_t c_in, uint64_t seed, int64_t epoch, int64_t batch_index, int64_t batch_size,
+                          const int64_t* order, float* coords, float* rgb, float* weight, int64_t* pixel_ids, int64_t* n_rows,
+                          void* stream);
 
 /* ---- the step after the path: 8-bit packing (SURVEY.md section 8(f) row f4) ----
  * Replaces: to8b(x) = (255 * clip(x, 0, 1)).astype(uint8) (utils/__init__.py:47) applied to the rendered frame before
