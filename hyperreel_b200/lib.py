@@ -11,7 +11,7 @@ import os
 import subprocess
 import threading
 
-HR_ABI_VERSION = 15
+HR_ABI_VERSION = 16
 HR_MAX_GROUPS = 4
 HR_MAX_LAYERS = 10
 HR_MAX_SAMPLES = 256
@@ -24,6 +24,7 @@ CONTRACT_NONE, CONTRACT_MIPNERF, CONTRACT_AFFINE = 0, 1, 2
 SHADE_SH, SHADE_RGB = 0, 1
 DENSE_RELU, DENSE_SOFTPLUS, DENSE_RELU_ABS = 0, 1, 2
 MLP_FP32_SIMT, MLP_BF16X3_TC, MLP_ZERO = 0, 1, 2
+SAMPLE_PERMUTE, SAMPLE_REPLACE = 0, 1  # hr_sample_train_rows modes
 # extra fields of the colour net (hr_render_fields): key of the reference's dict `x` -> HR_FIELD_* id
 FIELDS = {"points": 0, "distances": 1, "base_times": 2, "time_offset": 3, "times": 4, "viewdirs": 5, "weights": 6,
           "color_scale": 7, "color_shift": 8, "spatial_flow": 9, "sigma": 10, "point_sigma": 11, "point_offset": 12,
@@ -155,6 +156,9 @@ EXPORTS = {
     "hr_sample_train_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_uint64, C.c_int64,
                                          C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.POINTER(C.c_int64), C.c_void_p]),
+    "hr_sample_train_rows": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                        C.c_int64, C.c_int32, C.c_uint64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "hr_render_to8b": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "hr_render_frame_to8b_host": (C.c_int, [C.c_void_p, C.POINTER(hr_camera), C.c_void_p, C.c_int64]),
     "hr_encode_rays": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),

@@ -13,12 +13,17 @@ bit) and its colour ``u8 / 255`` (``T.ToTensor()``), weight 1.  ``INRSystem.trai
         batches.set_epoch(epoch)
         for batch in batches:
             system.training_step(batch)
+
+The shipped training configs train differently: they sample with replacement (``num_iters`` batches per epoch) from a table
+in which the video datasets keep only a per-frame subset of each view's pixels.  ``DeviceRayBatches.from_config`` reads both
+from a config, and ``hr_sample_train_rows`` (same file) generates those batches, again without any table in memory.
 """
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, Optional, Sequence
+from typing import Dict, List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from . import lib as L
@@ -43,6 +48,82 @@ def _as_image_stack(images) -> torch.Tensor:
     return images
 
 
+def regular_subsample_plan(frames: Sequence[int], *, load_full_step: int, subsample_keyframe_step: int,
+                           subsample_keyframe_frac: float, subsample_frac: float, counters: str = "technicolor",
+                           videos: Optional[Sequence[int]] = None) -> List[Tuple[int, int]]:
+    """The video datasets' per-frame pixel subsets as one ``(stride, offset)`` per training view, in the table's order: the
+    view keeps the pixels with ``(x + y + offset) % stride == 0`` (``stride == 1`` keeps every pixel).
+
+    ``frames[i]`` is view ``i``'s frame.  A frame with ``frame % load_full_step == 0`` is whole; otherwise one with ``frame %
+    subsample_keyframe_step == 0`` has stride ``round(1 / subsample_keyframe_frac)`` and every other frame ``round(1 /
+    subsample_frac)``; the offset is a running counter, one for each of the two kinds.  ``counters`` selects how they run:
+
+    * ``"technicolor"`` (datasets/technicolor.py:211-269): both start at 0 and advance over all views in order.
+    * ``"neural_3d"`` (datasets/neural_3d.py:168-185,217-269): ``videos[i]`` is view ``i``'s video index; views are video-major
+      with each video's frames consecutive.  Both counters restart at the video index, and each video's first view is whole
+      and advances neither.
+    """
+    frames = [int(f) for f in frames]
+    if any(f < 0 for f in frames):
+        raise ValueError("frames must be >= 0")
+    for name, step in (("load_full_step", load_full_step), ("subsample_keyframe_step", subsample_keyframe_step)):
+        if int(step) < 1:
+            raise ValueError(f"{name} must be >= 1, got {step}")
+    strides = {}
+    for name, frac in (("subsample_keyframe_frac", subsample_keyframe_frac), ("subsample_frac", subsample_frac)):
+        if not float(frac) > 0.0:
+            raise ValueError(f"{name} must be > 0, got {frac}")
+        strides[name] = int(round(1.0 / float(frac)))  # Python's round halves to even, as np.round does
+        if strides[name] < 1:
+            raise ValueError(f"{name}={frac} keeps more than every pixel (stride {strides[name]})")
+    if counters == "technicolor":
+        if videos is not None:
+            raise ValueError("videos is for counters='neural_3d'")
+        first_of_video = [False] * len(frames)
+        restart = [None] * len(frames)
+    elif counters == "neural_3d":
+        if videos is None or len(videos) != len(frames):
+            raise ValueError("counters='neural_3d' needs one video index per view")
+        videos = [int(v) for v in videos]
+        first_of_video = [i == 0 or videos[i] != videos[i - 1] for i in range(len(frames))]
+        seen = set()
+        for i, first in enumerate(first_of_video):
+            if first:
+                if videos[i] in seen:
+                    raise ValueError(f"views must be video-major: video {videos[i]} appears again at view {i}")
+                seen.add(videos[i])
+            elif frames[i] != frames[i - 1] + 1:
+                raise ValueError(f"views must be video-major with consecutive frames: view {i} has frame {frames[i]} "
+                                 f"after frame {frames[i - 1]}")
+        restart = [videos[i] if first else None for i, first in enumerate(first_of_video)]
+    else:
+        raise ValueError(f"counters must be 'technicolor' or 'neural_3d', got {counters!r}")
+    plan, key_offset, frame_offset = [], 0, 0
+    for i, f in enumerate(frames):
+        if restart[i] is not None:
+            key_offset = frame_offset = restart[i]
+        if first_of_video[i] or f % load_full_step == 0:
+            plan.append((1, 0))
+        elif f % subsample_keyframe_step == 0:
+            plan.append((strides["subsample_keyframe_frac"], key_offset))
+            key_offset += 1
+        else:
+            plan.append((strides["subsample_frac"], frame_offset))
+            frame_offset += 1
+    return plan
+
+
+def subset_rows(stride: int, offset: int, height: int, width: int) -> int:
+    """The number of pixels of an ``height x width`` view with ``(x + y + offset) % stride == 0``: every ``stride`` consecutive
+    rows hold ``width`` of them, and the rows past the last whole block are counted one by one."""
+    full = height // stride
+    n = full * width
+    for y in range(full * stride, height):
+        x0 = (stride - (y + offset) % stride) % stride
+        n += (width - 1 - x0) // stride + 1 if x0 < width else 0
+    return n
+
+
 class DeviceRayBatches:
     """Shuffled training batches ``{'coords' [B, c_in], 'rgb' [B, 3], 'weight' [B, 1]}`` (fp32, on the device) over every
     pixel of the training views, generated on the device per batch.
@@ -53,13 +134,24 @@ class DeviceRayBatches:
     is short, like the reference's last slice.  ``set_epoch(e)`` selects the order (0 at construction); ``len()`` is the
     number of batches per epoch and iterating yields them in turn.
 
+    Two options reproduce what the shipped training configs train on (``from_config`` sets both from a config):
+
+    * ``subsample``: one ``(stride, offset)`` per view (``regular_subsample_plan``).  The training table then holds, view by
+      view, only the pixels with ``(x + y + offset) % stride == 0``, each view's in row-major order: the order of the video
+      datasets' ``all_coords``.  ``n_rows`` is the table's size (``n*H*W`` without a plan); ``gather_rows`` returns rows by
+      table index.
+    * ``replacement=True`` with ``num_iters``: every batch is ``batch_size`` independent uniform draws from the table, keyed
+      by ``(seed, epoch, position)``, and an epoch is ``num_iters`` batches, as the reference's
+      ``RandomSampler(replacement=True, num_samples=num_iters * batch_size)`` (nlf/__init__.py:222-237).
+
     Only the reference's default training mode is provided.  The dataset options of the others (datasets/base.py:85-101)
     are accepted under the reference's names so that they can be refused: ``use_patches``, ``precrop_iters`` > 0 (crop),
     ``use_full_image`` and ``blur_radius`` > 0 raise ``ValueError``, as do views of different sizes and non-uint8 images."""
 
     def __init__(self, cameras: Sequence[Camera], images, batch_size: int, seed: int = 0, c_in: int = 8,
                  device: Optional[torch.device] = None, *, use_patches: bool = False, precrop_iters: int = 0,
-                 use_full_image: bool = False, blur_radius: int = 0):
+                 use_full_image: bool = False, blur_radius: int = 0, replacement: bool = False,
+                 num_iters: Optional[int] = None, subsample: Optional[Sequence[Tuple[int, int]]] = None):
         for name, value, default in (("use_patches", use_patches, False), ("precrop_iters", precrop_iters, 0),
                                      ("use_full_image", use_full_image, False), ("blur_radius", blur_radius, 0)):
             if value != default:
@@ -82,6 +174,24 @@ class DeviceRayBatches:
             if (int(cam.width), int(cam.height)) != (W, H):
                 raise ValueError(f"camera {i} is {cam.width}x{cam.height}, the images are {W}x{H}: every view needs the "
                                  "camera grid's size")
+        if replacement:
+            if num_iters is None or int(num_iters) < 1:
+                raise ValueError(f"replacement=True needs num_iters >= 1 (batches per epoch), got {num_iters!r}")
+        elif num_iters is not None:
+            raise ValueError("num_iters sets the epoch length of replacement=True; without replacement an epoch is "
+                             "ceil(n_rows / batch_size) batches")
+        if subsample is None:
+            rule = [(1, 0)] * n
+        else:
+            rule = [tuple(r) for r in subsample]
+            if len(rule) != n or any(len(r) != 2 for r in rule):
+                raise ValueError(f"subsample needs one (stride, offset) per view: {len(rule)} entries for {n} views")
+            if any(int(s) != s or int(o) != o or not 1 <= int(s) < 2 ** 31 for s, o in rule):
+                raise ValueError("subsample strides must be integers in [1, 2^31) and offsets integers")
+            rule = [(int(s), int(o) % int(s)) for s, o in rule]
+        counts = [subset_rows(s, o, H, W) for s, o in rule]
+        if sum(counts) < 1:
+            raise ValueError("subsample keeps no pixel: the training table is empty")
         if not torch.cuda.is_available():
             raise RuntimeError("hyperreel_b200.DeviceRayBatches needs a CUDA device (no CPU fallback)")
         if device is None:
@@ -97,40 +207,146 @@ class DeviceRayBatches:
         self.seed = int(seed) & ((1 << 64) - 1)
         self.c_in = int(c_in)
         self.epoch = 0
+        self.replacement = bool(replacement)
+        self.num_iters = int(num_iters) if replacement else None
+        self.subsample = None if subsample is None else rule
+        self.n_rows = int(sum(counts))
+        # the table's plan for hr_sample_train_rows: exclusive prefix of the per-view row counts, and (stride, offset) per view
+        self._view_start = torch.tensor(np.concatenate([[0], np.cumsum(counts)]), dtype=torch.int64, device=self.device)
+        self._view_rule = torch.tensor(rule, dtype=torch.int32, device=self.device).contiguous()
+        # the original path (every pixel, each once per epoch) keeps its own kernel
+        self._table_path = self.replacement or self.subsample is not None
+
+    @classmethod
+    def from_config(cls, cfg, cameras: Sequence[Camera], images, seed: int = 0, c_in: int = 8,
+                    device: Optional[torch.device] = None) -> "DeviceRayBatches":
+        """The training batches a reference config trains on: ``cfg.training.batch_size``, ``sample_with_replacement`` and
+        ``num_iters``, and for the ``technicolor`` and ``neural_3d`` datasets the per-frame pixel subsets of
+        ``cfg.dataset.{num_frames, load_full_step, subsample_keyframe_step, subsample_keyframe_frac, subsample_frac}``.
+
+        ``cameras`` and ``images`` must be the training views in the reference's training order: frame-major with the
+        held-out views removed for technicolor, video-major (each video's frames in order) for neural_3d.  A view's frame is
+        ``int(np.round(time * (num_frames - 1)))`` of its ``Camera.time``; for neural_3d each run of equal ``cam_idx`` is one
+        video, numbered 0, 1, ... in order (the reference numbers videos after removing the held-out one).  The ``immersive``
+        dataset's content-dependent ``importance_subsample``, and any other dataset that sets subsample keys, raise
+        ``ValueError``.
+
+        With replacement the reference runs with ``iters_per_epoch = num_iters`` (main.py:100-101), and its epoch-based
+        schedules are scaled by that value: an ``INRSystem`` built from the same config must be given
+        ``training.iters_per_epoch = num_iters``."""
+        training, dataset = cfg["training"], cfg["dataset"]
+        replacement = bool(training.get("sample_with_replacement", False))
+        num_iters = int(training["num_iters"]) if replacement else None
+        name = dataset.get("name", None)
+        keys = ("load_full_step", "subsample_keyframe_step", "subsample_keyframe_frac", "subsample_frac")
+        cameras = list(cameras)
+        subsample = None
+        if name in ("technicolor", "neural_3d"):
+            num_frames = int(dataset.get("num_frames", 1))
+            frames = [int(np.round(float(cam.time) * (num_frames - 1))) for cam in cameras]
+            videos = None
+            if name == "neural_3d":
+                videos, seen = [], set()
+                for i, cam in enumerate(cameras):
+                    if i == 0 or cam.cam_idx != cameras[i - 1].cam_idx:
+                        if cam.cam_idx in seen:
+                            raise ValueError(f"neural_3d views must be video-major: cam_idx {cam.cam_idx} appears again at "
+                                             f"view {i}")
+                        seen.add(cam.cam_idx)
+                    videos.append(len(seen) - 1)
+            subsample = regular_subsample_plan(
+                frames, load_full_step=dataset.get("load_full_step", 1),
+                subsample_keyframe_step=dataset.get("subsample_keyframe_step", 1),
+                subsample_keyframe_frac=dataset.get("subsample_keyframe_frac", 1.0),
+                subsample_frac=dataset.get("subsample_frac", 1.0), counters=name, videos=videos)
+        elif name == "immersive":
+            raise ValueError("the immersive dataset's importance_subsample depends on the images' content and is not "
+                             "supported")
+        elif any(k in dataset for k in keys):
+            raise ValueError(f"dataset {name!r} sets {[k for k in keys if k in dataset]}: only technicolor's and neural_3d's "
+                             "regular subsets are supported")
+        return cls(cameras, images, batch_size=int(training["batch_size"]), seed=seed, c_in=c_in, device=device,
+                   replacement=replacement, num_iters=num_iters, subsample=subsample)
 
     def __len__(self) -> int:
-        return -(-self.n_pixels // self.batch_size)
+        if self.replacement:
+            return self.num_iters
+        return -(-self.n_rows // self.batch_size)
 
     def set_epoch(self, epoch: int) -> None:
         self.epoch = int(epoch)
 
-    def batch(self, i: int, with_pixel_ids: bool = False) -> Dict[str, torch.Tensor]:
+    def batch(self, i: int, with_pixel_ids: bool = False, with_table_ids: bool = False) -> Dict[str, torch.Tensor]:
         """Batch ``i`` of the current epoch (``0 <= i < len(self)``).  ``with_pixel_ids=True`` adds ``'pixel_ids'`` [B] int64, the
-        pixel of each row (``view*H*W + y*W + x``), for callers that keep per-pixel state."""
+        pixel of each row (``view*H*W + y*W + x``), for callers that keep per-pixel state; ``with_table_ids=True`` adds
+        ``'table_ids'`` [B] int64, the training-table row of each row."""
         i = int(i)
         if not 0 <= i < len(self):
             raise IndexError(f"batch {i} outside [0, {len(self)})")
-        rows = min(self.batch_size, self.n_pixels - i * self.batch_size)
-        return self._launch(rows, i, None, with_pixel_ids)
+        if not self._table_path:
+            rows = min(self.batch_size, self.n_pixels - i * self.batch_size)
+            out = self._launch(rows, i, None, with_pixel_ids or with_table_ids)
+            if with_table_ids:  # without a plan the table is every pixel in order
+                out["table_ids"] = out["pixel_ids"].clone() if with_pixel_ids else out.pop("pixel_ids")
+            return out
+        rows = self.batch_size if self.replacement else min(self.batch_size, self.n_rows - i * self.batch_size)
+        return self._launch_rows(rows, i, None, with_pixel_ids, with_table_ids)
+
+    def gather_rows(self, table_ids, with_pixel_ids: bool = False) -> Dict[str, torch.Tensor]:
+        """The rows of the given training-table indices, in the given order, the table in the reference's ``all_coords``
+        order (views in order, each view's kept pixels row-major): for replaying the reference's own sampler indices.  An
+        index outside ``[0, n_rows)`` raises ``ValueError`` (for device indices the check synchronises with the device)."""
+        ids = self._check_ids(table_ids, self.n_rows, "table ids")
+        return self._launch_rows(ids.numel(), 0, ids, with_pixel_ids, False)
 
     def gather(self, pixel_ids, with_pixel_ids: bool = False) -> Dict[str, torch.Tensor]:
         """The rows of the given pixels, in the given order: for callers that bring their own order (the reference's
         ``np.random.permutation``, say).  An id outside ``[0, n*H*W)`` raises ``ValueError`` (for device ids the check
         synchronises with the device)."""
-        ids = torch.as_tensor(pixel_ids)
-        if ids.dim() != 1 or ids.numel() < 1:
-            raise ValueError(f"pixel_ids must be a non-empty 1-D tensor, got shape {tuple(ids.shape)}")
-        if ids.dtype.is_floating_point or ids.dtype == torch.bool or ids.is_complex():
-            raise ValueError(f"pixel_ids must be integers, got {ids.dtype}")
-        lo, hi = int(ids.min()), int(ids.max())
-        if lo < 0 or hi >= self.n_pixels:
-            raise ValueError(f"pixel ids must lie in [0, {self.n_pixels}), got [{lo}, {hi}]")
-        ids = ids.to(device=self.device, dtype=torch.int64).contiguous()
+        ids = self._check_ids(pixel_ids, self.n_pixels, "pixel ids")
         return self._launch(ids.numel(), 0, ids, with_pixel_ids)
 
     def __iter__(self):
         for i in range(len(self)):
             yield self.batch(i)
+
+    def _check_ids(self, ids, n: int, what: str) -> torch.Tensor:
+        ids = torch.as_tensor(ids)
+        name = what.replace(" ", "_")
+        if ids.dim() != 1 or ids.numel() < 1:
+            raise ValueError(f"{name} must be a non-empty 1-D tensor, got shape {tuple(ids.shape)}")
+        if ids.dtype.is_floating_point or ids.dtype == torch.bool or ids.is_complex():
+            raise ValueError(f"{name} must be integers, got {ids.dtype}")
+        lo, hi = int(ids.min()), int(ids.max())
+        if lo < 0 or hi >= n:
+            raise ValueError(f"{what} must lie in [0, {n}), got [{lo}, {hi}]")
+        return ids.to(device=self.device, dtype=torch.int64).contiguous()
+
+    def _launch_rows(self, rows: int, index: int, table_rows: Optional[torch.Tensor], with_pixel_ids: bool,
+                     with_table_ids: bool) -> Dict[str, torch.Tensor]:
+        dev = self.device
+        coords = torch.empty((rows, self.c_in), dtype=torch.float32, device=dev)
+        rgb = torch.empty((rows, 3), dtype=torch.float32, device=dev)
+        weight = torch.empty((rows, 1), dtype=torch.float32, device=dev)
+        pids = torch.empty((rows,), dtype=torch.int64, device=dev) if with_pixel_ids else None
+        tids = torch.empty((rows,), dtype=torch.int64, device=dev) if with_table_ids else None
+        n_rows = C.c_int64(0)
+        mode = L.SAMPLE_REPLACE if self.replacement else L.SAMPLE_PERMUTE
+        with torch.cuda.device(dev):
+            L.check(self._lib.hr_sample_train_rows(
+                self.cameras.data_ptr(), self.n_views, self.images.data_ptr(), self.height, self.width, self.c_in,
+                self._view_start.data_ptr(), self._view_rule.data_ptr(), self.n_rows, mode, self.seed, self.epoch, index,
+                rows if table_rows is not None else self.batch_size,
+                table_rows.data_ptr() if table_rows is not None else None, coords.data_ptr(), rgb.data_ptr(),
+                weight.data_ptr(), pids.data_ptr() if pids is not None else None,
+                tids.data_ptr() if tids is not None else None, C.byref(n_rows), torch.cuda.current_stream(dev).cuda_stream))
+        assert n_rows.value == rows, (n_rows.value, rows)
+        out = {"coords": coords, "rgb": rgb, "weight": weight}
+        if pids is not None:
+            out["pixel_ids"] = pids
+        if tids is not None:
+            out["table_ids"] = tids
+        return out
 
     def _launch(self, rows: int, index: int, order: Optional[torch.Tensor], with_ids: bool) -> Dict[str, torch.Tensor]:
         dev = self.device

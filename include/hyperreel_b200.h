@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define HR_ABI_VERSION 15
+#define HR_ABI_VERSION 16
 
 #define HR_MAX_GROUPS 4   /* ray-parameterisation groups feeding the sample net (ray.py:235-263) */
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
@@ -361,6 +361,32 @@ int hr_sample_train_batch(const hr_camera* cameras, int32_t n_views, const uint8
                           int32_t c_in, uint64_t seed, int64_t epoch, int64_t batch_index, int64_t batch_size,
                           const int64_t* order, float* coords, float* rgb, float* weight, int64_t* pixel_ids, int64_t* n_rows,
                           void* stream);
+
+/* Training batches over a table of per-view pixel subsets, drawn with or without replacement.
+ * Replaces: the training split of the video datasets (datasets/technicolor.py:211-269, datasets/neural_3d.py:168-185,217-269),
+ * which keep per view only the pixels with (x + y + offset) % stride == 0, sampled as the shipped training configs do
+ * (sample_with_replacement: RandomSampler(replacement=True, num_samples=num_iters * batch_size), nlf/__init__.py:222-237).
+ * cameras, images, n_views, height, width, c_in: as hr_sample_train_batch.  The table is implicit: view_start (device int64
+ * [n_views + 1]) is the exclusive prefix of the per-view row counts and view_rule (device int32 [n_views, 2]) each view's
+ * (stride >= 1, offset); table row k is in view v with view_start[v] <= k < view_start[v + 1], at rank k - view_start[v] of that
+ * view's kept pixels in row-major order (the reference's all_coords order).  Row r of the batch is table row
+ *   table_rows[r]                                       when table_rows (device int64, batch_size entries) is given;
+ *   element batch_index*batch_size + r of epoch's permutation of [0, n_table)   when mode == HR_SAMPLE_PERMUTE
+ *     (hr_sample_train_batch's permutation; batch_index in [0, ceil(n_table / batch_size)), the last batch short);
+ *   an independent uniform draw from [0, n_table), keyed by (seed, epoch, batch_index*batch_size + r)
+ *                                                       when mode == HR_SAMPLE_REPLACE (every batch full, batch_index >= 0).
+ * n_table lies in [1, n_views*height*width] and is view_start[n_views] for a well-formed plan.  Outputs: coords, rgb, weight as
+ * hr_sample_train_batch; pixel_ids [n] (may be NULL) view*H*W + y*W + x; table_ids [n] (may be NULL) the table row.  A row
+ * the plan does not hold (a table_rows entry outside [0, n_table), a malformed plan) gives a zero row of weight 0 and ids -1,
+ * and nothing outside the arrays is read or written.  coords, view_start and the int64 arrays 8-byte aligned, the rest 4.  No
+ * float atomics, no host synchronisation: two calls with the same arguments write the same bits. */
+#define HR_SAMPLE_PERMUTE 0
+#define HR_SAMPLE_REPLACE 1
+int hr_sample_train_rows(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height, int32_t width,
+                         int32_t c_in, const int64_t* view_start, const int32_t* view_rule, int64_t n_table, int32_t mode,
+                         uint64_t seed, int64_t epoch, int64_t batch_index, int64_t batch_size, const int64_t* table_rows,
+                         float* coords, float* rgb, float* weight, int64_t* pixel_ids, int64_t* table_ids, int64_t* n_rows,
+                         void* stream);
 
 /* ---- the step after the path: 8-bit packing (SURVEY.md section 8(f) row f4) ----
  * Replaces: to8b(x) = (255 * clip(x, 0, 1)).astype(uint8) (utils/__init__.py:47) applied to the rendered frame before
