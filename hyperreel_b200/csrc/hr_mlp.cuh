@@ -35,7 +35,8 @@ struct TcPass {
   int wait_a;       // the issuer must wait for the A chunks (first pass of a layer)
 };
 struct MlpTcPack {
-  const void* wpack;   // bf16 hi/lo weight images, K-major no-swizzle layout, consumption order
+  const void* wpack;   // bf16 hi/lo weight images, K-major no-swizzle layout, consumption order: columns [0, W/2) of
+                       // every pass, then columns [W/2, W) (wpack_bytes / 2 each)
   const float* bias;   // [bias_count]
   long long wpack_bytes;
   int n_passes;

@@ -4,7 +4,8 @@
 // hi = rn(w), lo = rn(w - hi) and laid out the way wgmma reads its B operand from shared memory: K-major,
 // no swizzle, core matrices of 8 rows x 16 bytes (LBO = N * 16 B between the two 8-wide k-groups of a 16-wide k-step,
 // SBO = 128 B between 8-row groups).  One image = one k-step of one pass = N x 16 bf16 hi followed by N x 16 bf16 lo;
-// images are concatenated in consumption order so the producer warp streams them with cp.async.bulk.
+// images are concatenated in consumption order so a producer warp streams them with cp.async.bulk (pack_mlp_tc2 packs
+// each column half of a pass as a pass of its own, one stream per half).
 #include <cuda_bf16.h>
 
 #include "hr_tc_prims.cuh"
