@@ -1,15 +1,17 @@
 """Camera -> rays on the device, and whole-frame rendering to 8-bit pixels (SURVEY.md section 8(f) rows f2 and f4).
 
 Mirrors ``get_coords_from_camera`` of the reference datasets (datasets/base.py:485-518: pixel grid ->
-``get_ray_directions_K`` -> ``get_rays`` -> optional ``to_ndc`` -> append camera id and time) and ``to8b``
+``get_ray_directions_K`` -> ``get_rays`` -> optional ``to_ndc`` -> append camera id and time), the fisheye cameras of
+``ImmersiveDataset.get_coords`` (``Camera(distortion=(k1, k2))``, datasets/immersive.py:494-573) and ``to8b``
 (utils/__init__.py:47).  The reference builds the rays on the CPU and uploads 32 B per ray for every frame
 (nlf/__init__.py:828-834); here only the pose and intrinsics cross PCIe and 3 B per pixel come back.
 """
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Optional, Sequence
+from typing import Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from . import lib as L
@@ -28,6 +30,25 @@ class Camera:
     normalize: bool = True
     use_ndc: bool = False
     ndc_near: float = 1.0
+    # (k1, k2): the Immersive dataset's fisheye camera (ImmersiveDataset.get_coords, datasets/immersive.py:494-573), the
+    # first two radial_distortion coefficients of models.json, rounded to float32 as the reference's .astype(np.float32).
+    # None is the pinhole.  (0, 0) is not: the fisheye model maps the radius r -> tan(r).
+    distortion: Optional[Sequence[float]] = None
+
+    def __post_init__(self):
+        self._distortion_f32()
+
+    def _distortion_f32(self) -> Optional[Tuple[float, float]]:
+        if self.distortion is None:
+            return None
+        d = np.asarray(self.distortion, dtype=np.float64).reshape(-1)
+        if d.shape != (2,):
+            raise ValueError(f"distortion must be (k1, k2), got {self.distortion!r}")
+        with np.errstate(over="ignore"):
+            k = d.astype(np.float32)
+        if not np.isfinite(k).all():
+            raise ValueError(f"distortion coefficients must be finite in float32, got {self.distortion!r}")
+        return float(k[0]), float(k[1])
 
     def to_c(self) -> L.hr_camera:
         c = L.hr_camera()
@@ -41,6 +62,9 @@ class Camera:
         c.centered_pixels, c.flipped = int(self.centered_pixels), int(self.flipped)
         c.normalize, c.use_ndc = int(self.normalize), int(self.use_ndc)
         c.ndc_near, c.cam_idx, c.time = float(self.ndc_near), float(self.cam_idx), float(self.time)
+        k = self._distortion_f32()
+        if k is not None:
+            c.fisheye, (c.k1, c.k2) = 1, k
         return c
 
 

@@ -837,10 +837,14 @@ int hr_render_to8b(hr_handle* h, const float* rays, int64_t n_rays, uint8_t* rgb
   return render_impl(h, rays, n_rays, nullptr, nullptr, nullptr, workspace, workspace_bytes, (cudaStream_t)stream, rgb8);
 }
 
+// A fisheye record needs finite coefficients: the Newton solve of camera_ray has no meaning otherwise.
+static bool bad_fisheye(const hr_camera& cam) { return cam.fisheye && !(std::isfinite(cam.k1) && std::isfinite(cam.k2)); }
+
 int hr_generate_rays(const hr_camera* cam, int32_t c_in, int64_t first_pixel, int64_t n_pixels, float* rays_out, void* stream) {
   if (!cam || !rays_out) return fail("hr_generate_rays: null argument");
   if (c_in != 6 && c_in != 8) return fail("hr_generate_rays: c_in must be 6 or 8");
   if (cam->width < 1 || cam->height < 1) return fail("hr_generate_rays: bad image size");
+  if (bad_fisheye(*cam)) return fail("hr_generate_rays: fisheye coefficients k1 = %g, k2 = %g are not finite", cam->k1, cam->k2);
   if (first_pixel < 0 || n_pixels < 0 || first_pixel + n_pixels > (int64_t)cam->width * cam->height)
     return fail("hr_generate_rays: pixel range outside the image");
   cudaError_t e = hr::launch_generate_rays(*cam, c_in, first_pixel, n_pixels, rays_out, (cudaStream_t)stream);
@@ -851,6 +855,8 @@ int hr_generate_rays(const hr_camera* cam, int32_t c_in, int64_t first_pixel, in
 int hr_render_frame_to8b_host(hr_handle* h, const hr_camera* cam, uint8_t* rgb8_host, int64_t chunk) {
   if (!h || !cam || !rgb8_host) return fail("hr_render_frame_to8b_host: null argument");
   if (!h->uploaded) return fail("hr_render_frame_to8b_host: parameters not uploaded");
+  if (bad_fisheye(*cam))
+    return fail("hr_render_frame_to8b_host: fisheye coefficients k1 = %g, k2 = %g are not finite", cam->k1, cam->k2);
   DeviceGuard guard(h->device);
   const hr_config& c = h->cfg;
   const int64_t n_rays = (int64_t)cam->width * cam->height;

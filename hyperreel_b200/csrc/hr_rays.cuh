@@ -1,7 +1,8 @@
-// Camera -> ray arithmetic, one definition shared by generate_rays_kernel (hr_rays.cu) and the training-batch kernel
+// Camera -> ray arithmetic, one definition shared by generate_rays_kernel (hr_rays.cu) and the training-batch kernels
 // (hr_train_batch.cu): a training row must be bit-identical to the row hr_generate_rays writes for the same pixel.
 // Reference: get_ray_directions_from_pixels_K / get_rays / get_ndc_rays_fx_fy (utils/ray_utils.py:98-164) as driven by
-// get_coords_from_camera (datasets/base.py:485-518).
+// get_coords_from_camera (datasets/base.py:485-518), and for fisheye cameras ImmersiveDataset.get_coords
+// (datasets/immersive.py:494-573).
 #pragma once
 #include "hr_common.cuh"
 
@@ -17,16 +18,65 @@ __host__ __device__ inline NdcScale ndc_scale(const hr_camera& cam) {
   return {-1.0f / ((float)cam.width / (2.0f * cam.fx)), -1.0f / ((float)cam.height / (2.0f * cam.fy))};
 }
 
+// The fisheye camera's direction for the pinhole direction (x, y, -1) (ImmersiveDataset.get_coords,
+// datasets/immersive.py:514-551): cv::fisheye::undistortPoints of OpenCV 4.x with K = I, D = (k1, k2, 0, 0), no R or P and
+// the default criteria (COUNT + EPS, 10 iterations, 1e-8), restated in fp64 in OpenCV's operation order with non-contracting
+// intrinsics, so that only tan (CUDA's, <= 2 ulp) can differ from the host library, and only below fp32 resolution.  The
+// zero k3, k4 terms are left out: they change nothing unless |theta| passes ~1e38, from which ten Newton steps cannot
+// converge either way.  Then F.normalize of (u, v, -1) in fp32.
+__device__ __forceinline__ float3 fisheye_direction(float xf, float yf, float k1f, float k2f) {
+  const double x = xf, y = yf, k1 = k1f, k2 = k2f;
+  constexpr double kHalfPi = 3.14159265358979323846 / 2.0;
+  // the model holds up to 180 degrees of field of view: OpenCV clamps theta_d to [-pi/2, pi/2]
+  const double theta_d = fmin(fmax(-kHalfPi, __dsqrt_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)))), kHalfPi);
+  double theta = theta_d, scale = 0.0;
+  bool converged = false;
+  if (fabs(theta_d) > 1e-8) {
+    for (int j = 0; j < 10; ++j) {  // Newton on theta * (1 + k1 theta^2 + k2 theta^4) = theta_d
+      const double t2 = __dmul_rn(theta, theta), t4 = __dmul_rn(t2, t2);
+      const double a = __dmul_rn(k1, t2), b = __dmul_rn(k2, t4);
+      const double fix = __ddiv_rn(__dsub_rn(__dmul_rn(theta, __dadd_rn(__dadd_rn(1.0, a), b)), theta_d),
+                                   __dadd_rn(__dadd_rn(1.0, __dmul_rn(3.0, a)), __dmul_rn(5.0, b)));
+      theta = __dsub_rn(theta, fix);
+      if (fabs(fix) < 1e-8) {
+        converged = true;
+        break;
+      }
+    }
+    scale = __ddiv_rn(tan(theta), theta_d);
+  } else {
+    converged = true;  // the principal point: scale 0
+  }
+  const bool flipped = (theta_d < 0.0 && theta > 0.0) || (theta_d > 0.0 && theta < 0.0);
+  float u = -1000000.0f, v = -1000000.0f;  // OpenCV's value for a point it cannot undistort
+  if (converged && !flipped) {
+    u = __double2float_rn(__dmul_rn(x, scale));
+    v = __double2float_rn(__dmul_rn(y, scale));
+  }
+  float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(u, u), __fmul_rn(v, v)), 1.0f));
+  nrm = fmaxf(nrm, 1e-12f);
+  return make_float3(__fdiv_rn(u, nrm), __fdiv_rn(v, nrm), __fdiv_rn(-1.0f, nrm));
+}
+
 // The ray of pixel (x, y) as the reference's coords row: origin, direction, then cam_idx and time (channels 6 and 7 when
-// c_in == 8, technicolor.py:389-393).
+// c_in == 8, technicolor.py:389-393).  kFisheye: records with cam.fisheye set take the fisheye direction (fisheye_direction);
+// without it every record is a pinhole.  The fp64 solve costs registers (DESIGN 4.4), out of line as well: a call keeps the
+// caller's live values and the callee's in one budget.  So generate_rays_kernel, whose one record the host reads, has a
+// pinhole instantiation with the pinhole path's registers; the training kernels read their records on the device and
+// always branch on the flag.
+template <bool kFisheye>
 __device__ __forceinline__ void camera_ray(const hr_camera& cam, int x, int y, NdcScale ndc, float (&row)[8]) {
   const float px = (float)x, py = (float)y;
   const float off = cam.centered_pixels ? 0.5f : 0.0f;
   // get_ray_directions_from_pixels_K (ray_utils.py:98-115)
-  const float dcx = __fdiv_rn(__fadd_rn(__fsub_rn(px, cam.cx), off), cam.fx);
+  float dcx = __fdiv_rn(__fadd_rn(__fsub_rn(px, cam.cx), off), cam.fx);
   float dcy = __fdiv_rn(__fadd_rn(__fsub_rn(py, cam.cy), off), cam.fy);
   if (!cam.flipped) dcy = -dcy;
-  const float dcz = -1.0f;
+  float dcz = -1.0f;
+  if (kFisheye && cam.fisheye) {
+    const float3 f = fisheye_direction(dcx, dcy, cam.k1, cam.k2);
+    dcx = f.x; dcy = f.y; dcz = f.z;
+  }
   // get_rays (ray_utils.py:121-135): rays_d = directions @ c2w[:, :3].T ; rays_o = c2w[:, 3]
   float d[3], o[3];
 #pragma unroll

@@ -14,7 +14,8 @@
 // uint64 arithmetic modulo 2^64.  tests/train_order_oracle.py restates it in NumPy.
 //
 // One thread per row: one 3-byte gather and one 48-byte row write (plus 8 B of pixel id when asked).  No float atomics, no
-// host synchronisation; two calls with the same arguments write the same bits.
+// host synchronisation; two calls with the same arguments write the same bits.  The camera records live on the device, so
+// each row branches on its own record's fisheye flag (camera_ray<true>) and one batch may mix fisheye and pinhole views.
 #include "hr_handle.h"
 #include "hr_rays.cuh"
 
@@ -78,7 +79,7 @@ train_batch_kernel(const hr_camera* __restrict__ cams, const uint8_t* __restrict
       const long long q = p - v * hw;
       const int y = (int)(q / width), x = (int)(q - (long long)y * width);
       const hr_camera& cam = cams[v];
-      camera_ray(cam, x, y, ndc_scale(cam), row);
+      camera_ray<true>(cam, x, y, ndc_scale(cam), row);
       const uint8_t* px = images + 3 * p;
       c0 = __fdiv_rn((float)px[0], 255.0f);
       c1 = __fdiv_rn((float)px[1], 255.0f);
@@ -198,7 +199,7 @@ train_rows_kernel(const hr_camera* __restrict__ cams, const uint8_t* __restrict_
     if (table_pixel(plan, start, height, width, k, v, y, x)) {
       p = v * hw + (long long)y * width + x;
       const hr_camera& cam = cams[v];
-      camera_ray(cam, x, y, ndc_scale(cam), row);
+      camera_ray<true>(cam, x, y, ndc_scale(cam), row);
       const uint8_t* px = images + 3 * p;
       c0 = __fdiv_rn((float)px[0], 255.0f);
       c1 = __fdiv_rn((float)px[1], 255.0f);

@@ -11,7 +11,7 @@ import os
 import subprocess
 import threading
 
-HR_ABI_VERSION = 16
+HR_ABI_VERSION = 17
 HR_MAX_GROUPS = 4
 HR_MAX_LAYERS = 10
 HR_MAX_SAMPLES = 256
@@ -131,7 +131,7 @@ class hr_camera(C.Structure):
         ("c2w", C.c_float * 12), ("fx", C.c_float), ("fy", C.c_float), ("cx", C.c_float), ("cy", C.c_float),
         ("width", C.c_int32), ("height", C.c_int32), ("centered_pixels", C.c_int32), ("flipped", C.c_int32),
         ("normalize", C.c_int32), ("use_ndc", C.c_int32), ("ndc_near", C.c_float), ("cam_idx", C.c_float),
-        ("time", C.c_float),
+        ("time", C.c_float), ("fisheye", C.c_int32), ("k1", C.c_float), ("k2", C.c_float),
     ]
 
 

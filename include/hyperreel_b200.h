@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define HR_ABI_VERSION 16
+#define HR_ABI_VERSION 17
 
 #define HR_MAX_GROUPS 4   /* ray-parameterisation groups feeding the sample net (ray.py:235-263) */
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
@@ -335,7 +335,17 @@ typedef struct hr_camera {
   int32_t use_ndc;          /* get_ndc_rays_fx_fy (ray_utils.py:137-164) with H, W, fx, fy of this camera */
   float ndc_near;           /* dataset.near                                                         */
   float cam_idx, time;      /* channels 6 and 7 when c_in == 8 (technicolor.py:389-393)             */
+  int32_t fisheye;          /* 0: pinhole; otherwise the two-coefficient fisheye below (ABI 17)     */
+  float k1, k2;             /* radial_distortion[:2] of the camera in models.json, as float32       */
 } hr_camera;
+/* Fisheye cameras (ABI 17): the Immersive dataset's train and validation views (ImmersiveDataset.get_coords,
+ * datasets/immersive.py:494-573).  When fisheye != 0 the pinhole direction's (x, y) -- centred pixels, y negated unless
+ * flipped -- is undistorted as cv2.fisheye.undistortPoints(points, I, [k1, k2, 0, 0]) does (perspective_to_fisheye, :43-48),
+ * the direction (u, v, -1) is normalised (F.normalize), then get_rays / NDC / cam_idx / time follow as for the pinhole.  A
+ * point the solve does not bring back (no convergence in 10 Newton steps, or a flipped angle) becomes OpenCV's (-1e6, -1e6)
+ * and its row is written like any other, as the reference does.  k1 = k2 = 0 is not the pinhole (the radius maps
+ * r -> tan r), hence the flag.  k1 and k2 must be finite: hr_generate_rays and hr_render_frame_to8b_host refuse a fisheye
+ * record otherwise and write nothing.  The render split's cameras (K * 0.75, no distortion) are pinholes. */
 
 /* rays_out [n_pixels, c_in] fp32 device, for pixels first_pixel .. first_pixel + n_pixels - 1; c_in is 6 or 8. */
 int hr_generate_rays(const hr_camera* cam, int32_t c_in, int64_t first_pixel, int64_t n_pixels, float* rays_out,
@@ -356,7 +366,9 @@ int hr_generate_rays(const hr_camera* cam, int32_t c_in, int64_t first_pixel, in
  *   coords [n, c_in] fp32, bit-identical to the row hr_generate_rays writes for that pixel of that view's camera; c_in 6 or 8;
  *   rgb [n, 3] fp32, u8 / 255 (T.ToTensor());  weight [n, 1] fp32, 1;  pixel_ids [n] int64 (may be NULL), the pixel of each row.
  * An order entry outside [0, N) gives a zero row of weight 0 and pixel id -1.  coords, order and pixel_ids 8-byte aligned, the
- * rest 4.  No float atomics, no host synchronisation: two calls with the same arguments write the same bits. */
+ * rest 4.  No float atomics, no host synchronisation: two calls with the same arguments write the same bits.
+ * Each row takes its view's camera model (ABI 17: a fisheye record's rays as hr_generate_rays writes them), so one batch may
+ * mix fisheye and pinhole views; the records' fisheye coefficients must be finite (the device array is not inspected). */
 int hr_sample_train_batch(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height, int32_t width,
                           int32_t c_in, uint64_t seed, int64_t epoch, int64_t batch_index, int64_t batch_size,
                           const int64_t* order, float* coords, float* rgb, float* weight, int64_t* pixel_ids, int64_t* n_rows,
