@@ -12,8 +12,8 @@ from .models import LightfieldModel, model_dict  # noqa: F401
 from .rendering import RenderLightfield, render_chunked, render_fn_dict  # noqa: F401
 from .signature import Signature, UnsupportedPipeline, lower  # noqa: F401
 from .system import INRSystem  # noqa: F401
-from .train_data import DeviceRayBatches, regular_subsample_plan  # noqa: F401
+from .train_data import DeviceRayBatches, importance_subsample_plan, regular_subsample_plan  # noqa: F401
 
-__all__ = ["camera", "Camera", "generate_rays", "configs", "metrics", "rays", "train_data", "DeviceRayBatches", "regular_subsample_plan", "Cfg", "to_cfg", "load_model_yaml", "epochs_to_iters", "LightfieldModel", "model_dict",
+__all__ = ["camera", "Camera", "generate_rays", "configs", "metrics", "rays", "train_data", "DeviceRayBatches", "importance_subsample_plan", "regular_subsample_plan", "Cfg", "to_cfg", "load_model_yaml", "epochs_to_iters", "LightfieldModel", "model_dict",
            "RenderLightfield", "render_chunked", "render_fn_dict", "Signature", "UnsupportedPipeline", "lower",
            "INRSystem"]

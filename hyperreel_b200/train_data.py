@@ -16,7 +16,9 @@ bit) and its colour ``u8 / 255`` (``T.ToTensor()``), weight 1.  ``INRSystem.trai
 
 The shipped training configs train differently: they sample with replacement (``num_iters`` batches per epoch) from a table
 in which the video datasets keep only a per-frame subset of each view's pixels.  ``DeviceRayBatches.from_config`` reads both
-from a config, and ``hr_sample_train_rows`` (same file) generates those batches, again without any table in memory.
+from a config, and ``hr_sample_train_rows`` (same file) generates those batches, again without any table in memory.  The
+Immersive dataset keeps its per-frame pixels by image content; ``hr_build_importance_table`` selects them on the device into a
+keep bitmask per frame and ``hr_sample_train_mask_rows`` samples from it.
 """
 from __future__ import annotations
 
@@ -46,6 +48,23 @@ def _as_image_stack(images) -> torch.Tensor:
     if images.dtype != torch.uint8:
         raise ValueError(f"DeviceRayBatches needs uint8 images, got {images.dtype}")
     return images
+
+
+def _video_major(frames: Sequence[int], videos: Sequence[int]) -> List[bool]:
+    """Whether each view is its video's first, checking that views are video-major with each video's frames consecutive."""
+    if len(videos) != len(frames):
+        raise ValueError(f"{len(videos)} video indices for {len(frames)} views: one per view is needed")
+    first = [i == 0 or videos[i] != videos[i - 1] for i in range(len(frames))]
+    seen = set()
+    for i, f in enumerate(first):
+        if f:
+            if videos[i] in seen:
+                raise ValueError(f"views must be video-major: video {videos[i]} appears again at view {i}")
+            seen.add(videos[i])
+        elif frames[i] != frames[i - 1] + 1:
+            raise ValueError(f"views must be video-major with consecutive frames: view {i} has frame {frames[i]} "
+                             f"after frame {frames[i - 1]}")
+    return first
 
 
 def regular_subsample_plan(frames: Sequence[int], *, load_full_step: int, subsample_keyframe_step: int,
@@ -85,16 +104,7 @@ def regular_subsample_plan(frames: Sequence[int], *, load_full_step: int, subsam
         if videos is None or len(videos) != len(frames):
             raise ValueError("counters='neural_3d' needs one video index per view")
         videos = [int(v) for v in videos]
-        first_of_video = [i == 0 or videos[i] != videos[i - 1] for i in range(len(frames))]
-        seen = set()
-        for i, first in enumerate(first_of_video):
-            if first:
-                if videos[i] in seen:
-                    raise ValueError(f"views must be video-major: video {videos[i]} appears again at view {i}")
-                seen.add(videos[i])
-            elif frames[i] != frames[i - 1] + 1:
-                raise ValueError(f"views must be video-major with consecutive frames: view {i} has frame {frames[i]} "
-                                 f"after frame {frames[i - 1]}")
+        first_of_video = _video_major(frames, videos)
         restart = [videos[i] if first else None for i, first in enumerate(first_of_video)]
     else:
         raise ValueError(f"counters must be 'technicolor' or 'neural_3d', got {counters!r}")
@@ -124,6 +134,48 @@ def subset_rows(stride: int, offset: int, height: int, width: int) -> int:
     return n
 
 
+def importance_subsample_plan(frames: Sequence[int], videos: Sequence[int], *, load_full_step: int,
+                              subsample_keyframe_step: int, subsample_keyframe_frac: float, subsample_frac: float,
+                              height: int, width: int) -> List[Optional[Tuple[int, int]]]:
+    """The Immersive dataset's per-frame pixel subsets (datasets/immersive.py:295-391) as one entry per training view, in the
+    table's order: ``None`` for a view that keeps every pixel, or ``(num_take, prev)`` for one that keeps the pixels whose
+    colour changed most since view ``prev`` (the previous frame of its video).
+
+    ``frames[i]`` and ``videos[i]`` are view ``i``'s frame and video; views are video-major with each video's frames
+    consecutive.  A video's first view is whole, as is a frame with ``frame % load_full_step == 0``.  Every other frame takes
+    ``num_take = int(np.round(H*W * frac))`` with ``frac = subsample_keyframe_frac`` when ``frame % subsample_keyframe_step ==
+    0`` and ``subsample_frac`` otherwise, and keeps the pixels whose mean absolute colour change exceeds that change's
+    ``num_take``-th largest value (ties excluded, so often fewer than ``num_take``) and whose ray points down the camera's
+    -z (direction z < -0.05).  ``DeviceRayBatches(..., importance=plan)`` builds that table on the device."""
+    frames, videos = [int(f) for f in frames], [int(v) for v in videos]
+    if any(f < 0 for f in frames):
+        raise ValueError("frames must be >= 0")
+    for name, step in (("load_full_step", load_full_step), ("subsample_keyframe_step", subsample_keyframe_step)):
+        if int(step) != step or int(step) < 1:
+            raise ValueError(f"{name} must be an integer >= 1, got {step}")
+    n = int(height) * int(width)
+    if int(height) < 1 or int(width) < 1:
+        raise ValueError(f"views must hold at least one pixel, got {height}x{width}")
+    take = {}
+    for name, frac in (("subsample_keyframe_frac", subsample_keyframe_frac), ("subsample_frac", subsample_frac)):
+        frac = float(frac)
+        if not 0.0 <= frac:
+            raise ValueError(f"{name} must be >= 0, got {frac}")
+        take[name] = int(np.round(n * frac * 1.0))  # importance_subsample's num_take (fac = 1.0)
+        if take[name] > n:
+            raise ValueError(f"{name}={frac} takes {take[name]} of {n} pixels: the reference's sorted[-num_take] fails")
+    first = _video_major(frames, videos)
+    plan: List[Optional[Tuple[int, int]]] = []
+    for i, f in enumerate(frames):
+        if first[i] or f % int(load_full_step) == 0:
+            plan.append(None)
+        elif f % int(subsample_keyframe_step) == 0:
+            plan.append((take["subsample_keyframe_frac"], i - 1))
+        else:
+            plan.append((take["subsample_frac"], i - 1))
+    return plan
+
+
 class DeviceRayBatches:
     """Shuffled training batches ``{'coords' [B, c_in], 'rgb' [B, 3], 'weight' [B, 1]}`` (fp32, on the device) over every
     pixel of the training views, generated on the device per batch.
@@ -140,6 +192,10 @@ class DeviceRayBatches:
       view, only the pixels with ``(x + y + offset) % stride == 0``, each view's in row-major order: the order of the video
       datasets' ``all_coords``.  ``n_rows`` is the table's size (``n*H*W`` without a plan); ``gather_rows`` returns rows by
       table index.
+    * ``importance``: the Immersive dataset's content-dependent subsets (``importance_subsample_plan``), built on the device
+      at construction into a keep bitmask per importance view (about 0.14 B per pixel); the table is then each view's kept
+      pixels in row-major order, as with ``subsample``, and ``view_rows`` gives the per-view counts.  Not combined with
+      ``subsample``.
     * ``replacement=True`` with ``num_iters``: every batch is ``batch_size`` independent uniform draws from the table, keyed
       by ``(seed, epoch, position)``, and an epoch is ``num_iters`` batches, as the reference's
       ``RandomSampler(replacement=True, num_samples=num_iters * batch_size)`` (nlf/__init__.py:222-237).
@@ -151,7 +207,8 @@ class DeviceRayBatches:
     def __init__(self, cameras: Sequence[Camera], images, batch_size: int, seed: int = 0, c_in: int = 8,
                  device: Optional[torch.device] = None, *, use_patches: bool = False, precrop_iters: int = 0,
                  use_full_image: bool = False, blur_radius: int = 0, replacement: bool = False,
-                 num_iters: Optional[int] = None, subsample: Optional[Sequence[Tuple[int, int]]] = None):
+                 num_iters: Optional[int] = None, subsample: Optional[Sequence[Tuple[int, int]]] = None,
+                 importance: Optional[Sequence[Optional[Tuple[int, int]]]] = None):
         for name, value, default in (("use_patches", use_patches, False), ("precrop_iters", precrop_iters, 0),
                                      ("use_full_image", use_full_image, False), ("blur_radius", blur_radius, 0)):
             if value != default:
@@ -180,6 +237,10 @@ class DeviceRayBatches:
         elif num_iters is not None:
             raise ValueError("num_iters sets the epoch length of replacement=True; without replacement an epoch is "
                              "ceil(n_rows / batch_size) batches")
+        if importance is not None:
+            if subsample is not None:
+                raise ValueError("importance and subsample are two different tables: give one of them")
+            importance = self._check_importance(importance, n, H * W)
         if subsample is None:
             rule = [(1, 0)] * n
         else:
@@ -210,26 +271,88 @@ class DeviceRayBatches:
         self.replacement = bool(replacement)
         self.num_iters = int(num_iters) if replacement else None
         self.subsample = None if subsample is None else rule
-        self.n_rows = int(sum(counts))
-        # the table's plan for hr_sample_train_rows: exclusive prefix of the per-view row counts, and (stride, offset) per view
-        self._view_start = torch.tensor(np.concatenate([[0], np.cumsum(counts)]), dtype=torch.int64, device=self.device)
-        self._view_rule = torch.tensor(rule, dtype=torch.int32, device=self.device).contiguous()
+        self.importance = importance
+        if importance is None:
+            self._n_rows = int(sum(counts))
+            # the table's plan for hr_sample_train_rows: exclusive prefix of the per-view row counts, and (stride, offset) per view
+            self._view_start = torch.tensor(np.concatenate([[0], np.cumsum(counts)]), dtype=torch.int64, device=self.device)
+            self._view_rule = torch.tensor(rule, dtype=torch.int32, device=self.device).contiguous()
+        else:
+            self._n_rows = None  # read from the device on first use
+            self._build_importance(importance)
         # the original path (every pixel, each once per epoch) keeps its own kernel
-        self._table_path = self.replacement or self.subsample is not None
+        self._table_path = self.replacement or self.subsample is not None or self.importance is not None
+
+    @staticmethod
+    def _check_importance(plan, n: int, hw: int) -> List[Optional[Tuple[int, int]]]:
+        plan = list(plan)
+        if len(plan) != n:
+            raise ValueError(f"importance needs one entry per view: {len(plan)} entries for {n} views")
+        out = []
+        for v, e in enumerate(plan):
+            if e is None:
+                out.append(None)
+                continue
+            e = tuple(e)
+            if len(e) != 2 or any(int(a) != a for a in e):
+                raise ValueError(f"importance entry {v} must be None or (num_take, prev), got {e!r}")
+            take, prev = int(e[0]), int(e[1])
+            if not 0 <= take <= hw:
+                raise ValueError(f"importance entry {v} takes {take} pixels, outside [0, {hw}]")
+            if prev != v - 1 or v == 0:
+                raise ValueError(f"importance entry {v}'s previous frame is view {prev}: it must be view {v - 1}, the "
+                                 "previous frame of the same video")
+            out.append((take, prev))
+        return out
+
+    def _build_importance(self, plan) -> None:
+        """Builds the keep masks of the importance views and the per-view row counts on the device (no synchronisation)."""
+        dev, n = self.device, self.n_views
+        n_slots = sum(e is not None for e in plan)
+        blocks = -(-self.height * self.width // 256)
+        host = np.array([(-1, -1) if e is None else e for e in plan], dtype=np.int64).reshape(n, 2)
+        self._view_slot = torch.empty((n,), dtype=torch.int32, device=dev)
+        self._block_start = torch.empty((max(n_slots, 1) * blocks,), dtype=torch.int32, device=dev)
+        self._masks = torch.empty((max(n_slots, 1) * blocks * 8,), dtype=torch.int32, device=dev)
+        self._view_rows = torch.empty((n,), dtype=torch.int64, device=dev)
+        self._view_start = torch.empty((n + 1,), dtype=torch.int64, device=dev)
+        ws_bytes = int(self._lib.hr_importance_workspace_bytes(n_slots))
+        ws = torch.empty((max(ws_bytes, 1),), dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            L.check(self._lib.hr_build_importance_table(
+                self.cameras.data_ptr(), n, self.images.data_ptr(), self.height, self.width,
+                host.ctypes.data_as(C.c_void_p), ws.data_ptr(), ws_bytes, self._view_slot.data_ptr(),
+                self._block_start.data_ptr(), self._masks.data_ptr(), self._view_rows.data_ptr(),
+                self._view_start.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+
+    @property
+    def n_rows(self) -> int:
+        """The training table's size; for an ``importance`` table, reading it waits for the table's build."""
+        if self._n_rows is None:
+            n = int(self._view_start[-1])
+            if n < 1:
+                raise ValueError("importance keeps no pixel: the training table is empty")
+            self._n_rows = n
+        return self._n_rows
+
+    @property
+    def view_rows(self) -> torch.Tensor:
+        """The number of table rows of each view, int64 [n_views] on the host."""
+        return self._view_start.diff().cpu()
 
     @classmethod
     def from_config(cls, cfg, cameras: Sequence[Camera], images, seed: int = 0, c_in: int = 8,
                     device: Optional[torch.device] = None) -> "DeviceRayBatches":
         """The training batches a reference config trains on: ``cfg.training.batch_size``, ``sample_with_replacement`` and
-        ``num_iters``, and for the ``technicolor`` and ``neural_3d`` datasets the per-frame pixel subsets of
-        ``cfg.dataset.{num_frames, load_full_step, subsample_keyframe_step, subsample_keyframe_frac, subsample_frac}``.
+        ``num_iters``, and for the ``technicolor``, ``neural_3d`` and ``immersive`` datasets the per-frame pixel subsets of
+        ``cfg.dataset.{num_frames, load_full_step, subsample_keyframe_step, subsample_keyframe_frac, subsample_frac}``
+        (``importance_subsample_plan`` for immersive, built on the device from the images).
 
         ``cameras`` and ``images`` must be the training views in the reference's training order: frame-major with the
-        held-out views removed for technicolor, video-major (each video's frames in order) for neural_3d.  A view's frame is
-        ``int(np.round(time * (num_frames - 1)))`` of its ``Camera.time``; for neural_3d each run of equal ``cam_idx`` is one
-        video, numbered 0, 1, ... in order (the reference numbers videos after removing the held-out one).  The ``immersive``
-        dataset's content-dependent ``importance_subsample``, and any other dataset that sets subsample keys, raise
-        ``ValueError``.
+        held-out views removed for technicolor, video-major (each video's frames in order) for neural_3d and immersive.  A
+        view's frame is ``int(np.round(time * (num_frames - 1)))`` of its ``Camera.time``; for neural_3d and immersive each
+        run of equal ``cam_idx`` is one video, numbered 0, 1, ... in order (the reference numbers videos after removing the
+        held-out one).  Any other dataset that sets subsample keys raises ``ValueError``.
 
         With replacement the reference runs with ``iters_per_epoch = num_iters`` (main.py:100-101), and its epoch-based
         schedules are scaled by that value: an ``INRSystem`` built from the same config must be given
@@ -240,33 +363,39 @@ class DeviceRayBatches:
         name = dataset.get("name", None)
         keys = ("load_full_step", "subsample_keyframe_step", "subsample_keyframe_frac", "subsample_frac")
         cameras = list(cameras)
-        subsample = None
-        if name in ("technicolor", "neural_3d"):
+        subsample = importance = None
+        steps = dict(load_full_step=dataset.get("load_full_step", 1),
+                     subsample_keyframe_step=dataset.get("subsample_keyframe_step", 1),
+                     subsample_keyframe_frac=dataset.get("subsample_keyframe_frac", 1.0),
+                     subsample_frac=dataset.get("subsample_frac", 1.0))
+        if name in ("technicolor", "neural_3d", "immersive"):
             num_frames = int(dataset.get("num_frames", 1))
             frames = [int(np.round(float(cam.time) * (num_frames - 1))) for cam in cameras]
             videos = None
-            if name == "neural_3d":
+            if name != "technicolor":
                 videos, seen = [], set()
                 for i, cam in enumerate(cameras):
                     if i == 0 or cam.cam_idx != cameras[i - 1].cam_idx:
                         if cam.cam_idx in seen:
-                            raise ValueError(f"neural_3d views must be video-major: cam_idx {cam.cam_idx} appears again at "
+                            raise ValueError(f"{name} views must be video-major: cam_idx {cam.cam_idx} appears again at "
                                              f"view {i}")
                         seen.add(cam.cam_idx)
                     videos.append(len(seen) - 1)
-            subsample = regular_subsample_plan(
-                frames, load_full_step=dataset.get("load_full_step", 1),
-                subsample_keyframe_step=dataset.get("subsample_keyframe_step", 1),
-                subsample_keyframe_frac=dataset.get("subsample_keyframe_frac", 1.0),
-                subsample_frac=dataset.get("subsample_frac", 1.0), counters=name, videos=videos)
-        elif name == "immersive":
-            raise ValueError("the immersive dataset's importance_subsample depends on the images' content and is not "
-                             "supported")
+            if name == "immersive":
+                if not cameras:
+                    raise ValueError("DeviceRayBatches needs at least one training view")
+                try:
+                    importance = importance_subsample_plan(frames, videos, height=int(cameras[0].height),
+                                                           width=int(cameras[0].width), **steps)
+                except ValueError as e:
+                    raise ValueError(f"immersive importance_subsample: {e}") from None
+            else:
+                subsample = regular_subsample_plan(frames, counters=name, videos=videos, **steps)
         elif any(k in dataset for k in keys):
-            raise ValueError(f"dataset {name!r} sets {[k for k in keys if k in dataset]}: only technicolor's and neural_3d's "
-                             "regular subsets are supported")
+            raise ValueError(f"dataset {name!r} sets {[k for k in keys if k in dataset]}: only technicolor's, neural_3d's "
+                             "and immersive's subsets are supported")
         return cls(cameras, images, batch_size=int(training["batch_size"]), seed=seed, c_in=c_in, device=device,
-                   replacement=replacement, num_iters=num_iters, subsample=subsample)
+                   replacement=replacement, num_iters=num_iters, subsample=subsample, importance=importance)
 
     def __len__(self) -> int:
         if self.replacement:
@@ -332,14 +461,18 @@ class DeviceRayBatches:
         tids = torch.empty((rows,), dtype=torch.int64, device=dev) if with_table_ids else None
         n_rows = C.c_int64(0)
         mode = L.SAMPLE_REPLACE if self.replacement else L.SAMPLE_PERMUTE
-        with torch.cuda.device(dev):
-            L.check(self._lib.hr_sample_train_rows(
-                self.cameras.data_ptr(), self.n_views, self.images.data_ptr(), self.height, self.width, self.c_in,
-                self._view_start.data_ptr(), self._view_rule.data_ptr(), self.n_rows, mode, self.seed, self.epoch, index,
-                rows if table_rows is not None else self.batch_size,
+        tail = (self.n_rows, mode, self.seed, self.epoch, index, rows if table_rows is not None else self.batch_size,
                 table_rows.data_ptr() if table_rows is not None else None, coords.data_ptr(), rgb.data_ptr(),
                 weight.data_ptr(), pids.data_ptr() if pids is not None else None,
-                tids.data_ptr() if tids is not None else None, C.byref(n_rows), torch.cuda.current_stream(dev).cuda_stream))
+                tids.data_ptr() if tids is not None else None, C.byref(n_rows), torch.cuda.current_stream(dev).cuda_stream)
+        head = (self.cameras.data_ptr(), self.n_views, self.images.data_ptr(), self.height, self.width, self.c_in,
+                self._view_start.data_ptr())
+        with torch.cuda.device(dev):
+            if self.importance is None:
+                L.check(self._lib.hr_sample_train_rows(*head, self._view_rule.data_ptr(), *tail))
+            else:
+                L.check(self._lib.hr_sample_train_mask_rows(*head, self._view_slot.data_ptr(), self._block_start.data_ptr(),
+                                                            self._masks.data_ptr(), *tail))
         assert n_rows.value == rows, (n_rows.value, rows)
         out = {"coords": coords, "rgb": rgb, "weight": weight}
         if pids is not None:

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define HR_ABI_VERSION 17
+#define HR_ABI_VERSION 18
 
 #define HR_MAX_GROUPS 4   /* ray-parameterisation groups feeding the sample net (ray.py:235-263) */
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
@@ -399,6 +399,37 @@ int hr_sample_train_rows(const hr_camera* cameras, int32_t n_views, const uint8_
                          uint64_t seed, int64_t epoch, int64_t batch_index, int64_t batch_size, const int64_t* table_rows,
                          float* coords, float* rgb, float* weight, int64_t* pixel_ids, int64_t* table_ids, int64_t* n_rows,
                          void* stream);
+
+/* The Immersive dataset's training table: per-view keep masks chosen by image content.
+ * Replaces: ImmersiveDataset.prepare_train_data / subsample / importance_subsample (datasets/immersive.py:295-391).  Views are
+ * video-major with each video's frames in order; an importance view v keeps the pixels with diff > thr and dz < -0.05 in
+ * row-major order, diff = mean over channels of |rgb_v - rgb_{v-1}| (u8 / 255 in fp32, ((d0 + d1) + d2) / 3), thr = diff's value
+ * of ascending rank (N - num_take) % N (N = height*width; duplicates counted), dz = channel 5 of hr_generate_rays's row for the
+ * pixel.  cameras, images, n_views, height, width: as hr_sample_train_batch (height*width < 2^31).  plan: HOST int64
+ * [n_views, 2], per view (num_take, prev): (-1, -1) for a whole view, else num_take in [0, N] and prev == v - 1 (the previous
+ * frame of the same video; v >= 1).  At most 65535 importance views per call; n_slots is their number.
+ * Outputs (device): view_slot int32 [n_views], the view's slot (its rank among the importance views) or -1;
+ *   masks uint32 [n_slots, B, 8], B = ceil(N / 256): bit (p & 31) of word p >> 5 of the slot's mask keeps pixel p;
+ *   block_start uint32 [n_slots, B]: exclusive prefix of the kept counts of each 256-pixel block within the view;
+ *   view_rows int64 [n_views]: the kept counts (N for whole views);  view_start int64 [n_views + 1]: their exclusive prefix.
+ * masks and block_start may be NULL when n_slots == 0.  workspace: device, 256-byte aligned, at least
+ * hr_importance_workspace_bytes(n_slots) bytes.  A malformed plan or argument returns non-zero and writes nothing.  A fixed
+ * number of launches whatever n_views, integer atomics only: two builds write the same bits.  No host synchronisation beyond
+ * the copy of the plan's slots from host memory. */
+int64_t hr_importance_workspace_bytes(int32_t n_slots);
+int hr_build_importance_table(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height, int32_t width,
+                              const int64_t* plan, void* workspace, int64_t workspace_bytes, int32_t* view_slot,
+                              uint32_t* block_start, uint32_t* masks, int64_t* view_rows, int64_t* view_start, void* stream);
+
+/* Training batches over a table of per-view keep masks (hr_build_importance_table's outputs): as hr_sample_train_rows, with
+ * view_slot, block_start and masks in place of view_rule.  Table row k is in view v with view_start[v] <= k < view_start[v + 1],
+ * at rank k - view_start[v] of that view's kept pixels in row-major order (every pixel for slot -1).  n_table is
+ * view_start[n_views] for a well-formed table; a row the table does not hold gives a zero row of weight 0 and ids -1. */
+int hr_sample_train_mask_rows(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height, int32_t width,
+                              int32_t c_in, const int64_t* view_start, const int32_t* view_slot, const uint32_t* block_start,
+                              const uint32_t* masks, int64_t n_table, int32_t mode, uint64_t seed, int64_t epoch,
+                              int64_t batch_index, int64_t batch_size, const int64_t* table_rows, float* coords, float* rgb,
+                              float* weight, int64_t* pixel_ids, int64_t* table_ids, int64_t* n_rows, void* stream);
 
 /* ---- the step after the path: 8-bit packing (SURVEY.md section 8(f) row f4) ----
  * Replaces: to8b(x) = (255 * clip(x, 0, 1)).astype(uint8) (utils/__init__.py:47) applied to the rendered frame before
