@@ -6,11 +6,14 @@ Only what sits on the hot path is kept: construction from the full config (``cfg
 checkpoints whose keys carry the ``render_fn.`` prefix, and -- SURVEY.md section 8 row f1 -- ``configure_optimizers`` /
 ``training_step`` (nlf/__init__.py:504-523, 634-709) over the differentiable path: image loss, manual optimisation with
 one Adam per optimiser group, the TensoRF regulariser (L1 + TV on the tables, nlf/regularizers/tensorf.py:35-96) and the grid
-up-sampling / occupancy-pruning schedule with its optimiser reset (tensorf_base.py:379-429,509-553,1151-1232).  Visualisers and
-datasets are out of scope (SURVEY.md section 2).
+up-sampling / occupancy-pruning schedule with its optimiser reset (tensorf_base.py:379-429,509-553,1151-1232), and, with
+``schedule="reference"``, the optimisers' own schedule: one learning-rate scheduler per group stepped by
+``training_epoch_end`` (utils/__init__.py:78-125, nlf/__init__.py:711-725) and the per-group ``reset_opt_list`` restarts
+(nlf/__init__.py:529-578).  Visualisers and datasets are out of scope (SURVEY.md section 2).
 """
 from __future__ import annotations
 
+from functools import partial
 from typing import Dict, Optional
 
 import torch
@@ -74,10 +77,49 @@ class TensoRFRegularizer:
             self.L1_reg_weight = float(self.cfg.L1_weight_rest)
 
 
+def exp_decay(decay_gamma, stop_epoch, decay_epoch, epoch):
+    """utils/__init__.py:78-84, the `exp` schedule's factor on the base learning rate."""
+    if epoch > stop_epoch:
+        return 0.0
+    return decay_gamma ** (epoch / decay_epoch)
+
+
+def poly_exp_decay(num_epochs, poly_exp, epoch):
+    """utils/__init__.py:86-87, the `poly` schedule's factor."""
+    return (1 - epoch / num_epochs) ** poly_exp
+
+
+def make_scheduler(oc, optimizer):
+    """get_scheduler (utils/__init__.py:89-125) for one group's config `oc` (cfg.training.optimizers.<group>): torch's own
+    LambdaLR / MultiStepLR / CosineAnnealingLR, stepped once per epoch.  The GradualWarmupScheduler wrapper of
+    `warmup_epochs > 0` is refused; no shipped training config sets it."""
+    kind = oc.get("lr_scheduler")
+    if oc.get("warmup_epochs", 0) > 0:
+        raise NotImplementedError("warmup_epochs > 0 (GradualWarmupScheduler) is not mirrored")
+    if kind == "exp":
+        fn = partial(exp_decay, oc.decay_gamma, oc.stop_epoch if "stop_epoch" in oc else float("inf"), float(oc.decay_epoch))
+        scheduler = torch.optim.lr_scheduler.LambdaLR(optimizer, fn)
+    elif kind == "steplr":
+        scheduler = torch.optim.lr_scheduler.MultiStepLR(optimizer, milestones=[oc.decay_epoch], gamma=oc.decay_gamma)
+    elif kind == "cosine":
+        scheduler = torch.optim.lr_scheduler.CosineAnnealingLR(optimizer, T_max=oc.num_epochs, eta_min=1e-8)
+    elif kind == "poly":
+        scheduler = torch.optim.lr_scheduler.LambdaLR(optimizer, partial(poly_exp_decay, oc.num_epochs, oc.poly_exp))
+    else:
+        raise NotImplementedError(f"lr_scheduler {kind!r}: only the reference's exp, steplr, cosine and poly are mirrored")
+    return scheduler
+
+
 class INRSystem(nn.Module):
     def __init__(self, cfg, dm=None, dataset: Optional[dict] = None, mlp_mode: str = "auto", train_net: str = "torch",
-                 ease: str = "elapsed"):
+                 ease: str = "elapsed", schedule: str = "constant"):
         super().__init__()
+        # "constant": every group trains at its configured lr, and every group restarts when the tables are re-created;
+        # "reference": the reference's per-group lr schedulers (stepped by training_epoch_end) and reset_opt_list restarts
+        if schedule not in ("constant", "reference"):
+            raise ValueError(f"schedule must be 'constant' or 'reference', got {schedule!r}")
+        self.schedule = schedule
+        self.training_started = False
         self.cfg = to_cfg(cfg)
         self.dm = dm
         training = self.cfg.get("training", Cfg())
@@ -137,28 +179,84 @@ class INRSystem(nn.Module):
             groups["embedding"] = emb
         return groups
 
-    def configure_optimizers(self):
+    def _group_cfg(self, key):
         training = self.cfg.get("training", Cfg())
-        ocfg = training.get("optimizers", Cfg())
-        self._optimizers = []
+        oc = training.get("optimizers", Cfg()).get(key, Cfg())
+        if self.schedule == "reference":
+            if "lr_scheduler" not in oc:
+                raise ValueError(f"schedule='reference' needs cfg.training.optimizers.{key}.lr_scheduler")
+            if training.get("multiscale", False):
+                raise NotImplementedError("multiscale training (the datamodule's per-scale cur_lr) is not mirrored")
+            for k in ("skip_opt_list", "remove_skip_opt_list"):
+                if k in oc:
+                    raise NotImplementedError(f"{k} is not mirrored: no shipped training config sets it")
+        return oc
+
+    def _adam(self, key, oc, params):
+        if oc.get("optimizer", "adam") != "adam":
+            raise NotImplementedError("only the reference's default optimizer (adam) is mirrored")
+        return torch.optim.Adam(params, lr=float(oc.get("lr", self.OPT_DEFAULTS[key])), eps=1e-8,
+                                weight_decay=float(oc.get("weight_decay", 0)), betas=(0.9, 0.99))
+
+    def configure_optimizers(self):
+        """One Adam per non-empty group; with schedule="reference" also its scheduler (nlf/__init__.py:504-527: the lr times
+        the datamodule's cur_lr, which is 1.0 without multiscale)."""
+        self._optimizers, self._schedulers, self._opt_keys, self._reset_iters = [], [], [], []
         self._opt_struct = self.render_fn.model.color_model.net.struct_version
         for key, params in self.optimizer_groups().items():
             params = [p for p in params if p.numel() > 0]
             if not params:
                 continue
-            oc = ocfg.get(key, Cfg())
-            if oc.get("optimizer", "adam") != "adam":
-                raise NotImplementedError("only the reference's default optimizer (adam) is mirrored")
-            self._optimizers.append(torch.optim.Adam(params, lr=float(oc.get("lr", self.OPT_DEFAULTS[key])), eps=1e-8,
-                                                     weight_decay=float(oc.get("weight_decay", 0)), betas=(0.9, 0.99)))
+            oc = self._group_cfg(key)
+            self._optimizers.append(self._adam(key, oc, params))
+            self._opt_keys.append(key)
+            if self.schedule == "reference":
+                self._schedulers.append(make_scheduler(oc, self._optimizers[-1]))
+                self._reset_iters.append(frozenset(oc.get("reset_opt_list", None) or ()))
         return self._optimizers
+
+    def optimizers(self):
+        """The optimisers training_step steps, one per group in optimizer_groups() order (LightningModule.optimizers)."""
+        return list(getattr(self, "_optimizers", []))
+
+    def lr_schedulers(self):
+        """Their schedulers with schedule="reference", in the same order; none with "constant"."""
+        return list(getattr(self, "_schedulers", []))
+
+    def _reference_restarts(self, train_iter: int):
+        """needs_opt_reset / reset_optimizers (nlf/__init__.py:529-578): a group whose reset_opt_list holds train_iter gets a
+        new Adam and a new scheduler (its lr back at the base); the others keep both.  The reference has no rule for tables
+        re-created (up-sampling, shrink) at an iteration its 'color' group does not list: its Adam would go on stepping the
+        stale Parameters.  Here the Adam of each group whose Parameters changed restarts on the new ones -- its moments and
+        step counts dropped, as in a new Adam -- and its scheduler carries on, so the lr stays on its curve (DESIGN §7)."""
+        net = self.render_fn.model.color_model.net
+        groups = None
+        if net.struct_version != self._opt_struct:
+            groups = self.optimizer_groups()
+            self._opt_struct = net.struct_version
+        for idx, key in enumerate(self._opt_keys):
+            listed = train_iter in self._reset_iters[idx]
+            if not listed and groups is None:
+                continue
+            params = [p for p in (groups or self.optimizer_groups())[key] if p.numel() > 0]
+            opt = self._optimizers[idx]
+            if listed:
+                oc = self._group_cfg(key)
+                self._optimizers[idx] = self._adam(key, oc, params)
+                self._schedulers[idx] = make_scheduler(oc, self._optimizers[idx])
+            elif len(params) != len(opt.param_groups[0]["params"]) or any(
+                    a is not b for a, b in zip(params, opt.param_groups[0]["params"])):
+                opt.param_groups[0]["params"] = params
+                opt.state.clear()
 
     def set_train_iter(self, train_iter: int):
         """The per-iteration hook of the reference's loop (nlf/__init__.py:592-632): the colour net's schedule (grid
-        up-sampling, tensorf_base.py:509-553) and the regularisers' (`L1_weight_rest`), then an optimiser rebuild when the
-        tables were re-created (`lr_upsample_reset`, nlf/__init__.py:541-578 -- here every group restarts, Adam state of the old
-        Parameter objects is meaningless for the new ones).  With ease="reference" the whole model's set_iter runs, as in the
-        reference (nlf/__init__.py:608-614), so its EaseValue heads are eased at `train_iter` for this step and later renders."""
+        up-sampling, tensorf_base.py:509-553) and the regularisers' (`L1_weight_rest`), then the optimiser restarts.  With
+        schedule="constant" every group restarts when the tables were re-created (`lr_upsample_reset`, nlf/__init__.py:541-578:
+        Adam state of the old Parameter objects is meaningless for the new ones); with schedule="reference" the groups restart
+        at their `reset_opt_list` iterations (_reference_restarts).  With ease="reference" the whole model's set_iter runs, as
+        in the reference (nlf/__init__.py:608-614), so its EaseValue heads are eased at `train_iter` for this step and later
+        renders."""
         model = self.render_fn.model
         if self.ease == "reference":
             model.set_iter(int(train_iter))  # includes the colour net's schedule
@@ -167,7 +265,10 @@ class INRSystem(nn.Module):
         for reg in self.regularizers:
             reg.set_iter(int(train_iter))
         net = model.color_model.net
-        if getattr(net, "needs_opt_reset", False) or (getattr(self, "_opt_struct", None) not in (None, net.struct_version)):
+        if self.schedule == "reference":
+            if getattr(self, "_optimizers", None):
+                self._reference_restarts(int(train_iter))
+        elif getattr(net, "needs_opt_reset", False) or (getattr(self, "_opt_struct", None) not in (None, net.struct_version)):
             self.configure_optimizers()
             net.needs_opt_reset = False
 
@@ -175,6 +276,7 @@ class INRSystem(nn.Module):
         """One iteration of nlf/__init__.py:634-709 on this path: batch {'coords' [N,C], 'rgb' [N,3], optional 'weight'};
         loss = MSE(rgb_pred * w, rgb * w) (losses.py 'mse') + regularisers, manual optimisation (zero_grad / backward / step
         per group).  `train_iter` (optional) drives the schedules like the reference's `set_train_iter`."""
+        self.training_started = True
         self.train()
         if train_iter is not None:
             self.set_train_iter(train_iter)
@@ -198,6 +300,20 @@ class INRSystem(nn.Module):
         with torch.no_grad():
             psnr = -10.0 * torch.log10(torch.mean((pred.detach() - rgb) ** 2))  # metrics.py:37-45
         return {"train/loss": loss.detach(), "train/psnr": psnr}
+
+    def training_epoch_end(self, outputs):
+        """nlf/__init__.py:711-725, to be called after an epoch's training_steps with their outputs: steps every scheduler
+        once if a training_step has run (the reference's `training_started`), and returns the epoch means of the outputs'
+        keys ('train/loss', 'train/psnr') as Python floats -- get_mean_outputs (metrics.py:60-82), fp32 means on the device,
+        read back in one copy, the epoch's one synchronisation."""
+        if self.training_started:
+            for scheduler in self.lr_schedulers():
+                scheduler.step()
+        if not outputs:
+            return {}
+        keys = list(outputs[0])
+        means = torch.stack([torch.stack([o[k] for o in outputs]).mean() for k in keys]).tolist()
+        return dict(zip(keys, means))
 
     # ---- nlf/__init__.py:895-982, 1015-1030
     def validation_image(self, batch, batch_idx: int = 0):
