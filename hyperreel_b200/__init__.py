@@ -6,7 +6,7 @@ Operator surface (same names as the reference's ``nlf`` package, SURVEY.md secti
 training images: ``DeviceRayBatches`` (train_data.py).  All compute is in ``libhyperreel_b200.so`` (csrc/, sm_90a CUDA behind the C-ABI of include/hyperreel_b200.h).
 """
 from . import camera, configs, metrics, rays, train_data  # noqa: F401
-from .camera import Camera, generate_rays  # noqa: F401
+from .camera import Camera, generate_rays, render_video, spiral_path  # noqa: F401
 from .config import Cfg, epochs_to_iters, load_model_yaml, to_cfg  # noqa: F401
 from .models import LightfieldModel, model_dict  # noqa: F401
 from .rendering import RenderLightfield, render_chunked, render_fn_dict  # noqa: F401
@@ -14,6 +14,6 @@ from .signature import Signature, UnsupportedPipeline, lower  # noqa: F401
 from .system import INRSystem  # noqa: F401
 from .train_data import DeviceRayBatches, importance_subsample_plan, regular_subsample_plan  # noqa: F401
 
-__all__ = ["camera", "Camera", "generate_rays", "configs", "metrics", "rays", "train_data", "DeviceRayBatches", "importance_subsample_plan", "regular_subsample_plan", "Cfg", "to_cfg", "load_model_yaml", "epochs_to_iters", "LightfieldModel", "model_dict",
+__all__ = ["camera", "Camera", "generate_rays", "render_video", "spiral_path", "configs", "metrics", "rays", "train_data", "DeviceRayBatches", "importance_subsample_plan", "regular_subsample_plan", "Cfg", "to_cfg", "load_model_yaml", "epochs_to_iters", "LightfieldModel", "model_dict",
            "RenderLightfield", "render_chunked", "render_fn_dict", "Signature", "UnsupportedPipeline", "lower",
            "INRSystem"]

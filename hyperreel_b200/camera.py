@@ -8,6 +8,7 @@ Mirrors ``get_coords_from_camera`` of the reference datasets (datasets/base.py:4
 """
 from __future__ import annotations
 
+import dataclasses
 from dataclasses import dataclass
 from typing import Optional, Sequence, Tuple
 
@@ -66,6 +67,162 @@ class Camera:
         if k is not None:
             c.fisheye, (c.k1, c.k2) = 1, k
         return c
+
+
+# ---- the render split's camera path: the poses and times of the reference's validation / render_only videos
+# (prepare_render_data of each dataset, rendered in order by validation_video, nlf/__init__.py:809-891), restated in fp64 numpy
+# in the reference's operation order and rounded to float32 where its get_coords makes tensors (torch.FloatTensor(pose),
+# `ones * time`).
+
+def _normalize(v):
+    return v / np.linalg.norm(v)
+
+
+def _average_poses(poses):  # utils/pose_utils.py:14-37
+    center = poses[..., 3].mean(0)
+    z = _normalize(poses[..., 2].mean(0))
+    y_ = poses[..., 1].mean(0)
+    x = _normalize(np.cross(y_, z))
+    y = np.cross(z, x)
+    return np.concatenate([np.stack([x, y, z], 1), center[..., None]], 1)
+
+
+def _viewmatrix(z, up, pos):  # utils/pose_utils.py:39-45
+    vec2 = _normalize(z)
+    vec0 = _normalize(np.cross(up, vec2))
+    vec1 = _normalize(np.cross(vec2, vec0))
+    return np.stack([vec0, vec1, vec2, pos], 1)
+
+
+def _spiral_poses(poses, rads, focal, n):  # create_spiral_poses (flip=False), utils/pose_utils.py:162-183
+    c2w = _average_poses(poses)
+    up = _normalize(poses[:, :3, 1].sum(0))
+    rads = np.array(list(rads) + [1.0])
+    out = []
+    for theta in np.linspace(0.0, 2.0 * np.pi * 2, n + 1)[:-1]:
+        c = np.dot(c2w[:3, :4], np.array([np.cos(theta), -np.sin(theta), -np.sin(theta * 0.5), 1.0]) * rads)
+        z = _normalize(c - np.dot(c2w[:3, :4], np.array([0, 0, -focal, 1.0])))
+        out.append(_viewmatrix(z, up, c))
+    return out
+
+
+def _interpolate_poses(poses, supersample):
+    """interpolate_poses (utils/pose_utils.py:269-356): `supersample` poses per gap, linear in the se(3) twist of each pose,
+    with scipy's logm / expm as the reference calls them; the last pose repeated `supersample` times."""
+    import scipy.linalg
+
+    p44 = np.concatenate([poses, np.tile(np.eye(4)[-1, :].reshape(1, 1, 4), [poses.shape[0], 1, 1])], 1)
+    twists = []
+    for p in p44:
+        M = scipy.linalg.logm(p)
+        twists.append(np.stack([M[..., 2, 1], M[..., 0, 2], M[..., 1, 0], M[..., 0, 3], M[..., 1, 3], M[..., 2, 3]], -1))
+    twists = np.stack(twists, 0)
+    t = np.linspace(0, 1, supersample, endpoint=False).reshape(1, supersample, 1)
+    tw = twists.reshape(-1, 1, twists.shape[-1])
+    tw = ((1 - t) * tw[:-1] + t * tw[1:]).reshape(-1, twists.shape[-1])
+    tw = np.concatenate([tw, np.tile(twists[-1:], [supersample, 1])], 0)
+    out = []
+    for w in tw:
+        z = np.zeros_like(w[0])
+        M = np.array([[z, -w[2], w[1], w[3]], [w[2], z, -w[0], w[4]], [-w[1], w[0], z, w[5]], [z, z, z, z]])
+        out.append(scipy.linalg.expm(M))
+    return np.stack(out, 0)[:, :3, :4]
+
+
+# video datasets: (percentile of |camera centre| per axis, scale of the x and y radii, scale of the z radius, focus depth
+# multiplier of a multi-frame video) of the spiral
+_VIDEO_SPIRALS = {
+    "technicolor": (60, 0.25, 1.0, 100.0),  # TechnicolorDataset.prepare_render_data, datasets/technicolor.py:294-353
+    "neural_3d": (50, 0.5, 1.0, 2.0),       # Neural3DVideoDataset.prepare_render_data, datasets/neural_3d.py:321-380
+    "immersive": (50, 1.0, 0.05, 1.0),      # ImmersiveDataset.prepare_render_data, datasets/immersive.py:427-487
+}
+SPIRAL_DATASETS = tuple(_VIDEO_SPIRALS) + ("donerf",)
+
+
+def spiral_path(dataset: str, camera: Camera, poses, bounds=None, num_frames: int = 1, supersample: int = 1,
+                interpolate: bool = False, interpolate_time: bool = False):
+    """The cameras and per-frame times of the reference's render-split video, for ``render_video``.
+
+    ``poses`` [N, 3, 4] and ``bounds`` are the dataset's ``poses`` and ``bounds`` as its read_meta leaves them for the
+    render split (pose-corrected, every camera of every frame: video datasets are frame-major with N / num_frames cameras
+    per frame); ``supersample``,
+    ``interpolate`` and ``interpolate_time`` are the config's ``render_params`` (supersample, interpolate, interpolate_time).
+    Video datasets (technicolor, neural_3d, immersive) fly a two-turn spiral around the middle frame's rig
+    (create_spiral_poses, utils/pose_utils.py:162-183) carried along the rig's per-frame motion (interpolate_poses), with
+    num_frames * supersample frames (120 for a one-frame dataset) and times over [0, 1] rounded to whole frames unless
+    interpolate_time; with ``interpolate`` the path goes through the given poses instead.  DoNeRF renders its render split's
+    poses (cam_path_pan.json) as they are (DONeRFDataset.prepare_render_data, datasets/donerf.py:216-217): pass those.
+    Every frame copies ``camera`` (intrinsics, size, ray flags, camera id) with the path's pose and time.  Returns
+    (list of Camera, times float32 [F])."""
+    if dataset not in SPIRAL_DATASETS:
+        raise ValueError(f"spiral_path: dataset must be one of {SPIRAL_DATASETS}, got {dataset!r}")
+    P = np.asarray(poses, dtype=np.float64)
+    if P.ndim != 3 or P.shape[1:] != (3, 4) or P.shape[0] < 1:
+        raise ValueError(f"spiral_path: poses must be [N, 3, 4] with N >= 1, got {P.shape}")
+    if not np.isfinite(P).all():
+        raise ValueError("spiral_path: poses must be finite")
+    num_frames, supersample = int(num_frames), int(supersample)
+    if dataset == "donerf":
+        path, times = list(P), np.zeros(P.shape[0])
+    else:
+        if num_frames < 1 or P.shape[0] % num_frames != 0:
+            raise ValueError(f"spiral_path: {P.shape[0]} poses are not num_frames = {num_frames} frames of one rig")
+        if supersample < 1:
+            raise ValueError(f"spiral_path: supersample must be >= 1, got {supersample}")
+        if interpolate:
+            path = list(_interpolate_poses(P, supersample))
+        else:
+            if bounds is None:
+                raise ValueError(f"spiral_path: the {dataset} spiral needs the dataset's bounds")
+            b = np.asarray(bounds, dtype=np.float64)
+            if b.size < 1 or not np.isfinite(b).all():
+                raise ValueError("spiral_path: bounds must be finite")
+            pct, s_xy, s_z, focus_mul = _VIDEO_SPIRALS[dataset]
+            close_depth, inf_depth = b.min() * 0.9, b.max() * 5.0
+            dt = 0.75
+            focus_depth = 1.0 / (((1.0 - dt) / close_depth + dt / inf_depth))
+            per_frame = P.shape[0] // num_frames
+            mid = (num_frames // 2) * per_frame
+            one_frame = P[mid:mid + per_frame]
+            radii = np.percentile(np.abs(one_frame[..., 3]), pct, axis=0)
+            radii[..., :2] *= s_xy
+            if s_z != 1.0:
+                radii[..., -1] *= s_z
+            if num_frames > 1:
+                each_frame = _interpolate_poses(P[::per_frame], supersample)
+                path = _spiral_poses(one_frame, radii, focus_depth * focus_mul, num_frames * supersample)
+                reference_pose = np.eye(4)
+                reference_pose[:3, :4] = P[mid]
+                reference_pose = np.linalg.inv(reference_pose)
+                for i in range(len(path)):
+                    cur = np.eye(4)
+                    cur[:3, :4] = path[i]
+                    path[i] = each_frame[i] @ (reference_pose @ cur)
+            else:
+                path = _spiral_poses(one_frame, radii, focus_depth * 100, 120)
+        if num_frames - 1 > 0:
+            times = np.linspace(0, num_frames - 1, len(path))
+            if not interpolate_time:
+                times = np.round(times)
+            times = times / (num_frames - 1)
+        else:
+            times = np.zeros(len(path))
+    poses32 = np.stack(path, 0).astype(np.float32)
+    times32 = np.asarray(times, dtype=np.float64).astype(np.float32)
+    cams = [dataclasses.replace(camera, pose=poses32[i], time=float(times32[i])) for i in range(len(path))]
+    return cams, times32
+
+
+def render_video(model_or_system, cameras: Sequence[Camera], times=None, out: Optional[torch.Tensor] = None,
+                 stream=None) -> torch.Tensor:
+    """uint8 video [F, H, W, 3] on the device of a LightfieldModel, RenderLightfield or INRSystem along ``cameras`` (one
+    size, pinhole or fisheye) at ``times`` (default each camera's ``time``): the reference's validation_video loop
+    (nlf/__init__.py:809-891) with its to8b, as one call that never synchronises (hr_render_video_to8b).  ``spiral_path``
+    gives the reference's cameras and times."""
+    target = model_or_system if hasattr(model_or_system, "render_video") else getattr(model_or_system, "model", None)
+    if target is None or not hasattr(target, "render_video"):
+        raise TypeError(f"render_video: expected a LightfieldModel, RenderLightfield or INRSystem, got {type(model_or_system)}")
+    return target.render_video(cameras, times, out=out, stream=stream)
 
 
 def generate_rays(camera: Camera, c_in: int = 8, device: Optional[torch.device] = None, first_pixel: int = 0,

@@ -26,6 +26,8 @@ cudaError_t launch_render_bwd(const hr_config& cfg, const Derived& dv, const Ren
                               float* g_color_embedding, const float* rays, const float* heads, const float* d_rgb, float* d_heads,
                               long long n, int clamp_output, int white_bg, int num_sms, cudaStream_t stream);
 cudaError_t launch_generate_rays(const hr_camera& cam, int c_in, long long first, long long n, float* out, cudaStream_t st);
+cudaError_t launch_generate_video_rays(const hr_camera* cams, const float* times, bool fisheye, int c_in, int width,
+                                       long long frame_px, long long first, long long n, float* out, cudaStream_t st);
 }  // namespace hr
 
 static thread_local std::string g_err;
@@ -894,6 +896,127 @@ int hr_render_frame_to8b_host(hr_handle* h, const hr_camera* cam, uint8_t* rgb8_
   }
   for (int i = 0; i < 3; ++i) CK(cudaStreamSynchronize(P.streams[i]));
   return 0;
+}
+
+// ---- videos: many frames per call, rays generated and rendered in sub-batches that span frame boundaries
+static int64_t align256(int64_t b) { return (b + 255) / 256 * 256; }
+
+// rays of the whole video, or -1 when F * H * W * 3 (the output's bytes) does not fit in int64
+static int64_t video_rays(int32_t n_frames, int32_t height, int32_t width) {
+  if (n_frames < 1 || height < 1 || width < 1) return -1;
+  int64_t px, n, bytes;
+  if (__builtin_mul_overflow((int64_t)height, (int64_t)width, &px) || __builtin_mul_overflow(px, (int64_t)n_frames, &n) ||
+      __builtin_mul_overflow(n, (int64_t)3, &bytes))
+    return -1;
+  return n;
+}
+
+// Workspace layout: the records [F] and times [F] on the device, then one slot per stream of the pipeline below (two when
+// the video is longer than one sub-batch), each a sub-batch's rays [sub, c_in] and render workspace.  The sub-batch is
+// hr_render's (16 sample-net tile waves unless hr_set_sub_batch says otherwise) whatever the frame size, so the scratch stays
+// bounded for any number of frames; "never split" does not apply here, a video is unbounded.
+static int64_t video_sub_rays(const hr_handle* h, int64_t n_rays) {
+  const int64_t sub = sub_batch_rays(h);
+  return n_rays < sub ? n_rays : sub;
+}
+
+static int64_t video_slot_bytes(const hr_handle* h, int64_t sub) {
+  return align256(sub * h->cfg.c_in * (int64_t)sizeof(float)) + align256(ws_bytes_for(h, sub));
+}
+
+int64_t hr_video_workspace_bytes(const hr_handle* h, int32_t n_frames, int32_t height, int32_t width) {
+  const int64_t n = video_rays(n_frames, height, width);
+  if (!h || n < 0) return -1;
+  const int64_t sub = video_sub_rays(h, n);
+  return align256((int64_t)n_frames * (int64_t)sizeof(hr_camera)) + align256((int64_t)n_frames * (int64_t)sizeof(float)) +
+         (n > sub ? 2 : 1) * video_slot_bytes(h, sub);
+}
+
+static bool finite_camera(const hr_camera& c) {
+  for (int i = 0; i < 12; ++i)
+    if (!std::isfinite(c.c2w[i])) return false;
+  return std::isfinite(c.fx) && std::isfinite(c.fy) && std::isfinite(c.cx) && std::isfinite(c.cy) && std::isfinite(c.ndc_near) &&
+         std::isfinite(c.cam_idx) && std::isfinite(c.time);
+}
+
+// Sub-batch i runs on stream i % 2 of the handle (forked from and joined back to the caller's stream by events) in slot
+// i % 2: its ray generation and sample net overlap the previous sub-batch's render kernel, where one stream would leave the
+// SMs idle between each sub-batch's render tail and the next one's ray generation.  Each stream runs its sub-batches in
+// order, so a slot is reused only after the sub-batch that last held it has finished.
+int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_frames, uint8_t* video,
+                         void* workspace, int64_t workspace_bytes, void* stream) {
+  if (!h || !cameras || !times || !video || !workspace) return fail("hr_render_video_to8b: null argument");
+  if (!h->uploaded) return fail("hr_render_video_to8b: parameters not uploaded");
+  if (n_frames < 1) return fail("hr_render_video_to8b: n_frames must be >= 1, got %d", n_frames);
+  const int32_t W = cameras[0].width, H = cameras[0].height;
+  const int64_t n = video_rays(n_frames, H, W);
+  if (n < 0) return fail("hr_render_video_to8b: %d frames of %d x %d pixels: bad size or output bytes overflow int64", n_frames, W, H);
+  bool fisheye = false;
+  for (int32_t f = 0; f < n_frames; ++f) {
+    const hr_camera& c = cameras[f];
+    if (c.width != W || c.height != H)
+      return fail("hr_render_video_to8b: frame %d is %d x %d, frame 0 is %d x %d", f, c.width, c.height, W, H);
+    if (!finite_camera(c)) return fail("hr_render_video_to8b: camera record of frame %d is not finite", f);
+    if (bad_fisheye(c))
+      return fail("hr_render_video_to8b: fisheye coefficients k1 = %g, k2 = %g of frame %d are not finite", c.k1, c.k2, f);
+    if (!std::isfinite(times[f])) return fail("hr_render_video_to8b: time of frame %d is not finite", f);
+    fisheye = fisheye || c.fisheye;
+  }
+  const int64_t need = hr_video_workspace_bytes(h, n_frames, H, W);
+  if (workspace_bytes < need) return fail("hr_render_video_to8b: workspace too small (%lld < %lld)", (long long)workspace_bytes, (long long)need);
+  if (((uintptr_t)workspace & 15) != 0) return fail("hr_render_video_to8b: workspace must be 16-byte aligned");
+  DeviceGuard guard(h->device);
+  const hr_config& c = h->cfg;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t sub = video_sub_rays(h, n);
+  const int n_slots = n > sub ? 2 : 1;
+  char* p = (char*)workspace;
+  hr_camera* d_cams = (hr_camera*)p;
+  p += align256((int64_t)n_frames * (int64_t)sizeof(hr_camera));
+  float* d_times = (float*)p;
+  p += align256((int64_t)n_frames * (int64_t)sizeof(float));
+  const int64_t slot_bytes = video_slot_bytes(h, sub), rays_bytes = align256(sub * c.c_in * (int64_t)sizeof(float));
+  // stream-ordered copies: a pageable source is staged before the call returns, without waiting for the device
+  CK(cudaMemcpyAsync(d_cams, cameras, (size_t)n_frames * sizeof(hr_camera), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_times, times, (size_t)n_frames * sizeof(float), cudaMemcpyHostToDevice, st));
+  cudaStream_t ss[2] = {st, st};
+  cudaEvent_t ev = nullptr;
+  if (n_slots == 2) {
+    for (int i = 0; i < 2; ++i) {
+      if (!h->pipe.streams[i]) CK(cudaStreamCreateWithFlags(&h->pipe.streams[i], cudaStreamNonBlocking));
+      ss[i] = h->pipe.streams[i];
+    }
+    CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    CK(cudaEventRecord(ev, st));
+    CK(cudaStreamWaitEvent(ss[0], ev, 0));
+    CK(cudaStreamWaitEvent(ss[1], ev, 0));
+    CK(cudaEventDestroy(ev));
+  }
+  const int64_t frame_px = (int64_t)W * H;
+  int rc = 0;
+  int64_t i = 0;
+  for (int64_t off = 0; off < n && !rc; off += sub, ++i) {
+    const int64_t m = (n - off < sub) ? (n - off) : sub;
+    cudaStream_t s = ss[i % 2];
+    char* slot = p + (i % n_slots) * slot_bytes;
+    float* d_rays = (float*)slot;
+    cudaError_t e = hr::launch_generate_video_rays(d_cams, d_times, fisheye, c.c_in, W, frame_px, off, m, d_rays, s);
+    if (e != cudaSuccess) {
+      rc = fail("video ray generation failed: %s", cudaGetErrorString(e));
+      break;
+    }
+    h->launches += 1;
+    rc = render_impl(h, d_rays, m, nullptr, nullptr, nullptr, slot + rays_bytes, slot_bytes - rays_bytes, s, video + off * 3);
+  }
+  if (n_slots == 2) {  // join, also after a failed launch: the caller's stream must not run ahead of enqueued work
+    for (int k = 0; k < 2; ++k) {
+      CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+      CK(cudaEventRecord(ev, ss[k]));
+      CK(cudaStreamWaitEvent(st, ev, 0));
+      CK(cudaEventDestroy(ev));
+    }
+  }
+  return rc;
 }
 
 int hr_render_host(hr_handle* h, const float* rays_host, int64_t n_rays, float* rgb_host, int64_t chunk) {

@@ -28,4 +28,36 @@ cudaError_t launch_generate_rays(const hr_camera& cam, int c_in, long long first
   return cudaGetLastError();
 }
 
+// Rays of a video (hr_render_video_to8b): global ray p = f * frame_px + y * width + x over n_frames records of one size,
+// rays first .. first + n - 1 of that sequence, so a batch may span frame boundaries.  Ray p is camera_ray of record f,
+// bit-identical to the row generate_rays_kernel writes for that record's pixel, with times[f] in the time column.  kFisheye
+// as in generate_rays_kernel: the host instantiates it when any record of the video is a fisheye, and then each row
+// branches on its own record's flag, so one batch may mix the two camera models.
+template <bool kFisheye>
+__global__ void generate_video_rays_kernel(const hr_camera* __restrict__ cams, const float* __restrict__ times, int c_in,
+                                           int width, long long frame_px, long long first, long long n,
+                                           float* __restrict__ out) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long p = first + i;
+    const long long f = p / frame_px, q = p - f * frame_px;
+    const hr_camera& cam = cams[f];
+    float row[8];
+    camera_ray<kFisheye>(cam, (int)(q % width), (int)(q / width), ndc_scale(cam), row);
+    float* r = out + i * c_in;
+    r[0] = row[0]; r[1] = row[1]; r[2] = row[2];
+    r[3] = row[3]; r[4] = row[4]; r[5] = row[5];
+    if (c_in >= 8) { r[6] = row[6]; r[7] = times[f]; }
+  }
+}
+
+cudaError_t launch_generate_video_rays(const hr_camera* cams, const float* times, bool fisheye, int c_in, int width,
+                                       long long frame_px, long long first, long long n, float* out, cudaStream_t st) {
+  if (n <= 0) return cudaSuccess;
+  long long g = (n + 255) / 256;
+  if (g > 148 * 16) g = 148 * 16;
+  if (fisheye) generate_video_rays_kernel<true><<<(unsigned)g, 256, 0, st>>>(cams, times, c_in, width, frame_px, first, n, out);
+  else generate_video_rays_kernel<false><<<(unsigned)g, 256, 0, st>>>(cams, times, c_in, width, frame_px, first, n, out);
+  return cudaGetLastError();
+}
+
 }  // namespace hr

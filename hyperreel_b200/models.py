@@ -496,6 +496,49 @@ class LightfieldModel(nn.Module):
         L.check(self._lib.hr_render_frame_to8b_host(self._handle, C.byref(cam), out_host.data_ptr(), chunk))
         return out_host
 
+    def render_video(self, cameras, times=None, out: Optional[torch.Tensor] = None, stream=None) -> torch.Tensor:
+        """Frames of ``cameras`` (hyperreel_b200.camera.Camera, one size, pinhole or fisheye) at ``times`` (one per camera;
+        default each camera's ``time``) -> uint8 video [F, H, W, 3] on the device, in one call that never synchronises
+        (hr_render_video_to8b): frame f is bit for bit the image render_frame_to8b makes of cameras[f] at times[f].  ``out``
+        (device uint8 [F, H, W, 3], contiguous) receives it when given; the work goes on ``stream`` (a torch.cuda.Stream;
+        default the current stream)."""
+        if self.training:
+            raise RuntimeError("hyperreel_b200.LightfieldModel implements the eval()/render path only; call .eval()")
+        cams = list(cameras)
+        if not cams:
+            raise ValueError("render_video: no cameras")
+        t = [float(c.time) for c in cams] if times is None else times
+        t = torch.as_tensor(t, dtype=torch.float64).reshape(-1).to(torch.float32)
+        if t.numel() != len(cams):
+            raise ValueError(f"render_video: {len(cams)} cameras but {t.numel()} times")
+        if not bool(torch.isfinite(t).all()):
+            raise ValueError("render_video: times must be finite in float32")
+        H, W = int(cams[0].height), int(cams[0].width)
+        for i, c in enumerate(cams):
+            if (int(c.height), int(c.width)) != (H, W):
+                raise ValueError(f"render_video: camera {i} is {int(c.width)} x {int(c.height)}, camera 0 is {W} x {H}")
+        if out is not None:
+            if not out.is_cuda or out.dtype != torch.uint8 or tuple(out.shape) != (len(cams), H, W, 3) or not out.is_contiguous():
+                raise ValueError(f"render_video: out must be a contiguous CUDA uint8 tensor of shape {(len(cams), H, W, 3)}, got "
+                                 f"{out.dtype} {tuple(out.shape)} on {out.device}")
+            dev = out.device
+        else:
+            dev = torch.device("cuda", self._device_index if self._device_index is not None else torch.cuda.current_device())
+        self._ensure_uploaded(dev)
+        need = int(self._lib.hr_video_workspace_bytes(self._handle, len(cams), H, W))
+        if need < 0:
+            raise ValueError(f"render_video: {len(cams)} frames of {W} x {H} pixels overflow a 64-bit size")
+        stream = stream if stream is not None else torch.cuda.current_stream(dev)
+        recs = (L.hr_camera * len(cams))(*[c.to_c() for c in cams])
+        tt = (C.c_float * len(cams))(*t.tolist())
+        with torch.cuda.stream(stream):  # the scratch (and a new out) belong to the stream the work runs on
+            ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            if out is None:
+                out = torch.empty((len(cams), H, W, 3), dtype=torch.uint8, device=dev)
+            L.check(self._lib.hr_render_video_to8b(self._handle, recs, tt, len(cams), out.data_ptr(), ws.data_ptr(), need,
+                                                   stream.cuda_stream))
+        return out
+
     def timing(self, enable: bool = True):
         L.check(self._lib.hr_timing_enable(self._handle, int(enable)))
         L.check(self._lib.hr_timing_reset(self._handle))

@@ -339,6 +339,16 @@ class INRSystem(nn.Module):
             self.train(was_training)
         return {"val/loss": loss, "val/psnr": psnr, "val/ssim": ssim[0]}
 
+    def render_video(self, cameras, times=None, out=None, stream=None):
+        """The render split's video (validation_video, nlf/__init__.py:809-891) as uint8 [F, H, W, 3] on the device:
+        hyperreel_b200.render_video of this system's model, rendered in eval() (the previous train / eval mode is restored)."""
+        was_training = self.training
+        self.eval()
+        try:
+            return self.render_fn.model.render_video(cameras, times, out=out, stream=stream)
+        finally:
+            self.train(was_training)
+
     @staticmethod
     def validation_epoch_end(outputs):
         """get_mean_outputs(outputs, cpu=True) (metrics.py): the NumPy mean over views of every key, as a Python float (a

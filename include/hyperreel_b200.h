@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define HR_ABI_VERSION 18
+#define HR_ABI_VERSION 19
 
 #define HR_MAX_GROUPS 4   /* ray-parameterisation groups feeding the sample net (ray.py:235-263) */
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
@@ -442,6 +442,24 @@ int hr_render_to8b(hr_handle* h, const float* rays, int64_t n_rays, uint8_t* rgb
  * (pinned) host buffer rgb8_host [width*height, 3]; synchronous.  Replaces one iteration of validation_video /
  * NeRFGUI.test_step (nlf/__init__.py:828-891, utils/gui_utils.py:139-212). */
 int hr_render_frame_to8b_host(hr_handle* h, const hr_camera* cam, uint8_t* rgb8_host, int64_t chunk);
+
+/* ---- videos on the device (ABI 19) ----
+ * Replaces: the loop of validation_video over the render dataset's poses (nlf/__init__.py:809-891, run every render_every
+ * epochs and by render_only, :998-1008): per frame, rays built on the CPU, uploaded, rendered, copied back, to8b.
+ * cameras: HOST array of n_frames records, all of one width x height, each pinhole or fisheye (ABI 17); times: HOST fp32
+ * [n_frames], frame f's time column (channel 7 when c_in == 8; the records' own `time` is not used).  video: DEVICE uint8
+ * [n_frames, height, width, 3], frame f's pixels as hr_render_frame_to8b_host renders records[f] with time = times[f], bit for
+ * bit.  workspace: device scratch of hr_video_workspace_bytes(h, n_frames, height, width) bytes (16B aligned), bounded
+ * whatever n_frames: the records and times, then two slots (one for a video of at most one sub-batch), each one sub-batch
+ * of rays (hr_render's sub-batch, 16 sample-net tile waves) and its render scratch.  The video's rays are generated and
+ * rendered sub-batch by sub-batch across frame boundaries, alternating between two streams of the handle that are forked
+ * from and joined back to `stream` by events: the call is ordered on `stream` like any other work.  No host
+ * synchronisation (the records and times are copied with cudaMemcpyAsync, so the host arrays may be reused when the call
+ * returns).  Refused before anything is enqueued: n_frames < 1, frames of
+ * different sizes, a size whose output bytes overflow int64, a non-finite record field, time or fisheye coefficient. */
+int64_t hr_video_workspace_bytes(const hr_handle* h, int32_t n_frames, int32_t height, int32_t width);
+int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_frames, uint8_t* video,
+                         void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- backward pass of the path (SURVEY.md section 8 row f1) ----
  * Replaces: what loss.backward() runs for the render path inside INRSystem.training_step (nlf/__init__.py:634-709): the
