@@ -2,7 +2,8 @@
 
 Mirrors ``get_coords_from_camera`` of the reference datasets (datasets/base.py:485-518: pixel grid ->
 ``get_ray_directions_K`` -> ``get_rays`` -> optional ``to_ndc`` -> append camera id and time), the fisheye cameras of
-``ImmersiveDataset.get_coords`` (``Camera(distortion=(k1, k2))``, datasets/immersive.py:494-573) and ``to8b``
+``ImmersiveDataset.get_coords`` (``Camera(distortion=(k1, k2))``, datasets/immersive.py:494-573), the Stanford light-field
+dataset's two-plane views (``TwoPlaneCamera``, ``get_lightfield_rays``, utils/ray_utils.py:14-45) and ``to8b``
 (utils/__init__.py:47).  The reference builds the rays on the CPU and uploads 32 B per ray for every frame
 (nlf/__init__.py:828-834); here only the pose and intrinsics cross PCIe and 3 B per pixel come back.
 """
@@ -66,6 +67,68 @@ class Camera:
         k = self._distortion_f32()
         if k is not None:
             c.fisheye, (c.k1, c.k2) = 1, k
+        return c
+
+
+def _f32(name: str, value) -> float:
+    with np.errstate(over="ignore", invalid="ignore"):
+        v = np.float32(np.float64(value))
+    if not np.isfinite(v):
+        raise ValueError(f"TwoPlaneCamera: {name} = {value!r} is not finite in float32")
+    return float(v)
+
+
+@dataclass
+class TwoPlaneCamera:
+    """One view of a two-plane light field: the Stanford light-field dataset's rays (``get_lightfield_rays``,
+    utils/ray_utils.py:14-45), pixel (x, y) -> origin (s * st_scale, t * st_scale, near) and direction
+    F.normalize(u * uv_scale - s * st_scale, v * uv_scale - t * st_scale, far - near) with u = linspace(-1, 1, width)[x]
+    and v = linspace(1, -1, height)[y] / aspect.  ``aspect`` defaults to width / height; the reference passes its dataset's
+    ``img_wh`` ratio, which differs from the view's when the view is cropped.  ``lightfield_cameras`` gives a split's views.
+
+    The reference makes fp32 tensors of these Python numbers, so each is rounded to float32 (s, t, st_scale, uv_scale,
+    near, aspect, and far - near, which it subtracts in double).  The device subtracts the rounded far and near in fp32, so a
+    pair whose float32 difference is not the rounded double difference raises ``ValueError``, as does a non-finite value or
+    an aspect that rounds to 0."""
+    width: int
+    height: int
+    s: float
+    t: float
+    st_scale: float = 1.0
+    uv_scale: float = 1.0
+    near: float = -1.0
+    far: float = 0.0
+    aspect: Optional[float] = None
+    time: float = 0.0
+    cam_idx: float = 0.0
+
+    def __post_init__(self):
+        self._fields_f32()
+
+    def _fields_f32(self) -> Tuple[float, ...]:
+        if int(self.width) < 1 or int(self.height) < 1:
+            raise ValueError(f"TwoPlaneCamera: bad size {self.width} x {self.height}")
+        aspect = float(self.width) / float(self.height) if self.aspect is None else self.aspect
+        f = tuple(_f32(n, v) for n, v in (("s", self.s), ("t", self.t), ("st_scale", self.st_scale),
+                                          ("uv_scale", self.uv_scale), ("near", self.near), ("far", self.far),
+                                          ("aspect", aspect), ("time", self.time), ("cam_idx", self.cam_idx)))
+        if f[6] == 0.0:
+            raise ValueError(f"TwoPlaneCamera: aspect = {aspect!r} is 0 in float32")
+        dz = _f32("far - near", float(self.far) - float(self.near))
+        if float(np.float32(f[5]) - np.float32(f[4])) != dz:
+            raise ValueError(f"TwoPlaneCamera: far - near of far = {self.far!r}, near = {self.near!r} in float32 is not the "
+                             "reference's (the difference in double, rounded): choose near and far whose float32 difference "
+                             "is exact")
+        return f
+
+    def to_c(self) -> L.hr_camera:
+        c = L.hr_camera()
+        s, t, st, uv, near, far, aspect, time, cam_idx = self._fields_f32()
+        c.width, c.height = int(self.width), int(self.height)
+        c.two_plane = 1
+        c.lf_s, c.lf_t, c.lf_st_scale, c.lf_uv_scale = s, t, st, uv
+        c.lf_near, c.lf_far, c.lf_aspect = near, far, aspect
+        c.time, c.cam_idx = time, cam_idx
         return c
 
 
@@ -216,7 +279,7 @@ def spiral_path(dataset: str, camera: Camera, poses, bounds=None, num_frames: in
 def render_video(model_or_system, cameras: Sequence[Camera], times=None, out: Optional[torch.Tensor] = None,
                  stream=None) -> torch.Tensor:
     """uint8 video [F, H, W, 3] on the device of a LightfieldModel, RenderLightfield or INRSystem along ``cameras`` (one
-    size, pinhole or fisheye) at ``times`` (default each camera's ``time``): the reference's validation_video loop
+    size, Camera or TwoPlaneCamera, models mixed freely) at ``times`` (default each camera's ``time``): the reference's validation_video loop
     (nlf/__init__.py:809-891) with its to8b, as one call that never synchronises (hr_render_video_to8b).  ``spiral_path``
     gives the reference's cameras and times."""
     target = model_or_system if hasattr(model_or_system, "render_video") else getattr(model_or_system, "model", None)

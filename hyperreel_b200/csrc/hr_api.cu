@@ -26,7 +26,7 @@ cudaError_t launch_render_bwd(const hr_config& cfg, const Derived& dv, const Ren
                               float* g_color_embedding, const float* rays, const float* heads, const float* d_rgb, float* d_heads,
                               long long n, int clamp_output, int white_bg, int num_sms, cudaStream_t stream);
 cudaError_t launch_generate_rays(const hr_camera& cam, int c_in, long long first, long long n, float* out, cudaStream_t st);
-cudaError_t launch_generate_video_rays(const hr_camera* cams, const float* times, bool fisheye, int c_in, int width,
+cudaError_t launch_generate_video_rays(const hr_camera* cams, const float* times, bool mixed, int c_in, int width,
                                        long long frame_px, long long first, long long n, float* out, cudaStream_t st);
 }  // namespace hr
 
@@ -842,11 +842,24 @@ int hr_render_to8b(hr_handle* h, const float* rays, int64_t n_rays, uint8_t* rgb
 // A fisheye record needs finite coefficients: the Newton solve of camera_ray has no meaning otherwise.
 static bool bad_fisheye(const hr_camera& cam) { return cam.fisheye && !(std::isfinite(cam.k1) && std::isfinite(cam.k2)); }
 
+// Why a two-plane record cannot be drawn, or nullptr: it is one model or the other, and its fields must be finite with a
+// nonzero aspect (lightfield_ray divides by it).
+static const char* bad_two_plane(const hr_camera& cam) {
+  if (!cam.two_plane) return nullptr;
+  if (cam.fisheye) return "two_plane and fisheye are both set";
+  const float f[7] = {cam.lf_s, cam.lf_t, cam.lf_st_scale, cam.lf_uv_scale, cam.lf_near, cam.lf_far, cam.lf_aspect};
+  for (float v : f)
+    if (!std::isfinite(v)) return "a two-plane field (lf_*) is not finite";
+  if (cam.lf_aspect == 0.0f) return "lf_aspect is 0";
+  return nullptr;
+}
+
 int hr_generate_rays(const hr_camera* cam, int32_t c_in, int64_t first_pixel, int64_t n_pixels, float* rays_out, void* stream) {
   if (!cam || !rays_out) return fail("hr_generate_rays: null argument");
   if (c_in != 6 && c_in != 8) return fail("hr_generate_rays: c_in must be 6 or 8");
   if (cam->width < 1 || cam->height < 1) return fail("hr_generate_rays: bad image size");
   if (bad_fisheye(*cam)) return fail("hr_generate_rays: fisheye coefficients k1 = %g, k2 = %g are not finite", cam->k1, cam->k2);
+  if (const char* why = bad_two_plane(*cam)) return fail("hr_generate_rays: %s", why);
   if (first_pixel < 0 || n_pixels < 0 || first_pixel + n_pixels > (int64_t)cam->width * cam->height)
     return fail("hr_generate_rays: pixel range outside the image");
   cudaError_t e = hr::launch_generate_rays(*cam, c_in, first_pixel, n_pixels, rays_out, (cudaStream_t)stream);
@@ -859,6 +872,7 @@ int hr_render_frame_to8b_host(hr_handle* h, const hr_camera* cam, uint8_t* rgb8_
   if (!h->uploaded) return fail("hr_render_frame_to8b_host: parameters not uploaded");
   if (bad_fisheye(*cam))
     return fail("hr_render_frame_to8b_host: fisheye coefficients k1 = %g, k2 = %g are not finite", cam->k1, cam->k2);
+  if (const char* why = bad_two_plane(*cam)) return fail("hr_render_frame_to8b_host: %s", why);
   DeviceGuard guard(h->device);
   const hr_config& c = h->cfg;
   const int64_t n_rays = (int64_t)cam->width * cam->height;
@@ -951,7 +965,7 @@ int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* ti
   const int32_t W = cameras[0].width, H = cameras[0].height;
   const int64_t n = video_rays(n_frames, H, W);
   if (n < 0) return fail("hr_render_video_to8b: %d frames of %d x %d pixels: bad size or output bytes overflow int64", n_frames, W, H);
-  bool fisheye = false;
+  bool mixed = false;  // any record not a pinhole: the ray kernel's instantiation that branches on each record's model
   for (int32_t f = 0; f < n_frames; ++f) {
     const hr_camera& c = cameras[f];
     if (c.width != W || c.height != H)
@@ -959,8 +973,9 @@ int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* ti
     if (!finite_camera(c)) return fail("hr_render_video_to8b: camera record of frame %d is not finite", f);
     if (bad_fisheye(c))
       return fail("hr_render_video_to8b: fisheye coefficients k1 = %g, k2 = %g of frame %d are not finite", c.k1, c.k2, f);
+    if (const char* why = bad_two_plane(c)) return fail("hr_render_video_to8b: frame %d: %s", f, why);
     if (!std::isfinite(times[f])) return fail("hr_render_video_to8b: time of frame %d is not finite", f);
-    fisheye = fisheye || c.fisheye;
+    mixed = mixed || c.fisheye || c.two_plane;
   }
   const int64_t need = hr_video_workspace_bytes(h, n_frames, H, W);
   if (workspace_bytes < need) return fail("hr_render_video_to8b: workspace too small (%lld < %lld)", (long long)workspace_bytes, (long long)need);
@@ -1000,7 +1015,7 @@ int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* ti
     cudaStream_t s = ss[i % 2];
     char* slot = p + (i % n_slots) * slot_bytes;
     float* d_rays = (float*)slot;
-    cudaError_t e = hr::launch_generate_video_rays(d_cams, d_times, fisheye, c.c_in, W, frame_px, off, m, d_rays, s);
+    cudaError_t e = hr::launch_generate_video_rays(d_cams, d_times, mixed, c.c_in, W, frame_px, off, m, d_rays, s);
     if (e != cudaSuccess) {
       rc = fail("video ray generation failed: %s", cudaGetErrorString(e));
       break;

@@ -1,8 +1,8 @@
 // Camera -> ray arithmetic, one definition shared by generate_rays_kernel (hr_rays.cu) and the training-batch kernels
 // (hr_train_batch.cu): a training row must be bit-identical to the row hr_generate_rays writes for the same pixel.
 // Reference: get_ray_directions_from_pixels_K / get_rays / get_ndc_rays_fx_fy (utils/ray_utils.py:98-164) as driven by
-// get_coords_from_camera (datasets/base.py:485-518), and for fisheye cameras ImmersiveDataset.get_coords
-// (datasets/immersive.py:494-573).
+// get_coords_from_camera (datasets/base.py:485-518), for fisheye cameras ImmersiveDataset.get_coords
+// (datasets/immersive.py:494-573), and for two-plane light-field views get_lightfield_rays (utils/ray_utils.py:14-45).
 #pragma once
 #include "hr_common.cuh"
 
@@ -58,14 +58,45 @@ __device__ __forceinline__ float3 fisheye_direction(float xf, float yf, float k1
   return make_float3(__fdiv_rn(u, nrm), __fdiv_rn(v, nrm), __fdiv_rn(-1.0f, nrm));
 }
 
+// Element i of torch.linspace(start, end, steps) in fp32 as torch's CPU kernel computes it: step = (end - start) / (steps - 1),
+// start + step * i below the midpoint steps / 2 and end - step * (steps - 1 - i) from it, each a fused multiply-add (the
+// kernel is compiled with contraction); [start] for one step.
+__device__ __forceinline__ float torch_linspace(float start, float end, int steps, int i) {
+  if (steps == 1) return start;
+  const float step = __fdiv_rn(__fsub_rn(end, start), (float)(steps - 1));
+  return i < steps / 2 ? __fmaf_rn(step, (float)i, start) : __fmaf_rn(-step, (float)(steps - 1 - i), end);
+}
+
+// The two-plane light-field ray of pixel (x, y) of a Stanford view (cam.two_plane; get_lightfield_rays, ray_utils.py:14-45):
+// u = linspace(-1, 1, W)[x] * uv_scale, v = (linspace(1, -1, H)[y] / aspect) * uv_scale, S = s * st_scale, T = t * st_scale
+// (the reference's `ones * s * st_scale`: s rounded to fp32, then one fp32 product), origin (S, T, near), direction
+// F.normalize((u - S, v - T, far - near)): x / max(|x|, 1e-12) with torch's CPU norm, sqrt(fma(x2, x2, fma(x1, x1, x0 x0)))
+// (not camera_ray's order: get_rays' norm is a different reduction).  Then cam_idx and time.
+__device__ __forceinline__ void lightfield_ray(const hr_camera& cam, int x, int y, float (&row)[8]) {
+  const float u = __fmul_rn(torch_linspace(-1.0f, 1.0f, cam.width, x), cam.lf_uv_scale);
+  const float v = __fmul_rn(__fdiv_rn(torch_linspace(1.0f, -1.0f, cam.height, y), cam.lf_aspect), cam.lf_uv_scale);
+  const float s = __fmul_rn(cam.lf_s, cam.lf_st_scale), t = __fmul_rn(cam.lf_t, cam.lf_st_scale);
+  const float d0 = __fsub_rn(u, s), d1 = __fsub_rn(v, t), d2 = __fsub_rn(cam.lf_far, cam.lf_near);
+  float nrm = sqrtf(__fmaf_rn(d2, d2, __fmaf_rn(d1, d1, __fmul_rn(d0, d0))));
+  nrm = fmaxf(nrm, 1e-12f);
+  row[0] = s; row[1] = t; row[2] = cam.lf_near;
+  row[3] = __fdiv_rn(d0, nrm); row[4] = __fdiv_rn(d1, nrm); row[5] = __fdiv_rn(d2, nrm);
+  row[6] = cam.cam_idx; row[7] = cam.time;
+}
+
 // The ray of pixel (x, y) as the reference's coords row: origin, direction, then cam_idx and time (channels 6 and 7 when
 // c_in == 8, technicolor.py:389-393).  kFisheye: records with cam.fisheye set take the fisheye direction (fisheye_direction);
 // without it every record is a pinhole.  The fp64 solve costs registers (DESIGN 4.4), out of line as well: a call keeps the
 // caller's live values and the callee's in one budget.  So generate_rays_kernel, whose one record the host reads, has a
 // pinhole instantiation with the pinhole path's registers; the training kernels read their records on the device and
-// always branch on the flag.
-template <bool kFisheye>
+// always branch on the flag.  kTwoPlane: records with cam.two_plane set are light-field views (lightfield_ray); without it
+// the flag is not read, and the code is what it was before two-plane records existed.
+template <bool kFisheye, bool kTwoPlane = false>
 __device__ __forceinline__ void camera_ray(const hr_camera& cam, int x, int y, NdcScale ndc, float (&row)[8]) {
+  if (kTwoPlane && cam.two_plane) {
+    lightfield_ray(cam, x, y, row);
+    return;
+  }
   const float px = (float)x, py = (float)y;
   const float off = cam.centered_pixels ? 0.5f : 0.0f;
   // get_ray_directions_from_pixels_K (ray_utils.py:98-115)

@@ -15,7 +15,8 @@
 //
 // One thread per row: one 3-byte gather and one 48-byte row write (plus 8 B of pixel id when asked).  No float atomics, no
 // host synchronisation; two calls with the same arguments write the same bits.  The camera records live on the device, so
-// each row branches on its own record's fisheye flag (camera_ray<true>) and one batch may mix fisheye and pinhole views.
+// each row branches on its own record's fisheye and two_plane flags (camera_ray<true, true>) and one batch may mix pinhole,
+// fisheye and two-plane views.
 #include <algorithm>
 #include <vector>
 
@@ -82,7 +83,7 @@ train_batch_kernel(const hr_camera* __restrict__ cams, const uint8_t* __restrict
       const long long q = p - v * hw;
       const int y = (int)(q / width), x = (int)(q - (long long)y * width);
       const hr_camera& cam = cams[v];
-      camera_ray<true>(cam, x, y, ndc_scale(cam), row);
+      camera_ray<true, true>(cam, x, y, ndc_scale(cam), row);
       const uint8_t* px = images + 3 * p;
       c0 = __fdiv_rn((float)px[0], 255.0f);
       c1 = __fdiv_rn((float)px[1], 255.0f);
@@ -265,7 +266,7 @@ train_rows_kernel(const hr_camera* __restrict__ cams, const uint8_t* __restrict_
     if (table_pixel(plan, start, height, width, k, v, y, x)) {
       p = v * hw + (long long)y * width + x;
       const hr_camera& cam = cams[v];
-      camera_ray<true>(cam, x, y, ndc_scale(cam), row);
+      camera_ray<true, true>(cam, x, y, ndc_scale(cam), row);
       const uint8_t* px = images + 3 * p;
       c0 = __fdiv_rn((float)px[0], 255.0f);
       c1 = __fdiv_rn((float)px[1], 255.0f);
@@ -404,7 +405,7 @@ importance_mask_kernel(const hr_camera* __restrict__ cams, const uint8_t* __rest
     if (p < hw && diff_key(cur + 3 * p, prev + 3 * p) > thr) {
       const int y = (int)(p / width), x = (int)(p - (long long)y * width);
       float row[8];
-      camera_ray<true>(cam, x, y, ndc_scale(cam), row);
+      camera_ray<true, true>(cam, x, y, ndc_scale(cam), row);
       keep = row[5] < -0.05f;  // coords[..., 5] < -0.05 of an fp32 tensor compares in fp32
     }
     const uint32_t bits = __ballot_sync(0xffffffffu, keep);

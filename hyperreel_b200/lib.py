@@ -11,7 +11,7 @@ import os
 import subprocess
 import threading
 
-HR_ABI_VERSION = 19
+HR_ABI_VERSION = 20
 HR_MAX_GROUPS = 4
 HR_MAX_LAYERS = 10
 HR_MAX_SAMPLES = 256
@@ -132,6 +132,8 @@ class hr_camera(C.Structure):
         ("width", C.c_int32), ("height", C.c_int32), ("centered_pixels", C.c_int32), ("flipped", C.c_int32),
         ("normalize", C.c_int32), ("use_ndc", C.c_int32), ("ndc_near", C.c_float), ("cam_idx", C.c_float),
         ("time", C.c_float), ("fisheye", C.c_int32), ("k1", C.c_float), ("k2", C.c_float),
+        ("two_plane", C.c_int32), ("lf_s", C.c_float), ("lf_t", C.c_float), ("lf_st_scale", C.c_float),
+        ("lf_uv_scale", C.c_float), ("lf_near", C.c_float), ("lf_far", C.c_float), ("lf_aspect", C.c_float),
     ]
 
 

@@ -481,7 +481,7 @@ class LightfieldModel(nn.Module):
         return out
 
     def render_frame_to8b(self, camera, out_host: Optional[torch.Tensor] = None, chunk: int = 0) -> torch.Tensor:
-        """One whole frame: rays generated on the device from ``camera`` (hyperreel_b200.camera.Camera), rendered,
+        """One whole frame: rays generated on the device from ``camera`` (hyperreel_b200.camera.Camera or TwoPlaneCamera), rendered,
         packed to 8 bit and copied into a pinned host image [H, W, 3] uint8 (hr_render_frame_to8b_host) -- one iteration of
         the reference's validation_video / viewer loop without the per-frame 32 B/ray upload."""
         if self.training:
@@ -497,7 +497,7 @@ class LightfieldModel(nn.Module):
         return out_host
 
     def render_video(self, cameras, times=None, out: Optional[torch.Tensor] = None, stream=None) -> torch.Tensor:
-        """Frames of ``cameras`` (hyperreel_b200.camera.Camera, one size, pinhole or fisheye) at ``times`` (one per camera;
+        """Frames of ``cameras`` (hyperreel_b200.camera.Camera or TwoPlaneCamera, one size, any mix of models) at ``times`` (one per camera;
         default each camera's ``time``) -> uint8 video [F, H, W, 3] on the device, in one call that never synchronises
         (hr_render_video_to8b): frame f is bit for bit the image render_frame_to8b makes of cameras[f] at times[f].  ``out``
         (device uint8 [F, H, W, 3], contiguous) receives it when given; the work goes on ``stream`` (a torch.cuda.Stream;

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define HR_ABI_VERSION 19
+#define HR_ABI_VERSION 20
 
 #define HR_MAX_GROUPS 4   /* ray-parameterisation groups feeding the sample net (ray.py:235-263) */
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
@@ -337,6 +337,14 @@ typedef struct hr_camera {
   float cam_idx, time;      /* channels 6 and 7 when c_in == 8 (technicolor.py:389-393)             */
   int32_t fisheye;          /* 0: pinhole; otherwise the two-coefficient fisheye below (ABI 17)     */
   float k1, k2;             /* radial_distortion[:2] of the camera in models.json, as float32       */
+  int32_t two_plane;        /* 0: c2w / K camera above; otherwise the light-field view below (ABI 20) */
+  float lf_s;               /* s of the view on the st plane (LightfieldDataset.get_coord), as float32 */
+  float lf_t;               /* t of the view, as float32                                            */
+  float lf_st_scale;        /* st_scale (vis_st_scale for the render split), as float32             */
+  float lf_uv_scale;        /* uv_scale (vis_uv_scale for the render split), as float32             */
+  float lf_near;            /* near plane z (lightfield.near, default -1), as float32               */
+  float lf_far;             /* far plane z (lightfield.far, default 0), as float32                  */
+  float lf_aspect;          /* the dataset's aspect, img_wh[0] / img_wh[1], as float32; nonzero     */
 } hr_camera;
 /* Fisheye cameras (ABI 17): the Immersive dataset's train and validation views (ImmersiveDataset.get_coords,
  * datasets/immersive.py:494-573).  When fisheye != 0 the pinhole direction's (x, y) -- centred pixels, y negated unless
@@ -345,7 +353,20 @@ typedef struct hr_camera {
  * point the solve does not bring back (no convergence in 10 Newton steps, or a flipped angle) becomes OpenCV's (-1e6, -1e6)
  * and its row is written like any other, as the reference does.  k1 = k2 = 0 is not the pinhole (the radius maps
  * r -> tan r), hence the flag.  k1 and k2 must be finite: hr_generate_rays and hr_render_frame_to8b_host refuse a fisheye
- * record otherwise and write nothing.  The render split's cameras (K * 0.75, no distortion) are pinholes. */
+ * record otherwise and write nothing.  The render split's cameras (K * 0.75, no distortion) are pinholes.
+ * Two-plane light-field views (ABI 20): the Stanford light-field dataset's views (get_lightfield_rays, utils/ray_utils.py:14-45,
+ * as LightfieldDataset.get_coords drives it, datasets/lightfield.py:193-219).  When two_plane != 0, c2w, K, centered_pixels,
+ * flipped, normalize, use_ndc, ndc_near and the fisheye fields are ignored, and pixel (x, y) of the width x height view is the
+ * row, in fp32 with each operation rounded as torch's CPU kernels round it,
+ *   S = s * st_scale, T = t * st_scale, u = linspace(-1, 1, width)[x] * uv_scale, v = (linspace(1, -1, height)[y] / aspect) * uv_scale,
+ *   origin (S, T, near), direction F.normalize((u - S, v - T, far - near)),
+ * with linspace evaluated as torch's CPU kernel does (fma(step, i, start) below the midpoint, fma(-step, steps - 1 - i, end)
+ * from it; [start] for one step) and the norm as sqrt(fma(dz, dz, fma(dy, dy, dx * dx))), then cam_idx and time as for the
+ * other models.  The reference subtracts far - near in double; the record's
+ * far - near in fp32 must be that value rounded (hyperreel_b200.TwoPlaneCamera checks it).  hr_generate_rays,
+ * hr_render_frame_to8b_host and hr_render_video_to8b refuse, and write nothing for, a record with both two_plane and fisheye
+ * set, a non-finite lf_* field or lf_aspect == 0.  The training entry points read their records on the device and do not
+ * inspect them: the same must hold there. */
 
 /* rays_out [n_pixels, c_in] fp32 device, for pixels first_pixel .. first_pixel + n_pixels - 1; c_in is 6 or 8. */
 int hr_generate_rays(const hr_camera* cam, int32_t c_in, int64_t first_pixel, int64_t n_pixels, float* rays_out,
@@ -367,8 +388,9 @@ int hr_generate_rays(const hr_camera* cam, int32_t c_in, int64_t first_pixel, in
  *   rgb [n, 3] fp32, u8 / 255 (T.ToTensor());  weight [n, 1] fp32, 1;  pixel_ids [n] int64 (may be NULL), the pixel of each row.
  * An order entry outside [0, N) gives a zero row of weight 0 and pixel id -1.  coords, order and pixel_ids 8-byte aligned, the
  * rest 4.  No float atomics, no host synchronisation: two calls with the same arguments write the same bits.
- * Each row takes its view's camera model (ABI 17: a fisheye record's rays as hr_generate_rays writes them), so one batch may
- * mix fisheye and pinhole views; the records' fisheye coefficients must be finite (the device array is not inspected). */
+ * Each row takes its view's camera model (ABI 17: a fisheye record's rays as hr_generate_rays writes them; ABI 20: a two-plane
+ * record's), so one batch may mix pinhole, fisheye and two-plane views; the records' fisheye coefficients must be finite and
+ * their two-plane records well formed as hr_generate_rays requires (the device array is not inspected). */
 int hr_sample_train_batch(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height, int32_t width,
                           int32_t c_in, uint64_t seed, int64_t epoch, int64_t batch_index, int64_t batch_size,
                           const int64_t* order, float* coords, float* rgb, float* weight, int64_t* pixel_ids, int64_t* n_rows,
@@ -446,7 +468,7 @@ int hr_render_frame_to8b_host(hr_handle* h, const hr_camera* cam, uint8_t* rgb8_
 /* ---- videos on the device (ABI 19) ----
  * Replaces: the loop of validation_video over the render dataset's poses (nlf/__init__.py:809-891, run every render_every
  * epochs and by render_only, :998-1008): per frame, rays built on the CPU, uploaded, rendered, copied back, to8b.
- * cameras: HOST array of n_frames records, all of one width x height, each pinhole or fisheye (ABI 17); times: HOST fp32
+ * cameras: HOST array of n_frames records, all of one width x height, each pinhole, fisheye (ABI 17) or two-plane (ABI 20); times: HOST fp32
  * [n_frames], frame f's time column (channel 7 when c_in == 8; the records' own `time` is not used).  video: DEVICE uint8
  * [n_frames, height, width, 3], frame f's pixels as hr_render_frame_to8b_host renders records[f] with time = times[f], bit for
  * bit.  workspace: device scratch of hr_video_workspace_bytes(h, n_frames, height, width) bytes (16B aligned), bounded
@@ -456,7 +478,8 @@ int hr_render_frame_to8b_host(hr_handle* h, const hr_camera* cam, uint8_t* rgb8_
  * from and joined back to `stream` by events: the call is ordered on `stream` like any other work.  No host
  * synchronisation (the records and times are copied with cudaMemcpyAsync, so the host arrays may be reused when the call
  * returns).  Refused before anything is enqueued: n_frames < 1, frames of
- * different sizes, a size whose output bytes overflow int64, a non-finite record field, time or fisheye coefficient. */
+ * different sizes, a size whose output bytes overflow int64, a non-finite record field, time or fisheye coefficient, a
+ * malformed two-plane record (ABI 20). */
 int64_t hr_video_workspace_bytes(const hr_handle* h, int32_t n_frames, int32_t height, int32_t width);
 int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_frames, uint8_t* video,
                          void* workspace, int64_t workspace_bytes, void* stream);
