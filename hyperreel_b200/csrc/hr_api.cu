@@ -21,10 +21,9 @@ namespace hr {
 cudaError_t launch_render(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs, const float* rays,
                           const float* heads, const RgbDst& rgb, long long n, const ExtraOut* so, int num_sms,
                           cudaStream_t stream, unsigned char* rgb8);
-cudaError_t launch_render_bwd(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs, float* const* g_sig_space,
-                              float* const* g_sig_second, float* const* g_app_space, float* const* g_app_second, float* g_basis,
-                              float* g_color_embedding, const float* rays, const float* heads, const float* d_rgb, float* d_heads,
-                              long long n, int clamp_output, int white_bg, int num_sms, cudaStream_t stream);
+cudaError_t launch_render_bwd(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs, const GradTabs& gt, const float* rays,
+                              const float* heads, const float* d_rgb, float* d_heads, long long n, int clamp_output, int white_bg,
+                              int num_sms, cudaStream_t stream);
 cudaError_t launch_generate_rays(const hr_camera& cam, int c_in, long long first, long long n, float* out, cudaStream_t st);
 cudaError_t launch_generate_video_rays(const hr_camera* cams, const float* times, bool mixed, int c_in, int width,
                                        long long frame_px, long long first, long long n, float* out, cudaStream_t st);
@@ -33,16 +32,6 @@ cudaError_t launch_generate_video_rays(const hr_camera* cams, const float* times
 static thread_local std::string g_err;
 
 int hr_fail(const char* fmt, ...) {
-  char buf[1024];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  g_err = buf;
-  return 1;
-}
-
-static int fail(const char* fmt, ...) {
   char buf[1024];
   va_list ap;
   va_start(ap, fmt);
@@ -65,10 +54,10 @@ struct DeviceGuard {
   }
 };
 
-#define CK(expr)                                                                                   \
-  do {                                                                                             \
-    cudaError_t _e = (expr);                                                                       \
-    if (_e != cudaSuccess) return fail("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
+#define CK(expr)                                                                                                        \
+  do {                                                                                                                  \
+    cudaError_t _e = (expr);                                                                                            \
+    if (_e != cudaSuccess) return hr_fail("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
   } while (0)
 
 #include "hr_handle.h"
@@ -275,7 +264,7 @@ int dev_alloc(hr_handle* h, void** p, size_t bytes) {
     h->slots.push_back({nullptr, 0});
   }
   cudaError_t e = cudaMalloc(p, bytes);
-  if (e != cudaSuccess) return fail("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
+  if (e != cudaSuccess) return hr_fail("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
   h->slots[i] = {*p, bytes};
   return 0;
 }
@@ -288,78 +277,78 @@ int stage_in(const float* src, size_t count, int on_device, cudaStream_t st, std
   }
   void* d = nullptr;
   cudaError_t e = cudaMalloc(&d, count * sizeof(float));
-  if (e != cudaSuccess) return fail("cudaMalloc(temp %zu) failed: %s", count * sizeof(float), cudaGetErrorString(e));
+  if (e != cudaSuccess) return hr_fail("cudaMalloc(temp %zu) failed: %s", count * sizeof(float), cudaGetErrorString(e));
   temps.push_back(d);
   e = cudaMemcpyAsync(d, src, count * sizeof(float), cudaMemcpyHostToDevice, st);
-  if (e != cudaSuccess) return fail("H2D of parameters failed: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return hr_fail("H2D of parameters failed: %s", cudaGetErrorString(e));
   *out = (const float*)d;
   return 0;
 }
 
 int validate(const hr_config& c) {
-  if (c.abi_version != HR_ABI_VERSION) return fail("hr_config.abi_version %d != %d", c.abi_version, HR_ABI_VERSION);
-  if (hr::eases_density(c) && c.n_samples > 64) return fail("eased density heads above 64 samples per ray are not supported");
-  if (c.c_in != 6 && c.c_in != 8) return fail("unsupported c_in %d (6: static rays, 8: video rays)", c.c_in);
-  if (c.n_groups < 1 || c.n_groups > HR_MAX_GROUPS) return fail("unsupported n_groups %d", c.n_groups);
-  if (c.mlp_mode != HR_MLP_FP32_SIMT && c.mlp_mode != HR_MLP_BF16X3_TC && c.mlp_mode != HR_MLP_ZERO) return fail("unsupported mlp_mode");
+  if (c.abi_version != HR_ABI_VERSION) return hr_fail("hr_config.abi_version %d != %d", c.abi_version, HR_ABI_VERSION);
+  if (hr::eases_density(c) && c.n_samples > 64) return hr_fail("eased density heads above 64 samples per ray are not supported");
+  if (c.c_in != 6 && c.c_in != 8) return hr_fail("unsupported c_in %d (6: static rays, 8: video rays)", c.c_in);
+  if (c.n_groups < 1 || c.n_groups > HR_MAX_GROUPS) return hr_fail("unsupported n_groups %d", c.n_groups);
+  if (c.mlp_mode != HR_MLP_FP32_SIMT && c.mlp_mode != HR_MLP_BF16X3_TC && c.mlp_mode != HR_MLP_ZERO) return hr_fail("unsupported mlp_mode");
   const bool has_net = c.mlp_mode != HR_MLP_ZERO;
-  if (has_net && (c.mlp_layers < 2 || c.mlp_layers > HR_MAX_LAYERS)) return fail("unsupported mlp_layers %d", c.mlp_layers);
-  if (has_net && c.mlp_width != 128 && c.mlp_width != 256) return fail("unsupported mlp_width %d (128 or 256)", c.mlp_width);
-  if (c.mlp_in < 1 || c.mlp_in > 64) return fail("unsupported mlp_in %d", c.mlp_in);
-  if (has_net && c.mlp_skip != -1 && (c.mlp_skip < 1 || c.mlp_skip > c.mlp_layers - 2)) return fail("bad mlp_skip %d", c.mlp_skip);
-  if (c.n_samples < 1 || c.n_samples > HR_MAX_SAMPLES) return fail("unsupported n_samples %d (max %d)", c.n_samples, HR_MAX_SAMPLES);
-  if (c.mlp_out != c.n_samples * c.head_stride) return fail("mlp_out %d != S*head_stride %d", c.mlp_out, c.n_samples * c.head_stride);
-  if (c.off_z < 0) return fail("z_vals head is required");
-  if ((c.isect_type == HR_ISECT_Z_PLANE || c.isect_type == HR_ISECT_DISTANCE) && c.n_z != 1) return fail("z_plane / euclidean_distance need 1 z channel");
-  if ((c.isect_type == HR_ISECT_SPHERE || c.isect_type == HR_ISECT_CYLINDER) && c.n_z != 4) return fail("sphere / cylinder need 4 z channels");
-  if (c.isect_type == HR_ISECT_SPHERE_NEW && c.n_z != 8) return fail("sphere_new needs 8 z channels");
-  if (c.isect_type < HR_ISECT_Z_PLANE || c.isect_type > HR_ISECT_PLANE) return fail("unsupported intersect type %d", c.isect_type);
+  if (has_net && (c.mlp_layers < 2 || c.mlp_layers > HR_MAX_LAYERS)) return hr_fail("unsupported mlp_layers %d", c.mlp_layers);
+  if (has_net && c.mlp_width != 128 && c.mlp_width != 256) return hr_fail("unsupported mlp_width %d (128 or 256)", c.mlp_width);
+  if (c.mlp_in < 1 || c.mlp_in > 64) return hr_fail("unsupported mlp_in %d", c.mlp_in);
+  if (has_net && c.mlp_skip != -1 && (c.mlp_skip < 1 || c.mlp_skip > c.mlp_layers - 2)) return hr_fail("bad mlp_skip %d", c.mlp_skip);
+  if (c.n_samples < 1 || c.n_samples > HR_MAX_SAMPLES) return hr_fail("unsupported n_samples %d (max %d)", c.n_samples, HR_MAX_SAMPLES);
+  if (c.mlp_out != c.n_samples * c.head_stride) return hr_fail("mlp_out %d != S*head_stride %d", c.mlp_out, c.n_samples * c.head_stride);
+  if (c.off_z < 0) return hr_fail("z_vals head is required");
+  if ((c.isect_type == HR_ISECT_Z_PLANE || c.isect_type == HR_ISECT_DISTANCE) && c.n_z != 1) return hr_fail("z_plane / euclidean_distance need 1 z channel");
+  if ((c.isect_type == HR_ISECT_SPHERE || c.isect_type == HR_ISECT_CYLINDER) && c.n_z != 4) return hr_fail("sphere / cylinder need 4 z channels");
+  if (c.isect_type == HR_ISECT_SPHERE_NEW && c.n_z != 8) return hr_fail("sphere_new needs 8 z channels");
+  if (c.isect_type < HR_ISECT_Z_PLANE || c.isect_type > HR_ISECT_PLANE) return hr_fail("unsupported intersect type %d", c.isect_type);
   if (c.isect_type == HR_ISECT_VOXEL && (c.n_z != 1 || c.isect_axes != 3 || c.n_samples % 3 != 0))
-    return fail("voxel_grid needs 1 z channel and a multiple of 3 samples");
+    return hr_fail("voxel_grid needs 1 z channel and a multiple of 3 samples");
   if (c.isect_type == HR_ISECT_PLANE && (c.n_z != 4 || c.isect_axes < 1 || c.isect_axes > 3 || c.n_samples % c.isect_axes != 0))
-    return fail("deformable_voxel_grid needs 4 z channels and 1-3 axes dividing the sample count");
+    return hr_fail("deformable_voxel_grid needs 4 z channels and 1-3 axes dividing the sample count");
   if (c.cascade) {
-    if (c.pre_samples < 1 || c.pre_samples > 32 || c.n_samples % c.pre_samples != 0) return fail("cascade: bad pre_samples %d", c.pre_samples);
-    if (c.mlp_mode == HR_MLP_ZERO) return fail("cascade: the point net cannot be a zero net");
-    if (c.pre_mlp_mode != HR_MLP_ZERO && c.pre_mlp_mode != c.mlp_mode) return fail("cascade: pre_mlp_mode must be zero or mlp_mode");
+    if (c.pre_samples < 1 || c.pre_samples > 32 || c.n_samples % c.pre_samples != 0) return hr_fail("cascade: bad pre_samples %d", c.pre_samples);
+    if (c.mlp_mode == HR_MLP_ZERO) return hr_fail("cascade: the point net cannot be a zero net");
+    if (c.pre_mlp_mode != HR_MLP_ZERO && c.pre_mlp_mode != c.mlp_mode) return hr_fail("cascade: pre_mlp_mode must be zero or mlp_mode");
     if (c.pre_head_stride < 1 || c.pre_off_z < 0 || c.pre_off_z >= c.pre_head_stride || c.pre_off_sigma >= c.pre_head_stride)
-      return fail("cascade: bad first-stage head layout");
+      return hr_fail("cascade: bad first-stage head layout");
     if (c.pre_mlp_mode != HR_MLP_ZERO) {
-      if (c.pre_n_groups < 1 || c.pre_n_groups > HR_MAX_GROUPS) return fail("cascade: unsupported pre_n_groups %d", c.pre_n_groups);
-      if (c.pre_mlp_layers < 2 || c.pre_mlp_layers > HR_MAX_LAYERS) return fail("cascade: unsupported pre_mlp_layers %d", c.pre_mlp_layers);
-      if (c.pre_mlp_width != 128 && c.pre_mlp_width != 256) return fail("cascade: unsupported pre_mlp_width %d", c.pre_mlp_width);
-      if (c.pre_mlp_in < 1 || c.pre_mlp_in > 64) return fail("cascade: unsupported pre_mlp_in %d", c.pre_mlp_in);
-      if (c.pre_mlp_skip != -1 && (c.pre_mlp_skip < 1 || c.pre_mlp_skip > c.pre_mlp_layers - 2)) return fail("cascade: bad pre_mlp_skip");
-      if ((c.pre_samples * c.pre_head_stride) % 4 != 0) return fail("cascade: first-stage output width must be a multiple of 4");
+      if (c.pre_n_groups < 1 || c.pre_n_groups > HR_MAX_GROUPS) return hr_fail("cascade: unsupported pre_n_groups %d", c.pre_n_groups);
+      if (c.pre_mlp_layers < 2 || c.pre_mlp_layers > HR_MAX_LAYERS) return hr_fail("cascade: unsupported pre_mlp_layers %d", c.pre_mlp_layers);
+      if (c.pre_mlp_width != 128 && c.pre_mlp_width != 256) return hr_fail("cascade: unsupported pre_mlp_width %d", c.pre_mlp_width);
+      if (c.pre_mlp_in < 1 || c.pre_mlp_in > 64) return hr_fail("cascade: unsupported pre_mlp_in %d", c.pre_mlp_in);
+      if (c.pre_mlp_skip != -1 && (c.pre_mlp_skip < 1 || c.pre_mlp_skip > c.pre_mlp_layers - 2)) return hr_fail("cascade: bad pre_mlp_skip");
+      if ((c.pre_samples * c.pre_head_stride) % 4 != 0) return hr_fail("cascade: first-stage output width must be a multiple of 4");
     }
-    if ((c.mlp_out / c.pre_samples) % 4 != 0) return fail("cascade: the point net's output width must be a multiple of 4");
+    if ((c.mlp_out / c.pre_samples) % 4 != 0) return hr_fail("cascade: the point net's output width must be a multiple of 4");
     for (int g = 0; g < c.n_groups; ++g)
-      if (c.groups[g].start < 0 || c.groups[g].end > 8) return fail("cascade: point-net param group outside the 8-channel row");
+      if (c.groups[g].start < 0 || c.groups[g].end > 8) return hr_fail("cascade: point-net param group outside the 8-channel row");
   }
-  if (c.n_color_views < 0) return fail("bad n_color_views");
-  if (c.n_color_views > 0 && c.c_in != 8) return fail("colour transform needs 8-channel rays (camera id = rays[:, -2])");
-  if (c.n_color_views > 0 && c.off_cscale_global >= 0) return fail("colour transform and global colour heads are exclusive");
+  if (c.n_color_views < 0) return hr_fail("bad n_color_views");
+  if (c.n_color_views > 0 && c.c_in != 8) return hr_fail("colour transform needs 8-channel rays (camera id = rays[:, -2])");
+  if (c.n_color_views > 0 && c.off_cscale_global >= 0) return hr_fail("colour transform and global colour heads are exclusive");
   if (c.contract_type != HR_CONTRACT_NONE && c.contract_type != HR_CONTRACT_MIPNERF && c.contract_type != HR_CONTRACT_AFFINE)
-    return fail("unsupported contract type");
+    return hr_fail("unsupported contract type");
   if (c.contract_type == HR_CONTRACT_AFFINE) {
     for (int i = 0; i < 3; ++i)
-      if (c.contract_affine_den[i] == 0.0f) return fail("affine contraction: zero extent on axis %d", i);
-    if (c.contract_dist_fac == 0.0f) return fail("affine contraction: zero distance factor");
+      if (c.contract_affine_den[i] == 0.0f) return hr_fail("affine contraction: zero extent on axis %d", i);
+    if (c.contract_dist_fac == 0.0f) return hr_fail("affine contraction: zero distance factor");
   }
-  if ((c.off_cscale_global >= 0) != (c.off_cshift_global >= 0)) return fail("color_scale_global and color_shift_global come together");
-  if (c.off_cscale_global + 3 > c.head_stride || c.off_cshift_global + 3 > c.head_stride) return fail("global colour heads out of range");
-  if (c.use_flow && (c.off_flow < 0 || c.num_keyframes < 1 || c.num_frames < 1)) return fail("flow needs spatial_flow head and K,F");
-  if (c.use_offset && c.off_offset < 0) return fail("point_offset needs point_offset head");
-  if (c.use_color_scale_shift && (c.off_cscale < 0 || c.off_cshift < 0)) return fail("colour scale/shift heads missing");
-  if (c.dynamic && (c.num_keyframes < 1 || c.num_frames < 1)) return fail("dynamic net needs K,F");
+  if ((c.off_cscale_global >= 0) != (c.off_cshift_global >= 0)) return hr_fail("color_scale_global and color_shift_global come together");
+  if (c.off_cscale_global + 3 > c.head_stride || c.off_cshift_global + 3 > c.head_stride) return hr_fail("global colour heads out of range");
+  if (c.use_flow && (c.off_flow < 0 || c.num_keyframes < 1 || c.num_frames < 1)) return hr_fail("flow needs spatial_flow head and K,F");
+  if (c.use_offset && c.off_offset < 0) return hr_fail("point_offset needs point_offset head");
+  if (c.use_color_scale_shift && (c.off_cscale < 0 || c.off_cshift < 0)) return hr_fail("colour scale/shift heads missing");
+  if (c.dynamic && (c.num_keyframes < 1 || c.num_frames < 1)) return hr_fail("dynamic net needs K,F");
   for (int i = 0; i < 3; ++i)
-    if (c.n_sigma[i] != c.n_app[i]) return fail("n_lamb_sigma != n_lamb_sh not supported");
+    if (c.n_sigma[i] != c.n_app[i]) return hr_fail("n_lamb_sigma != n_lamb_sh not supported");
   const int* s = c.n_sigma;
   bool ok = (s[0] == 8 && s[1] == 0 && s[2] == 0) || (s[0] == 8 && s[1] == 4 && s[2] == 4) || (s[0] == 8 && s[1] == 8 && s[2] == 8);
-  if (!ok) return fail("unsupported component layout [%d,%d,%d]", s[0], s[1], s[2]);
-  if (c.shading == HR_SHADE_SH && c.app_dim != 27) return fail("SH shading needs app_dim 27");
-  if (c.shading == HR_SHADE_RGB && c.app_dim != 3) return fail("RGB shading needs app_dim 3");
-  if (c.shading != HR_SHADE_SH && c.shading != HR_SHADE_RGB) return fail("unsupported shading");
+  if (!ok) return hr_fail("unsupported component layout [%d,%d,%d]", s[0], s[1], s[2]);
+  if (c.shading == HR_SHADE_SH && c.app_dim != 27) return hr_fail("SH shading needs app_dim 27");
+  if (c.shading == HR_SHADE_RGB && c.app_dim != 3) return hr_fail("RGB shading needs app_dim 3");
+  if (c.shading != HR_SHADE_SH && c.shading != HR_SHADE_RGB) return hr_fail("unsupported shading");
   return 0;
 }
 
@@ -388,42 +377,37 @@ int hr_abi_version(void) { return HR_ABI_VERSION; }
 const char* hr_last_error(void) { return g_err.c_str(); }
 
 int hr_create(const hr_config* cfg, int device, hr_handle** out) {
-  if (!cfg || !out) return fail("hr_create: null argument");
+  if (!cfg || !out) return hr_fail("hr_create: null argument");
   *out = nullptr;
   if (validate(*cfg)) return 1;
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0) return fail("hr_create: no CUDA device (%s); there is no CPU fallback", cudaGetErrorString(e));
-  if (device < 0 || device >= ndev) return fail("hr_create: device %d out of range (%d devices)", device, ndev);
+  if (e != cudaSuccess || ndev == 0) return hr_fail("hr_create: no CUDA device (%s); there is no CPU fallback", cudaGetErrorString(e));
+  if (device < 0 || device >= ndev) return hr_fail("hr_create: device %d out of range (%d devices)", device, ndev);
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
   if (prop.major != 9 || prop.minor != 0)
-    return fail("hr_create: device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
+    return hr_fail("hr_create: device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
   DeviceGuard guard(device);
   hr_handle* h = new (std::nothrow) hr_handle();
-  if (!h) return fail("hr_create: out of memory");
+  if (!h) return hr_fail("hr_create: out of memory");
   h->cfg = *cfg;
   h->device = device;
   h->num_sms = prop.multiProcessorCount;
   derive(h->cfg, h->dv);
-  memset(&h->tabs, 0, sizeof(h->tabs));
-  memset(&h->simt, 0, sizeof(h->simt));
-  memset(&h->tc, 0, sizeof(h->tc));
-  memset(&h->simt_pre, 0, sizeof(h->simt_pre));
-  memset(&h->tc_pre, 0, sizeof(h->tc_pre));
-  h->cfg_net = h->cfg;
-  h->cfg_pre = h->cfg;
+  h->net.cfg = h->cfg;
+  h->pre.cfg = h->cfg;
   if (h->cfg.cascade) {
     const hr_config& c = h->cfg;
     // the point net: one 8-float row per first-stage point in, n_samples / pre_samples samples out, columns in the
     // reference's order (n_samples = 1 makes the packers' channel-major permutation the identity)
-    hr_config& n = h->cfg_net;
+    hr_config& n = h->net.cfg;
     n.c_in = 8;
     n.mlp_out = c.mlp_out / c.pre_samples;
     n.n_samples = 1;
     n.head_stride = n.mlp_out;
     // the first-stage ray net
-    hr_config& q = h->cfg_pre;
+    hr_config& q = h->pre.cfg;
     q.n_groups = c.pre_n_groups;
     for (int g = 0; g < HR_MAX_GROUPS; ++g) q.groups[g] = c.pre_groups[g];
     q.mlp_in = c.pre_mlp_in; q.mlp_width = c.pre_mlp_width; q.mlp_layers = c.pre_mlp_layers; q.mlp_skip = c.pre_mlp_skip;
@@ -438,8 +422,49 @@ int hr_create(const hr_config* cfg, int device, hr_handle** out) {
 
 static void drop_host_graph(hr_handle* h);
 
+// Packs one sample net for both kernels: the fp32 CUDA-core layers, and the wgmma images when the net runs on the tensor cores.
+static int pack_net(hr_handle* h, SampleNet& net, const float* const* wsrc, const float* const* bsrc, int on_device, cudaStream_t st,
+                    std::vector<void*>& temps) {
+  const hr_config& nc = net.cfg;
+  hr::MlpSimtPack& simt = net.simt;
+  const int L = nc.mlp_layers, W = nc.mlp_width;
+  const int in_pad = (nc.mlp_in + 15) / 16 * 16;
+  simt.in_pad = in_pad;
+  simt.n_layers = L;
+  simt.skip = nc.mlp_skip;
+  net.tc_ready = false;
+  const float* w_dev[HR_MAX_LAYERS] = {nullptr};
+  const float* b_dev[HR_MAX_LAYERS] = {nullptr};
+  int r = 0;
+  for (int l = 0; l < L && !r && nc.mlp_mode != HR_MLP_ZERO; ++l) {
+    if (!wsrc[l] || !bsrc[l]) return hr_fail("hr_upload: mlp layer %d missing", l);
+    const bool first = (l == 0), last = (l == L - 1), skip = (l == nc.mlp_skip);
+    const int in_src = first ? nc.mlp_in : (skip ? nc.mlp_in + W : W);
+    const int out_ch = last ? nc.mlp_out : W;
+    const int Kp = first ? in_pad : (skip ? in_pad + W : W);
+    const int Np = last ? (nc.mlp_out + W - 1) / W * W : W;
+    if ((r = stage_in(wsrc[l], (size_t)out_ch * in_src, on_device, st, temps, &w_dev[l]))) break;
+    if ((r = stage_in(bsrc[l], (size_t)out_ch, on_device, st, temps, &b_dev[l]))) break;
+    float *Wt = nullptr, *bias = nullptr;
+    if ((r = dev_alloc(h, (void**)&Wt, (size_t)Kp * Np * sizeof(float)))) break;
+    if ((r = dev_alloc(h, (void**)&bias, (size_t)Np * sizeof(float)))) break;
+    pack_simt_layer<<<grid_for((long long)Kp * Np + Np), 256, 0, st>>>(
+        w_dev[l], b_dev[l], Wt, bias, Kp, Np, out_ch, in_src, nc.mlp_in, in_pad, (first || skip) ? 1 : 0, skip ? 1 : 0, W,
+        last ? nc.n_samples : 0, nc.head_stride);
+    simt.Wt[l] = Wt;
+    simt.bias[l] = bias;
+    simt.Kp[l] = Kp;
+    simt.Np[l] = Np;
+  }
+  if (!r && nc.mlp_mode == HR_MLP_BF16X3_TC) {
+    r = hr::pack_mlp_tc2(net, w_dev, b_dev, st);
+    if (!r) net.tc_ready = true;
+  }
+  return r;
+}
+
 int hr_upload(hr_handle* h, const hr_params* p, void* stream) {
-  if (!h || !p) return fail("hr_upload: null argument");
+  if (!h || !p) return hr_fail("hr_upload: null argument");
   DeviceGuard guard(h->device);
   drop_host_graph(h);
   cudaStream_t st = (cudaStream_t)stream;
@@ -448,58 +473,19 @@ int hr_upload(hr_handle* h, const hr_params* p, void* stream) {
   // enqueued on `st` that reads the old contents is ordered before the pack kernels below (same stream).
   h->slot_cursor = 0;
   h->uploaded = false;
-  h->tc_ready = false;
+  h->net.tc_ready = h->pre.tc_ready = false;
   std::vector<void*> temps;
   int rc = 0;
 
   // ---- sample net(s) ----
-  auto pack_net = [&](const hr_config& nc, const float* const* wsrc, const float* const* bsrc, hr::MlpSimtPack& simt,
-                      hr::MlpTcPack& tc, bool& tc_ready, size_t& tc_bytes, int& tc_bias) -> int {
-    const int L = nc.mlp_layers, W = nc.mlp_width;
-    const int in_pad = (nc.mlp_in + 15) / 16 * 16;
-    simt.in_pad = in_pad;
-    simt.n_layers = L;
-    simt.skip = nc.mlp_skip;
-    tc_ready = false;
-    const float* w_dev[HR_MAX_LAYERS] = {nullptr};
-    const float* b_dev[HR_MAX_LAYERS] = {nullptr};
-    int r = 0;
-    for (int l = 0; l < L && !r && nc.mlp_mode != HR_MLP_ZERO; ++l) {
-      if (!wsrc[l] || !bsrc[l]) return fail("hr_upload: mlp layer %d missing", l);
-      const bool first = (l == 0), last = (l == L - 1), skip = (l == nc.mlp_skip);
-      const int in_src = first ? nc.mlp_in : (skip ? nc.mlp_in + W : W);
-      const int out_ch = last ? nc.mlp_out : W;
-      const int Kp = first ? in_pad : (skip ? in_pad + W : W);
-      const int Np = last ? (nc.mlp_out + W - 1) / W * W : W;
-      if ((r = stage_in(wsrc[l], (size_t)out_ch * in_src, p->on_device, st, temps, &w_dev[l]))) break;
-      if ((r = stage_in(bsrc[l], (size_t)out_ch, p->on_device, st, temps, &b_dev[l]))) break;
-      float *Wt = nullptr, *bias = nullptr;
-      if ((r = dev_alloc(h, (void**)&Wt, (size_t)Kp * Np * sizeof(float)))) break;
-      if ((r = dev_alloc(h, (void**)&bias, (size_t)Np * sizeof(float)))) break;
-      pack_simt_layer<<<grid_for((long long)Kp * Np + Np), 256, 0, st>>>(
-          w_dev[l], b_dev[l], Wt, bias, Kp, Np, out_ch, in_src, nc.mlp_in, in_pad, (first || skip) ? 1 : 0, skip ? 1 : 0, W,
-          last ? nc.n_samples : 0, nc.head_stride);
-      simt.Wt[l] = Wt;
-      simt.bias[l] = bias;
-      simt.Kp[l] = Kp;
-      simt.Np[l] = Np;
-    }
-    if (!r && nc.mlp_mode == HR_MLP_BF16X3_TC) {
-      r = hr::pack_mlp_tc2(h, nc, tc, tc_bytes, tc_bias, w_dev, b_dev, st);
-      if (!r) tc_ready = true;
-    }
-    return r;
-  };
-  rc = pack_net(h->cfg_net, p->mlp_weight, p->mlp_bias, h->simt, h->tc, h->tc_ready, h->tc_alloc_bytes, h->tc_alloc_bias);
-  if (!rc && c.cascade)
-    rc = pack_net(h->cfg_pre, p->pre_mlp_weight, p->pre_mlp_bias, h->simt_pre, h->tc_pre, h->tc_pre_ready, h->tc_pre_alloc_bytes,
-                  h->tc_pre_alloc_bias);
+  rc = pack_net(h, h->net, p->mlp_weight, p->mlp_bias, p->on_device, st, temps);
+  if (!rc && c.cascade) rc = pack_net(h, h->pre, p->pre_mlp_weight, p->pre_mlp_bias, p->on_device, st, temps);
 
   // ---- VM tables, channel-last ----
   auto pack_tab = [&](const float* src, int C, int H, int Wd, const float** out) -> int {
     *out = nullptr;
     if (C == 0) return 0;
-    if (!src) return fail("hr_upload: table with C=%d missing", C);
+    if (!src) return hr_fail("hr_upload: table with C=%d missing", C);
     const float* d = nullptr;
     if (stage_in(src, (size_t)C * H * Wd, p->on_device, st, temps, &d)) return 1;
     float* dst = nullptr;
@@ -520,7 +506,7 @@ int hr_upload(hr_handle* h, const hr_params* p, void* stream) {
     ts.W = ta.W = p->plane_w[i];
     ts.H2 = ta.H2 = H2;
     ts.L = ta.L = p->second_len[i];
-    if (C > 0 && (ts.H < 2 || ts.W < 2 || ts.L < 2)) { rc = fail("hr_upload: plane %d too small (%dx%d, L=%d)", i, ts.H, ts.W, ts.L); break; }
+    if (C > 0 && (ts.H < 2 || ts.W < 2 || ts.L < 2)) { rc = hr_fail("hr_upload: plane %d too small (%dx%d, L=%d)", i, ts.H, ts.W, ts.L); break; }
     if ((rc = pack_tab(p->sigma_plane[i], C, ts.H, ts.W, &ts.space))) break;
     if ((rc = pack_tab(p->app_plane[i], C, ts.H, ts.W, &ta.space))) break;
     // second factor: static [C][L][1] -> [1][L][C]; dynamic [C][K][L] -> K pre-blended keyframe lines [K][L][C]
@@ -528,10 +514,10 @@ int hr_upload(hr_handle* h, const hr_params* p, void* stream) {
       if ((rc = pack_tab(p->sigma_second[i], C, H2, ts.L, &ts.second))) break;
       if ((rc = pack_tab(p->app_second[i], C, H2, ts.L, &ta.second))) break;
     } else if (C > 0) {
-      if (H2 < 2) { rc = fail("hr_upload: the keyframe (time) planes need at least 2 keyframes"); break; }
+      if (H2 < 2) { rc = hr_fail("hr_upload: the keyframe (time) planes need at least 2 keyframes"); break; }
       for (int f = 0; f < 2 && !rc; ++f) {
         const float* srcp = f ? p->app_second[i] : p->sigma_second[i];
-        if (!srcp) { rc = fail("hr_upload: time plane %d missing", i); break; }
+        if (!srcp) { rc = hr_fail("hr_upload: time plane %d missing", i); break; }
         const float* d = nullptr;
         if ((rc = stage_in(srcp, (size_t)C * H2 * ts.L, p->on_device, st, temps, &d))) break;
         float* dst = nullptr;
@@ -549,14 +535,14 @@ int hr_upload(hr_handle* h, const hr_params* p, void* stream) {
     const int rx = p->plane_w[0], ry = p->plane_h[0], rz = p->second_len[0];
     h->dv.res[0] = rx; h->dv.res[1] = ry; h->dv.res[2] = rz;
     h->dv.kt = c.dynamic ? c.num_keyframes : 1;
-    if (c.dynamic && c.num_keyframes < 2) rc = fail("hr_upload: the keyframe (time) planes need at least 2 keyframes");
+    if (c.dynamic && c.num_keyframes < 2) rc = hr_fail("hr_upload: the keyframe (time) planes need at least 2 keyframes");
     if (c.n_sigma[1] > 0 && (p->plane_w[1] != rx || p->plane_h[1] != rz || p->second_len[1] != ry))
-      rc = fail("hr_upload: table group 1 is inconsistent with grid %dx%dx%d", rx, ry, rz);
+      rc = hr_fail("hr_upload: table group 1 is inconsistent with grid %dx%dx%d", rx, ry, rz);
     if (!rc && c.n_sigma[2] > 0 && (p->plane_w[2] != ry || p->plane_h[2] != rz || p->second_len[2] != rx))
-      rc = fail("hr_upload: table group 2 is inconsistent with grid %dx%dx%d", rx, ry, rz);
+      rc = hr_fail("hr_upload: table group 2 is inconsistent with grid %dx%dx%d", rx, ry, rz);
   }
   if (!rc) {
-    if (!p->basis_mat) rc = fail("hr_upload: basis_mat missing");
+    if (!p->basis_mat) rc = hr_fail("hr_upload: basis_mat missing");
     else {
       const float* d = nullptr;
       size_t cnt = (size_t)c.app_dim * n_app_total;
@@ -566,7 +552,7 @@ int hr_upload(hr_handle* h, const hr_params* p, void* stream) {
         rc = dev_alloc(h, (void**)&dst, cnt * sizeof(float));
         if (!rc) {
           cudaError_t e = cudaMemcpyAsync(dst, d, cnt * sizeof(float), cudaMemcpyDeviceToDevice, st);
-          if (e != cudaSuccess) rc = fail("basis copy failed: %s", cudaGetErrorString(e));
+          if (e != cudaSuccess) rc = hr_fail("basis copy failed: %s", cudaGetErrorString(e));
           h->tabs.basis = dst;
           h->tabs.n_app_total = n_app_total;
         }
@@ -576,7 +562,7 @@ int hr_upload(hr_handle* h, const hr_params* p, void* stream) {
   if (!rc) {
     h->tabs.color_embedding = nullptr;
     if (c.n_color_views > 0) {
-      if (!p->color_embedding) rc = fail("hr_upload: color_embedding missing (n_color_views = %d)", c.n_color_views);
+      if (!p->color_embedding) rc = hr_fail("hr_upload: color_embedding missing (n_color_views = %d)", c.n_color_views);
       else {
         const float* d = nullptr;
         const size_t cnt = (size_t)c.n_color_views * 12;
@@ -585,14 +571,14 @@ int hr_upload(hr_handle* h, const hr_params* p, void* stream) {
         if (!rc) rc = dev_alloc(h, (void**)&dst, cnt * sizeof(float));
         if (!rc) {
           cudaError_t e = cudaMemcpyAsync(dst, d, cnt * sizeof(float), cudaMemcpyDeviceToDevice, st);
-          if (e != cudaSuccess) rc = fail("color_embedding copy failed: %s", cudaGetErrorString(e));
+          if (e != cudaSuccess) rc = hr_fail("color_embedding copy failed: %s", cudaGetErrorString(e));
           h->tabs.color_embedding = dst;
         }
       }
     }
   }
   cudaError_t le = cudaGetLastError();
-  if (!rc && le != cudaSuccess) rc = fail("hr_upload: pack kernel launch failed: %s", cudaGetErrorString(le));
+  if (!rc && le != cudaSuccess) rc = hr_fail("hr_upload: pack kernel launch failed: %s", cudaGetErrorString(le));
   if (!temps.empty()) {  // host sources only: the staging copies must outlive the pack kernels
     cudaStreamSynchronize(st);
     for (void* t : temps) cudaFree(t);
@@ -609,8 +595,7 @@ int hr_upload(hr_handle* h, const hr_params* p, void* stream) {
 
 // bytes of a heads scratch for n rays: one [mlp_out] fp32 row per ray
 static int64_t heads_bytes(const hr_handle* h, int64_t n_rays) {
-  int64_t b = n_rays * (int64_t)h->cfg.mlp_out * (int64_t)sizeof(float);
-  return (b + 255) / 256 * 256 + 256;
+  return align256(n_rays * (int64_t)h->cfg.mlp_out * (int64_t)sizeof(float)) + 256;
 }
 
 // hr_render walks a large batch in sub-batches (sample net, then render kernel, per sub-batch) so that the heads scratch
@@ -621,17 +606,24 @@ static int64_t sub_batch_rays(const hr_handle* h) {
   return (int64_t)h->num_sms * 128 * 16;
 }
 
-// scratch of the first stage of a cascaded pipeline for n rays, placed after the heads: first-stage heads [n][S0*stride0],
-// point rows [n*S0][8], point-net output [n][mlp_out] (reference order, before the channel-major permutation)
-static int64_t cascade_bytes(const hr_handle* h, int64_t n_rays) {
-  const hr_config& c = h->cfg;
-  if (!c.cascade) return 0;
-  auto seg = [](int64_t floats) { return (floats * (int64_t)sizeof(float) + 255) / 256 * 256; };  // each buffer 256-byte aligned
-  return seg(n_rays * c.pre_samples * c.pre_head_stride) + seg(n_rays * c.pre_samples * 8) + seg(n_rays * (int64_t)c.mlp_out);
+// scratch of the first stage of a cascaded pipeline for n rays, placed after the heads (byte offsets, each 256-byte aligned):
+// first-stage heads [n][S0*stride0] channel-major, point rows [n*S0][8], point-net output [n*S0][mlp_out/S0] = [n][S][stride]
+// (reference order, before the channel-major permutation).  total is 0 for a pipeline that is not cascaded.
+struct CascadeLayout {
+  int64_t heads0, rows, out, total;
+};
+static CascadeLayout cascade_layout(const hr_config& c, int64_t n_rays) {
+  CascadeLayout t{0, 0, 0, 0};
+  if (!c.cascade) return t;
+  const int64_t f = (int64_t)sizeof(float);
+  t.rows = t.heads0 + align256(n_rays * c.pre_samples * c.pre_head_stride * f);
+  t.out = t.rows + align256(n_rays * c.pre_samples * 8 * f);
+  t.total = t.out + align256(n_rays * (int64_t)c.mlp_out * f);
+  return t;
 }
 
 // workspace of one render call over n rays that is not split further
-static int64_t ws_bytes_for(const hr_handle* h, int64_t n_rays) { return heads_bytes(h, n_rays) + cascade_bytes(h, n_rays); }
+static int64_t ws_bytes_for(const hr_handle* h, int64_t n_rays) { return heads_bytes(h, n_rays) + cascade_layout(h->cfg, n_rays).total; }
 
 int64_t hr_workspace_bytes(const hr_handle* h, int64_t n_rays) {
   if (!h || n_rays < 0) return -1;
@@ -645,7 +637,7 @@ int64_t hr_train_workspace_bytes(const hr_handle* h, int64_t n_rays) {
 }
 
 int hr_set_sub_batch(hr_handle* h, int64_t rays) {
-  if (!h) return fail("hr_set_sub_batch: null handle");
+  if (!h) return hr_fail("hr_set_sub_batch: null handle");
   h->sub_rays = rays;
   return 0;
 }
@@ -657,50 +649,91 @@ static void drop_host_graph(hr_handle* h) {
   h->pipe.g_rays = nullptr; h->pipe.g_rgb = nullptr; h->pipe.g_n = 0; h->pipe.g_chunk = 0;
 }
 
+// stream i of the host pipelines, created on first use
+static int pipe_stream(hr_handle* h, int i) {
+  if (!h->pipe.streams[i]) CK(cudaStreamCreateWithFlags(&h->pipe.streams[i], cudaStreamNonBlocking));
+  return 0;
+}
+
+// Device scratch of the host pipelines: three slots, each the rays, the pixels (fp32 rgb, or an 8-bit tile stored in the rgb
+// slot) and the render workspace of `rays_per_slot` rays.  It only grows; growing drops the cached graph, whose nodes hold
+// the old pointers.
+static int ensure_pipe(hr_handle* h, int64_t rays_per_slot) {
+  HostPipe& P = h->pipe;
+  if (P.chunk >= rays_per_slot) return 0;
+  drop_host_graph(h);
+  P.chunk = 0;
+  for (int i = 0; i < 3; ++i) {
+    if (P.d_rays[i]) cudaFree(P.d_rays[i]);
+    if (P.d_rgb[i]) cudaFree(P.d_rgb[i]);
+    if (P.d_ws[i]) cudaFree(P.d_ws[i]);
+    P.d_rays[i] = P.d_rgb[i] = nullptr; P.d_ws[i] = nullptr;
+    if (pipe_stream(h, i)) return 1;
+  }
+  P.ws_bytes = ws_bytes_for(h, rays_per_slot);
+  for (int i = 0; i < 3; ++i) {
+    CK(cudaMalloc((void**)&P.d_rays[i], (size_t)rays_per_slot * h->cfg.c_in * sizeof(float)));
+    CK(cudaMalloc((void**)&P.d_rgb[i], (size_t)rays_per_slot * 3 * sizeof(float)));
+    CK(cudaMalloc(&P.d_ws[i], (size_t)P.ws_bytes));
+  }
+  P.chunk = rays_per_slot;
+  return 0;
+}
+
 // one net (ray net or point net) over `rows` input rows -> out [rows][nc.mlp_out]
-static int launch_net(hr_handle* h, const hr_config& nc, const hr::MlpSimtPack& simt, const hr::MlpTcPack& tc, bool tc_ready,
-                      const float* in, int64_t rows, float* out, cudaStream_t st) {
+static int launch_net(hr_handle* h, const SampleNet& net, const float* in, int64_t rows, float* out, cudaStream_t st) {
+  const hr_config& nc = net.cfg;
   cudaError_t e;
   if (nc.mlp_mode == HR_MLP_ZERO) {  // ZeroMLP (nlf/nets/mlp.py:29-30): x.new_zeros(N, out_channels)
     e = cudaMemsetAsync(out, 0, (size_t)rows * nc.mlp_out * sizeof(float), st);
-    if (e != cudaSuccess) return fail("heads memset failed: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return hr_fail("heads memset failed: %s", cudaGetErrorString(e));
     return 0;
   }
   if (nc.mlp_mode == HR_MLP_BF16X3_TC) {
-    if (!tc_ready) return fail("hr_render: tensor-core pack missing");
-    e = hr::launch_mlp_tc2(nc, tc, in, out, rows, h->num_sms, st);
+    if (!net.tc_ready) return hr_fail("hr_render: tensor-core pack missing");
+    e = hr::launch_mlp_tc2(nc, net.tc, in, out, rows, h->num_sms, st);
   } else {
-    e = hr::launch_mlp_simt(nc, simt, in, out, rows, h->num_sms, st);
+    e = hr::launch_mlp_simt(nc, net.simt, in, out, rows, h->num_sms, st);
   }
-  if (e != cudaSuccess) return fail("sample-net launch failed: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return hr_fail("sample-net launch failed: %s", cudaGetErrorString(e));
   h->launches += 1;
   return 0;
 }
 
-// rays [n, c_in] -> heads scratch [n, mlp_out] (channel-major per ray).  `scratch` (cascade_bytes(h, n), only read for a
+// heads of n rays between the reference's order [n][s*stride+c] and the kernels' channel-major rows [n][c*S+s]
+static cudaError_t permute_heads_async(const hr_config& c, const float* src, float* dst, int64_t n, cudaStream_t st) {
+  permute_heads<<<grid_for(n * (long long)c.mlp_out), 256, 0, st>>>(src, dst, n, c.n_samples, c.head_stride);
+  return cudaGetLastError();
+}
+
+static cudaError_t unpermute_heads_async(const hr_config& c, const float* src, float* dst, int64_t n, cudaStream_t st) {
+  unpermute_heads<<<grid_for(n * (long long)c.mlp_out), 256, 0, st>>>(src, dst, n, c.n_samples, c.head_stride);
+  return cudaGetLastError();
+}
+
+// rays [n, c_in] -> heads scratch [n, mlp_out] (channel-major per ray).  `scratch` (cascade_layout(c, n).total bytes, only read for a
 // cascaded pipeline) holds the first stage's intermediates.
 static int launch_sample_net(hr_handle* h, const float* rays, int64_t n, float* heads, cudaStream_t st, void* scratch = nullptr) {
   const hr_config& c = h->cfg;
-  if (!c.cascade) return launch_net(h, h->cfg_net, h->simt, h->tc, h->tc_ready, rays, n, heads, st);
-  if (!scratch) return fail("hr_render: cascade scratch missing");
+  if (!c.cascade) return launch_net(h, h->net, rays, n, heads, st);
+  if (!scratch) return hr_fail("hr_render: cascade scratch missing");
   // PointPredictionEmbedding (nlf/embedding/point.py:142-206): ray net -> S0 z-planes -> one point-net row per point
-  auto seg = [](int64_t floats) { return (floats * (int64_t)sizeof(float) + 255) / 256 * 256; };  // as in cascade_bytes
-  float* heads0 = (float*)scratch;                                                                // [n][S0*stride0] channel-major
-  float* rows = (float*)((char*)heads0 + seg(n * c.pre_samples * c.pre_head_stride));              // [n*S0][8]
-  float* out = (float*)((char*)rows + seg(n * c.pre_samples * 8));                                 // [n*S0][mlp_out/S0] = [n][S][stride]
+  const CascadeLayout t = cascade_layout(c, n);
+  float* heads0 = (float*)((char*)scratch + t.heads0);
+  float* rows = (float*)((char*)scratch + t.rows);
+  float* out = (float*)((char*)scratch + t.out);
   const bool has_pre = c.pre_mlp_mode != HR_MLP_ZERO;
   if (has_pre) {
-    int rc = launch_net(h, h->cfg_pre, h->simt_pre, h->tc_pre, h->tc_pre_ready, rays, n, heads0, st);
+    int rc = launch_net(h, h->pre, rays, n, heads0, st);
     if (rc) return rc;
   }
   cascade_points_kernel<<<grid_for(n * 32), 256, 0, st>>>(c, rays, has_pre ? heads0 : nullptr, rows, n);
   cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail("cascade point kernel launch failed: %s", cudaGetErrorString(e));
-  int rc = launch_net(h, h->cfg_net, h->simt, h->tc, h->tc_ready, rows, n * c.pre_samples, out, st);
+  if (e != cudaSuccess) return hr_fail("cascade point kernel launch failed: %s", cudaGetErrorString(e));
+  int rc = launch_net(h, h->net, rows, n * c.pre_samples, out, st);
   if (rc) return rc;
-  permute_heads<<<grid_for(n * (long long)c.mlp_out), 256, 0, st>>>(out, heads, n, c.n_samples, c.head_stride);
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return fail("heads permutation launch failed: %s", cudaGetErrorString(e));
+  e = permute_heads_async(c, out, heads, n, st);
+  if (e != cudaSuccess) return hr_fail("heads permutation launch failed: %s", cudaGetErrorString(e));
   h->launches += 2;
   return 0;
 }
@@ -713,15 +746,19 @@ static hr::RgbDst one_dst(float* rgb) {
   return d;
 }
 
+// channels of every extra field (HR_FIELD_*, in the enum's order): points, view directions, flow, offset and the colour
+// scales / shifts are 3-vectors
+constexpr int kFieldWidth[HR_N_FIELDS] = {3, 1, 1, 1, 1, 3, 1, 3, 3, 3, 1, 1, 3, 3, 3};
+
 static int render_impl(hr_handle* h, const float* rays, int64_t n, float* rgb, float* mlp_out, const hr::ExtraOut* so,
                        void* workspace, int64_t ws_bytes, cudaStream_t st, unsigned char* rgb8 = nullptr,
                        const hr::RgbDst* scatter = nullptr) {
-  if (!h) return fail("hr_render: null handle");
-  if (!h->uploaded) return fail("hr_render: parameters not uploaded (call hr_upload)");
+  if (!h) return hr_fail("hr_render: null handle");
+  if (!h->uploaded) return hr_fail("hr_render: parameters not uploaded (call hr_upload)");
   if (n == 0) return 0;
-  if (!rays || (!rgb && !rgb8 && !scatter) || !workspace) return fail("hr_render: null buffer");
-  if (ws_bytes < hr_workspace_bytes(h, n)) return fail("hr_render: workspace too small (%lld < %lld)", (long long)ws_bytes, (long long)hr_workspace_bytes(h, n));
-  if (((uintptr_t)workspace & 15) != 0) return fail("hr_render: workspace must be 16-byte aligned");
+  if (!rays || (!rgb && !rgb8 && !scatter) || !workspace) return hr_fail("hr_render: null buffer");
+  if (ws_bytes < hr_workspace_bytes(h, n)) return hr_fail("hr_render: workspace too small (%lld < %lld)", (long long)ws_bytes, (long long)hr_workspace_bytes(h, n));
+  if (((uintptr_t)workspace & 15) != 0) return hr_fail("hr_render: workspace must be 16-byte aligned");
   float* heads = (float*)workspace;
   const hr_config& c = h->cfg;
   const bool timing = h->timing && h->ev_render.size() < 8192;
@@ -750,14 +787,11 @@ static int render_impl(hr_handle* h, const float* rays, int64_t n, float* rgb, f
       if (so_off.rgb_samples) so_off.rgb_samples += off * S * 3;
       for (int f = 0; f < HR_N_FIELDS; ++f) {
         if (!so_off.field_out[f]) continue;
-        const bool three = f == HR_FIELD_POINTS || f == HR_FIELD_VIEWDIRS || f == HR_FIELD_COLOR_SCALE || f == HR_FIELD_COLOR_SHIFT ||
-                           f == HR_FIELD_SPATIAL_FLOW || f == HR_FIELD_POINT_OFFSET || f == HR_FIELD_COLOR_SCALE_GLOBAL ||
-                           f == HR_FIELD_COLOR_SHIFT_GLOBAL;
-        so_off.field_out[f] += off * (three ? 3 : 1) * (so_off.field_mode[f] == HR_FIELD_NO_OVER ? S : 1);
+        so_off.field_out[f] += off * kFieldWidth[f] * (so_off.field_mode[f] == HR_FIELD_NO_OVER ? S : 1);
       }
     }
     cudaError_t e = hr::launch_render(c, h->dv, h->tabs, r, heads, d, m, so ? &so_off : nullptr, h->num_sms, st, rgb8 ? rgb8 + off * 3 : nullptr);
-    if (e != cudaSuccess) return fail("render launch failed: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return hr_fail("render launch failed: %s", cudaGetErrorString(e));
     if (timing) {
       CK(cudaEventRecord(er.b, st));
       h->ev_mlp.push_back(em);
@@ -765,9 +799,8 @@ static int render_impl(hr_handle* h, const float* rays, int64_t n, float* rgb, f
     }
     h->launches += 1;
     if (mlp_out) {
-      unpermute_heads<<<grid_for(m * (long long)c.mlp_out), 256, 0, st>>>(heads, mlp_out + off * c.mlp_out, m, c.n_samples, c.head_stride);
-      e = cudaGetLastError();
-      if (e != cudaSuccess) return fail("unpermute launch failed: %s", cudaGetErrorString(e));
+      e = unpermute_heads_async(c, heads, mlp_out + off * c.mlp_out, m, st);
+      if (e != cudaSuccess) return hr_fail("unpermute launch failed: %s", cudaGetErrorString(e));
       h->launches += 1;
     }
   }
@@ -783,13 +816,13 @@ int hr_render(hr_handle* h, const float* rays, int64_t n_rays, float* rgb, void*
 
 int hr_render_scatter(hr_handle* h, const float* rays, int64_t n_rays, float* const* dst, int32_t n_dst, int64_t row0,
                       void* workspace, int64_t workspace_bytes, void* stream) {
-  if (!h) return fail("hr_render_scatter: null handle");
-  if (!dst || n_dst < 1 || n_dst > HR_MAX_PEERS) return fail("hr_render_scatter: 1..%d destination buffers", HR_MAX_PEERS);
-  if (row0 < 0) return fail("hr_render_scatter: negative row offset");
+  if (!h) return hr_fail("hr_render_scatter: null handle");
+  if (!dst || n_dst < 1 || n_dst > HR_MAX_PEERS) return hr_fail("hr_render_scatter: 1..%d destination buffers", HR_MAX_PEERS);
+  if (row0 < 0) return hr_fail("hr_render_scatter: negative row offset");
   DeviceGuard guard(h->device);
   hr::RgbDst d{};
   for (int i = 0; i < n_dst; ++i) {
-    if (!dst[i]) return fail("hr_render_scatter: null destination %d", i);
+    if (!dst[i]) return hr_fail("hr_render_scatter: null destination %d", i);
     d.p[i] = dst[i];
   }
   d.n = n_dst;
@@ -808,24 +841,24 @@ int hr_render_stages(hr_handle* h, const float* rays, int64_t n_rays, float* rgb
 
 int hr_render_fields(hr_handle* h, const float* rays, int64_t n_rays, float* rgb, float* render_weights,
                      const hr_field_request* req, int32_t n_req, void* workspace, int64_t workspace_bytes, void* stream) {
-  if (!h) return fail("hr_render_fields: null handle");
-  if (n_req < 0 || (n_req > 0 && !req)) return fail("hr_render_fields: bad request list");
+  if (!h) return hr_fail("hr_render_fields: null handle");
+  if (n_req < 0 || (n_req > 0 && !req)) return hr_fail("hr_render_fields: bad request list");
   DeviceGuard guard(h->device);
   const hr_config& c = h->cfg;
   hr::ExtraOut so{};
   so.weights = render_weights;
   for (int i = 0; i < n_req; ++i) {
     const int f = req[i].field, m = req[i].mode;
-    if (f < 0 || f >= HR_N_FIELDS) return fail("hr_render_fields: unknown field %d", f);
-    if (m != HR_FIELD_OVER && m != HR_FIELD_NO_OVER && m != HR_FIELD_PRED_WEIGHTS) return fail("hr_render_fields: unknown mode %d", m);
-    if (!req[i].out) return fail("hr_render_fields: null output for field %d", f);
-    if (so.field_out[f]) return fail("hr_render_fields: field %d requested twice", f);
+    if (f < 0 || f >= HR_N_FIELDS) return hr_fail("hr_render_fields: unknown field %d", f);
+    if (m != HR_FIELD_OVER && m != HR_FIELD_NO_OVER && m != HR_FIELD_PRED_WEIGHTS) return hr_fail("hr_render_fields: unknown mode %d", m);
+    if (!req[i].out) return hr_fail("hr_render_fields: null output for field %d", f);
+    if (so.field_out[f]) return hr_fail("hr_render_fields: field %d requested twice", f);
     // fields the pipeline does not carry (reference: KeyError on x[key])
     if ((f == HR_FIELD_BASE_TIMES || f == HR_FIELD_TIME_OFFSET) && !(c.dynamic || c.use_flow))
-      return fail("hr_render_fields: this pipeline has no keyframe times");
+      return hr_fail("hr_render_fields: this pipeline has no keyframe times");
     const int head_off[HR_N_FIELDS] = {0, 0, 0, 0, 0, 0, 0, c.off_cscale, c.off_cshift, c.off_flow, c.off_sigma,
                                        c.off_point_sigma, c.off_offset, c.off_cscale_global, c.off_cshift_global};
-    if (f >= HR_FIELD_COLOR_SCALE && head_off[f] < 0) return fail("hr_render_fields: the sample net has no head for field %d", f);
+    if (f >= HR_FIELD_COLOR_SCALE && head_off[f] < 0) return hr_fail("hr_render_fields: the sample net has no head for field %d", f);
     so.field_out[f] = req[i].out;
     so.field_mode[f] = m;
   }
@@ -835,7 +868,7 @@ int hr_render_fields(hr_handle* h, const float* rays, int64_t n_rays, float* rgb
 int hr_render_to8b(hr_handle* h, const float* rays, int64_t n_rays, uint8_t* rgb8, void* workspace, int64_t workspace_bytes,
                    void* stream) {
   DeviceGuard guard(h ? h->device : 0);
-  if (!rgb8) return fail("hr_render_to8b: null output");
+  if (!rgb8) return hr_fail("hr_render_to8b: null output");
   return render_impl(h, rays, n_rays, nullptr, nullptr, nullptr, workspace, workspace_bytes, (cudaStream_t)stream, rgb8);
 }
 
@@ -855,54 +888,37 @@ static const char* bad_two_plane(const hr_camera& cam) {
 }
 
 int hr_generate_rays(const hr_camera* cam, int32_t c_in, int64_t first_pixel, int64_t n_pixels, float* rays_out, void* stream) {
-  if (!cam || !rays_out) return fail("hr_generate_rays: null argument");
-  if (c_in != 6 && c_in != 8) return fail("hr_generate_rays: c_in must be 6 or 8");
-  if (cam->width < 1 || cam->height < 1) return fail("hr_generate_rays: bad image size");
-  if (bad_fisheye(*cam)) return fail("hr_generate_rays: fisheye coefficients k1 = %g, k2 = %g are not finite", cam->k1, cam->k2);
-  if (const char* why = bad_two_plane(*cam)) return fail("hr_generate_rays: %s", why);
+  if (!cam || !rays_out) return hr_fail("hr_generate_rays: null argument");
+  if (c_in != 6 && c_in != 8) return hr_fail("hr_generate_rays: c_in must be 6 or 8");
+  if (cam->width < 1 || cam->height < 1) return hr_fail("hr_generate_rays: bad image size");
+  if (bad_fisheye(*cam)) return hr_fail("hr_generate_rays: fisheye coefficients k1 = %g, k2 = %g are not finite", cam->k1, cam->k2);
+  if (const char* why = bad_two_plane(*cam)) return hr_fail("hr_generate_rays: %s", why);
   if (first_pixel < 0 || n_pixels < 0 || first_pixel + n_pixels > (int64_t)cam->width * cam->height)
-    return fail("hr_generate_rays: pixel range outside the image");
+    return hr_fail("hr_generate_rays: pixel range outside the image");
   cudaError_t e = hr::launch_generate_rays(*cam, c_in, first_pixel, n_pixels, rays_out, (cudaStream_t)stream);
-  if (e != cudaSuccess) return fail("hr_generate_rays: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return hr_fail("hr_generate_rays: %s", cudaGetErrorString(e));
   return 0;
 }
 
 int hr_render_frame_to8b_host(hr_handle* h, const hr_camera* cam, uint8_t* rgb8_host, int64_t chunk) {
-  if (!h || !cam || !rgb8_host) return fail("hr_render_frame_to8b_host: null argument");
-  if (!h->uploaded) return fail("hr_render_frame_to8b_host: parameters not uploaded");
+  if (!h || !cam || !rgb8_host) return hr_fail("hr_render_frame_to8b_host: null argument");
+  if (!h->uploaded) return hr_fail("hr_render_frame_to8b_host: parameters not uploaded");
   if (bad_fisheye(*cam))
-    return fail("hr_render_frame_to8b_host: fisheye coefficients k1 = %g, k2 = %g are not finite", cam->k1, cam->k2);
-  if (const char* why = bad_two_plane(*cam)) return fail("hr_render_frame_to8b_host: %s", why);
+    return hr_fail("hr_render_frame_to8b_host: fisheye coefficients k1 = %g, k2 = %g are not finite", cam->k1, cam->k2);
+  if (const char* why = bad_two_plane(*cam)) return hr_fail("hr_render_frame_to8b_host: %s", why);
   DeviceGuard guard(h->device);
   const hr_config& c = h->cfg;
   const int64_t n_rays = (int64_t)cam->width * cam->height;
   if (chunk <= 0) chunk = (h->cfg.mlp_mode == HR_MLP_BF16X3_TC) ? (int64_t)h->num_sms * 128 * 14 : 262144;  // whole tile waves
   if (chunk > n_rays) chunk = n_rays;
   HostPipe& P = h->pipe;
-  // device scratch per slot: rays, 8-bit tile (stored in the rgb slot), workspace
-  if (P.chunk < chunk) {
-    drop_host_graph(h);
-    for (int i = 0; i < 3; ++i) {
-      if (P.d_rays[i]) cudaFree(P.d_rays[i]);
-      if (P.d_rgb[i]) cudaFree(P.d_rgb[i]);
-      if (P.d_ws[i]) cudaFree(P.d_ws[i]);
-      P.d_rays[i] = P.d_rgb[i] = nullptr; P.d_ws[i] = nullptr;
-      if (!P.streams[i]) CK(cudaStreamCreateWithFlags(&P.streams[i], cudaStreamNonBlocking));
-    }
-    P.ws_bytes = ws_bytes_for(h, chunk);
-    for (int i = 0; i < 3; ++i) {
-      CK(cudaMalloc((void**)&P.d_rays[i], (size_t)chunk * c.c_in * sizeof(float)));
-      CK(cudaMalloc((void**)&P.d_rgb[i], (size_t)chunk * 3 * sizeof(float)));
-      CK(cudaMalloc(&P.d_ws[i], (size_t)P.ws_bytes));
-    }
-    P.chunk = chunk;
-  }
+  if (ensure_pipe(h, chunk)) return 1;
   int slot = 0;
   for (int64_t off = 0; off < n_rays; off += chunk, slot = (slot + 1) % 3) {
     const int64_t m = (n_rays - off < chunk) ? (n_rays - off) : chunk;
     cudaStream_t st = P.streams[slot];
     cudaError_t e = hr::launch_generate_rays(*cam, c.c_in, off, m, P.d_rays[slot], st);
-    if (e != cudaSuccess) return fail("ray generation failed: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return hr_fail("ray generation failed: %s", cudaGetErrorString(e));
     h->launches += 1;
     int rc = render_impl(h, P.d_rays[slot], m, nullptr, nullptr, nullptr, P.d_ws[slot], P.ws_bytes, st, (unsigned char*)P.d_rgb[slot]);
     if (rc) return rc;
@@ -913,8 +929,6 @@ int hr_render_frame_to8b_host(hr_handle* h, const hr_camera* cam, uint8_t* rgb8_
 }
 
 // ---- videos: many frames per call, rays generated and rendered in sub-batches that span frame boundaries
-static int64_t align256(int64_t b) { return (b + 255) / 256 * 256; }
-
 // rays of the whole video, or -1 when F * H * W * 3 (the output's bytes) does not fit in int64
 static int64_t video_rays(int32_t n_frames, int32_t height, int32_t width) {
   if (n_frames < 1 || height < 1 || width < 1) return -1;
@@ -959,27 +973,27 @@ static bool finite_camera(const hr_camera& c) {
 // order, so a slot is reused only after the sub-batch that last held it has finished.
 int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_frames, uint8_t* video,
                          void* workspace, int64_t workspace_bytes, void* stream) {
-  if (!h || !cameras || !times || !video || !workspace) return fail("hr_render_video_to8b: null argument");
-  if (!h->uploaded) return fail("hr_render_video_to8b: parameters not uploaded");
-  if (n_frames < 1) return fail("hr_render_video_to8b: n_frames must be >= 1, got %d", n_frames);
+  if (!h || !cameras || !times || !video || !workspace) return hr_fail("hr_render_video_to8b: null argument");
+  if (!h->uploaded) return hr_fail("hr_render_video_to8b: parameters not uploaded");
+  if (n_frames < 1) return hr_fail("hr_render_video_to8b: n_frames must be >= 1, got %d", n_frames);
   const int32_t W = cameras[0].width, H = cameras[0].height;
   const int64_t n = video_rays(n_frames, H, W);
-  if (n < 0) return fail("hr_render_video_to8b: %d frames of %d x %d pixels: bad size or output bytes overflow int64", n_frames, W, H);
+  if (n < 0) return hr_fail("hr_render_video_to8b: %d frames of %d x %d pixels: bad size or output bytes overflow int64", n_frames, W, H);
   bool mixed = false;  // any record not a pinhole: the ray kernel's instantiation that branches on each record's model
   for (int32_t f = 0; f < n_frames; ++f) {
     const hr_camera& c = cameras[f];
     if (c.width != W || c.height != H)
-      return fail("hr_render_video_to8b: frame %d is %d x %d, frame 0 is %d x %d", f, c.width, c.height, W, H);
-    if (!finite_camera(c)) return fail("hr_render_video_to8b: camera record of frame %d is not finite", f);
+      return hr_fail("hr_render_video_to8b: frame %d is %d x %d, frame 0 is %d x %d", f, c.width, c.height, W, H);
+    if (!finite_camera(c)) return hr_fail("hr_render_video_to8b: camera record of frame %d is not finite", f);
     if (bad_fisheye(c))
-      return fail("hr_render_video_to8b: fisheye coefficients k1 = %g, k2 = %g of frame %d are not finite", c.k1, c.k2, f);
-    if (const char* why = bad_two_plane(c)) return fail("hr_render_video_to8b: frame %d: %s", f, why);
-    if (!std::isfinite(times[f])) return fail("hr_render_video_to8b: time of frame %d is not finite", f);
+      return hr_fail("hr_render_video_to8b: fisheye coefficients k1 = %g, k2 = %g of frame %d are not finite", c.k1, c.k2, f);
+    if (const char* why = bad_two_plane(c)) return hr_fail("hr_render_video_to8b: frame %d: %s", f, why);
+    if (!std::isfinite(times[f])) return hr_fail("hr_render_video_to8b: time of frame %d is not finite", f);
     mixed = mixed || c.fisheye || c.two_plane;
   }
   const int64_t need = hr_video_workspace_bytes(h, n_frames, H, W);
-  if (workspace_bytes < need) return fail("hr_render_video_to8b: workspace too small (%lld < %lld)", (long long)workspace_bytes, (long long)need);
-  if (((uintptr_t)workspace & 15) != 0) return fail("hr_render_video_to8b: workspace must be 16-byte aligned");
+  if (workspace_bytes < need) return hr_fail("hr_render_video_to8b: workspace too small (%lld < %lld)", (long long)workspace_bytes, (long long)need);
+  if (((uintptr_t)workspace & 15) != 0) return hr_fail("hr_render_video_to8b: workspace must be 16-byte aligned");
   DeviceGuard guard(h->device);
   const hr_config& c = h->cfg;
   cudaStream_t st = (cudaStream_t)stream;
@@ -998,7 +1012,7 @@ int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* ti
   cudaEvent_t ev = nullptr;
   if (n_slots == 2) {
     for (int i = 0; i < 2; ++i) {
-      if (!h->pipe.streams[i]) CK(cudaStreamCreateWithFlags(&h->pipe.streams[i], cudaStreamNonBlocking));
+      if (pipe_stream(h, i)) return 1;
       ss[i] = h->pipe.streams[i];
     }
     CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
@@ -1017,7 +1031,7 @@ int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* ti
     float* d_rays = (float*)slot;
     cudaError_t e = hr::launch_generate_video_rays(d_cams, d_times, mixed, c.c_in, W, frame_px, off, m, d_rays, s);
     if (e != cudaSuccess) {
-      rc = fail("video ray generation failed: %s", cudaGetErrorString(e));
+      rc = hr_fail("video ray generation failed: %s", cudaGetErrorString(e));
       break;
     }
     h->launches += 1;
@@ -1034,11 +1048,20 @@ int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* ti
   return rc;
 }
 
+// the device's view of a pinned (device-addressable) host buffer, or null
+static float* device_view(const void* host) {
+  cudaPointerAttributes pa;
+  if (cudaPointerGetAttributes(&pa, host) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer != nullptr)
+    return (float*)pa.devicePointer;
+  cudaGetLastError();  // pageable memory: not an error, just not device-addressable
+  return nullptr;
+}
+
 int hr_render_host(hr_handle* h, const float* rays_host, int64_t n_rays, float* rgb_host, int64_t chunk) {
-  if (!h) return fail("hr_render_host: null handle");
-  if (!h->uploaded) return fail("hr_render_host: parameters not uploaded");
+  if (!h) return hr_fail("hr_render_host: null handle");
+  if (!h->uploaded) return hr_fail("hr_render_host: parameters not uploaded");
   if (n_rays == 0) return 0;
-  if (!rays_host || !rgb_host) return fail("hr_render_host: null buffer");
+  if (!rays_host || !rgb_host) return hr_fail("hr_render_host: null buffer");
   DeviceGuard guard(h->device);
   const hr_config& c = h->cfg;
   HostPipe& P = h->pipe;
@@ -1047,44 +1070,14 @@ int hr_render_host(hr_handle* h, const float* rays_host, int64_t n_rays, float* 
   // `chunk` rays (default: whole waves for the tensor-core net, 32 768 rays for the CUDA-core net) on three streams.
   // (a cascaded pipeline runs its nets on point rows: it takes the plain chunked pipeline)
   const bool whole = chunk <= 0 && c.mlp_mode == HR_MLP_BF16X3_TC && n_rays <= 16 * wave && !c.cascade;  // the batch stays whole on the device
-  const float* rays_dev_view = nullptr;
-  if (whole && h->tc_ready && !h->timing) {
-    cudaPointerAttributes pa;
-    if (cudaPointerGetAttributes(&pa, rays_host) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer != nullptr)
-      rays_dev_view = (const float*)pa.devicePointer;
-    else
-      cudaGetLastError();  // pageable memory: not an error, just not device-addressable
-  }
+  const float* rays_dev_view = (whole && h->net.tc_ready && !h->timing) ? device_view(rays_host) : nullptr;
   const bool zero_copy = rays_dev_view != nullptr;
-  float* rgb_dev_view = nullptr;
-  if (zero_copy) {
-    cudaPointerAttributes pa;
-    if (cudaPointerGetAttributes(&pa, rgb_host) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer != nullptr)
-      rgb_dev_view = (float*)pa.devicePointer;
-    else
-      cudaGetLastError();
-  }
+  float* rgb_dev_view = zero_copy ? device_view(rgb_host) : nullptr;
   const bool split = !zero_copy && whole && n_rays > wave;
   if (chunk <= 0) chunk = (c.mlp_mode == HR_MLP_BF16X3_TC) ? wave : 32768;
   if (chunk > n_rays) chunk = n_rays;
   const int64_t alloc = (split || zero_copy) ? n_rays : chunk;  // rays per device slot
-  if (P.chunk < alloc) {
-    drop_host_graph(h);
-    for (int i = 0; i < 3; ++i) {
-      if (P.d_rays[i]) cudaFree(P.d_rays[i]);
-      if (P.d_rgb[i]) cudaFree(P.d_rgb[i]);
-      if (P.d_ws[i]) cudaFree(P.d_ws[i]);
-      P.d_rays[i] = P.d_rgb[i] = nullptr; P.d_ws[i] = nullptr;
-      if (!P.streams[i]) CK(cudaStreamCreateWithFlags(&P.streams[i], cudaStreamNonBlocking));
-    }
-    P.ws_bytes = ws_bytes_for(h, alloc);
-    for (int i = 0; i < 3; ++i) {
-      CK(cudaMalloc((void**)&P.d_rays[i], (size_t)alloc * c.c_in * sizeof(float)));
-      CK(cudaMalloc((void**)&P.d_rgb[i], (size_t)alloc * 3 * sizeof(float)));
-      CK(cudaMalloc(&P.d_ws[i], (size_t)P.ws_bytes));
-    }
-    P.chunk = alloc;
-  }
+  if (ensure_pipe(h, alloc)) return 1;
   if (!P.fork_ev) {
     CK(cudaEventCreateWithFlags(&P.fork_ev, cudaEventDisableTiming));
     for (int i = 0; i < 3; ++i) CK(cudaEventCreateWithFlags(&P.join_ev[i], cudaEventDisableTiming));
@@ -1103,6 +1096,27 @@ int hr_render_host(hr_handle* h, const float* rays_host, int64_t n_rays, float* 
     }
     return 0;
   };
+  // The whole batch on the device (rays, heads and rgb of slot 0): the render kernel on stream 0 in `pieces` launches
+  // (event Rj after piece j), the rgb of piece j copied out on stream 2 after Rj.
+  auto render_pieces = [&](int pieces) -> int {
+    cudaStream_t s0 = P.streams[0], s2 = P.streams[2];
+    const float* d_rays = P.d_rays[0];
+    float* d_rgb = P.d_rgb[0];
+    const float* heads = (const float*)P.d_ws[0];
+    const int64_t per = ((n_rays + pieces - 1) / pieces + 255) / 256 * 256;
+    int j = 0;
+    for (int64_t off = 0; off < n_rays; off += per, ++j) {
+      const int64_t m = (n_rays - off < per) ? (n_rays - off) : per;
+      cudaError_t e = hr::launch_render(c, h->dv, h->tabs, d_rays + off * c.c_in, heads + off * (int64_t)c.mlp_out, one_dst(d_rgb + off * 3), m,
+                                        nullptr, h->num_sms, s0, nullptr);
+      if (e != cudaSuccess) return hr_fail("render launch failed: %s", cudaGetErrorString(e));
+      h->launches += 1;
+      CK(cudaEventRecord(P.dep_ev[2 + j], s0));
+      CK(cudaStreamWaitEvent(s2, P.dep_ev[2 + j], 0));
+      CK(cudaMemcpyAsync(rgb_host + off * 3, d_rgb + off * 3, (size_t)m * 3 * sizeof(float), cudaMemcpyDeviceToHost, s2));
+    }
+    return 0;
+  };
   // Wave-split pipeline: splitting a batch into independent chunks costs one cold sample-net launch and one render tail
   // per chunk, which eats what the copy overlap wins (measured: 0.404 ms unsplit vs 0.410 ms in four chunks).  Instead the
   // batch stays whole on the device and only the edges are split:
@@ -1112,9 +1126,8 @@ int hr_render_host(hr_handle* h, const float* rays_host, int64_t n_rays, float* 
   //   copy-out (stream 2): rgb of piece j after Rj
   // so only the first wave's H2D and the last piece's D2H are exposed.
   auto enqueue_split = [&]() -> int {
-    cudaStream_t s0 = P.streams[0], s1 = P.streams[1], s2 = P.streams[2];
+    cudaStream_t s0 = P.streams[0], s1 = P.streams[1];
     float* d_rays = P.d_rays[0];
-    float* d_rgb = P.d_rgb[0];
     float* heads = (float*)P.d_ws[0];
     const int64_t nA = wave, nB = n_rays - wave;
     CK(cudaMemcpyAsync(d_rays, rays_host, (size_t)nA * c.c_in * sizeof(float), cudaMemcpyHostToDevice, s1));
@@ -1127,56 +1140,29 @@ int hr_render_host(hr_handle* h, const float* rays_host, int64_t n_rays, float* 
     CK(cudaStreamWaitEvent(s0, P.dep_ev[1], 0));
     rc = launch_sample_net(h, d_rays + nA * c.c_in, nB, heads + nA * (int64_t)c.mlp_out, s0);
     if (rc) return rc;
-    const int pieces = 4;
-    const int64_t per = ((n_rays + pieces - 1) / pieces + 255) / 256 * 256;
-    int j = 0;
-    for (int64_t off = 0; off < n_rays; off += per, ++j) {
-      const int64_t m = (n_rays - off < per) ? (n_rays - off) : per;
-      cudaError_t e = hr::launch_render(c, h->dv, h->tabs, d_rays + off * c.c_in, heads + off * (int64_t)c.mlp_out, one_dst(d_rgb + off * 3), m,
-                                        nullptr, h->num_sms, s0, nullptr);
-      if (e != cudaSuccess) return fail("render launch failed: %s", cudaGetErrorString(e));
-      h->launches += 1;
-      CK(cudaEventRecord(P.dep_ev[2 + j], s0));
-      CK(cudaStreamWaitEvent(s2, P.dep_ev[2 + j], 0));
-      CK(cudaMemcpyAsync(rgb_host + off * 3, d_rgb + off * 3, (size_t)m * 3 * sizeof(float), cudaMemcpyDeviceToHost, s2));
-    }
-    return 0;
+    return render_pieces(4);
   };
   // Zero-copy input: when the caller's rays are pinned (device-addressable) host memory and the second tensor-core layout
   // is in use, the sample net reads them straight over PCIe -- its two encoder warps work one tile ahead of the tensor
   // pipe, so the transfer hides under the math without splitting any launch -- and leaves a device copy for the render
   // kernel.  The render kernel then runs in two pieces so that half of the D2H overlaps it.
   auto enqueue_zero_copy = [&]() -> int {
-    cudaStream_t s0 = P.streams[0], s2 = P.streams[2];
+    cudaStream_t s0 = P.streams[0];
     float* d_rays = P.d_rays[0];
-    float* d_rgb = P.d_rgb[0];
     float* heads = (float*)P.d_ws[0];
-    cudaError_t e = hr::launch_mlp_tc2(c, h->tc, rays_dev_view, heads, n_rays, h->num_sms, s0, d_rays);
-    if (e != cudaSuccess) return fail("sample-net launch failed: %s", cudaGetErrorString(e));
+    cudaError_t e = hr::launch_mlp_tc2(c, h->net.tc, rays_dev_view, heads, n_rays, h->num_sms, s0, d_rays);
+    if (e != cudaSuccess) return hr_fail("sample-net launch failed: %s", cudaGetErrorString(e));
     h->launches += 1;
     if (rgb_dev_view != nullptr) {
       // Zero-copy output: the caller's rgb buffer is device-addressable pinned memory too -- the render kernel's epilogue
       // stores the pixels straight into it (12 bytes per ray as posted writes over PCIe, spread over the kernel's whole run),
       // so there is no D2H copy and no reason to split the launch.  Completion of the stream makes the writes visible.
       e = hr::launch_render(c, h->dv, h->tabs, d_rays, heads, one_dst(rgb_dev_view), n_rays, nullptr, h->num_sms, s0, nullptr);
-      if (e != cudaSuccess) return fail("render launch failed: %s", cudaGetErrorString(e));
+      if (e != cudaSuccess) return hr_fail("render launch failed: %s", cudaGetErrorString(e));
       h->launches += 1;
       return 0;
     }
-    const int pieces = 2;
-    const int64_t per = ((n_rays + pieces - 1) / pieces + 255) / 256 * 256;
-    int j = 0;
-    for (int64_t off = 0; off < n_rays; off += per, ++j) {
-      const int64_t m = (n_rays - off < per) ? (n_rays - off) : per;
-      e = hr::launch_render(c, h->dv, h->tabs, d_rays + off * c.c_in, heads + off * (int64_t)c.mlp_out, one_dst(d_rgb + off * 3), m, nullptr,
-                            h->num_sms, s0, nullptr);
-      if (e != cudaSuccess) return fail("render launch failed: %s", cudaGetErrorString(e));
-      h->launches += 1;
-      CK(cudaEventRecord(P.dep_ev[2 + j], s0));
-      CK(cudaStreamWaitEvent(s2, P.dep_ev[2 + j], 0));
-      CK(cudaMemcpyAsync(rgb_host + off * 3, d_rgb + off * 3, (size_t)m * 3 * sizeof(float), cudaMemcpyDeviceToHost, s2));
-    }
-    return 0;
+    return render_pieces(2);
   };
   auto enqueue = [&]() -> int { return zero_copy ? enqueue_zero_copy() : (split ? enqueue_split() : enqueue_chunks()); };
   const int64_t n_chunks = (n_rays + chunk - 1) / chunk;
@@ -1200,10 +1186,10 @@ int hr_render_host(hr_handle* h, const float* rays_host, int64_t n_rays, float* 
       P.g_launches = h->launches - launches_before;
       h->launches = launches_before;  // capture enqueued nothing; the replay below is what runs
       if (rc) { if (g) cudaGraphDestroy(g); return rc; }
-      if (ce != cudaSuccess) return fail("hr_render_host: graph capture failed: %s", cudaGetErrorString(ce));
+      if (ce != cudaSuccess) return hr_fail("hr_render_host: graph capture failed: %s", cudaGetErrorString(ce));
       ce = cudaGraphInstantiate(&P.graph, g, 0);
       cudaGraphDestroy(g);
-      if (ce != cudaSuccess) { P.graph = nullptr; return fail("hr_render_host: graph instantiate failed: %s", cudaGetErrorString(ce)); }
+      if (ce != cudaSuccess) { P.graph = nullptr; return hr_fail("hr_render_host: graph instantiate failed: %s", cudaGetErrorString(ce)); }
       P.g_rays = rays_host; P.g_rgb = rgb_host; P.g_n = n_rays; P.g_chunk = key_chunk;
     }
     CK(cudaGraphLaunch(P.graph, P.streams[0]));
@@ -1219,63 +1205,72 @@ int hr_render_host(hr_handle* h, const float* rays_host, int64_t n_rays, float* 
 
 // ---- backward pass (SURVEY.md 8 f1) ----
 static int train_supported(const hr_config& c) {
-  if (c.isect_type == HR_ISECT_SPHERE_NEW) return fail("backward: the sphere_new primitive is not supported yet");
+  if (c.isect_type == HR_ISECT_SPHERE_NEW) return hr_fail("backward: the sphere_new primitive is not supported yet");
   if (c.mlp_mode == HR_MLP_ZERO) { /* no sample net: d heads is simply unused by the caller */ }
   if ((c.isect_type == HR_ISECT_SPHERE || c.isect_type == HR_ISECT_CYLINDER) && c.sphere_origin_scale != 0.0f)
-    return fail("backward: learned primitive origins (origin_scale_factor != 0) are not supported yet");
+    return hr_fail("backward: learned primitive origins (origin_scale_factor != 0) are not supported yet");
   // the colour transform's gradient is summed per CTA in shared memory
-  if (c.n_color_views > 512) return fail("backward: more than 512 colour-transform views are not supported");
-  if (c.n_samples > 64) return fail("backward: more than 64 samples per ray are not supported yet");
-  if (c.cascade) return fail("backward: cascaded (point_prediction) pipelines are not supported yet");
+  if (c.n_color_views > 512) return hr_fail("backward: more than 512 colour-transform views are not supported");
+  if (c.n_samples > 64) return hr_fail("backward: more than 64 samples per ray are not supported yet");
+  if (c.cascade) return hr_fail("backward: cascaded (point_prediction) pipelines are not supported yet");
   return 0;
+}
+
+// the fourteen gradient tables as one list, in g_sizes' order: (sigma, appearance) x (space, second) x 3 groups, the basis,
+// the colour transform
+static void grad_bufs(hr::GradTabs& g, float** out[kGradTables]) {
+  for (int i = 0; i < 3; ++i) {
+    out[i] = &g.sig_space[i]; out[3 + i] = &g.sig_second[i]; out[6 + i] = &g.app_space[i]; out[9 + i] = &g.app_second[i];
+  }
+  out[kGradBasis] = &g.basis;
+  out[kGradColorEmbedding] = &g.color_embedding;
 }
 
 static int ensure_grad_tables(hr_handle* h, cudaStream_t st) {
   const hr_config& c = h->cfg;
-  size_t want[14];
+  size_t want[kGradTables];
   for (int i = 0; i < 3; ++i) {
     const hr::PlaneTab& t = h->tabs.sig[i];
     const size_t sp = (size_t)t.C * t.H * t.W, se = (size_t)t.C * t.H2 * t.L;
     want[i] = sp; want[3 + i] = se; want[6 + i] = sp; want[9 + i] = se;
   }
-  want[12] = (size_t)c.app_dim * h->tabs.n_app_total;
-  want[13] = (size_t)c.n_color_views * 12;
-  float** bufs[14] = {&h->g_sig_space[0], &h->g_sig_space[1], &h->g_sig_space[2], &h->g_sig_second[0], &h->g_sig_second[1],
-                      &h->g_sig_second[2], &h->g_app_space[0], &h->g_app_space[1], &h->g_app_space[2], &h->g_app_second[0],
-                      &h->g_app_second[1], &h->g_app_second[2], &h->g_basis, &h->g_color_embedding};
-  for (int i = 0; i < 14; ++i) {
+  want[kGradBasis] = (size_t)c.app_dim * h->tabs.n_app_total;
+  want[kGradColorEmbedding] = (size_t)c.n_color_views * 12;
+  float** bufs[kGradTables];
+  grad_bufs(h->grads, bufs);
+  for (int i = 0; i < kGradTables; ++i) {
     if (h->g_sizes[i] == want[i] && (*bufs[i] || want[i] == 0)) continue;
     if (*bufs[i]) cudaFree(*bufs[i]);
     *bufs[i] = nullptr;
     h->g_sizes[i] = 0;
     if (want[i] == 0) continue;
     cudaError_t e = cudaMalloc((void**)bufs[i], want[i] * sizeof(float));
-    if (e != cudaSuccess) return fail("cudaMalloc(gradient table %zu floats): %s", want[i], cudaGetErrorString(e));
+    if (e != cudaSuccess) return hr_fail("cudaMalloc(gradient table %zu floats): %s", want[i], cudaGetErrorString(e));
     e = cudaMemsetAsync(*bufs[i], 0, want[i] * sizeof(float), st);
-    if (e != cudaSuccess) return fail("cudaMemsetAsync: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) return hr_fail("cudaMemsetAsync: %s", cudaGetErrorString(e));
     h->g_sizes[i] = want[i];
   }
   return 0;
 }
 
 int hr_encode_rays(hr_handle* h, const float* rays, int64_t n_rays, float* enc, void* stream) {
-  if (!h || !rays || !enc) return fail("hr_encode_rays: null argument");
-  if (h->cfg.cascade) return fail("hr_encode_rays: a cascaded pipeline has two nets; its training path is not built");
+  if (!h || !rays || !enc) return hr_fail("hr_encode_rays: null argument");
+  if (h->cfg.cascade) return hr_fail("hr_encode_rays: a cascaded pipeline has two nets; its training path is not built");
   if (n_rays == 0) return 0;
   DeviceGuard guard(h->device);
   encode_rays_kernel<<<grid_for(n_rays), 256, 0, (cudaStream_t)stream>>>(h->cfg, rays, enc, n_rays);
   cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail("hr_encode_rays: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return hr_fail("hr_encode_rays: %s", cudaGetErrorString(e));
   h->launches += 1;
   return 0;
 }
 
 int hr_render_heads(hr_handle* h, const float* rays, const float* heads, int64_t n, float* rgb, const hr_train_opts* opts,
                     void* workspace, int64_t workspace_bytes, void* stream) {
-  if (!h || !rays || !heads || !rgb || !opts || !workspace) return fail("hr_render_heads: null argument");
-  if (!h->uploaded) return fail("hr_render_heads: parameters not uploaded");
+  if (!h || !rays || !heads || !rgb || !opts || !workspace) return hr_fail("hr_render_heads: null argument");
+  if (!h->uploaded) return hr_fail("hr_render_heads: parameters not uploaded");
   if (n == 0) return 0;
-  if (workspace_bytes < heads_bytes(h, n)) return fail("hr_render_heads: workspace too small");
+  if (workspace_bytes < heads_bytes(h, n)) return hr_fail("hr_render_heads: workspace too small");
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   hr_config c = h->cfg;
@@ -1283,59 +1278,57 @@ int hr_render_heads(hr_handle* h, const float* rays, const float* heads, int64_t
   c.white_bg = opts->white_bg ? 1 : 0;
   if (opts->white_bg) c.black_bg = 0;
   float* hcm = (float*)workspace;
-  permute_heads<<<grid_for(n * (long long)c.mlp_out), 256, 0, st>>>(heads, hcm, n, c.n_samples, c.head_stride);
-  cudaError_t e = hr::launch_render(c, h->dv, h->tabs, rays, hcm, one_dst(rgb), n, nullptr, h->num_sms, st, nullptr);
-  if (e != cudaSuccess) return fail("hr_render_heads: %s", cudaGetErrorString(e));
+  cudaError_t e = permute_heads_async(c, heads, hcm, n, st);
+  if (e == cudaSuccess) e = hr::launch_render(c, h->dv, h->tabs, rays, hcm, one_dst(rgb), n, nullptr, h->num_sms, st, nullptr);
+  if (e != cudaSuccess) return hr_fail("hr_render_heads: %s", cudaGetErrorString(e));
   h->launches += 2;
   return 0;
 }
 
 int hr_render_backward(hr_handle* h, const float* rays, const float* heads, int64_t n, const float* d_rgb, float* d_heads,
                        const hr_train_opts* opts, void* workspace, int64_t workspace_bytes, void* stream) {
-  if (!h || !rays || !heads || !d_rgb || !d_heads || !opts || !workspace) return fail("hr_render_backward: null argument");
-  if (!h->uploaded) return fail("hr_render_backward: parameters not uploaded");
+  if (!h || !rays || !heads || !d_rgb || !d_heads || !opts || !workspace) return hr_fail("hr_render_backward: null argument");
+  if (!h->uploaded) return hr_fail("hr_render_backward: parameters not uploaded");
   if (train_supported(h->cfg)) return 1;
   if (n == 0) return 0;
-  if (workspace_bytes < 2 * heads_bytes(h, n)) return fail("hr_render_backward: workspace too small (hr_train_workspace_bytes)");
+  if (workspace_bytes < 2 * heads_bytes(h, n)) return hr_fail("hr_render_backward: workspace too small (hr_train_workspace_bytes)");
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   const hr_config& c = h->cfg;
   if (ensure_grad_tables(h, st)) return 1;
   float* hcm = (float*)workspace;
   float* gcm = (float*)((char*)workspace + heads_bytes(h, n));
-  permute_heads<<<grid_for(n * (long long)c.mlp_out), 256, 0, st>>>(heads, hcm, n, c.n_samples, c.head_stride);
+  cudaError_t e = permute_heads_async(c, heads, hcm, n, st);
+  if (e != cudaSuccess) return hr_fail("hr_render_backward: %s", cudaGetErrorString(e));
   const int white = opts->white_bg ? 1 : 0;
   EventPair eb{nullptr, nullptr};
   const bool timing = h->timing && h->ev_bwd.size() < 8192;
   if (timing) { CK(cudaEventCreate(&eb.a)); CK(cudaEventCreate(&eb.b)); CK(cudaEventRecord(eb.a, st)); }
-  cudaError_t e = hr::launch_render_bwd(c, h->dv, h->tabs, h->g_sig_space, h->g_sig_second, h->g_app_space, h->g_app_second, h->g_basis,
-                                        h->g_color_embedding, rays, hcm, d_rgb, gcm, n, opts->clamp_output ? 1 : 0, white, h->num_sms, st);
-  if (e != cudaSuccess) return fail("hr_render_backward: %s", cudaGetErrorString(e));
+  e = hr::launch_render_bwd(c, h->dv, h->tabs, h->grads, rays, hcm, d_rgb, gcm, n, opts->clamp_output ? 1 : 0, white, h->num_sms, st);
+  if (e != cudaSuccess) return hr_fail("hr_render_backward: %s", cudaGetErrorString(e));
   if (timing) { CK(cudaEventRecord(eb.b, st)); h->ev_bwd.push_back(eb); }
-  unpermute_heads<<<grid_for(n * (long long)c.mlp_out), 256, 0, st>>>(gcm, d_heads, n, c.n_samples, c.head_stride);
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return fail("hr_render_backward: %s", cudaGetErrorString(e));
+  e = unpermute_heads_async(c, gcm, d_heads, n, st);
+  if (e != cudaSuccess) return hr_fail("hr_render_backward: %s", cudaGetErrorString(e));
   h->launches += 3;
   return 0;
 }
 
 int hr_grad_zero(hr_handle* h, void* stream) {
-  if (!h) return fail("hr_grad_zero: null handle");
-  if (!h->uploaded) return fail("hr_grad_zero: parameters not uploaded");
+  if (!h) return hr_fail("hr_grad_zero: null handle");
+  if (!h->uploaded) return hr_fail("hr_grad_zero: parameters not uploaded");
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   if (ensure_grad_tables(h, st)) return 1;
-  float* bufs[14] = {h->g_sig_space[0], h->g_sig_space[1], h->g_sig_space[2], h->g_sig_second[0], h->g_sig_second[1], h->g_sig_second[2],
-                     h->g_app_space[0], h->g_app_space[1], h->g_app_space[2], h->g_app_second[0], h->g_app_second[1], h->g_app_second[2],
-                     h->g_basis, h->g_color_embedding};
-  for (int i = 0; i < 14; ++i)
-    if (bufs[i]) CK(cudaMemsetAsync(bufs[i], 0, h->g_sizes[i] * sizeof(float), st));
+  float** bufs[kGradTables];
+  grad_bufs(h->grads, bufs);
+  for (int i = 0; i < kGradTables; ++i)
+    if (*bufs[i]) CK(cudaMemsetAsync(*bufs[i], 0, h->g_sizes[i] * sizeof(float), st));
   return 0;
 }
 
 int hr_grad_read(hr_handle* h, const hr_grads* out, void* stream) {
-  if (!h || !out) return fail("hr_grad_read: null argument");
-  if (!h->uploaded) return fail("hr_grad_read: parameters not uploaded");
+  if (!h || !out) return hr_fail("hr_grad_read: null argument");
+  if (!h->uploaded) return hr_fail("hr_grad_read: parameters not uploaded");
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   if (ensure_grad_tables(h, st)) return 1;
@@ -1346,8 +1339,8 @@ int hr_grad_read(hr_handle* h, const hr_grads* out, void* stream) {
     for (int f = 0; f < 2; ++f) {
       float* dsp = f ? out->app_plane[i] : out->sigma_plane[i];
       float* dse = f ? out->app_second[i] : out->sigma_second[i];
-      const float* gsp = f ? h->g_app_space[i] : h->g_sig_space[i];
-      const float* gse = f ? h->g_app_second[i] : h->g_sig_second[i];
+      const float* gsp = f ? h->grads.app_space[i] : h->grads.sig_space[i];
+      const float* gse = f ? h->grads.app_second[i] : h->grads.sig_second[i];
       if (dsp) unpack_channel_last<<<grid_for((long long)t.C * t.H * t.W), 256, 0, st>>>(gsp, dsp, t.C, t.H, t.W);
       if (dse) {
         if (c.dynamic)
@@ -1358,21 +1351,22 @@ int hr_grad_read(hr_handle* h, const hr_grads* out, void* stream) {
       }
     }
   }
-  if (out->basis_mat) CK(cudaMemcpyAsync(out->basis_mat, h->g_basis, h->g_sizes[12] * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  if (out->color_embedding && h->g_sizes[13])
-    CK(cudaMemcpyAsync(out->color_embedding, h->g_color_embedding, h->g_sizes[13] * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (out->basis_mat) CK(cudaMemcpyAsync(out->basis_mat, h->grads.basis, h->g_sizes[kGradBasis] * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (out->color_embedding && h->g_sizes[kGradColorEmbedding])
+    CK(cudaMemcpyAsync(out->color_embedding, h->grads.color_embedding, h->g_sizes[kGradColorEmbedding] * sizeof(float),
+                       cudaMemcpyDeviceToDevice, st));
   cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail("hr_grad_read: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return hr_fail("hr_grad_read: %s", cudaGetErrorString(e));
   return 0;
 }
 
 // ---- the sample net's training forward / backward on the tensor cores (hr_mlp_tc2.cu, hr_mlp_train.cu) ----
 static int train_net_supported(const hr_handle* h, const char* fn) {
   const hr_config& c = h->cfg;
-  if (c.cascade) return fail("%s: cascaded (point_prediction) pipelines have two sample nets; only single-net pipelines train on the tensor cores", fn);
-  if (c.mlp_mode == HR_MLP_ZERO) return fail("%s: a zero sample net has no layers to train", fn);
-  if (c.mlp_mode != HR_MLP_BF16X3_TC) return fail("%s: the training forward is the wgmma sample net: create the handle with mlp_mode HR_MLP_BF16X3_TC", fn);
-  if (!h->uploaded || !h->tc_ready) return fail("%s: parameters not uploaded", fn);
+  if (c.cascade) return hr_fail("%s: cascaded (point_prediction) pipelines have two sample nets; only single-net pipelines train on the tensor cores", fn);
+  if (c.mlp_mode == HR_MLP_ZERO) return hr_fail("%s: a zero sample net has no layers to train", fn);
+  if (c.mlp_mode != HR_MLP_BF16X3_TC) return hr_fail("%s: the training forward is the wgmma sample net: create the handle with mlp_mode HR_MLP_BF16X3_TC", fn);
+  if (!h->uploaded || !h->net.tc_ready) return hr_fail("%s: parameters not uploaded", fn);
   return 0;
 }
 
@@ -1383,29 +1377,29 @@ int64_t hr_train_net_workspace_bytes(const hr_handle* h, int64_t n_rays) {
 
 int hr_train_net_forward(hr_handle* h, const float* rays, int64_t n, float* heads, void* workspace, int64_t workspace_bytes,
                          void* stream) {
-  if (!h || !rays || !heads || !workspace) return fail("hr_train_net_forward: null argument");
+  if (!h || !rays || !heads || !workspace) return hr_fail("hr_train_net_forward: null argument");
   if (train_net_supported(h, "hr_train_net_forward")) return 1;
   if (n == 0) return 0;
   const hr::TrainNetLayout t = hr::train_net_layout(h->cfg, n, h->num_sms);
-  if (workspace_bytes < (int64_t)t.total) return fail("hr_train_net_forward: workspace too small (hr_train_net_workspace_bytes)");
-  if (((uintptr_t)workspace & 255) != 0) return fail("hr_train_net_forward: workspace must be 256-byte aligned");
+  if (workspace_bytes < (int64_t)t.total) return hr_fail("hr_train_net_forward: workspace too small (hr_train_net_workspace_bytes)");
+  if (((uintptr_t)workspace & 255) != 0) return hr_fail("hr_train_net_forward: workspace must be 256-byte aligned");
   DeviceGuard guard(h->device);
   uint8_t* ws = (uint8_t*)workspace;
   const hr::TrainSave sv{(float*)(ws + t.enc), (float*)(ws + t.act), (long long)t.act_stride, t.ld_enc};
-  cudaError_t e = hr::launch_mlp_tc2_train(h->cfg, h->tc, rays, heads, n, h->num_sms, (cudaStream_t)stream, sv);
-  if (e != cudaSuccess) return fail("hr_train_net_forward: %s", cudaGetErrorString(e));
+  cudaError_t e = hr::launch_mlp_tc2_train(h->cfg, h->net.tc, rays, heads, n, h->num_sms, (cudaStream_t)stream, sv);
+  if (e != cudaSuccess) return hr_fail("hr_train_net_forward: %s", cudaGetErrorString(e));
   h->launches += 1;
   return 0;
 }
 
 int hr_train_net_backward(hr_handle* h, const float* d_heads, int64_t n, const hr_net_grads* out, void* workspace,
                           int64_t workspace_bytes, void* stream) {
-  if (!h || !d_heads || !out || !workspace) return fail("hr_train_net_backward: null argument");
+  if (!h || !d_heads || !out || !workspace) return hr_fail("hr_train_net_backward: null argument");
   if (train_net_supported(h, "hr_train_net_backward")) return 1;
   const hr_config& c = h->cfg;
   const int L = c.mlp_layers, W = c.mlp_width;
   for (int l = 0; l < L; ++l)
-    if (!out->weight[l] || !out->bias[l]) return fail("hr_train_net_backward: gradient buffers of layer %d missing", l);
+    if (!out->weight[l] || !out->bias[l]) return hr_fail("hr_train_net_backward: gradient buffers of layer %d missing", l);
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   if (n == 0) {  // no rays: every gradient is zero
@@ -1417,12 +1411,12 @@ int hr_train_net_backward(hr_handle* h, const float* d_heads, int64_t n, const h
     return 0;
   }
   const hr::TrainNetLayout t = hr::train_net_layout(c, n, h->num_sms);
-  if (workspace_bytes < (int64_t)t.total) return fail("hr_train_net_backward: workspace too small (hr_train_net_workspace_bytes)");
-  if (((uintptr_t)workspace & 255) != 0) return fail("hr_train_net_backward: workspace must be 256-byte aligned");
+  if (workspace_bytes < (int64_t)t.total) return hr_fail("hr_train_net_backward: workspace too small (hr_train_net_workspace_bytes)");
+  if (((uintptr_t)workspace & 255) != 0) return hr_fail("hr_train_net_backward: workspace must be 256-byte aligned");
   uint8_t* ws = (uint8_t*)workspace;
-  permute_heads<<<grid_for(n * (long long)c.mlp_out), 256, 0, st>>>(d_heads, (float*)(ws + t.dlast), n, c.n_samples, c.head_stride);
-  cudaError_t e = hr::train_net_backward(c, h->simt, n, out->weight, out->bias, ws, h->num_sms, st);
-  if (e != cudaSuccess) return fail("hr_train_net_backward: %s", cudaGetErrorString(e));
+  cudaError_t e = permute_heads_async(c, d_heads, (float*)(ws + t.dlast), n, st);
+  if (e == cudaSuccess) e = hr::train_net_backward(c, h->net.simt, n, out->weight, out->bias, ws, h->num_sms, st);
+  if (e != cudaSuccess) return hr_fail("hr_train_net_backward: %s", cudaGetErrorString(e));
   h->launches += 1 + 3 * L;
   return 0;
 }
@@ -1435,23 +1429,23 @@ static hr_act hr_config::* const kActMembers[] = {
     &hr_config::pre_act_z, &hr_config::pre_act_sigma, &hr_config::pre_isect_act};
 
 int hr_set_activations(hr_handle* h, const hr_config* cfg) {
-  if (!h || !cfg) return fail("hr_set_activations: null argument");
+  if (!h || !cfg) return hr_fail("hr_set_activations: null argument");
   // everything but the activations must be the handle's configuration (hr_config has no padding: 4-byte members only)
   hr_config probe = *cfg;
   for (hr_act hr_config::* m : kActMembers) probe.*m = h->cfg.*m;
   if (memcmp(&probe, &h->cfg, sizeof(hr_config)) != 0)
-    return fail("hr_set_activations: the configuration differs from the handle's beyond its activations (create a new handle)");
+    return hr_fail("hr_set_activations: the configuration differs from the handle's beyond its activations (create a new handle)");
   for (hr_act hr_config::* m : kActMembers) {
     const hr_act& a = cfg->*m;
     if (a.kind != HR_ACT_IDENTITY && a.kind != HR_ACT_SIGMOID && a.kind != HR_ACT_TANH)
-      return fail("hr_set_activations: unknown activation kind %d", a.kind);
+      return hr_fail("hr_set_activations: unknown activation kind %d", a.kind);
     if (a.eased && m != &hr_config::act_sigma && m != &hr_config::act_point_sigma && m != &hr_config::pre_act_sigma)
-      return fail("hr_set_activations: only act_sigma, act_point_sigma and pre_act_sigma may be eased");
+      return hr_fail("hr_set_activations: only act_sigma, act_point_sigma and pre_act_sigma may be eased");
   }
   if (hr::eases_density(*cfg) && cfg->n_samples > 64)
-    return fail("hr_set_activations: eased density heads above 64 samples per ray are not supported");
-  // the nets' configurations (cfg_net / cfg_pre) are copies of cfg: keep their activations in step, although no net reads them
-  for (hr_act hr_config::* m : kActMembers) h->cfg.*m = h->cfg_net.*m = h->cfg_pre.*m = cfg->*m;
+    return hr_fail("hr_set_activations: eased density heads above 64 samples per ray are not supported");
+  // the nets' configurations (net.cfg / pre.cfg) are copies of cfg: keep their activations in step, although no net reads them
+  for (hr_act hr_config::* m : kActMembers) h->cfg.*m = h->net.cfg.*m = h->pre.cfg.*m = cfg->*m;
   drop_host_graph(h);  // its kernel nodes hold the old configuration by value
   return 0;
 }
@@ -1459,7 +1453,7 @@ int hr_set_activations(hr_handle* h, const hr_config* cfg) {
 int64_t hr_launch_count(const hr_handle* h) { return h ? h->launches : -1; }
 
 int hr_timing_enable(hr_handle* h, int enable) {
-  if (!h) return fail("null handle");
+  if (!h) return hr_fail("null handle");
   h->timing = enable != 0;
   return 0;
 }
@@ -1470,7 +1464,7 @@ static void drop_events(std::vector<EventPair>& v) {
 }
 
 int hr_timing_reset(hr_handle* h) {
-  if (!h) return fail("null handle");
+  if (!h) return hr_fail("null handle");
   drop_events(h->ev_render);
   drop_events(h->ev_mlp);
   drop_events(h->ev_bwd);
@@ -1478,13 +1472,20 @@ int hr_timing_reset(hr_handle* h) {
   return 0;
 }
 
-int hr_timing_read_backward(hr_handle* h, double* backward_ms_avg, int64_t* launches) {
-  if (!h) return fail("null handle");
-  double sb = 0;
-  for (auto& p : h->ev_bwd) {
+// waits for every pair and adds up their elapsed times
+static int sum_event_ms(std::vector<EventPair>& v, double* sum) {
+  *sum = 0;
+  for (auto& p : v) {
     CK(cudaEventSynchronize(p.b));
-    float ms = 0; CK(cudaEventElapsedTime(&ms, p.a, p.b)); sb += ms;
+    float ms = 0; CK(cudaEventElapsedTime(&ms, p.a, p.b)); *sum += ms;
   }
+  return 0;
+}
+
+int hr_timing_read_backward(hr_handle* h, double* backward_ms_avg, int64_t* launches) {
+  if (!h) return hr_fail("null handle");
+  double sb = 0;
+  if (sum_event_ms(h->ev_bwd, &sb)) return 1;
   const size_t k = h->ev_bwd.size();
   if (backward_ms_avg) *backward_ms_avg = k ? sb / k : 0.0;
   if (launches) *launches = (int64_t)k;
@@ -1492,16 +1493,9 @@ int hr_timing_read_backward(hr_handle* h, double* backward_ms_avg, int64_t* laun
 }
 
 int hr_timing_read(hr_handle* h, double* render_ms_avg, double* mlp_ms_avg, int64_t* launches) {
-  if (!h) return fail("null handle");
+  if (!h) return hr_fail("null handle");
   double sr = 0, sm = 0;
-  for (auto& p : h->ev_render) {
-    CK(cudaEventSynchronize(p.b));
-    float ms = 0; CK(cudaEventElapsedTime(&ms, p.a, p.b)); sr += ms;
-  }
-  for (auto& p : h->ev_mlp) {
-    CK(cudaEventSynchronize(p.b));
-    float ms = 0; CK(cudaEventElapsedTime(&ms, p.a, p.b)); sm += ms;
-  }
+  if (sum_event_ms(h->ev_render, &sr) || sum_event_ms(h->ev_mlp, &sm)) return 1;
   // per hr_render call: a call may run several sub-batches, i.e. several launches of each kernel
   const size_t k = h->timed_calls;
   if (render_ms_avg) *render_ms_avg = k ? sr / k : 0.0;
@@ -1514,22 +1508,19 @@ int hr_destroy(hr_handle* h) {
   if (!h) return 0;
   DeviceGuard guard(h->device);
   for (auto& sl : h->slots) cudaFree(sl.ptr);
-  for (int i = 0; i < 3; ++i) {
-    cudaFree(h->g_sig_space[i]); cudaFree(h->g_sig_second[i]); cudaFree(h->g_app_space[i]); cudaFree(h->g_app_second[i]);
-  }
-  cudaFree(h->g_basis);
-  cudaFree(h->g_color_embedding);
-  hr::free_mlp_tc2(h);
+  float** grads[kGradTables];
+  grad_bufs(h->grads, grads);
+  for (float** g : grads) cudaFree(*g);
+  hr::free_mlp_tc2(h->net);
+  hr::free_mlp_tc2(h->pre);
   drop_events(h->ev_render);
   drop_events(h->ev_mlp);
   drop_events(h->ev_bwd);
+  drop_host_graph(h);
+  if (h->pipe.fork_ev) cudaEventDestroy(h->pipe.fork_ev);
+  for (int k = 0; k < 8; ++k)
+    if (h->pipe.dep_ev[k]) cudaEventDestroy(h->pipe.dep_ev[k]);
   for (int i = 0; i < 3; ++i) {
-    if (i == 0) {
-      drop_host_graph(h);
-      if (h->pipe.fork_ev) cudaEventDestroy(h->pipe.fork_ev);
-      for (int k = 0; k < 8; ++k)
-        if (h->pipe.dep_ev[k]) cudaEventDestroy(h->pipe.dep_ev[k]);
-    }
     if (h->pipe.join_ev[i]) cudaEventDestroy(h->pipe.join_ev[i]);
     if (h->pipe.d_rays[i]) cudaFree(h->pipe.d_rays[i]);
     if (h->pipe.d_rgb[i]) cudaFree(h->pipe.d_rgb[i]);

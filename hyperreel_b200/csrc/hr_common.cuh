@@ -26,6 +26,16 @@ struct RenderTabs {
   const float* color_embedding;  // [n_color_views][12] per-camera colour transform + shift (point.py:558-592), or null
 };
 
+// Gradient tables: same channel-last layout as the forward's PlaneTab (second factor: pre-blended keyframe lines / lines).
+struct GradTabs {
+  float* sig_space[3];
+  float* sig_second[3];
+  float* app_space[3];
+  float* app_second[3];
+  float* basis;  // [app_dim][NT]
+  float* color_embedding;  // [n_color_views][12] (RARE variants only; null without a colour transform)
+};
+
 // Host-derived scalars (computed in double on the host, then rounded once to fp32, the way the
 // reference's Python-float constants meet fp32 tensors).
 struct Derived {

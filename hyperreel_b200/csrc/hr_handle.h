@@ -28,6 +28,22 @@ struct HostPipe {
   cudaEvent_t dep_ev[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // wave-split pipeline edges
 };
 
+// One sample net as hr_upload packs it: its configuration (a copy of the handle's with the net's own shape) and both packs.
+struct SampleNet {
+  hr_config cfg;
+  hr::MlpSimtPack simt{};
+  hr::MlpTcPack tc{};
+  bool tc_ready = false;
+  size_t tc_alloc_bytes = 0;  // current allocation behind tc.wpack / tc.bias (reused while the layout is unchanged)
+  int tc_alloc_bias = 0;
+};
+
+// hr::GradTabs' buffers as a flat list (hr_api.cu: grad_bufs): their number, and the two read by name
+constexpr int kGradTables = 14, kGradBasis = 12, kGradColorEmbedding = 13;
+
+// every size of a workspace segment is rounded up to 256 bytes, so that every segment starts 256-byte aligned
+static inline int64_t align256(int64_t bytes) { return (bytes + 255) / 256 * 256; }
+
 struct hr_handle {
   hr_config cfg;
   hr::Derived dv;
@@ -37,29 +53,14 @@ struct hr_handle {
   struct Slot { void* ptr; size_t bytes; };
   std::vector<Slot> slots;   // device allocations of packed parameters, in hr_upload's request order
   size_t slot_cursor = 0;
-  hr::RenderTabs tabs;
-  // the net behind the final heads (cfg_net == cfg, or the point net of a cascaded pipeline evaluated on 8-float point rows)
-  hr_config cfg_net;
-  hr::MlpSimtPack simt;
-  hr::MlpTcPack tc;
-  bool tc_ready = false;
-  size_t tc_alloc_bytes = 0;  // current allocation behind tc.wpack / tc.bias (reused while the layout is unchanged)
-  int tc_alloc_bias = 0;
+  hr::RenderTabs tabs{};
+  // the net behind the final heads (net.cfg == cfg, or the point net of a cascaded pipeline evaluated on 8-float point rows)
+  SampleNet net;
   // cascaded pipelines only: the first-stage ray net (cfg.pre_*), same kernels
-  hr_config cfg_pre;
-  hr::MlpSimtPack simt_pre;
-  hr::MlpTcPack tc_pre;
-  bool tc_pre_ready = false;
-  size_t tc_pre_alloc_bytes = 0;
-  int tc_pre_alloc_bias = 0;
+  SampleNet pre;
   // gradient tables of the backward pass (hr_render_backward), packed like the forward tables; allocated on first use
-  float* g_sig_space[3] = {nullptr, nullptr, nullptr};
-  float* g_sig_second[3] = {nullptr, nullptr, nullptr};
-  float* g_app_space[3] = {nullptr, nullptr, nullptr};
-  float* g_app_second[3] = {nullptr, nullptr, nullptr};
-  float* g_basis = nullptr;
-  float* g_color_embedding = nullptr;  // [n_color_views][12], the colour transform's table (none without one)
-  size_t g_sizes[14] = {0};   // element counts of the 14 buffers above (to notice a resized grid)
+  hr::GradTabs grads{};
+  size_t g_sizes[kGradTables] = {0};  // element counts of grad_bufs' buffers (to notice a resized grid)
   int64_t launches = 0;
   bool timing = false;
   size_t timed_calls = 0;      // hr_render calls covered by ev_render / ev_mlp (a call may run several sub-batches)

@@ -78,11 +78,10 @@ cudaError_t train_net_backward(const hr_config& c, const MlpSimtPack& simt, long
                                float* const* bias, uint8_t* ws, int num_sms, cudaStream_t st);
 }  // namespace hr
 
-struct hr_handle;
-struct hr_params;
+struct SampleNet;
 namespace hr {
-// packs the net `c` describes into `pk`; alloc_bytes / alloc_bias remember the allocation behind pk (reused while unchanged)
-int pack_mlp_tc2(hr_handle* h, const hr_config& c, MlpTcPack& pk, size_t& alloc_bytes, int& alloc_bias,
-                 const float* const* w_dev, const float* const* b_dev, cudaStream_t st);
-void free_mlp_tc2(hr_handle* h);
+// packs the net `net.cfg` describes into net.tc; net.tc_alloc_bytes / tc_alloc_bias remember the allocation behind it
+// (reused while unchanged)
+int pack_mlp_tc2(SampleNet& net, const float* const* w_dev, const float* const* b_dev, cudaStream_t st);
+void free_mlp_tc2(SampleNet& net);
 }

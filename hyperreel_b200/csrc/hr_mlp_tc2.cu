@@ -397,8 +397,11 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
 }
 
 // Pass table + weight images (format: hr_tc_pack.cu).  Called by hr_upload with the handle's device current.
-int pack_mlp_tc2(hr_handle* h, const hr_config& c, MlpTcPack& pk, size_t& alloc_bytes, int& alloc_bias,
-                 const float* const* w_dev, const float* const* b_dev, cudaStream_t st) {
+int pack_mlp_tc2(SampleNet& net, const float* const* w_dev, const float* const* b_dev, cudaStream_t st) {
+  const hr_config& c = net.cfg;
+  MlpTcPack& pk = net.tc;
+  size_t& alloc_bytes = net.tc_alloc_bytes;
+  int& alloc_bias = net.tc_alloc_bias;
   const int W = c.mlp_width;
   if (W != 128 && W != 256) return hr_fail("tensor-core sample net: hidden width must be 128 or 256 (got %d)", W);
   if (c.mlp_in > 64) return hr_fail("tensor-core sample net: encoded input wider than 64 features (%d)", c.mlp_in);
@@ -476,15 +479,11 @@ int pack_mlp_tc2(hr_handle* h, const hr_config& c, MlpTcPack& pk, size_t& alloc_
   return 0;
 }
 
-void free_mlp_tc2(hr_handle* h) {
-  if (h->tc.wpack) cudaFree(const_cast<void*>(h->tc.wpack));
-  if (h->tc.bias) cudaFree(const_cast<float*>(h->tc.bias));
-  h->tc.wpack = nullptr; h->tc.bias = nullptr;
-  h->tc_alloc_bytes = 0; h->tc_alloc_bias = 0;
-  if (h->tc_pre.wpack) cudaFree(const_cast<void*>(h->tc_pre.wpack));
-  if (h->tc_pre.bias) cudaFree(const_cast<float*>(h->tc_pre.bias));
-  h->tc_pre.wpack = nullptr; h->tc_pre.bias = nullptr;
-  h->tc_pre_alloc_bytes = 0; h->tc_pre_alloc_bias = 0;
+void free_mlp_tc2(SampleNet& net) {
+  if (net.tc.wpack) cudaFree(const_cast<void*>(net.tc.wpack));
+  if (net.tc.bias) cudaFree(const_cast<float*>(net.tc.bias));
+  net.tc.wpack = nullptr; net.tc.bias = nullptr;
+  net.tc_alloc_bytes = 0; net.tc_alloc_bias = 0;
 }
 
 cudaError_t launch_mlp_tc2(const hr_config& cfg, const MlpTcPack& pk, const float* rays, float* heads, long long n, int num_sms,

@@ -4,17 +4,9 @@
 
 namespace hr {
 
-cudaError_t launch_render_bwd(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs, float* const* g_sig_space,
-                              float* const* g_sig_second, float* const* g_app_space, float* const* g_app_second, float* g_basis,
-                              float* g_color_embedding, const float* rays, const float* heads, const float* d_rgb, float* d_heads,
-                              long long n, int clamp_output, int white_bg, int num_sms, cudaStream_t stream) {
-  GradTabs gt;
-  for (int i = 0; i < 3; ++i) {
-    gt.sig_space[i] = g_sig_space[i]; gt.sig_second[i] = g_sig_second[i];
-    gt.app_space[i] = g_app_space[i]; gt.app_second[i] = g_app_second[i];
-  }
-  gt.basis = g_basis;
-  gt.color_embedding = g_color_embedding;
+cudaError_t launch_render_bwd(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs, const GradTabs& gt, const float* rays,
+                              const float* heads, const float* d_rgb, float* d_heads, long long n, int clamp_output, int white_bg,
+                              int num_sms, cudaStream_t stream) {
   BwdOpts opt{clamp_output, white_bg};
   if (eases_density(cfg)) return launch_render_bwd_ease(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, stream);
   if (needs_rare_bwd(cfg)) return launch_render_bwd_rare(cfg, dv, tabs, gt, rays, heads, d_rgb, d_heads, n, opt, num_sms, stream);

@@ -176,16 +176,6 @@ __device__ __forceinline__ void red_add4(float* p, float a, float b, float c, fl
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
-// Gradient tables: same channel-last layout as the forward's PlaneTab (second factor: pre-blended keyframe lines / lines).
-struct GradTabs {
-  float* sig_space[3];
-  float* sig_second[3];
-  float* app_space[3];
-  float* app_second[3];
-  float* basis;  // [app_dim][NT]
-  float* color_embedding;  // [n_color_views][12] (RARE variants only; null without a colour transform)
-};
-
 // One channel quad (4 channels starting at ch0) of one VM group for one sample: forward values and coordinate slopes.
 struct Quad {
   float A[4], dAa[4], dAb[4];  // space plane value, d/d fa, d/d fb (per texel unit)

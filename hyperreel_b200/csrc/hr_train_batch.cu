@@ -565,8 +565,6 @@ int sample_rows(const char* fn, const Plan& plan, const hr_camera* cameras, int3
   return 0;
 }
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 // Workspace of hr_build_importance_table: the slots, the select state and one histogram per slot.
 size_t importance_workspace(int64_t n_slots) {
   return align256((size_t)n_slots * sizeof(hr::ImportanceSlot)) + align256((size_t)n_slots * 2 * sizeof(uint32_t)) +
