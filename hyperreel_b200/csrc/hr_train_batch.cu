@@ -18,6 +18,7 @@
 // each row branches on its own record's fisheye and two_plane flags (camera_ray<true, true>) and one batch may mix pinhole,
 // fisheye and two-plane views.
 #include <algorithm>
+#include <type_traits>
 #include <vector>
 
 #include "hr_handle.h"
@@ -68,41 +69,47 @@ __device__ __forceinline__ uint64_t feistel_permute(uint64_t x, const FeistelKey
   return x;
 }
 
-__global__ void __launch_bounds__(256)
-train_batch_kernel(const hr_camera* __restrict__ cams, const uint8_t* __restrict__ images, int height, int width,
-                   const __grid_constant__ FeistelKey key, long long first, long long rows, const int64_t* __restrict__ order,
-                   int c_in, float* __restrict__ coords, float* __restrict__ rgb, float* __restrict__ weight,
-                   int64_t* __restrict__ pixel_ids) {
+// ---- the training tables: train_rows_kernel<Plan> maps table row k to its pixel through the plan's table_pixel ----
+// table_pixel(plan, start, height, width, k, v, y, x) gives the pixel of table row k as (view, y, x); false for a row the plan
+// does not hold (k outside [0, n_table), or a malformed plan), so a malformed plan reads and writes nothing out of bounds.
+// start: the plan's prefix, staged in shared memory by the kernel when it fits.
+
+// Every pixel of every view (hr_sample_train_batch): table row k is pixel k.  It has no view prefix, so the kernel stages
+// nothing and searches nothing.  The kernel also tests kWhole where hr_sample_train_batch's arguments are fixed (permute
+// mode, no table ids, the row's pixel id is k), so that instantiation does no per-row work that only the other plans need.
+struct WholePlan {
+  long long n_table;  // n_views*H*W
+};
+template <class Plan>
+constexpr bool kWhole = std::is_same<Plan, WholePlan>::value;
+
+__device__ __forceinline__ bool table_pixel(const WholePlan& plan, const int64_t*, int height, int width, long long k,
+                                            int& v, int& y, int& x) {
+  if (k < 0 || k >= plan.n_table) return false;
   const long long hw = (long long)height * width;
-  for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < rows; r += (long long)gridDim.x * blockDim.x) {
-    long long p = order ? (long long)order[r] : (long long)feistel_permute((uint64_t)(first + r), key);
-    float row[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    float c0 = 0.f, c1 = 0.f, c2 = 0.f, w = 0.f;
-    if (p >= 0 && p < (long long)key.n) {
-      const int v = (int)(p / hw);
-      const long long q = p - v * hw;
-      const int y = (int)(q / width), x = (int)(q - (long long)y * width);
-      const hr_camera& cam = cams[v];
-      camera_ray<true, true>(cam, x, y, ndc_scale(cam), row);
-      const uint8_t* px = images + 3 * p;
-      c0 = __fdiv_rn((float)px[0], 255.0f);
-      c1 = __fdiv_rn((float)px[1], 255.0f);
-      c2 = __fdiv_rn((float)px[2], 255.0f);
-      w = 1.0f;
-    } else {
-      p = -1;  // an explicit order entry outside [0, N): a zero row of weight 0 (the host binding refuses such orders)
-    }
-    float2* cr = reinterpret_cast<float2*>(coords + r * c_in);
-    cr[0] = make_float2(row[0], row[1]);
-    cr[1] = make_float2(row[2], row[3]);
-    cr[2] = make_float2(row[4], row[5]);
-    if (c_in == 8) cr[3] = make_float2(row[6], row[7]);
-    rgb[3 * r + 0] = c0;
-    rgb[3 * r + 1] = c1;
-    rgb[3 * r + 2] = c2;
-    weight[r] = w;
-    if (pixel_ids) pixel_ids[r] = p;
+  v = (int)(k / hw);
+  const long long q = k - v * hw;
+  y = (int)(q / width);
+  x = (int)(q - (long long)y * width);
+  return true;
+}
+
+// The view of table row k, for the plans with a per-view row prefix: the last view v with start[v] <= k, and k's rank q
+// within it; false for k outside [0, n_table) or a prefix that does not bracket k.
+__device__ __forceinline__ bool find_view(const int64_t* start, int n_views, long long n_table, long long k, int& v,
+                                          long long& q) {
+  if (k < 0 || k >= n_table) return false;
+  int lo = 0, hi = n_views;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (start[mid] <= k) lo = mid;
+    else hi = mid;
   }
+  v = lo;
+  const long long s0 = start[v];
+  if (k < s0 || k >= start[v + 1]) return false;
+  q = k - s0;
+  return true;
 }
 
 // ---- training table of per-view pixel subsets (hr_sample_train_rows) ----
@@ -131,25 +138,13 @@ struct TablePlan {
   long long n_table;     // rows drawn or permuted: [0, n_table)
 };
 
-// The pixel of table row k as (view, y, x); false for a row the plan does not hold (k outside [0, n_table), a start prefix
-// that does not bracket k, a stride < 1, or a rank past the view's last kept pixel), so a malformed plan reads and writes
-// nothing out of bounds.
-// start: the plan's prefix, staged in shared memory by the caller when it fits.
+// Not held besides the rows find_view refuses: a stride < 1, or a rank past the view's last kept pixel.
 __device__ __forceinline__ bool table_pixel(const TablePlan& plan, const int64_t* start, int height, int width, long long k,
                                             int& v, int& y, int& x) {
-  if (k < 0 || k >= plan.n_table) return false;
-  int lo = 0, hi = plan.n_views;  // the largest v in [0, n_views) with start[v] <= k
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (start[mid] <= k) lo = mid;
-    else hi = mid;
-  }
-  v = lo;
-  const long long s0 = start[v];
-  if (k < s0 || k >= start[v + 1]) return false;
+  long long q;
+  if (!find_view(start, plan.n_views, plan.n_table, k, v, q)) return false;
   const int s = plan.rule[2 * v], o = plan.rule[2 * v + 1];
   if (s < 1) return false;
-  const long long q = k - s0;
   long long block, rem;
   if (q <= 0x7fffffffLL) {  // 32-bit division for every view of fewer than 2^31 pixels
     block = (unsigned)q / (unsigned)width;
@@ -194,20 +189,12 @@ struct MaskPlan {
   long long n_table;            // rows drawn or permuted: [0, n_table)
 };
 
-// The pixel of table row k as (view, y, x); false for a row the plan does not hold, as the rule plan's table_pixel.
+// Not held besides the rows find_view refuses: a rank past the view's last kept pixel.
 __device__ __forceinline__ bool table_pixel(const MaskPlan& plan, const int64_t* start, int height, int width, long long k,
                                             int& v, int& y, int& x) {
-  if (k < 0 || k >= plan.n_table) return false;
-  int lo = 0, hi = plan.n_views;  // the largest v in [0, n_views) with start[v] <= k
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (start[mid] <= k) lo = mid;
-    else hi = mid;
-  }
-  v = lo;
-  const long long s0 = start[v];
-  if (k < s0 || k >= start[v + 1]) return false;
-  const long long q = k - s0, hw = (long long)height * width;
+  long long q;
+  if (!find_view(start, plan.n_views, plan.n_table, k, v, q)) return false;
+  const long long hw = (long long)height * width;
   long long p = q;
   const int slot = plan.slot[v];
   if (slot >= 0) {
@@ -238,7 +225,7 @@ __device__ __forceinline__ bool table_pixel(const MaskPlan& plan, const int64_t*
 
 constexpr int kStagedViews = 4095;  // prefixes of up to this many views are staged in shared memory (32 KB)
 
-// Plan: TablePlan (a (stride, offset) rule per view) or MaskPlan (a keep mask per view).
+// Plan: WholePlan (every pixel), TablePlan (a (stride, offset) rule per view) or MaskPlan (a keep mask per view).
 template <class Plan>
 __global__ void __launch_bounds__(256)
 train_rows_kernel(const hr_camera* __restrict__ cams, const uint8_t* __restrict__ images, int height, int width,
@@ -246,25 +233,28 @@ train_rows_kernel(const hr_camera* __restrict__ cams, const uint8_t* __restrict_
                   long long first, long long rows, const int64_t* __restrict__ table_rows, int c_in, float* __restrict__ coords,
                   float* __restrict__ rgb, float* __restrict__ weight, int64_t* __restrict__ pixel_ids,
                   int64_t* __restrict__ table_ids) {
-  extern __shared__ int64_t staged[];
-  const int64_t* start = plan.start;
-  if (plan.n_views <= kStagedViews) {  // the binary search's dependent loads then hit shared memory
-    for (int i = threadIdx.x; i <= plan.n_views; i += blockDim.x) staged[i] = plan.start[i];
-    __syncthreads();
-    start = staged;
+  const int64_t* start = nullptr;
+  if constexpr (!kWhole<Plan>) {
+    extern __shared__ int64_t staged[];
+    start = plan.start;
+    if (plan.n_views <= kStagedViews) {  // the binary search's dependent loads then hit shared memory
+      for (int i = threadIdx.x; i <= plan.n_views; i += blockDim.x) staged[i] = plan.start[i];
+      __syncthreads();
+      start = staged;
+    }
   }
   const long long hw = (long long)height * width;
   for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < rows; r += (long long)gridDim.x * blockDim.x) {
     long long k;
     if (table_rows) k = (long long)table_rows[r];
-    else if (mode == HR_SAMPLE_PERMUTE) k = (long long)feistel_permute((uint64_t)(first + r), key);
+    else if (kWhole<Plan> || mode == HR_SAMPLE_PERMUTE) k = (long long)feistel_permute((uint64_t)(first + r), key);
     else k = (long long)__umul64hi(mix64(dkey + kGolden * ((uint64_t)(first + r) + 1)), (uint64_t)plan.n_table);
     float row[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     float c0 = 0.f, c1 = 0.f, c2 = 0.f, w = 0.f;
     long long p = -1;
     int v, y, x;
     if (table_pixel(plan, start, height, width, k, v, y, x)) {
-      p = v * hw + (long long)y * width + x;
+      p = kWhole<Plan> ? k : v * hw + (long long)y * width + x;
       const hr_camera& cam = cams[v];
       camera_ray<true, true>(cam, x, y, ndc_scale(cam), row);
       const uint8_t* px = images + 3 * p;
@@ -285,7 +275,7 @@ train_rows_kernel(const hr_camera* __restrict__ cams, const uint8_t* __restrict_
     rgb[3 * r + 2] = c2;
     weight[r] = w;
     if (pixel_ids) pixel_ids[r] = p;
-    if (table_ids) table_ids[r] = k;
+    if (!kWhole<Plan> && table_ids) table_ids[r] = k;
   }
 }
 
@@ -315,6 +305,22 @@ __device__ __forceinline__ uint32_t diff_key(const uint8_t* cur, const uint8_t* 
   for (int c = 0; c < 3; ++c)
     d[c] = fabsf(__fsub_rn(__fdiv_rn((float)cur[c], 255.0f), __fdiv_rn((float)prev[c], 255.0f)));
   return __float_as_uint(__fdiv_rn(__fadd_rn(__fadd_rn(d[0], d[1]), d[2]), 3.0f));
+}
+
+// Inclusive scan over a CTA of kThreads threads, one value per thread, through the shared array part[kThreads]; returns this
+// thread's inclusive sum.  Ends with a barrier, so every thread may then read any element of part.
+template <class T, int kThreads>
+__device__ __forceinline__ T block_inclusive_scan(T* part, T value) {
+  const int t = threadIdx.x;
+  part[t] = value;
+  __syncthreads();
+  for (int off = 1; off < kThreads; off <<= 1) {
+    const T add = t >= off ? part[t - off] : T(0);
+    __syncthreads();
+    part[t] += add;
+    __syncthreads();
+  }
+  return part[t];
 }
 
 // grid (chunks, n_slots): histogram of pass kPass over the keys whose bits above this pass's equal the slot's prefix.
@@ -357,19 +363,12 @@ importance_select_kernel(const ImportanceSlot* __restrict__ slots, uint32_t* __r
     c[j] = g[t * kPer + j];
     sum += c[j];
   }
-  part[t] = sum;
-  __syncthreads();
-  for (int off = 1; off < 256; off <<= 1) {  // inclusive scan of the per-thread sums
-    const uint32_t add = t >= off ? part[t - off] : 0u;
-    __syncthreads();
-    part[t] += add;
-    __syncthreads();
-  }
+  const uint32_t incl = block_inclusive_scan<uint32_t, 256>(part, sum);
   const uint32_t prefix = kPass == 0 ? 0u : state[2 * s];
   const uint32_t rank = kPass == 0 ? slots[s].rank : state[2 * s + 1];
-  uint32_t before = part[t] - sum;
+  uint32_t before = incl - sum;
   __syncthreads();  // every thread has read state before the owner of the rank overwrites it
-  if (rank >= before && rank < part[t]) {
+  if (rank >= before && rank < incl) {
 #pragma unroll
     for (int j = 0; j < kPer; ++j) {
       if (rank < before + c[j]) {
@@ -434,21 +433,14 @@ importance_scan_kernel(int blocks, const ImportanceSlot* __restrict__ slots, uin
   const int per = (blocks + 255) / 256, b0 = min(blocks, t * per), b1 = min(blocks, b0 + per);
   uint32_t sum = 0;
   for (int b = b0; b < b1; ++b) sum += bs[b];
-  part[t] = sum;
-  __syncthreads();
-  for (int off = 1; off < 256; off <<= 1) {
-    const uint32_t add = t >= off ? part[t - off] : 0u;
-    __syncthreads();
-    part[t] += add;
-    __syncthreads();
-  }
-  uint32_t run = part[t] - sum;
+  const uint32_t incl = block_inclusive_scan<uint32_t, 256>(part, sum);
+  uint32_t run = incl - sum;
   for (int b = b0; b < b1; ++b) {
     const uint32_t n = bs[b];
     bs[b] = run;
     run += n;
   }
-  if (t == 255) view_rows[slots[s].view] = part[255];
+  if (t == 255) view_rows[slots[s].view] = incl;
 }
 
 // one block of 1024 threads: whole views' row counts (H*W) and the exclusive int64 prefix over all views.
@@ -463,15 +455,7 @@ importance_views_kernel(int n_views, long long hw, const int32_t* __restrict__ v
     if (view_slot[v] < 0) view_rows[v] = hw;
     sum += view_rows[v];
   }
-  part[t] = sum;
-  __syncthreads();
-  for (int off = 1; off < 1024; off <<= 1) {
-    const long long add = t >= off ? part[t - off] : 0;
-    __syncthreads();
-    part[t] += add;
-    __syncthreads();
-  }
-  long long run = part[t] - sum;
+  long long run = block_inclusive_scan<long long, 1024>(part, sum) - sum;
   if (t == 0) view_start[0] = 0;
   for (int v = v0; v < v1; ++v) {
     run += view_rows[v];
@@ -482,43 +466,9 @@ importance_views_kernel(int n_views, long long hw, const int32_t* __restrict__ v
 }  // namespace
 }  // namespace hr
 
-extern "C" int hr_sample_train_batch(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height,
-                                     int32_t width, int32_t c_in, uint64_t seed, int64_t epoch, int64_t batch_index,
-                                     int64_t batch_size, const int64_t* order, float* coords, float* rgb, float* weight,
-                                     int64_t* pixel_ids, int64_t* n_rows, void* stream) {
-  if (!cameras || !images || !coords || !rgb || !weight) return hr_fail("hr_sample_train_batch: null argument");
-  if (n_views < 1 || height < 1 || width < 1)
-    return hr_fail("hr_sample_train_batch: bad image stack %d x %d x %d", n_views, height, width);
-  if (c_in != 6 && c_in != 8) return hr_fail("hr_sample_train_batch: c_in must be 6 or 8, got %d", c_in);
-  if (batch_size < 1) return hr_fail("hr_sample_train_batch: batch_size must be >= 1, got %lld", (long long)batch_size);
-  if (((uintptr_t)coords % 8) || ((uintptr_t)rgb % 4) || ((uintptr_t)weight % 4) || ((uintptr_t)pixel_ids % 8) ||
-      ((uintptr_t)order % 8) || ((uintptr_t)cameras % 4))
-    return hr_fail("hr_sample_train_batch: misaligned pointer (coords and pixel_ids / order need 8 bytes, the rest 4)");
-  const uint64_t n = (uint64_t)n_views * (uint64_t)height * (uint64_t)width;
-  if (n > (1ull << 62)) return hr_fail("hr_sample_train_batch: %llu pixels, at most 2^62", (unsigned long long)n);
-  long long first = 0, rows = batch_size;
-  if (!order) {
-    const int64_t n_batches = (int64_t)((n + (uint64_t)batch_size - 1) / (uint64_t)batch_size);
-    if (batch_index < 0 || batch_index >= n_batches)
-      return hr_fail("hr_sample_train_batch: batch_index %lld outside [0, %lld)", (long long)batch_index,
-                     (long long)n_batches);
-    first = batch_index * batch_size;
-    if ((uint64_t)(first + rows) > n) rows = (long long)(n - (uint64_t)first);  // the epoch's short last batch
-  }
-  const hr::FeistelKey key = hr::feistel_key(seed, epoch, n);
-  long long g = (rows + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
-  hr::train_batch_kernel<<<(unsigned)g, 256, 0, (cudaStream_t)stream>>>(cameras, images, height, width, key, first, rows, order,
-                                                                       c_in, coords, rgb, weight, pixel_ids);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return hr_fail("hr_sample_train_batch: %s", cudaGetErrorString(e));
-  if (n_rows) *n_rows = rows;
-  return 0;
-}
-
 namespace {
 
-// The checks, batch range and launch shared by hr_sample_train_rows and hr_sample_train_mask_rows; `plan` carries the table.
+// The checks, batch range and launch shared by the three sampling entry points; `plan` carries the table.
 template <class Plan>
 int sample_rows(const char* fn, const Plan& plan, const hr_camera* cameras, int32_t n_views, const uint8_t* images,
                 int32_t height, int32_t width, int32_t c_in, int32_t mode, uint64_t seed, int64_t epoch, int64_t batch_index,
@@ -529,8 +479,10 @@ int sample_rows(const char* fn, const Plan& plan, const hr_camera* cameras, int3
   if (c_in != 6 && c_in != 8) return hr_fail("%s: c_in must be 6 or 8, got %d", fn, c_in);
   if (mode != HR_SAMPLE_PERMUTE && mode != HR_SAMPLE_REPLACE) return hr_fail("%s: unknown mode %d", fn, mode);
   if (batch_size < 1) return hr_fail("%s: batch_size must be >= 1, got %lld", fn, (long long)batch_size);
+  uintptr_t view_start = 0;  // WholePlan has none
+  if constexpr (!hr::kWhole<Plan>) view_start = (uintptr_t)plan.start;
   if (((uintptr_t)coords % 8) || ((uintptr_t)rgb % 4) || ((uintptr_t)weight % 4) || ((uintptr_t)pixel_ids % 8) ||
-      ((uintptr_t)table_ids % 8) || ((uintptr_t)table_rows % 8) || ((uintptr_t)plan.start % 8) || ((uintptr_t)cameras % 4))
+      ((uintptr_t)table_ids % 8) || ((uintptr_t)table_rows % 8) || (view_start % 8) || ((uintptr_t)cameras % 4))
     return hr_fail("%s: misaligned pointer (coords, view_start and the int64 row arrays need 8 bytes, the rest 4)", fn);
   const uint64_t n = (uint64_t)n_views * (uint64_t)height * (uint64_t)width;
   if (n > (1ull << 62)) return hr_fail("%s: %llu pixels, at most 2^62", fn, (unsigned long long)n);
@@ -541,11 +493,11 @@ int sample_rows(const char* fn, const Plan& plan, const hr_camera* cameras, int3
   if (!table_rows) {
     if (batch_index < 0) return hr_fail("%s: batch_index %lld < 0", fn, (long long)batch_index);
     if (mode == HR_SAMPLE_PERMUTE) {
-      const int64_t n_batches = (n_table + batch_size - 1) / batch_size;
+      const int64_t n_batches = (n_table - 1) / batch_size + 1;  // ceil(n_table / batch_size) without overflow
       if (batch_index >= n_batches)
         return hr_fail("%s: batch_index %lld outside [0, %lld)", fn, (long long)batch_index, (long long)n_batches);
       first = batch_index * batch_size;
-      if (first + rows > n_table) rows = n_table - first;  // the epoch's short last batch
+      if (rows > n_table - first) rows = n_table - first;  // the epoch's short last batch
     } else {
       if (batch_index > (INT64_MAX - batch_size) / batch_size)
         return hr_fail("%s: batch_index %lld too large", fn, (long long)batch_index);
@@ -555,7 +507,8 @@ int sample_rows(const char* fn, const Plan& plan, const hr_camera* cameras, int3
   const hr::FeistelKey key = hr::feistel_key(seed, epoch, (uint64_t)n_table);
   long long g = (rows + 255) / 256;
   if (g > 148 * 16) g = 148 * 16;
-  const size_t smem = n_views <= hr::kStagedViews ? (size_t)(n_views + 1) * sizeof(int64_t) : 0;
+  const size_t smem =
+      !hr::kWhole<Plan> && n_views <= hr::kStagedViews ? (size_t)(n_views + 1) * sizeof(int64_t) : 0;
   hr::train_rows_kernel<Plan><<<(unsigned)g, 256, smem, (cudaStream_t)stream>>>(
       cameras, images, height, width, plan, key, hr::draw_key(seed, epoch), mode, first, rows, table_rows, c_in, coords, rgb,
       weight, pixel_ids, table_ids);
@@ -572,6 +525,20 @@ size_t importance_workspace(int64_t n_slots) {
 }
 
 }  // namespace
+
+extern "C" int hr_sample_train_batch(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height,
+                                     int32_t width, int32_t c_in, uint64_t seed, int64_t epoch, int64_t batch_index,
+                                     int64_t batch_size, const int64_t* order, float* coords, float* rgb, float* weight,
+                                     int64_t* pixel_ids, int64_t* n_rows, void* stream) {
+  if (!cameras || !images || !coords || !rgb || !weight) return hr_fail("hr_sample_train_batch: null argument");
+  if (((uintptr_t)coords % 8) || ((uintptr_t)rgb % 4) || ((uintptr_t)weight % 4) || ((uintptr_t)pixel_ids % 8) ||
+      ((uintptr_t)order % 8) || ((uintptr_t)cameras % 4))
+    return hr_fail("hr_sample_train_batch: misaligned pointer (coords and pixel_ids / order need 8 bytes, the rest 4)");
+  // the table is every pixel (sample_rows refuses a bad image stack and more than 2^62 pixels before n_table is used)
+  const hr::WholePlan plan{(long long)((uint64_t)n_views * (uint64_t)height * (uint64_t)width)};
+  return sample_rows("hr_sample_train_batch", plan, cameras, n_views, images, height, width, c_in, HR_SAMPLE_PERMUTE, seed,
+                     epoch, batch_index, batch_size, order, coords, rgb, weight, pixel_ids, nullptr, n_rows, stream);
+}
 
 extern "C" int hr_sample_train_rows(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height,
                                     int32_t width, int32_t c_in, const int64_t* view_start, const int32_t* view_rule,

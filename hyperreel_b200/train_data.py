@@ -280,8 +280,6 @@ class DeviceRayBatches:
         else:
             self._n_rows = None  # read from the device on first use
             self._build_importance(importance)
-        # the original path (every pixel, each once per epoch) keeps its own kernel
-        self._table_path = self.replacement or self.subsample is not None or self.importance is not None
 
     @staticmethod
     def _check_importance(plan, n: int, hw: int) -> List[Optional[Tuple[int, int]]]:
@@ -412,28 +410,22 @@ class DeviceRayBatches:
         i = int(i)
         if not 0 <= i < len(self):
             raise IndexError(f"batch {i} outside [0, {len(self)})")
-        if not self._table_path:
-            rows = min(self.batch_size, self.n_pixels - i * self.batch_size)
-            out = self._launch(rows, i, None, with_pixel_ids or with_table_ids)
-            if with_table_ids:  # without a plan the table is every pixel in order
-                out["table_ids"] = out["pixel_ids"].clone() if with_pixel_ids else out.pop("pixel_ids")
-            return out
         rows = self.batch_size if self.replacement else min(self.batch_size, self.n_rows - i * self.batch_size)
-        return self._launch_rows(rows, i, None, with_pixel_ids, with_table_ids)
+        return self._launch(rows, i, None, with_pixel_ids, with_table_ids)
 
     def gather_rows(self, table_ids, with_pixel_ids: bool = False) -> Dict[str, torch.Tensor]:
         """The rows of the given training-table indices, in the given order, the table in the reference's ``all_coords``
         order (views in order, each view's kept pixels row-major): for replaying the reference's own sampler indices.  An
         index outside ``[0, n_rows)`` raises ``ValueError`` (for device indices the check synchronises with the device)."""
         ids = self._check_ids(table_ids, self.n_rows, "table ids")
-        return self._launch_rows(ids.numel(), 0, ids, with_pixel_ids, False)
+        return self._launch(ids.numel(), 0, ids, with_pixel_ids, False)
 
     def gather(self, pixel_ids, with_pixel_ids: bool = False) -> Dict[str, torch.Tensor]:
         """The rows of the given pixels, in the given order: for callers that bring their own order (the reference's
         ``np.random.permutation``, say).  An id outside ``[0, n*H*W)`` raises ``ValueError`` (for device ids the check
         synchronises with the device)."""
         ids = self._check_ids(pixel_ids, self.n_pixels, "pixel ids")
-        return self._launch(ids.numel(), 0, ids, with_pixel_ids)
+        return self._launch(ids.numel(), 0, ids, with_pixel_ids, False, ids_are_pixels=True)
 
     def __iter__(self):
         for i in range(len(self)):
@@ -451,51 +443,45 @@ class DeviceRayBatches:
             raise ValueError(f"{what} must lie in [0, {n}), got [{lo}, {hi}]")
         return ids.to(device=self.device, dtype=torch.int64).contiguous()
 
-    def _launch_rows(self, rows: int, index: int, table_rows: Optional[torch.Tensor], with_pixel_ids: bool,
-                     with_table_ids: bool) -> Dict[str, torch.Tensor]:
+    def _launch(self, rows: int, index: int, ids: Optional[torch.Tensor], with_pixel_ids: bool, with_table_ids: bool,
+                ids_are_pixels: bool = False) -> Dict[str, torch.Tensor]:
+        """Batch ``index`` of the epoch, or the rows of the explicit ``ids`` (table rows, or pixels with ``ids_are_pixels``).
+        Explicit pixels and the permuted batches without a plan go through ``hr_sample_train_batch``, everything else
+        through the plan's entry (``hr_sample_train_rows`` or ``hr_sample_train_mask_rows``)."""
         dev = self.device
+        whole = ids_are_pixels or (ids is None and not self.replacement and self.subsample is None and
+                                   self.importance is None)
         coords = torch.empty((rows, self.c_in), dtype=torch.float32, device=dev)
         rgb = torch.empty((rows, 3), dtype=torch.float32, device=dev)
         weight = torch.empty((rows, 1), dtype=torch.float32, device=dev)
-        pids = torch.empty((rows,), dtype=torch.int64, device=dev) if with_pixel_ids else None
-        tids = torch.empty((rows,), dtype=torch.int64, device=dev) if with_table_ids else None
+        pids = torch.empty((rows,), dtype=torch.int64, device=dev) if with_pixel_ids or (whole and with_table_ids) else None
+        tids = torch.empty((rows,), dtype=torch.int64, device=dev) if with_table_ids and not whole else None
+        ptr = lambda t: t.data_ptr() if t is not None else None
         n_rows = C.c_int64(0)
-        mode = L.SAMPLE_REPLACE if self.replacement else L.SAMPLE_PERMUTE
-        tail = (self.n_rows, mode, self.seed, self.epoch, index, rows if table_rows is not None else self.batch_size,
-                table_rows.data_ptr() if table_rows is not None else None, coords.data_ptr(), rgb.data_ptr(),
-                weight.data_ptr(), pids.data_ptr() if pids is not None else None,
-                tids.data_ptr() if tids is not None else None, C.byref(n_rows), torch.cuda.current_stream(dev).cuda_stream)
-        head = (self.cameras.data_ptr(), self.n_views, self.images.data_ptr(), self.height, self.width, self.c_in,
-                self._view_start.data_ptr())
+        head = (self.cameras.data_ptr(), self.n_views, self.images.data_ptr(), self.height, self.width, self.c_in)
+        # an explicit list is the whole batch; otherwise the entry shortens the epoch's last batch
+        batch = (index, rows if ids is not None else self.batch_size, ptr(ids), coords.data_ptr(), rgb.data_ptr(),
+                 weight.data_ptr(), ptr(pids))
+        stream = torch.cuda.current_stream(dev).cuda_stream
         with torch.cuda.device(dev):
-            if self.importance is None:
-                L.check(self._lib.hr_sample_train_rows(*head, self._view_rule.data_ptr(), *tail))
+            if whole:
+                L.check(self._lib.hr_sample_train_batch(*head, self.seed, self.epoch, *batch, C.byref(n_rows), stream))
             else:
-                L.check(self._lib.hr_sample_train_mask_rows(*head, self._view_slot.data_ptr(), self._block_start.data_ptr(),
-                                                            self._masks.data_ptr(), *tail))
+                mode = L.SAMPLE_REPLACE if self.replacement else L.SAMPLE_PERMUTE
+                tail = (self.n_rows, mode, self.seed, self.epoch, *batch, ptr(tids), C.byref(n_rows), stream)
+                if self.importance is None:
+                    L.check(self._lib.hr_sample_train_rows(*head, self._view_start.data_ptr(), self._view_rule.data_ptr(),
+                                                           *tail))
+                else:
+                    L.check(self._lib.hr_sample_train_mask_rows(*head, self._view_start.data_ptr(),
+                                                                self._view_slot.data_ptr(), self._block_start.data_ptr(),
+                                                                self._masks.data_ptr(), *tail))
         assert n_rows.value == rows, (n_rows.value, rows)
+        if whole and with_table_ids:  # without a plan, table ids are pixel ids
+            tids = pids.clone() if with_pixel_ids else pids
         out = {"coords": coords, "rgb": rgb, "weight": weight}
-        if pids is not None:
+        if with_pixel_ids:
             out["pixel_ids"] = pids
-        if tids is not None:
+        if with_table_ids:
             out["table_ids"] = tids
-        return out
-
-    def _launch(self, rows: int, index: int, order: Optional[torch.Tensor], with_ids: bool) -> Dict[str, torch.Tensor]:
-        dev = self.device
-        coords = torch.empty((rows, self.c_in), dtype=torch.float32, device=dev)
-        rgb = torch.empty((rows, 3), dtype=torch.float32, device=dev)
-        weight = torch.empty((rows, 1), dtype=torch.float32, device=dev)
-        ids = torch.empty((rows,), dtype=torch.int64, device=dev) if with_ids else None
-        n_rows = C.c_int64(0)
-        with torch.cuda.device(dev):
-            L.check(self._lib.hr_sample_train_batch(
-                self.cameras.data_ptr(), self.n_views, self.images.data_ptr(), self.height, self.width, self.c_in, self.seed,
-                self.epoch, index, rows if order is not None else self.batch_size,
-                order.data_ptr() if order is not None else None, coords.data_ptr(), rgb.data_ptr(), weight.data_ptr(),
-                ids.data_ptr() if ids is not None else None, C.byref(n_rows), torch.cuda.current_stream(dev).cuda_stream))
-        assert n_rows.value == rows, (n_rows.value, rows)
-        out = {"coords": coords, "rgb": rgb, "weight": weight}
-        if ids is not None:
-            out["pixel_ids"] = ids
         return out

@@ -1,8 +1,8 @@
 """Times the camera-model kernels with pinhole and fisheye cameras, and the pinhole path against another build of the library.
 
   (a) generate_rays_kernel on a 1280x960 frame (the Immersive dataset's training size), pinhole against fisheye;
-  (b) train_batch_kernel (every pixel, permuted) and train_rows_kernel (replacement draws) at 16,384 and 65,536 rows over
-      20 views of 1280x960, all pinhole against all fisheye;
+  (b) train_rows_kernel over every pixel, permuted (hr_sample_train_batch), and with replacement draws
+      (hr_sample_train_rows), at 16,384 and 65,536 rows over 20 views of 1280x960, all pinhole against all fisheye;
   (c) with --other-lib PATH (a libhyperreel_b200.so of an earlier ABI, whose hr_camera is the pinhole prefix of this one): the
       pinhole workloads of (a) and (b) through both libraries, alternated round by round in one process.
 
@@ -21,6 +21,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 W, H, N_VIEWS = 1280, 960, 20
 PINHOLE_FIELDS = 14  # fields of hr_camera before the fisheye members (ABI <= 16)
+# the every-pixel kernel: train_rows_kernel<WholePlan>, named train_batch_kernel in earlier builds (both match, so builds compare)
+WHOLE_IMAGE_KERNEL = ("WholePlan", "train_batch_kernel")
 
 
 def main():
@@ -77,9 +79,9 @@ def main():
     out = {"gpu": gpu_facts(), "frame": f"{W}x{H}", "views": N_VIEWS, "calls": args.calls}
 
     def workloads(lib, host_cam, dev_cams):
-        """name -> (kernel name, call)"""
+        """name -> (kernel names, call)"""
         frame = torch.empty((W * H, 8), dtype=torch.float32, device=dev)
-        w = {"generate_rays 1280x960": ("generate_rays_kernel", lambda: lib.hr_generate_rays(
+        w = {"generate_rays 1280x960": (("generate_rays_kernel",), lambda: lib.hr_generate_rays(
             C.byref(host_cam), 8, 0, W * H, frame.data_ptr(), stream))}
         for B in (16384, 65536):
             coords = torch.empty((B, 8), dtype=torch.float32, device=dev)
@@ -100,11 +102,11 @@ def main():
                                                 state[0], B, None, coords.data_ptr(), rgb.data_ptr(), weight.data_ptr(),
                                                 None, None, None, stream)
 
-            w[f"train_batch {B}"] = ("train_batch_kernel", batch)
-            w[f"train_rows replace {B}"] = ("train_rows_kernel", rows)
+            w[f"train_batch {B}"] = (WHOLE_IMAGE_KERNEL, batch)
+            w[f"train_rows replace {B}"] = (("train_rows_kernel",), rows)
         return w
 
-    def kernel_us(name, fn):
+    def kernel_us(names, fn):
         for _ in range(5):
             assert fn() == 0
         torch.cuda.synchronize()
@@ -112,10 +114,10 @@ def main():
             for _ in range(args.calls):
                 fn()
             torch.cuda.synchronize()
-        kern = [e for e in prof.key_averages() if name in e.key]
+        kern = [e for e in prof.key_averages() if any(n in e.key for n in names)]
         total = sum(getattr(e, "device_time_total", 0.0) or getattr(e, "cuda_time_total", 0.0) for e in kern)
         count = sum(e.count for e in kern)
-        assert count >= args.calls - 2, (name, count)  # a session may drop an event at its start
+        assert count >= args.calls - 2, (names, count)  # a session may drop an event at its start
         return total / count
 
     this = open_lib(L.LIB_PATH)

@@ -1,8 +1,8 @@
 """Times the ray kernels with two-plane light-field views against pinhole cameras, and the pinhole path against another build.
 
   (a) generate_rays_kernel on a 1024x1024 view (the large Stanford configs' tarot_small size), pinhole against two-plane;
-  (b) train_batch_kernel (every pixel, permuted) and train_rows_kernel (replacement draws) at 16,384 and 65,536 rows over
-      17 views of 1024x1024, all pinhole against all two-plane;
+  (b) train_rows_kernel over every pixel, permuted (hr_sample_train_batch), and with replacement draws
+      (hr_sample_train_rows), at 16,384 and 65,536 rows over 17 views of 1024x1024, all pinhole against all two-plane;
   (c) render_video of the 120-frame render path of a Stanford spiral (lightfield_cameras(split="render")) at 512x512 with
       the shipped stanford_z_plane model, against 120 pinhole frames of the same size;
   (d) with --other-lib PATH (a libhyperreel_b200.so of an earlier ABI, whose hr_camera is a prefix of this one): the pinhole
@@ -23,6 +23,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 W, H, N_VIEWS = 1024, 1024, 17
 VW, VH = 512, 512
+# the every-pixel kernel: train_rows_kernel<WholePlan>, named train_batch_kernel in earlier builds (both match, so builds compare)
+WHOLE_IMAGE_KERNEL = ("WholePlan", "train_batch_kernel")
 
 
 def main():
@@ -80,9 +82,9 @@ def main():
     out = {"gpu": gpu_facts(), "frame": f"{W}x{H}", "views": N_VIEWS, "calls": args.calls}
 
     def workloads(lib, host_cam, dev_cams):
-        """name -> (kernel name, call)"""
+        """name -> (kernel names, call)"""
         frame = torch.empty((W * H, 6), dtype=torch.float32, device=dev)
-        w = {f"generate_rays {W}x{H}": ("generate_rays_kernel", lambda: lib.hr_generate_rays(
+        w = {f"generate_rays {W}x{H}": (("generate_rays_kernel",), lambda: lib.hr_generate_rays(
             C.byref(host_cam), 6, 0, W * H, frame.data_ptr(), stream))}
         for B in (16384, 65536):
             coords = torch.empty((B, 6), dtype=torch.float32, device=dev)
@@ -103,11 +105,11 @@ def main():
                                                 state[0], B, None, coords.data_ptr(), rgb.data_ptr(), weight.data_ptr(),
                                                 None, None, None, stream)
 
-            w[f"train_batch {B}"] = ("train_batch_kernel", batch)
-            w[f"train_rows replace {B}"] = ("train_rows_kernel", rows)
+            w[f"train_batch {B}"] = (WHOLE_IMAGE_KERNEL, batch)
+            w[f"train_rows replace {B}"] = (("train_rows_kernel",), rows)
         return w
 
-    def kernel_us(name, fn):
+    def kernel_us(names, fn):
         for _ in range(5):
             assert fn() == 0
         torch.cuda.synchronize()
@@ -115,10 +117,10 @@ def main():
             for _ in range(args.calls):
                 fn()
             torch.cuda.synchronize()
-        kern = [e for e in prof.key_averages() if name in e.key]
+        kern = [e for e in prof.key_averages() if any(n in e.key for n in names)]
         total = sum(getattr(e, "device_time_total", 0.0) or getattr(e, "cuda_time_total", 0.0) for e in kern)
         count = sum(e.count for e in kern)
-        assert count >= args.calls - 2, (name, count)  # a session may drop an event at its start
+        assert count >= args.calls - 2, (names, count)  # a session may drop an event at its start
         return total / count
 
     this = open_lib(L.LIB_PATH)

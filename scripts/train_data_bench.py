@@ -6,7 +6,7 @@ train_net="tc"), at 16,384 and 65,536 rays per step:
       np.random.permutation + gather, timed), then per step a consecutive slice copied to the GPU with .cuda(), from pinned
       memory (non_blocking, what the DataLoader's pin_memory gives) and from pageable memory, and split by format_batch.
       The DataLoader's per-row __getitem__ and collate are not included, so (a) is a lower bound of the reference's cost;
-  (b) DeviceRayBatches.batch(i) alone: the train_batch_kernel time (torch.profiler, a run of its own), the device time per
+  (b) DeviceRayBatches.batch(i) alone: the every-pixel kernel's time (torch.profiler, a run of its own), the device time per
       call (CUDA events over back-to-back calls) and the host time to issue a call;
   (c) training_step fed by each of them, and by one batch kept resident on the device (no data path at all), alternated
       round by round; CUDA events per step, mean over the steps of a round.
@@ -26,6 +26,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 W, H = 2048, 1088
 HBM_BYTES_S = 3.35e12  # NVIDIA H100 SXM data sheet (700 W card)
+# the every-pixel kernel: train_rows_kernel<WholePlan>, named train_batch_kernel in earlier builds (both match, so builds compare)
+WHOLE_IMAGE_KERNEL = ("WholePlan", "train_batch_kernel")
 
 
 def rig_cameras(hb, n_views, near):
@@ -143,7 +145,7 @@ def main():
             for _ in range(args.calls):
                 feed("device")
             torch.cuda.synchronize()
-        kern = [e for e in prof.key_averages() if "train_batch_kernel" in e.key]
+        kern = [e for e in prof.key_averages() if any(n in e.key for n in WHOLE_IMAGE_KERNEL)]
         kernel_ms = (sum(getattr(e, "device_time_total", 0.0) or getattr(e, "cuda_time_total", 0.0) for e in kern) / 1e3 /
                      max(1, sum(e.count for e in kern)))
         write_bytes, read_bytes = B * 48, B * 32  # 48 B row written; each 3 B gather touches one 32 B sector (more if it straddles)

@@ -25,6 +25,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 W, H = 2048, 1088
 N_FRAMES = 50
 TECHNICOLOR = dict(load_full_step=8, subsample_keyframe_step=4, subsample_keyframe_frac=0.25, subsample_frac=0.125)
+# the every-pixel kernel: train_rows_kernel<WholePlan>, named train_batch_kernel in earlier builds (both match, so builds compare)
+WHOLE_IMAGE_KERNEL = ("WholePlan", "train_batch_kernel")
 
 
 def train_cameras(hb):
@@ -80,13 +82,13 @@ def main():
         torch.cuda.synchronize()
         return a.elapsed_time(b) / k
 
-    def kernel_ms(fn, name):
+    def kernel_ms(fn, names):
         torch.cuda.synchronize()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             for _ in range(args.calls):
                 fn()
             torch.cuda.synchronize()
-        kern = [e for e in prof.key_averages() if name in e.key]
+        kern = [e for e in prof.key_averages() if any(n in e.key for n in names)]
         return (sum(getattr(e, "device_time_total", 0.0) or getattr(e, "cuda_time_total", 0.0) for e in kern) / 1e3 /
                 max(1, sum(e.count for e in kern)))
 
@@ -109,7 +111,7 @@ def main():
 
             for _ in range(5):
                 call()
-            kname = "train_batch_kernel" if "train_batch" in name else "train_rows_kernel"
+            kname = WHOLE_IMAGE_KERNEL if "train_batch" in name else ("train_rows_kernel",)
             res[name] = {"device_ms_per_call": events(call, args.calls), "kernel_ms": kernel_ms(call, kname),
                          "table_rows": d.n_rows, "batches_per_epoch": len(d)}
         out["batches"].append(res)

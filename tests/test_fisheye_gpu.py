@@ -66,7 +66,7 @@ def _check(out, rows, images):
 def test_mixed_fisheye_and_pinhole_batches_equal_generate_rays():
     cams, images, rows = _mixed_views()
     n = rows.shape[0]
-    # every pixel, permuted (train_batch_kernel)
+    # every pixel, permuted (train_rows_kernel<WholePlan>)
     d = hb.DeviceRayBatches(cams, images, batch_size=1000, seed=3)
     seen = []
     for i in range(len(d)):
@@ -77,7 +77,7 @@ def test_mixed_fisheye_and_pinhole_batches_equal_generate_rays():
     ids = torch.randint(0, n, (4096,), generator=torch.Generator().manual_seed(1))
     out = d.gather(ids, with_pixel_ids=True)
     _check(out, rows, images)
-    # per-view subsets, permuted and with replacement (train_rows_kernel)
+    # per-view subsets, permuted and with replacement (train_rows_kernel<TablePlan>)
     plan = [(1, 0), (4, 1), (2, 1)]
     for kw in ({}, {"replacement": True, "num_iters": 5}):
         d = hb.DeviceRayBatches(cams, images, batch_size=700, seed=5, subsample=plan, **kw)

@@ -82,7 +82,7 @@ def _check(out, rows, images):
 def test_mixed_model_batches_equal_generate_rays():
     cams, images, rows = _mixed_views()
     n = rows.shape[0]
-    d = hb.DeviceRayBatches(cams, images, batch_size=1100, seed=3)  # train_batch_kernel
+    d = hb.DeviceRayBatches(cams, images, batch_size=1100, seed=3)  # train_rows_kernel<WholePlan>
     seen = []
     for i in range(len(d)):
         out = d.batch(i, with_pixel_ids=True)
@@ -91,7 +91,7 @@ def test_mixed_model_batches_equal_generate_rays():
     assert torch.equal(torch.cat(seen).sort().values.cpu(), torch.arange(n))
     _check(d.gather(torch.randint(0, n, (4096,), generator=torch.Generator().manual_seed(1)), with_pixel_ids=True),
            rows, images)
-    plan = [(1, 0), (3, 1), (2, 1), (1, 0), (5, 4)]  # train_rows_kernel, rule plan
+    plan = [(1, 0), (3, 1), (2, 1), (1, 0), (5, 4)]  # train_rows_kernel<TablePlan>
     for kw in ({}, {"replacement": True, "num_iters": 5}):
         d = hb.DeviceRayBatches(cams, images, batch_size=700, seed=5, subsample=plan, **kw)
         for i in range(len(d)):
