@@ -27,6 +27,8 @@ cudaError_t launch_render_bwd(const hr_config& cfg, const Derived& dv, const Ren
 cudaError_t launch_generate_rays(const hr_camera& cam, int c_in, long long first, long long n, float* out, cudaStream_t st);
 cudaError_t launch_generate_video_rays(const hr_camera* cams, const float* times, bool mixed, int c_in, int width,
                                        long long frame_px, long long first, long long n, float* out, cudaStream_t st);
+cudaError_t launch_image_metrics_u8(const float* pred, const uint8_t* gt, int32_t n, int32_t H, int32_t W, double* out,
+                                    double* partial, cudaStream_t st);
 }  // namespace hr
 
 static thread_local std::string g_err;
@@ -967,6 +969,23 @@ static bool finite_camera(const hr_camera& c) {
          std::isfinite(c.cam_idx) && std::isfinite(c.time);
 }
 
+// The records and times of a video or split: one size (frame 0's), finite fields and times, well-formed fisheye and two-plane
+// records.  *mixed: any record is not a pinhole, so the ray kernel's instantiation that branches on each record's model runs.
+static int check_frames(const char* fn, const hr_camera* cameras, const float* times, int32_t n_frames, bool* mixed) {
+  const int32_t W = cameras[0].width, H = cameras[0].height;
+  *mixed = false;
+  for (int32_t f = 0; f < n_frames; ++f) {
+    const hr_camera& c = cameras[f];
+    if (c.width != W || c.height != H) return hr_fail("%s: frame %d is %d x %d, frame 0 is %d x %d", fn, f, c.width, c.height, W, H);
+    if (!finite_camera(c)) return hr_fail("%s: camera record of frame %d is not finite", fn, f);
+    if (bad_fisheye(c)) return hr_fail("%s: fisheye coefficients k1 = %g, k2 = %g of frame %d are not finite", fn, c.k1, c.k2, f);
+    if (const char* why = bad_two_plane(c)) return hr_fail("%s: frame %d: %s", fn, f, why);
+    if (!std::isfinite(times[f])) return hr_fail("%s: time of frame %d is not finite", fn, f);
+    *mixed = *mixed || c.fisheye || c.two_plane;
+  }
+  return 0;
+}
+
 // Sub-batch i runs on stream i % 2 of the handle (forked from and joined back to the caller's stream by events) in slot
 // i % 2: its ray generation and sample net overlap the previous sub-batch's render kernel, where one stream would leave the
 // SMs idle between each sub-batch's render tail and the next one's ray generation.  Each stream runs its sub-batches in
@@ -979,18 +998,8 @@ int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* ti
   const int32_t W = cameras[0].width, H = cameras[0].height;
   const int64_t n = video_rays(n_frames, H, W);
   if (n < 0) return hr_fail("hr_render_video_to8b: %d frames of %d x %d pixels: bad size or output bytes overflow int64", n_frames, W, H);
-  bool mixed = false;  // any record not a pinhole: the ray kernel's instantiation that branches on each record's model
-  for (int32_t f = 0; f < n_frames; ++f) {
-    const hr_camera& c = cameras[f];
-    if (c.width != W || c.height != H)
-      return hr_fail("hr_render_video_to8b: frame %d is %d x %d, frame 0 is %d x %d", f, c.width, c.height, W, H);
-    if (!finite_camera(c)) return hr_fail("hr_render_video_to8b: camera record of frame %d is not finite", f);
-    if (bad_fisheye(c))
-      return hr_fail("hr_render_video_to8b: fisheye coefficients k1 = %g, k2 = %g of frame %d are not finite", c.k1, c.k2, f);
-    if (const char* why = bad_two_plane(c)) return hr_fail("hr_render_video_to8b: frame %d: %s", f, why);
-    if (!std::isfinite(times[f])) return hr_fail("hr_render_video_to8b: time of frame %d is not finite", f);
-    mixed = mixed || c.fisheye || c.two_plane;
-  }
+  bool mixed = false;
+  if (check_frames("hr_render_video_to8b", cameras, times, n_frames, &mixed)) return 1;
   const int64_t need = hr_video_workspace_bytes(h, n_frames, H, W);
   if (workspace_bytes < need) return hr_fail("hr_render_video_to8b: workspace too small (%lld < %lld)", (long long)workspace_bytes, (long long)need);
   if (((uintptr_t)workspace & 15) != 0) return hr_fail("hr_render_video_to8b: workspace must be 16-byte aligned");
@@ -1045,6 +1054,166 @@ int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* ti
       CK(cudaEventDestroy(ev));
     }
   }
+  return rc;
+}
+
+// ---- held-out splits: every view rendered into a ring of whole fp32 frames and scored against its uint8 ground truth
+// Frames of the ring: what two sub-batches cover and one more (so the sub-batch after next is the first that may wait for a
+// frame's scoring), at most the split; bounded by the sub-batch, whatever n_views.  -1 when the ring's bytes overflow.
+static int64_t score_ring_frames(int64_t sub, int64_t frame_px, int32_t n_views) {
+  int64_t r = (2 * sub + frame_px - 1) / frame_px + 1;
+  if (r > n_views) r = n_views;
+  if (r > 65535) r = 65535;  // frames per metrics launch
+  int64_t bytes;
+  if (__builtin_mul_overflow(r * frame_px, (int64_t)(3 * sizeof(float)), &bytes)) return -1;
+  return r;
+}
+
+// Workspace layout (each part 256-byte aligned): two record windows (ring frames records and times each), the fp32 ring
+// [R][H][W][3], two metrics partial buffers (one per stream, R frames each), then the video path's one or two slots.
+struct ScoreLayout {
+  int64_t sub, ring, win_cams, win_times, ring_off, partial_off, partial_bytes, slots_off, slot_bytes, total;
+  int n_slots;
+};
+
+static bool score_layout(const hr_handle* h, int32_t n_views, int32_t height, int32_t width, ScoreLayout* L) {
+  if (!h || height < 11 || width < 11) return false;
+  const int64_t n = video_rays(n_views, height, width);
+  if (n < 0) return false;
+  const int64_t frame_px = (int64_t)height * width;
+  L->sub = video_sub_rays(h, n);
+  L->ring = score_ring_frames(L->sub, frame_px, n_views);
+  if (L->ring < 1) return false;
+  L->n_slots = n > L->sub ? 2 : 1;
+  L->win_cams = align256(L->ring * (int64_t)sizeof(hr_camera));
+  L->win_times = align256(L->ring * (int64_t)sizeof(float));
+  L->ring_off = 2 * (L->win_cams + L->win_times);
+  L->partial_off = L->ring_off + align256(L->ring * frame_px * 3 * (int64_t)sizeof(float));
+  L->partial_bytes = align256(hr_image_metrics_workspace_bytes((int32_t)L->ring, height, width));
+  L->slots_off = L->partial_off + 2 * L->partial_bytes;
+  L->slot_bytes = video_slot_bytes(h, L->sub);
+  L->total = L->slots_off + L->n_slots * L->slot_bytes;
+  return true;
+}
+
+int64_t hr_score_views_workspace_bytes(const hr_handle* h, int32_t n_views, int32_t height, int32_t width) {
+  ScoreLayout L;
+  return score_layout(h, n_views, height, width, &L) ? L.total : -1;
+}
+
+// The split is one ray sequence walked in the video path's sub-batches on its two streams, each sub-batch also cut where it
+// would wrap the ring, so its pixels land in consecutive ring positions.  A sub-batch copies its frames' records and times
+// into its stream's window, generates their rays, renders them into the ring and, when it completes frames, scores them with
+// one metrics launch on its own stream.  Cross-stream order comes from events: a frame begun by the previous sub-batch (the
+// other stream) is scored after that sub-batch's render, and a ring frame is rendered again only after the launch that
+// scored its previous frame.  Each stream runs its sub-batches in order, so its slot, window and partials are reused safely.
+int hr_score_views(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views, const uint8_t* gt, double* out,
+                   void* workspace, int64_t workspace_bytes, void* stream) {
+  if (!h || !cameras || !times || !gt || !out || !workspace) return hr_fail("hr_score_views: null argument");
+  if (!h->uploaded) return hr_fail("hr_score_views: parameters not uploaded");
+  if (n_views < 1) return hr_fail("hr_score_views: n_views must be >= 1, got %d", n_views);
+  const int32_t W = cameras[0].width, H = cameras[0].height;
+  if (H < 11 || W < 11) return hr_fail("hr_score_views: height and width must be >= 11 (the SSIM window), got %d x %d", H, W);
+  ScoreLayout lay;
+  if (!score_layout(h, n_views, H, W, &lay))
+    return hr_fail("hr_score_views: %d views of %d x %d pixels: bad size or bytes overflow int64", n_views, W, H);
+  bool mixed = false;
+  if (check_frames("hr_score_views", cameras, times, n_views, &mixed)) return 1;
+  if (((uintptr_t)out & 7) != 0) return hr_fail("hr_score_views: out must be 8-byte aligned");
+  if (((uintptr_t)workspace & 15) != 0) return hr_fail("hr_score_views: workspace must be 16-byte aligned");
+  if (workspace_bytes < lay.total)
+    return hr_fail("hr_score_views: workspace too small (%lld < %lld)", (long long)workspace_bytes, (long long)lay.total);
+  DeviceGuard guard(h->device);
+  const hr_config& c = h->cfg;
+  cudaStream_t st = (cudaStream_t)stream;
+  char* base = (char*)workspace;
+  float* ring = (float*)(base + lay.ring_off);
+  const int64_t frame_px = (int64_t)W * H, n = frame_px * n_views, ring_rays = lay.ring * frame_px;
+  const int64_t rays_bytes = align256(lay.sub * c.c_in * (int64_t)sizeof(float));
+  cudaStream_t ss[2] = {st, st};
+  std::vector<cudaEvent_t> evs;  // every event of the call, destroyed at the end (a destroyed event's pending work still runs)
+  auto new_event = [&](cudaEvent_t* ev) -> int {
+    CK(cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
+    evs.push_back(*ev);
+    return 0;
+  };
+  // scored[k]: recorded after the metrics launch that read ring frame k last; done[s]: after stream s's last render
+  std::vector<cudaEvent_t> scored(lay.n_slots == 2 ? lay.ring : 0, nullptr);
+  cudaEvent_t done[2] = {nullptr, nullptr};
+  int rc = 0;
+  if (lay.n_slots == 2) {
+    cudaEvent_t fork;
+    for (int i = 0; i < 2; ++i) {
+      if (pipe_stream(h, i)) return 1;
+      ss[i] = h->pipe.streams[i];
+    }
+    if (new_event(&fork)) return 1;
+    CK(cudaEventRecord(fork, st));
+    CK(cudaStreamWaitEvent(ss[0], fork, 0));
+    CK(cudaStreamWaitEvent(ss[1], fork, 0));
+    for (auto& e : scored)
+      if ((rc = new_event(&e))) break;
+    for (int i = 0; i < 2 && !rc; ++i) rc = new_event(&done[i]);
+  }
+  int64_t next = 0;  // first frame not yet scored
+  int64_t i = 0;
+  for (int64_t off = 0; off < n && !rc; ++i) {
+    const int k = (int)(i % 2);
+    cudaStream_t s = ss[k];
+    const int64_t pos = off % ring_rays;
+    int64_t m = n - off < lay.sub ? n - off : lay.sub;
+    if (pos + m > ring_rays) m = ring_rays - pos;
+    const int64_t f0 = off / frame_px, f1 = (off + m - 1) / frame_px, f_end = (off + m) / frame_px;
+    auto fail = [&](const char* what, cudaError_t e) { return hr_fail("hr_score_views: %s: %s", what, cudaGetErrorString(e)); };
+    cudaError_t e = cudaSuccess;
+    if (lay.n_slots == 2)  // ring frames rendered again: after the scoring of the frames they held
+      for (int64_t f = f0 < lay.ring ? lay.ring : f0; f <= f1 && e == cudaSuccess; ++f)
+        e = cudaStreamWaitEvent(s, scored[f % lay.ring], 0);
+    hr_camera* win_c = (hr_camera*)(base + k * (lay.win_cams + lay.win_times));
+    float* win_t = (float*)((char*)win_c + lay.win_cams);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(win_c, cameras + f0, (size_t)(f1 - f0 + 1) * sizeof(hr_camera), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(win_t, times + f0, (size_t)(f1 - f0 + 1) * sizeof(float), cudaMemcpyHostToDevice, s);
+    if (e != cudaSuccess) {
+      rc = fail("record copy", e);
+      break;
+    }
+    char* slot = base + lay.slots_off + (i % lay.n_slots) * lay.slot_bytes;
+    e = hr::launch_generate_video_rays(win_c, win_t, mixed, c.c_in, W, frame_px, off - f0 * frame_px, m, (float*)slot, s);
+    if (e != cudaSuccess) {
+      rc = fail("ray generation", e);
+      break;
+    }
+    h->launches += 1;
+    rc = render_impl(h, (const float*)slot, m, ring + pos * 3, nullptr, nullptr, slot + rays_bytes, lay.slot_bytes - rays_bytes, s);
+    if (rc) break;
+    if (f_end > next) {  // frames next .. f_end - 1 are complete, in consecutive ring frames
+      if (lay.n_slots == 2 && next * frame_px < off) e = cudaStreamWaitEvent(s, done[1 - k], 0);
+      if (e == cudaSuccess)
+        e = hr::launch_image_metrics_u8(ring + (next % lay.ring) * frame_px * 3, gt + next * frame_px * 3, (int32_t)(f_end - next),
+                                        H, W, out + 2 * next, (double*)(base + lay.partial_off + k * lay.partial_bytes), s);
+      for (int64_t f = next; f < f_end && e == cudaSuccess && lay.n_slots == 2; ++f) e = cudaEventRecord(scored[f % lay.ring], s);
+      if (e != cudaSuccess) {
+        rc = fail("metrics launch", e);
+        break;
+      }
+      h->launches += 2;
+      next = f_end;
+    }
+    if (lay.n_slots == 2 && (e = cudaEventRecord(done[k], s)) != cudaSuccess) {
+      rc = fail("event record", e);
+      break;
+    }
+    off += m;
+  }
+  if (lay.n_slots == 2) {  // join, also after a failed launch: the caller's stream must not run ahead of enqueued work
+    for (int k = 0; k < 2; ++k) {
+      cudaEvent_t ev;
+      if (new_event(&ev)) break;
+      CK(cudaEventRecord(ev, ss[k]));
+      CK(cudaStreamWaitEvent(st, ev, 0));
+    }
+  }
+  for (cudaEvent_t ev : evs) cudaEventDestroy(ev);
   return rc;
 }
 

@@ -1,4 +1,5 @@
-// Held-out view scoring: per-image MSE and SSIM of [n, H, W, 3] fp32 image pairs on the device.
+// Held-out view scoring: per-image MSE and SSIM of [n, H, W, 3] image pairs on the device, the prediction fp32 and the
+// ground truth fp32 or uint8.
 // Reference: metrics.psnr / metrics.ssim (metrics.py:25-34), i.e. scikit-image's peak_signal_noise_ratio(data_range=1) and
 // structural_similarity(win_size=11, multichannel, gaussian_weights, data_range=1), called by INRSystem.validation_image
 // (nlf/__init__.py:976-980) on the host copy of every held-out frame.
@@ -10,7 +11,12 @@
 // same CTA sums the squared error of its own tile (border pixels included).  Per-tile partials go to the workspace and a
 // second kernel sums each image's partials in a fixed order: no float atomics, so results are bit-reproducible and do not
 // depend on the batch an image is scored in.
+//
+// uint8 ground truth (hr_score_views) is converted while the tile is staged, as u8 / 255 correctly rounded: what
+// T.ToTensor() (a CPU division) gives the reference, and what the training batches use.  Everything after staging is shared,
+// so a uint8 frame scores bit for bit like that fp32 conversion of it.
 #include <cmath>
+#include <cstdint>
 
 #include "hr_handle.h"
 
@@ -59,8 +65,12 @@ __device__ __forceinline__ void block_sum2(double& a, double& b, double (*red)[M
   }
 }
 
+__device__ __forceinline__ float load_gt(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float load_gt(const uint8_t* p) { return __fdiv_rn((float)__ldg(p), 255.0f); }
+
+template <typename GtT>
 __global__ void __launch_bounds__(MTHREADS, 2)
-image_metrics_tile_kernel(const float* __restrict__ pred, const float* __restrict__ gt, int H, int W,
+image_metrics_tile_kernel(const float* __restrict__ pred, const GtT* __restrict__ gt, int H, int W,
                           const __grid_constant__ GaussTaps g, double* __restrict__ partial) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   MetricsSmem& s = *reinterpret_cast<MetricsSmem*>(smem_raw);
@@ -83,7 +93,7 @@ image_metrics_tile_kernel(const float* __restrict__ pred, const float* __restric
     if (e < N_STAGE && r >= 0 && r < H && c >= 0 && c < W) {
       const size_t i = base + ((size_t)r * W + c) * 3 + ch;
       xs[it] = __ldg(pred + i);
-      ys[it] = __ldg(gt + i);
+      ys[it] = load_gt(gt + i);
     }
   }
   double sse = 0.0;
@@ -210,7 +220,43 @@ int64_t metrics_tiles(int32_t h, int32_t w) {
   return (int64_t)((h + MT_H - 1) / MT_H) * ((w + MT_W - 1) / MT_W);
 }
 
+// SciPy's _gaussian_kernel1d(sigma=1.5, order=0, radius=5): exp(-0.5 / sigma^2 * x^2), normalised by NumPy's sum of the 11
+// values (pairwise: eight partial sums combined as a tree, then the last three added in order)
+GaussTaps gauss_taps() {
+  GaussTaps g;
+  const double sigma2 = 1.5 * 1.5;
+  for (int t = 0; t < MTAPS; ++t) g.w[t] = std::exp(-0.5 / sigma2 * (double)((t - MR) * (t - MR)));
+  double sum = ((g.w[0] + g.w[1]) + (g.w[2] + g.w[3])) + ((g.w[4] + g.w[5]) + (g.w[6] + g.w[7]));
+  for (int t = 8; t < MTAPS; ++t) sum += g.w[t];
+  for (int t = 0; t < MTAPS; ++t) g.w[t] /= sum;
+  return g;
+}
+
+// The tile kernel and the per-image reduction of n images on `st`; `partial` holds hr_image_metrics_workspace_bytes(n, H, W).
+template <typename GtT>
+cudaError_t launch_metrics(const float* pred, const GtT* gt, int32_t n, int32_t H, int32_t W, double* out, double* partial,
+                           cudaStream_t st) {
+  const cudaError_t e = cudaFuncSetAttribute(image_metrics_tile_kernel<GtT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)sizeof(MetricsSmem));
+  if (e != cudaSuccess) return e;
+  const dim3 grid((W + MT_W - 1) / MT_W, (H + MT_H - 1) / MT_H, n);
+  image_metrics_tile_kernel<GtT><<<grid, MTHREADS, sizeof(MetricsSmem), st>>>(pred, gt, H, W, gauss_taps(), partial);
+  image_metrics_reduce_kernel<<<n, MTHREADS, 0, st>>>(partial, (int)metrics_tiles(H, W), 3.0 * H * W,
+                                                      3.0 * (H - 2 * MR) * (W - 2 * MR), out);
+  return cudaGetLastError();
+}
+
 }  // namespace
+
+namespace hr {
+
+// hr_score_views' scoring of whole frames of its fp32 ring against their uint8 ground truth (arguments checked by the caller)
+cudaError_t launch_image_metrics_u8(const float* pred, const uint8_t* gt, int32_t n, int32_t H, int32_t W, double* out,
+                                    double* partial, cudaStream_t st) {
+  return launch_metrics(pred, gt, n, H, W, out, partial, st);
+}
+
+}  // namespace hr
 
 extern "C" {
 
@@ -231,26 +277,7 @@ int hr_image_metrics(const float* pred, const float* gt, int32_t n_images, int32
   if (workspace_bytes < need)
     return hr_fail("hr_image_metrics: workspace of %lld bytes, %lld needed", (long long)workspace_bytes, (long long)need);
 
-  // SciPy's _gaussian_kernel1d(sigma=1.5, order=0, radius=5): exp(-0.5 / sigma^2 * x^2), normalised by NumPy's sum of the 11
-  // values (pairwise: eight partial sums combined as a tree, then the last three added in order)
-  GaussTaps g;
-  const double sigma2 = 1.5 * 1.5;
-  for (int t = 0; t < MTAPS; ++t) g.w[t] = std::exp(-0.5 / sigma2 * (double)((t - MR) * (t - MR)));
-  double sum = ((g.w[0] + g.w[1]) + (g.w[2] + g.w[3])) + ((g.w[4] + g.w[5]) + (g.w[6] + g.w[7]));
-  for (int t = 8; t < MTAPS; ++t) sum += g.w[t];
-  for (int t = 0; t < MTAPS; ++t) g.w[t] /= sum;
-
-  cudaStream_t st = (cudaStream_t)stream;
-  cudaError_t e = cudaFuncSetAttribute(image_metrics_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)sizeof(MetricsSmem));
-  if (e != cudaSuccess) return hr_fail("hr_image_metrics: %s", cudaGetErrorString(e));
-  const dim3 grid((width + MT_W - 1) / MT_W, (height + MT_H - 1) / MT_H, n_images);
-  double* partial = (double*)workspace;
-  image_metrics_tile_kernel<<<grid, MTHREADS, sizeof(MetricsSmem), st>>>(pred, gt, height, width, g, partial);
-  image_metrics_reduce_kernel<<<n_images, MTHREADS, 0, st>>>(partial, (int)metrics_tiles(height, width),
-                                                             3.0 * height * width, 3.0 * (height - 2 * MR) * (width - 2 * MR),
-                                                             out);
-  e = cudaGetLastError();
+  const cudaError_t e = launch_metrics(pred, gt, n_images, height, width, out, (double*)workspace, (cudaStream_t)stream);
   if (e != cudaSuccess) return hr_fail("hr_image_metrics: %s", cudaGetErrorString(e));
   return 0;
 }

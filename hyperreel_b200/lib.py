@@ -11,7 +11,7 @@ import os
 import subprocess
 import threading
 
-HR_ABI_VERSION = 20
+HR_ABI_VERSION = 21
 HR_MAX_GROUPS = 4
 HR_MAX_LAYERS = 10
 HR_MAX_SAMPLES = 256
@@ -173,6 +173,9 @@ EXPORTS = {
     "hr_video_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]),
     "hr_render_video_to8b": (C.c_int, [C.c_void_p, C.POINTER(hr_camera), C.POINTER(C.c_float), C.c_int32, C.c_void_p, C.c_void_p,
                                         C.c_int64, C.c_void_p]),
+    "hr_score_views_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]),
+    "hr_score_views": (C.c_int, [C.c_void_p, C.POINTER(hr_camera), C.POINTER(C.c_float), C.c_int32, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_int64, C.c_void_p]),
     "hr_encode_rays": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "hr_render_heads": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.POINTER(hr_train_opts), C.c_void_p,
                                    C.c_int64, C.c_void_p]),

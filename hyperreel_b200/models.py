@@ -539,6 +539,59 @@ class LightfieldModel(nn.Module):
                                                    stream.cuda_stream))
         return out
 
+    def score_views(self, cameras, images: torch.Tensor, times=None, out: Optional[torch.Tensor] = None, stream=None):
+        """(mse, ssim) of every held-out view, fp64 [n] device tensors: view i rendered from ``cameras[i]`` at ``times[i]``
+        (default each camera's ``time``) in one call that never synchronises (hr_score_views), scored against ``images[i]``
+        (uint8 [n, H, W, 3] on the device, contiguous) like ``metrics.image_metrics(pred, images[i] / 255)`` (correctly rounded, as T.ToTensor() converts) of the
+        view's eval render, bit for bit.  ``out`` (device fp64 [n, 2], contiguous) receives (mse, ssim) when given; the work
+        goes on ``stream`` (a torch.cuda.Stream; default the current stream)."""
+        if self.training:
+            raise RuntimeError("hyperreel_b200.LightfieldModel implements the eval()/render path only; call .eval()")
+        cams = list(cameras)
+        if not cams:
+            raise ValueError("score_views: no cameras")
+        t = [float(c.time) for c in cams] if times is None else times
+        t = torch.as_tensor(t, dtype=torch.float64).reshape(-1).to(torch.float32)
+        if t.numel() != len(cams):
+            raise ValueError(f"score_views: {len(cams)} cameras but {t.numel()} times")
+        if not bool(torch.isfinite(t).all()):
+            raise ValueError("score_views: times must be finite in float32")
+        H, W = int(cams[0].height), int(cams[0].width)
+        for i, c in enumerate(cams):
+            if (int(c.height), int(c.width)) != (H, W):
+                raise ValueError(f"score_views: camera {i} is {int(c.width)} x {int(c.height)}, camera 0 is {W} x {H}")
+        if H < 11 or W < 11:
+            raise ValueError(f"score_views: views must be at least 11 x 11 (the SSIM window), got {W} x {H}")
+        shape = (len(cams), H, W, 3)
+        if not isinstance(images, torch.Tensor) or images.dtype != torch.uint8 or tuple(images.shape) != shape \
+                or not images.is_contiguous():
+            got = f"{images.dtype} {tuple(images.shape)}" if isinstance(images, torch.Tensor) else type(images).__name__
+            raise ValueError(f"score_views: images must be a contiguous uint8 tensor of shape {shape}, got {got}")
+        if not images.is_cuda:
+            raise RuntimeError("hyperreel_b200 scores views on an H100 only: images must be a CUDA tensor (no CPU fallback)")
+        dev = images.device
+        p = next(self.parameters(), None)
+        if p is not None and p.is_cuda and p.device != dev:
+            raise ValueError(f"score_views: images are on {dev}, the model on {p.device}")
+        if out is not None and (not out.is_cuda or out.dtype != torch.float64 or tuple(out.shape) != (len(cams), 2)
+                                or not out.is_contiguous() or out.device != dev):
+            raise ValueError(f"score_views: out must be a contiguous float64 tensor of shape {(len(cams), 2)} on {dev}, got "
+                             f"{out.dtype} {tuple(out.shape)} on {out.device}")
+        self._ensure_uploaded(dev)
+        need = int(self._lib.hr_score_views_workspace_bytes(self._handle, len(cams), H, W))
+        if need < 0:
+            raise ValueError(f"score_views: {len(cams)} views of {W} x {H} pixels overflow a 64-bit size")
+        stream = stream if stream is not None else torch.cuda.current_stream(dev)
+        recs = (L.hr_camera * len(cams))(*[c.to_c() for c in cams])
+        tt = (C.c_float * len(cams))(*t.tolist())
+        with torch.cuda.stream(stream):  # the scratch (and a new out) belong to the stream the work runs on
+            ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            if out is None:
+                out = torch.empty((len(cams), 2), dtype=torch.float64, device=dev)
+            L.check(self._lib.hr_score_views(self._handle, recs, tt, len(cams), images.data_ptr(), out.data_ptr(), ws.data_ptr(),
+                                             need, stream.cuda_stream))
+        return out[:, 0], out[:, 1]
+
     def timing(self, enable: bool = True):
         L.check(self._lib.hr_timing_enable(self._handle, int(enable)))
         L.check(self._lib.hr_timing_reset(self._handle))

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define HR_ABI_VERSION 20
+#define HR_ABI_VERSION 21
 
 #define HR_MAX_GROUPS 4   /* ray-parameterisation groups feeding the sample net (ray.py:235-263) */
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
@@ -483,6 +483,27 @@ int hr_render_frame_to8b_host(hr_handle* h, const hr_camera* cam, uint8_t* rgb8_
 int64_t hr_video_workspace_bytes(const hr_handle* h, int32_t n_frames, int32_t height, int32_t width);
 int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_frames, uint8_t* video,
                          void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ---- held-out splits scored on the device (ABI 21) ----
+ * Replaces: the reference's evaluation of a validation / test split (nlf/__init__.py:249-265, :895-982, :1015-1030): per
+ * view, rays built on the CPU, the view rendered, copied to the host and scored with scikit-image.  cameras / times: HOST
+ * arrays of n_views records (one width x height, >= 11 x 11, pinhole, fisheye and two-plane mixed freely) and fp32 times, as
+ * hr_render_video_to8b takes them.  gt: DEVICE uint8 [n_views, height, width, 3], the views' ground truth.  out: DEVICE fp64
+ * [n_views][2] = (mse, ssim) of each view, bit for bit hr_image_metrics of the fp32 frame hr_render makes of the view's rays
+ * (clamped output, the configured background, no to8b) against gt / 255 correctly rounded in fp32 (T.ToTensor()'s conversion; NumPy's, and torch's on the CPU).
+ * workspace: device scratch of hr_score_views_workspace_bytes(h, n_views, height, width) bytes (16B aligned, -1 for a size
+ * hr_score_views refuses), bounded whatever n_views: two windows of ring-many records and times, a ring of whole fp32
+ * frames (enough for two sub-batches and one frame more), two metrics partial buffers and the video path's one or two
+ * slots.  The split is one ray sequence rendered in hr_render_video_to8b's sub-batches on its two streams (forked from and
+ * joined back to `stream` by events), a sub-batch also cut where it would wrap the ring; a sub-batch that completes frames
+ * scores them with one metrics launch on its own stream, after an event of the other stream for a frame that straddles
+ * the two, and a ring frame is reused only after the launch that scored it.  No host synchronisation, no float atomics:
+ * two calls write the same bits.  Refused before anything is enqueued (out untouched): null or misaligned pointers
+ * (out 8B, workspace 16B), n_views < 1, views of different sizes or smaller than 11 x 11, a size whose bytes overflow int64,
+ * a non-finite record field, time or fisheye coefficient, a malformed two-plane record, a workspace too small. */
+int64_t hr_score_views_workspace_bytes(const hr_handle* h, int32_t n_views, int32_t height, int32_t width);
+int hr_score_views(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views, const uint8_t* gt, double* out,
+                   void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- backward pass of the path (SURVEY.md section 8 row f1) ----
  * Replaces: what loss.backward() runs for the render path inside INRSystem.training_step (nlf/__init__.py:634-709): the
