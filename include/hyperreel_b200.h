@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define HR_ABI_VERSION 21
+#define HR_ABI_VERSION 22
 
 #define HR_MAX_GROUPS 4   /* ray-parameterisation groups feeding the sample net (ray.py:235-263) */
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
@@ -593,6 +593,35 @@ int hr_set_activations(hr_handle* h, const hr_config* cfg);
 int64_t hr_image_metrics_workspace_bytes(int32_t n_images, int32_t height, int32_t width);
 int hr_image_metrics(const float* pred, const float* gt, int32_t n_images, int32_t height, int32_t width, double* out,
                      void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ---- frame resize to the training resolution (handle-free) ----
+ * Replaces: the resize in the datasets' get_rgb, run on the host per image: Pillow's Image.resize (datasets/technicolor.py,
+ * llff.py, spaces.py, stanford.py: LANCZOS to _img_wh, then BOX to img_wh) and cv2.resize (datasets/neural_3d.py,
+ * immersive.py: the flag they pass sits in the dst slot, so both of their steps are OpenCV's default INTER_LINEAR).
+ * src: DEVICE uint8 [n, H0, W0, 3] contiguous.  dst: DEVICE uint8, frame f's row y at dst + (f * H + y) * dst_row_stride
+ * (dst_row_stride >= 3 * W bytes), so a slice of a larger [N, H, W, 3] tensor can be written in place.  method: one of
+ * HR_RESIZE_*; bit for bit the library's result on each frame (Pillow 12's 8-bit convolution resampler with its filter;
+ * OpenCV 4's CV_8UC3 INTER_LINEAR, or INTER_AREA for integer factors, with INTER_LINEAR sent to INTER_AREA at exactly 2x).
+ * A frame of the same size is copied, as both libraries do.  flags: HR_RESIZE_BGR reads src as BGR (channels 0 and 2
+ * swapped), which is what OpenCV decodes; dst is RGB.  workspace: device, 256-byte aligned, at least
+ * hr_resize_workspace_bytes(n, H0, W0, H, W, method) bytes (-1 for sizes or a method hr_resize_frames refuses; 0 for the
+ * copy and the INTER_AREA paths): the coefficient tables, copied in with the launch, and for the two Pillow passes the uint8
+ * intermediate of the rows the vertical pass reads.  Kernels use integer multiply-adds only (INTER_AREA at factors other
+ * than 2 x 2 rounds sum * (1.f / area) in fp32, as OpenCV does), no float atomics and no host synchronisation: two calls
+ * write the same bits.  Refused before anything is enqueued (dst untouched): null pointers, unknown method or flags, sizes
+ * < 1, an enlargement in either direction, cv2_area at a non-integer factor, a Pillow reduction needing more filter
+ * coefficients than Pillow allows (outSize > INT_MAX / (ksize * 8), where Pillow raises MemoryError), source, destination
+ * or workspace bytes that overflow int64, a short dst_row_stride, a missing, misaligned or short workspace. */
+#define HR_RESIZE_PIL_LANCZOS 0
+#define HR_RESIZE_PIL_BICUBIC 1
+#define HR_RESIZE_PIL_BOX 2
+#define HR_RESIZE_CV2_LINEAR 3
+#define HR_RESIZE_CV2_AREA 4
+#define HR_RESIZE_BGR 1
+int64_t hr_resize_workspace_bytes(int32_t n, int32_t H0, int32_t W0, int32_t H, int32_t W, int32_t method);
+int hr_resize_frames(const uint8_t* src, int32_t n, int32_t H0, int32_t W0, uint8_t* dst, int32_t H, int32_t W,
+                     int64_t dst_row_stride, int32_t method, int32_t flags, void* workspace, int64_t workspace_bytes,
+                     void* stream);
 
 /* Number of kernels hr_render launched since creation (bench.py's gpu_launches). */
 int64_t hr_launch_count(const hr_handle* h);
