@@ -289,16 +289,18 @@ def render_video(model_or_system, cameras: Sequence[Camera], times=None, out: Op
 
 
 def score_views(model_or_system, cameras: Sequence[Camera], images: torch.Tensor, times=None, out: Optional[torch.Tensor] = None,
-                stream=None):
+                stream=None, *, rgba: bool = False):
     """(mse, ssim), fp64 [n] device tensors, of a held-out split: view i of a LightfieldModel, RenderLightfield or INRSystem
     rendered from ``cameras[i]`` (one size, Camera or TwoPlaneCamera, models mixed freely) at ``times[i]`` (default each
     camera's ``time``) and scored against ``images[i]`` (uint8 [n, H, W, 3], contiguous, on the model's device) -- the
     reference's evaluation of a split (nlf/__init__.py:895-982) as one call that never synchronises (hr_score_views).  Each
-    pair equals ``metrics.image_metrics`` of the view's eval render against ``images[i] / 255`` correctly rounded in fp32 (T.ToTensor()'s conversion), bit for bit."""
+    pair equals ``metrics.image_metrics`` of the view's eval render against ``images[i] / 255`` correctly rounded in fp32 (T.ToTensor()'s conversion), bit for bit.
+    ``rgba=True``: ``images`` are uint8 RGBA [n, H, W, 4] (the DoNeRF and Catacaustics frames) and each view is scored
+    against its composite over white, ``rgb * a + (1 - a)`` as their ``get_rgb`` computes it, bit for bit."""
     target = model_or_system if hasattr(model_or_system, "score_views") else getattr(model_or_system, "model", None)
     if target is None or not hasattr(target, "score_views"):
         raise TypeError(f"score_views: expected a LightfieldModel, RenderLightfield or INRSystem, got {type(model_or_system)}")
-    return target.score_views(cameras, images, times, out=out, stream=stream)
+    return target.score_views(cameras, images, times, out=out, stream=stream, rgba=rgba)
 
 
 def generate_rays(camera: Camera, c_in: int = 8, device: Optional[torch.device] = None, first_pixel: int = 0,

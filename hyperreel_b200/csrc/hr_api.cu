@@ -29,6 +29,8 @@ cudaError_t launch_generate_video_rays(const hr_camera* cams, const float* times
                                        long long frame_px, long long first, long long n, float* out, cudaStream_t st);
 cudaError_t launch_image_metrics_u8(const float* pred, const uint8_t* gt, int32_t n, int32_t H, int32_t W, double* out,
                                     double* partial, cudaStream_t st);
+cudaError_t launch_image_metrics_rgba8(const float* pred, const uint8_t* gt, int32_t n, int32_t H, int32_t W, double* out,
+                                       double* partial, cudaStream_t st);
 }  // namespace hr
 
 static thread_local std::string g_err;
@@ -1107,22 +1109,28 @@ int64_t hr_score_views_workspace_bytes(const hr_handle* h, int32_t n_views, int3
 // one metrics launch on its own stream.  Cross-stream order comes from events: a frame begun by the previous sub-batch (the
 // other stream) is scored after that sub-batch's render, and a ring frame is rendered again only after the launch that
 // scored its previous frame.  Each stream runs its sub-batches in order, so its slot, window and partials are reused safely.
-int hr_score_views(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views, const uint8_t* gt, double* out,
-                   void* workspace, int64_t workspace_bytes, void* stream) {
-  if (!h || !cameras || !times || !gt || !out || !workspace) return hr_fail("hr_score_views: null argument");
-  if (!h->uploaded) return hr_fail("hr_score_views: parameters not uploaded");
-  if (n_views < 1) return hr_fail("hr_score_views: n_views must be >= 1, got %d", n_views);
+// gt of pixel_format (HR_PIXEL_*); fn names the entry point in refusals
+static int score_views(const char* fn, hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views,
+                       const uint8_t* gt, int32_t pixel_format, double* out, void* workspace, int64_t workspace_bytes,
+                       void* stream) {
+  if (!h || !cameras || !times || !gt || !out || !workspace) return hr_fail("%s: null argument", fn);
+  if (!h->uploaded) return hr_fail("%s: parameters not uploaded", fn);
+  if (n_views < 1) return hr_fail("%s: n_views must be >= 1, got %d", fn, n_views);
   const int32_t W = cameras[0].width, H = cameras[0].height;
-  if (H < 11 || W < 11) return hr_fail("hr_score_views: height and width must be >= 11 (the SSIM window), got %d x %d", H, W);
+  if (H < 11 || W < 11) return hr_fail("%s: height and width must be >= 11 (the SSIM window), got %d x %d", fn, H, W);
   ScoreLayout lay;
   if (!score_layout(h, n_views, H, W, &lay))
-    return hr_fail("hr_score_views: %d views of %d x %d pixels: bad size or bytes overflow int64", n_views, W, H);
+    return hr_fail("%s: %d views of %d x %d pixels: bad size or bytes overflow int64", fn, n_views, W, H);
   bool mixed = false;
-  if (check_frames("hr_score_views", cameras, times, n_views, &mixed)) return 1;
-  if (((uintptr_t)out & 7) != 0) return hr_fail("hr_score_views: out must be 8-byte aligned");
-  if (((uintptr_t)workspace & 15) != 0) return hr_fail("hr_score_views: workspace must be 16-byte aligned");
+  if (check_frames(fn, cameras, times, n_views, &mixed)) return 1;
+  if (((uintptr_t)out & 7) != 0) return hr_fail("%s: out must be 8-byte aligned", fn);
+  if (((uintptr_t)workspace & 15) != 0) return hr_fail("%s: workspace must be 16-byte aligned", fn);
+  if (pixel_format != HR_PIXEL_RGB8 && pixel_format != HR_PIXEL_RGBA8)
+    return hr_fail("%s: unknown pixel format %d", fn, pixel_format);
+  const int gt_px = pixel_format == HR_PIXEL_RGBA8 ? 4 : 3;  // bytes per ground-truth pixel
+  if (gt_px == 4 && ((uintptr_t)gt & 3) != 0) return hr_fail("%s: RGBA gt must be 4-byte aligned", fn);
   if (workspace_bytes < lay.total)
-    return hr_fail("hr_score_views: workspace too small (%lld < %lld)", (long long)workspace_bytes, (long long)lay.total);
+    return hr_fail("%s: workspace too small (%lld < %lld)", fn, (long long)workspace_bytes, (long long)lay.total);
   DeviceGuard guard(h->device);
   const hr_config& c = h->cfg;
   cudaStream_t st = (cudaStream_t)stream;
@@ -1164,7 +1172,7 @@ int hr_score_views(hr_handle* h, const hr_camera* cameras, const float* times, i
     int64_t m = n - off < lay.sub ? n - off : lay.sub;
     if (pos + m > ring_rays) m = ring_rays - pos;
     const int64_t f0 = off / frame_px, f1 = (off + m - 1) / frame_px, f_end = (off + m) / frame_px;
-    auto fail = [&](const char* what, cudaError_t e) { return hr_fail("hr_score_views: %s: %s", what, cudaGetErrorString(e)); };
+    auto fail = [&](const char* what, cudaError_t e) { return hr_fail("%s: %s: %s", fn, what, cudaGetErrorString(e)); };
     cudaError_t e = cudaSuccess;
     if (lay.n_slots == 2)  // ring frames rendered again: after the scoring of the frames they held
       for (int64_t f = f0 < lay.ring ? lay.ring : f0; f <= f1 && e == cudaSuccess; ++f)
@@ -1189,8 +1197,9 @@ int hr_score_views(hr_handle* h, const hr_camera* cameras, const float* times, i
     if (f_end > next) {  // frames next .. f_end - 1 are complete, in consecutive ring frames
       if (lay.n_slots == 2 && next * frame_px < off) e = cudaStreamWaitEvent(s, done[1 - k], 0);
       if (e == cudaSuccess)
-        e = hr::launch_image_metrics_u8(ring + (next % lay.ring) * frame_px * 3, gt + next * frame_px * 3, (int32_t)(f_end - next),
-                                        H, W, out + 2 * next, (double*)(base + lay.partial_off + k * lay.partial_bytes), s);
+        e = (gt_px == 4 ? hr::launch_image_metrics_rgba8 : hr::launch_image_metrics_u8)(
+            ring + (next % lay.ring) * frame_px * 3, gt + next * frame_px * gt_px, (int32_t)(f_end - next), H, W, out + 2 * next,
+            (double*)(base + lay.partial_off + k * lay.partial_bytes), s);
       for (int64_t f = next; f < f_end && e == cudaSuccess && lay.n_slots == 2; ++f) e = cudaEventRecord(scored[f % lay.ring], s);
       if (e != cudaSuccess) {
         rc = fail("metrics launch", e);
@@ -1215,6 +1224,17 @@ int hr_score_views(hr_handle* h, const hr_camera* cameras, const float* times, i
   }
   for (cudaEvent_t ev : evs) cudaEventDestroy(ev);
   return rc;
+}
+
+int hr_score_views(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views, const uint8_t* gt, double* out,
+                   void* workspace, int64_t workspace_bytes, void* stream) {
+  return score_views("hr_score_views", h, cameras, times, n_views, gt, HR_PIXEL_RGB8, out, workspace, workspace_bytes, stream);
+}
+
+int hr_score_views_fmt(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views, const uint8_t* gt,
+                       int32_t pixel_format, double* out, void* workspace, int64_t workspace_bytes, void* stream) {
+  return score_views("hr_score_views_fmt", h, cameras, times, n_views, gt, pixel_format, out, workspace, workspace_bytes,
+                     stream);
 }
 
 // the device's view of a pinned (device-addressable) host buffer, or null

@@ -13,10 +13,13 @@
 // depend on the batch an image is scored in.
 //
 // uint8 ground truth (hr_score_views) is converted while the tile is staged, as u8 / 255 correctly rounded: what
-// T.ToTensor() (a CPU division) gives the reference, and what the training batches use.  Everything after staging is shared,
-// so a uint8 frame scores bit for bit like that fp32 conversion of it.
+// T.ToTensor() (a CPU division) gives the reference, and what the training batches use.  RGBA ground truth (the DoNeRF and
+// Catacaustics datasets) is composited over white while it is staged, rgb * a + (1 - a) of those values with each operation
+// rounded on its own (no FMA), as their get_rgb computes it with torch on the CPU.  Everything after staging is shared, so a
+// uint8 frame scores bit for bit like that fp32 conversion (or composite) of it.
 #include <cmath>
 #include <cstdint>
+#include <type_traits>
 
 #include "hr_handle.h"
 
@@ -68,6 +71,19 @@ __device__ __forceinline__ void block_sum2(double& a, double& b, double (*red)[M
 __device__ __forceinline__ float load_gt(const float* p) { return __ldg(p); }
 __device__ __forceinline__ float load_gt(const uint8_t* p) { return __fdiv_rn((float)__ldg(p), 255.0f); }
 
+// One RGBA uint8 pixel, loaded whole
+struct __align__(4) Rgba8 {
+  uint8_t v[4];
+};
+
+// Channel ch of an RGBA pixel composited over white, as get_rgb: c * a + (1 - a), c and a u8 / 255
+__device__ __forceinline__ float load_gt(const Rgba8* p, int ch) {
+  const uint32_t q = __ldg(reinterpret_cast<const unsigned int*>(p));
+  const float a = __fdiv_rn((float)(q >> 24), 255.0f);
+  const float c = __fdiv_rn((float)((q >> (8 * ch)) & 0xffu), 255.0f);
+  return __fadd_rn(__fmul_rn(c, a), __fsub_rn(1.0f, a));
+}
+
 template <typename GtT>
 __global__ void __launch_bounds__(MTHREADS, 2)
 image_metrics_tile_kernel(const float* __restrict__ pred, const GtT* __restrict__ gt, int H, int W,
@@ -93,7 +109,10 @@ image_metrics_tile_kernel(const float* __restrict__ pred, const GtT* __restrict_
     if (e < N_STAGE && r >= 0 && r < H && c >= 0 && c < W) {
       const size_t i = base + ((size_t)r * W + c) * 3 + ch;
       xs[it] = __ldg(pred + i);
-      ys[it] = load_gt(gt + i);
+      if constexpr (std::is_same<GtT, Rgba8>::value)
+        ys[it] = load_gt(gt + (size_t)blockIdx.z * H * W + (size_t)r * W + c, ch);
+      else
+        ys[it] = load_gt(gt + i);
     }
   }
   double sse = 0.0;
@@ -254,6 +273,12 @@ namespace hr {
 cudaError_t launch_image_metrics_u8(const float* pred, const uint8_t* gt, int32_t n, int32_t H, int32_t W, double* out,
                                     double* partial, cudaStream_t st) {
   return launch_metrics(pred, gt, n, H, W, out, partial, st);
+}
+
+// The same against RGBA uint8 ground truth [n][H][W][4] (4-byte aligned), composited over white while it is staged
+cudaError_t launch_image_metrics_rgba8(const float* pred, const uint8_t* gt, int32_t n, int32_t H, int32_t W, double* out,
+                                       double* partial, cudaStream_t st) {
+  return launch_metrics(pred, reinterpret_cast<const Rgba8*>(gt), n, H, W, out, partial, st);
 }
 
 }  // namespace hr

@@ -18,6 +18,10 @@
 // * OpenCV INTER_AREA for integer factors (resizeAreaFast_): (sum + 2) >> 2 at 2 x 2, otherwise sum * (1.f / area) in fp32
 //   rounded half to even.  The same kernel with a 1 x 1 box is the identity (both libraries copy a frame of the same size).
 //
+// RGBA (HR_PIXEL_RGBA8; datasets/donerf.py and catacaustics.py): OpenCV resamples the four channels independently; Pillow's
+// Image.resize converts an RGBA image to premultiplied RGBa, resamples that and converts back, on every call, so the Pillow
+// passes premultiply on load from the source and unpremultiply on the store into dst (Convert.c's rgbA2rgba / rgba2rgbA).
+//
 // No host synchronisation, no float atomics: two calls with the same arguments write the same bits.
 #include <algorithm>
 #include <cmath>
@@ -151,10 +155,10 @@ struct Plan {
   int kh = 0, kv = 0, y0 = 0, rows = 0;      // kPil: tap counts, first and number of intermediate rows
   std::vector<int32_t> th, tv;               // kPil tables
   std::vector<int4> lx, ly;                  // kLinear tables
-  size_t tab_bytes = 0, tmp_bytes = 0;       // workspace: tables, then the uint8 intermediate
+  size_t tab_bytes = 0, tmp_bytes = 0;       // workspace: tables, then the uint8 intermediate (premultiplied for RGBA)
 };
 
-// ---- kernels: one thread per output pixel (3 channels), grid-stride over all frames
+// ---- kernels: one thread per output pixel (kC = 3 or 4 channels), grid-stride over all frames
 
 __device__ __forceinline__ void load3(const uint8_t* p, bool swap, int& c0, int& c1, int& c2) {
   c0 = p[0];
@@ -169,13 +173,28 @@ __device__ __forceinline__ void load3(const uint8_t* p, bool swap, int& c0, int&
 
 __device__ __forceinline__ uint8_t clip8(int acc) { return (uint8_t)min(max(acc >> kPrecisionBits, 0), 255); }
 
+// Pillow's RGBA -> RGBa (rgbA2rgba): MULDIV255(c, a) = ((t >> 8) + t) >> 8 with t = c * a + 128
+__device__ __forceinline__ int premultiply(int c, int a) {
+  const int t = c * a + 128;
+  return ((t >> 8) + t) >> 8;
+}
+
+// Pillow's RGBa -> RGBA (rgba2rgbA): c unchanged for a of 0 or 255, else min(255, 255 * c / a) in integers
+__device__ __forceinline__ uint8_t unpremultiply(int c, int a) {
+  return (a == 0 || a == 255) ? (uint8_t)c : (uint8_t)min(255, (255 * c) / a);
+}
+
 // One Pillow pass.  Horizontal (vertical = 0): output (f, y, x) reads source row y0 + y at columns tab[x]; vertical: output
-// (f, y, x) reads column x at rows tab[y].  tab: [out][2 + ksize] as pil_table writes it.
+// (f, y, x) reads column x at rows tab[y].  tab: [out][2 + ksize] as pil_table writes it.  RGBA (kC = 4) resamples Pillow's
+// premultiplied RGBa, as Image.resize does: premul premultiplies each tap as it is loaded from the RGBA source (a per-pixel
+// function, so the same as premultiplying the frame first), unpremul converts back to RGBA in the store; an intermediate
+// between two passes stays premultiplied, as Pillow's does.
+template <int kC>
 __global__ void __launch_bounds__(kThreads) pil_pass_kernel(const uint8_t* __restrict__ src, int64_t src_frame, int64_t src_row,
                                                             int y0, uint8_t* __restrict__ dst, int64_t dst_frame,
                                                             int64_t dst_row, int n, int rows, int cols,
                                                             const int32_t* __restrict__ tab, int ksize, int vertical,
-                                                            int swap) {
+                                                            int swap, int premul, int unpremul) {
   const int64_t total = (int64_t)n * rows * cols;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int x = (int)(i % cols);
@@ -183,21 +202,44 @@ __global__ void __launch_bounds__(kThreads) pil_pass_kernel(const uint8_t* __res
     const int y = (int)(fy % rows), f = (int)(fy / rows);
     const int32_t* t = tab + (int64_t)(vertical ? y : x) * (2 + ksize);
     const int first = t[0], count = t[1];
-    const int64_t step = vertical ? src_row : 3;
-    const uint8_t* p = src + f * src_frame + (vertical ? (int64_t)x * 3 : (int64_t)(y0 + y) * src_row) + first * step;
-    int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0;
+    const int64_t step = vertical ? src_row : kC;
+    const uint8_t* p = src + f * src_frame + (vertical ? (int64_t)x * kC : (int64_t)(y0 + y) * src_row) + first * step;
+    int a0 = 1 << (kPrecisionBits - 1), a1 = a0, a2 = a0, a3 = a0;
     for (int k = 0; k < count; ++k, p += step) {
       int c0, c1, c2;
       load3(p, swap, c0, c1, c2);
       const int w = t[2 + k];
+      if constexpr (kC == 4) {
+        const int c3 = p[3];
+        if (premul) {
+          c0 = premultiply(c0, c3);
+          c1 = premultiply(c1, c3);
+          c2 = premultiply(c2, c3);
+        }
+        a3 += c3 * w;
+      }
       a0 += c0 * w;
       a1 += c1 * w;
       a2 += c2 * w;
     }
-    uint8_t* o = dst + f * dst_frame + y * dst_row + (int64_t)x * 3;
-    o[0] = clip8(a0);
-    o[1] = clip8(a1);
-    o[2] = clip8(a2);
+    uint8_t* o = dst + f * dst_frame + y * dst_row + (int64_t)x * kC;
+    if constexpr (kC == 4) {
+      const uint8_t al = clip8(a3);
+      if (unpremul) {
+        o[0] = unpremultiply(clip8(a0), al);
+        o[1] = unpremultiply(clip8(a1), al);
+        o[2] = unpremultiply(clip8(a2), al);
+      } else {
+        o[0] = clip8(a0);
+        o[1] = clip8(a1);
+        o[2] = clip8(a2);
+      }
+      o[3] = al;
+    } else {
+      o[0] = clip8(a0);
+      o[1] = clip8(a1);
+      o[2] = clip8(a2);
+    }
   }
 }
 
@@ -234,36 +276,41 @@ __global__ void __launch_bounds__(kThreads) cv_linear_kernel(const uint8_t* __re
   }
 }
 
-// OpenCV INTER_AREA for integer factors (ix x iy box); a 1 x 1 box copies
+// OpenCV INTER_AREA for integer factors (ix x iy box); a 1 x 1 box copies.  RGBA (kC = 4): OpenCV resamples the four
+// channels independently, alpha like the others.
+template <int kC>
 __global__ void __launch_bounds__(kThreads) cv_area_kernel(const uint8_t* __restrict__ src, int H0, int W0,
                                                            uint8_t* __restrict__ dst, int64_t dst_row, int n, int H, int W,
                                                            int ix, int iy, float inv_area, int swap) {
   const int64_t total = (int64_t)n * H * W;
-  const int64_t src_row = (int64_t)W0 * 3;
+  const int64_t src_row = (int64_t)W0 * kC;
   const bool two = ix == 2 && iy == 2;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int x = (int)(i % W);
     const int64_t fy = i / W;
     const int y = (int)(fy % H), f = (int)(fy / H);
-    const uint8_t* p = src + (int64_t)f * H0 * src_row + (int64_t)y * iy * src_row + (int64_t)x * ix * 3;
-    int s0 = 0, s1 = 0, s2 = 0;
+    const uint8_t* p = src + (int64_t)f * H0 * src_row + (int64_t)y * iy * src_row + (int64_t)x * ix * kC;
+    int s0 = 0, s1 = 0, s2 = 0, s3 = 0;
     for (int r = 0; r < iy; ++r, p += src_row)
       for (int c = 0; c < ix; ++c) {
         int c0, c1, c2;
-        load3(p + c * 3, swap, c0, c1, c2);
+        load3(p + c * kC, swap, c0, c1, c2);
         s0 += c0;
         s1 += c1;
         s2 += c2;
+        if constexpr (kC == 4) s3 += p[c * kC + 3];
       }
-    uint8_t* o = dst + (int64_t)f * H * dst_row + y * dst_row + (int64_t)x * 3;
+    uint8_t* o = dst + (int64_t)f * H * dst_row + y * dst_row + (int64_t)x * kC;
     if (two) {
       o[0] = (uint8_t)((s0 + 2) >> 2);
       o[1] = (uint8_t)((s1 + 2) >> 2);
       o[2] = (uint8_t)((s2 + 2) >> 2);
+      if constexpr (kC == 4) o[3] = (uint8_t)((s3 + 2) >> 2);
     } else {
       o[0] = (uint8_t)min(max(__float2int_rn(__fmul_rn((float)s0, inv_area)), 0), 255);
       o[1] = (uint8_t)min(max(__float2int_rn(__fmul_rn((float)s1, inv_area)), 0), 255);
       o[2] = (uint8_t)min(max(__float2int_rn(__fmul_rn((float)s2, inv_area)), 0), 255);
+      if constexpr (kC == 4) o[3] = (uint8_t)min(max(__float2int_rn(__fmul_rn((float)s3, inv_area)), 0), 255);
     }
   }
 }
@@ -278,10 +325,13 @@ bool mul_ok(int64_t& r, int64_t a, int64_t b, int64_t c, int64_t d) {
 }
 
 // Validates the call's shape and method and builds its tables; false with the refusal in msg.
-bool make_plan(const char* fn, int32_t n, int32_t H0, int32_t W0, int32_t H, int32_t W, int32_t method, Plan& p,
+// kC: channels per pixel, 3 (RGB) or 4 (RGBA).
+bool make_plan(const char* fn, int32_t n, int32_t H0, int32_t W0, int32_t H, int32_t W, int32_t method, int kC, Plan& p,
                char* msg, size_t len) {
   if (method < HR_RESIZE_PIL_LANCZOS || method > HR_RESIZE_CV2_AREA)
     return snprintf(msg, len, "%s: unknown method %d", fn, method), false;
+  if (kC == 4 && method == HR_RESIZE_CV2_LINEAR)
+    return snprintf(msg, len, "%s: cv2_linear is not supported for RGBA frames", fn), false;
   if (n < 1 || H0 < 1 || W0 < 1 || H < 1 || W < 1)
     return snprintf(msg, len, "%s: bad sizes %d x %d x %d -> %d x %d", fn, n, H0, W0, H, W), false;
   if (H > H0 || W > W0)
@@ -289,7 +339,7 @@ bool make_plan(const char* fn, int32_t n, int32_t H0, int32_t W0, int32_t H, int
                     W, H), false;
   // every byte count the call addresses fits int64 (the destination's is checked with its row stride)
   int64_t bytes;
-  if (!mul_ok(bytes, n, H0, W0, 3))
+  if (!mul_ok(bytes, n, H0, W0, kC))
     return snprintf(msg, len, "%s: %d frames of %d x %d overflow a 64-bit size", fn, n, W0, H0), false;
   if (H == H0 && W == W0) {
     p.path = kCopy;
@@ -327,7 +377,7 @@ bool make_plan(const char* fn, int32_t n, int32_t H0, int32_t W0, int32_t H, int
   p.tab_bytes = align256((int64_t)p.th.size() * 4) + align256((int64_t)p.tv.size() * 4);
   if (p.need_h && p.need_v) {
     // at most the source's bytes (rows <= H0, W <= W0), but the sum with the tables must fit too
-    if (!mul_ok(bytes, n, p.rows, W, 3) || bytes > INT64_MAX - 512 - (int64_t)p.tab_bytes)
+    if (!mul_ok(bytes, n, p.rows, W, kC) || bytes > INT64_MAX - 512 - (int64_t)p.tab_bytes)
       return snprintf(msg, len, "%s: the intermediate of %d frames of %d x %d overflows a 64-bit size", fn, n, W, p.rows),
              false;
     p.tmp_bytes = (size_t)align256(bytes);
@@ -335,47 +385,31 @@ bool make_plan(const char* fn, int32_t n, int32_t H0, int32_t W0, int32_t H, int
   return true;
 }
 
-}  // namespace
+// channels per pixel of an HR_PIXEL_* format, 0 for an unknown one
+int format_channels(int32_t pixel_format) {
+  return pixel_format == HR_PIXEL_RGB8 ? 3 : pixel_format == HR_PIXEL_RGBA8 ? 4 : 0;
+}
 
-extern "C" int64_t hr_resize_workspace_bytes(int32_t n, int32_t H0, int32_t W0, int32_t H, int32_t W, int32_t method) {
+int64_t workspace_bytes(const char* fn, int32_t n, int32_t H0, int32_t W0, int32_t H, int32_t W, int32_t method, int kC) {
   Plan p;
   char msg[256];
-  if (!make_plan("hr_resize_workspace_bytes", n, H0, W0, H, W, method, p, msg, sizeof msg)) return -1;
+  if (kC == 0 || !make_plan(fn, n, H0, W0, H, W, method, kC, p, msg, sizeof msg)) return -1;
   return (int64_t)(p.tab_bytes + p.tmp_bytes);
 }
 
-extern "C" int hr_resize_frames(const uint8_t* src, int32_t n, int32_t H0, int32_t W0, uint8_t* dst, int32_t H, int32_t W,
-                                int64_t dst_row_stride, int32_t method, int32_t flags, void* workspace,
-                                int64_t workspace_bytes, void* stream) {
-  const char* fn = "hr_resize_frames";
-  if (!src || !dst) return hr_fail("%s: null argument", fn);
-  if (flags & ~HR_RESIZE_BGR) return hr_fail("%s: unknown flags 0x%x", fn, (unsigned)flags);
-  Plan p;
-  char msg[256];
-  if (!make_plan(fn, n, H0, W0, H, W, method, p, msg, sizeof msg)) return hr_fail("%s", msg);
-  if (dst_row_stride < (int64_t)W * 3)
-    return hr_fail("%s: dst_row_stride %lld is less than a row's %lld bytes", fn, (long long)dst_row_stride, (long long)W * 3);
-  int64_t dst_bytes;
-  if (!mul_ok(dst_bytes, n, H, dst_row_stride, 1))
-    return hr_fail("%s: %d frames of %d rows of %lld bytes overflow a 64-bit size", fn, n, H, (long long)dst_row_stride);
-  const int64_t need = (int64_t)(p.tab_bytes + p.tmp_bytes);
-  if (need > 0 && (!workspace || ((uintptr_t)workspace % 256)))
-    return hr_fail("%s: a workspace of %lld bytes is needed (device, 256-byte aligned)", fn, (long long)need);
-  if (workspace_bytes < need)
-    return hr_fail("%s: workspace of %lld bytes, %lld needed", fn, (long long)workspace_bytes, (long long)need);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int swap = (flags & HR_RESIZE_BGR) ? 1 : 0;
+template <int kC>
+cudaError_t launch_plan(const Plan& p, const uint8_t* src, int32_t n, int32_t H0, int32_t W0, uint8_t* dst, int32_t H,
+                        int32_t W, int64_t dst_row_stride, int swap, char* ws, cudaStream_t st) {
   const int64_t total = (int64_t)n * H * W;
-  const int64_t src_row = (int64_t)W0 * 3, src_frame = src_row * H0, dst_frame = dst_row_stride * H;
-  char* ws = (char*)workspace;
+  const int64_t src_row = (int64_t)W0 * kC, src_frame = src_row * H0, dst_frame = dst_row_stride * H;
   cudaError_t e = cudaSuccess;
   switch (p.path) {
     case kCopy:
     case kArea:
-      cv_area_kernel<<<grid_for(total), kThreads, 0, st>>>(src, H0, W0, dst, dst_row_stride, n, H, W, p.ix, p.iy,
-                                                           1.f / (float)(p.ix * p.iy), swap);
+      cv_area_kernel<kC><<<grid_for(total), kThreads, 0, st>>>(src, H0, W0, dst, dst_row_stride, n, H, W, p.ix, p.iy,
+                                                               1.f / (float)(p.ix * p.iy), swap);
       break;
-    case kLinear: {
+    case kLinear: {  // RGB only (make_plan refuses it for RGBA)
       int4* tx = (int4*)ws;
       int4* ty = (int4*)(ws + align256((int64_t)W * sizeof(int4)));
       e = cudaMemcpyAsync(tx, p.lx.data(), p.lx.size() * sizeof(int4), cudaMemcpyHostToDevice, st);
@@ -391,26 +425,81 @@ extern "C" int hr_resize_frames(const uint8_t* src, int32_t n, int32_t H0, int32
       e = cudaMemcpyAsync(th, p.th.data(), p.th.size() * 4, cudaMemcpyHostToDevice, st);
       if (e == cudaSuccess) e = cudaMemcpyAsync(tv, p.tv.data(), p.tv.size() * 4, cudaMemcpyHostToDevice, st);
       if (e != cudaSuccess) break;
+      // RGBA: the pass that reads the source premultiplies, the pass that writes dst unpremultiplies (ignored for RGB)
       if (p.need_h) {
         // into the intermediate (rows y0 .. y0 + rows of the source), or straight into dst when the height is kept
         uint8_t* o = p.need_v ? tmp : dst;
-        const int64_t o_row = p.need_v ? (int64_t)W * 3 : dst_row_stride;
+        const int64_t o_row = p.need_v ? (int64_t)W * kC : dst_row_stride;
         const int rows = p.need_v ? p.rows : H0;
         const int y0 = p.need_v ? p.y0 : 0;
-        pil_pass_kernel<<<grid_for((int64_t)n * rows * W), kThreads, 0, st>>>(src, src_frame, src_row, y0, o, o_row * rows,
-                                                                              o_row, n, rows, W, th, p.kh, 0, swap);
+        pil_pass_kernel<kC><<<grid_for((int64_t)n * rows * W), kThreads, 0, st>>>(
+            src, src_frame, src_row, y0, o, o_row * rows, o_row, n, rows, W, th, p.kh, 0, swap, 1, p.need_v ? 0 : 1);
       }
       if (p.need_v) {
         const uint8_t* in = p.need_h ? tmp : src;
-        const int64_t in_row = p.need_h ? (int64_t)W * 3 : src_row;
+        const int64_t in_row = p.need_h ? (int64_t)W * kC : src_row;
         const int64_t in_frame = p.need_h ? in_row * p.rows : src_frame;
-        pil_pass_kernel<<<grid_for(total), kThreads, 0, st>>>(in, in_frame, in_row, 0, dst, dst_frame, dst_row_stride, n, H,
-                                                              W, tv, p.kv, 1, p.need_h ? 0 : swap);
+        pil_pass_kernel<kC><<<grid_for(total), kThreads, 0, st>>>(in, in_frame, in_row, 0, dst, dst_frame, dst_row_stride, n,
+                                                                  H, W, tv, p.kv, 1, p.need_h ? 0 : swap,
+                                                                  p.need_h ? 0 : 1, 1);
       }
       break;
     }
   }
+  return e;
+}
+
+int resize_frames(const char* fn, const uint8_t* src, int32_t n, int32_t H0, int32_t W0, uint8_t* dst, int32_t H, int32_t W,
+                  int64_t dst_row_stride, int32_t method, int32_t flags, int32_t pixel_format, void* workspace,
+                  int64_t workspace_bytes, void* stream) {
+  if (!src || !dst) return hr_fail("%s: null argument", fn);
+  if (flags & ~HR_RESIZE_BGR) return hr_fail("%s: unknown flags 0x%x", fn, (unsigned)flags);
+  const int kC = format_channels(pixel_format);
+  if (kC == 0) return hr_fail("%s: unknown pixel format %d", fn, pixel_format);
+  Plan p;
+  char msg[256];
+  if (!make_plan(fn, n, H0, W0, H, W, method, kC, p, msg, sizeof msg)) return hr_fail("%s", msg);
+  if (dst_row_stride < (int64_t)W * kC)
+    return hr_fail("%s: dst_row_stride %lld is less than a row's %lld bytes", fn, (long long)dst_row_stride,
+                   (long long)W * kC);
+  int64_t dst_bytes;
+  if (!mul_ok(dst_bytes, n, H, dst_row_stride, 1))
+    return hr_fail("%s: %d frames of %d rows of %lld bytes overflow a 64-bit size", fn, n, H, (long long)dst_row_stride);
+  const int64_t need = (int64_t)(p.tab_bytes + p.tmp_bytes);
+  if (need > 0 && (!workspace || ((uintptr_t)workspace % 256)))
+    return hr_fail("%s: a workspace of %lld bytes is needed (device, 256-byte aligned)", fn, (long long)need);
+  if (workspace_bytes < need)
+    return hr_fail("%s: workspace of %lld bytes, %lld needed", fn, (long long)workspace_bytes, (long long)need);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int swap = (flags & HR_RESIZE_BGR) ? 1 : 0;
+  cudaError_t e = kC == 4 ? launch_plan<4>(p, src, n, H0, W0, dst, H, W, dst_row_stride, swap, (char*)workspace, st)
+                          : launch_plan<3>(p, src, n, H0, W0, dst, H, W, dst_row_stride, swap, (char*)workspace, st);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) return hr_fail("%s: %s", fn, cudaGetErrorString(e));
   return 0;
+}
+
+}  // namespace
+
+extern "C" int64_t hr_resize_workspace_bytes(int32_t n, int32_t H0, int32_t W0, int32_t H, int32_t W, int32_t method) {
+  return workspace_bytes("hr_resize_workspace_bytes", n, H0, W0, H, W, method, 3);
+}
+
+extern "C" int64_t hr_resize_workspace_bytes_fmt(int32_t n, int32_t H0, int32_t W0, int32_t H, int32_t W, int32_t method,
+                                                 int32_t pixel_format) {
+  return workspace_bytes("hr_resize_workspace_bytes_fmt", n, H0, W0, H, W, method, format_channels(pixel_format));
+}
+
+extern "C" int hr_resize_frames(const uint8_t* src, int32_t n, int32_t H0, int32_t W0, uint8_t* dst, int32_t H, int32_t W,
+                                int64_t dst_row_stride, int32_t method, int32_t flags, void* workspace,
+                                int64_t workspace_bytes, void* stream) {
+  return resize_frames("hr_resize_frames", src, n, H0, W0, dst, H, W, dst_row_stride, method, flags, HR_PIXEL_RGB8,
+                       workspace, workspace_bytes, stream);
+}
+
+extern "C" int hr_resize_frames_fmt(const uint8_t* src, int32_t n, int32_t H0, int32_t W0, uint8_t* dst, int32_t H,
+                                    int32_t W, int64_t dst_row_stride, int32_t method, int32_t flags, int32_t pixel_format,
+                                    void* workspace, int64_t workspace_bytes, void* stream) {
+  return resize_frames("hr_resize_frames_fmt", src, n, H0, W0, dst, H, W, dst_row_stride, method, flags, pixel_format,
+                       workspace, workspace_bytes, stream);
 }

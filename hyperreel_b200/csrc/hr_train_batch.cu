@@ -13,7 +13,11 @@
 // epoch_key = mix64(mix64(seed) + G*(epoch + 1)), round_key[i] = mix64(epoch_key + G*(i + 1)), G = 0x9E3779B97F4A7C15, all
 // uint64 arithmetic modulo 2^64.  tests/train_order_oracle.py restates it in NumPy.
 //
-// One thread per row: one 3-byte gather and one 48-byte row write (plus 8 B of pixel id when asked).  No float atomics, no
+// RGBA images (HR_PIXEL_RGBA8, the DoNeRF and Catacaustics datasets): a row's colour is the composite their get_rgb returns,
+// rgb * a + (1 - a) of the u8 / 255 values, each operation rounded on its own as torch rounds it on the CPU (no FMA
+// contraction: __fmul_rn, __fsub_rn, __fadd_rn), from one aligned 4-byte load of the pixel.
+//
+// One thread per row: one 3-byte (or 4-byte) gather and one 48-byte row write (plus 8 B of pixel id when asked).  No float atomics, no
 // host synchronisation; two calls with the same arguments write the same bits.  The camera records live on the device, so
 // each row branches on its own record's fisheye and two_plane flags (camera_ray<true, true>) and one batch may mix pinhole,
 // fisheye and two-plane views.
@@ -225,8 +229,9 @@ __device__ __forceinline__ bool table_pixel(const MaskPlan& plan, const int64_t*
 
 constexpr int kStagedViews = 4095;  // prefixes of up to this many views are staged in shared memory (32 KB)
 
-// Plan: WholePlan (every pixel), TablePlan (a (stride, offset) rule per view) or MaskPlan (a keep mask per view).
-template <class Plan>
+// Plan: WholePlan (every pixel), TablePlan (a (stride, offset) rule per view) or MaskPlan (a keep mask per view).  kC: bytes
+// per pixel, 3 (RGB) or 4 (RGBA, composited over white).
+template <class Plan, int kC>
 __global__ void __launch_bounds__(256)
 train_rows_kernel(const hr_camera* __restrict__ cams, const uint8_t* __restrict__ images, int height, int width,
                   const __grid_constant__ Plan plan, const __grid_constant__ FeistelKey key, uint64_t dkey, int mode,
@@ -257,10 +262,18 @@ train_rows_kernel(const hr_camera* __restrict__ cams, const uint8_t* __restrict_
       p = kWhole<Plan> ? k : v * hw + (long long)y * width + x;
       const hr_camera& cam = cams[v];
       camera_ray<true, true>(cam, x, y, ndc_scale(cam), row);
-      const uint8_t* px = images + 3 * p;
-      c0 = __fdiv_rn((float)px[0], 255.0f);
-      c1 = __fdiv_rn((float)px[1], 255.0f);
-      c2 = __fdiv_rn((float)px[2], 255.0f);
+      if constexpr (kC == 4) {
+        const uint32_t q = *reinterpret_cast<const uint32_t*>(images + 4 * p);  // 4-byte aligned (checked by the host)
+        const float a = __fdiv_rn((float)(q >> 24), 255.0f), ia = __fsub_rn(1.0f, a);
+        c0 = __fadd_rn(__fmul_rn(__fdiv_rn((float)(q & 0xffu), 255.0f), a), ia);
+        c1 = __fadd_rn(__fmul_rn(__fdiv_rn((float)((q >> 8) & 0xffu), 255.0f), a), ia);
+        c2 = __fadd_rn(__fmul_rn(__fdiv_rn((float)((q >> 16) & 0xffu), 255.0f), a), ia);
+      } else {
+        const uint8_t* px = images + 3 * p;
+        c0 = __fdiv_rn((float)px[0], 255.0f);
+        c1 = __fdiv_rn((float)px[1], 255.0f);
+        c2 = __fdiv_rn((float)px[2], 255.0f);
+      }
       w = 1.0f;
     } else {
       k = -1;  // a row the plan does not hold: a zero row of weight 0 (the Python binding validates plans and rows)
@@ -468,8 +481,9 @@ importance_views_kernel(int n_views, long long hw, const int32_t* __restrict__ v
 
 namespace {
 
-// The checks, batch range and launch shared by the three sampling entry points; `plan` carries the table.
-template <class Plan>
+// The checks, batch range and launch shared by the three sampling entry points; `plan` carries the table, kC the bytes per
+// pixel of `images` (3 or 4).
+template <class Plan, int kC = 3>
 int sample_rows(const char* fn, const Plan& plan, const hr_camera* cameras, int32_t n_views, const uint8_t* images,
                 int32_t height, int32_t width, int32_t c_in, int32_t mode, uint64_t seed, int64_t epoch, int64_t batch_index,
                 int64_t batch_size, const int64_t* table_rows, float* coords, float* rgb, float* weight, int64_t* pixel_ids,
@@ -484,6 +498,7 @@ int sample_rows(const char* fn, const Plan& plan, const hr_camera* cameras, int3
   if (((uintptr_t)coords % 8) || ((uintptr_t)rgb % 4) || ((uintptr_t)weight % 4) || ((uintptr_t)pixel_ids % 8) ||
       ((uintptr_t)table_ids % 8) || ((uintptr_t)table_rows % 8) || (view_start % 8) || ((uintptr_t)cameras % 4))
     return hr_fail("%s: misaligned pointer (coords, view_start and the int64 row arrays need 8 bytes, the rest 4)", fn);
+  if (kC == 4 && ((uintptr_t)images % 4)) return hr_fail("%s: misaligned pointer (RGBA images need 4 bytes)", fn);
   const uint64_t n = (uint64_t)n_views * (uint64_t)height * (uint64_t)width;
   if (n > (1ull << 62)) return hr_fail("%s: %llu pixels, at most 2^62", fn, (unsigned long long)n);
   const int64_t n_table = plan.n_table;
@@ -509,7 +524,7 @@ int sample_rows(const char* fn, const Plan& plan, const hr_camera* cameras, int3
   if (g > 148 * 16) g = 148 * 16;
   const size_t smem =
       !hr::kWhole<Plan> && n_views <= hr::kStagedViews ? (size_t)(n_views + 1) * sizeof(int64_t) : 0;
-  hr::train_rows_kernel<Plan><<<(unsigned)g, 256, smem, (cudaStream_t)stream>>>(
+  hr::train_rows_kernel<Plan, kC><<<(unsigned)g, 256, smem, (cudaStream_t)stream>>>(
       cameras, images, height, width, plan, key, hr::draw_key(seed, epoch), mode, first, rows, table_rows, c_in, coords, rgb,
       weight, pixel_ids, table_ids);
   const cudaError_t e = cudaGetLastError();
@@ -526,18 +541,63 @@ size_t importance_workspace(int64_t n_slots) {
 
 }  // namespace
 
+namespace {
+
+int sample_batch(const char* fn, const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t pixel_format,
+                 int32_t height, int32_t width, int32_t c_in, uint64_t seed, int64_t epoch, int64_t batch_index,
+                 int64_t batch_size, const int64_t* order, float* coords, float* rgb, float* weight, int64_t* pixel_ids,
+                 int64_t* n_rows, void* stream) {
+  if (!cameras || !images || !coords || !rgb || !weight) return hr_fail("%s: null argument", fn);
+  if (((uintptr_t)coords % 8) || ((uintptr_t)rgb % 4) || ((uintptr_t)weight % 4) || ((uintptr_t)pixel_ids % 8) ||
+      ((uintptr_t)order % 8) || ((uintptr_t)cameras % 4))
+    return hr_fail("%s: misaligned pointer (coords and pixel_ids / order need 8 bytes, the rest 4)", fn);
+  if (pixel_format != HR_PIXEL_RGB8 && pixel_format != HR_PIXEL_RGBA8)
+    return hr_fail("%s: unknown pixel format %d", fn, pixel_format);
+  // the table is every pixel (sample_rows refuses a bad image stack and more than 2^62 pixels before n_table is used)
+  const hr::WholePlan plan{(long long)((uint64_t)n_views * (uint64_t)height * (uint64_t)width)};
+  return pixel_format == HR_PIXEL_RGBA8
+             ? sample_rows<hr::WholePlan, 4>(fn, plan, cameras, n_views, images, height, width, c_in, HR_SAMPLE_PERMUTE,
+                                             seed, epoch, batch_index, batch_size, order, coords, rgb, weight, pixel_ids,
+                                             nullptr, n_rows, stream)
+             : sample_rows(fn, plan, cameras, n_views, images, height, width, c_in, HR_SAMPLE_PERMUTE, seed, epoch,
+                           batch_index, batch_size, order, coords, rgb, weight, pixel_ids, nullptr, n_rows, stream);
+}
+
+int sample_table_rows(const char* fn, const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t pixel_format,
+                      int32_t height, int32_t width, int32_t c_in, const int64_t* view_start, const int32_t* view_rule,
+                      int64_t n_table, int32_t mode, uint64_t seed, int64_t epoch, int64_t batch_index, int64_t batch_size,
+                      const int64_t* table_rows, float* coords, float* rgb, float* weight, int64_t* pixel_ids,
+                      int64_t* table_ids, int64_t* n_rows, void* stream) {
+  if (!cameras || !images || !view_start || !view_rule || !coords || !rgb || !weight) return hr_fail("%s: null argument", fn);
+  if ((uintptr_t)view_rule % 4) return hr_fail("%s: misaligned pointer (view_rule needs 4 bytes)", fn);
+  if (pixel_format != HR_PIXEL_RGB8 && pixel_format != HR_PIXEL_RGBA8)
+    return hr_fail("%s: unknown pixel format %d", fn, pixel_format);
+  const hr::TablePlan plan{view_start, view_rule, n_views, n_table};
+  return pixel_format == HR_PIXEL_RGBA8
+             ? sample_rows<hr::TablePlan, 4>(fn, plan, cameras, n_views, images, height, width, c_in, mode, seed, epoch,
+                                             batch_index, batch_size, table_rows, coords, rgb, weight, pixel_ids, table_ids,
+                                             n_rows, stream)
+             : sample_rows(fn, plan, cameras, n_views, images, height, width, c_in, mode, seed, epoch, batch_index,
+                           batch_size, table_rows, coords, rgb, weight, pixel_ids, table_ids, n_rows, stream);
+}
+
+}  // namespace
+
 extern "C" int hr_sample_train_batch(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height,
                                      int32_t width, int32_t c_in, uint64_t seed, int64_t epoch, int64_t batch_index,
                                      int64_t batch_size, const int64_t* order, float* coords, float* rgb, float* weight,
                                      int64_t* pixel_ids, int64_t* n_rows, void* stream) {
-  if (!cameras || !images || !coords || !rgb || !weight) return hr_fail("hr_sample_train_batch: null argument");
-  if (((uintptr_t)coords % 8) || ((uintptr_t)rgb % 4) || ((uintptr_t)weight % 4) || ((uintptr_t)pixel_ids % 8) ||
-      ((uintptr_t)order % 8) || ((uintptr_t)cameras % 4))
-    return hr_fail("hr_sample_train_batch: misaligned pointer (coords and pixel_ids / order need 8 bytes, the rest 4)");
-  // the table is every pixel (sample_rows refuses a bad image stack and more than 2^62 pixels before n_table is used)
-  const hr::WholePlan plan{(long long)((uint64_t)n_views * (uint64_t)height * (uint64_t)width)};
-  return sample_rows("hr_sample_train_batch", plan, cameras, n_views, images, height, width, c_in, HR_SAMPLE_PERMUTE, seed,
-                     epoch, batch_index, batch_size, order, coords, rgb, weight, pixel_ids, nullptr, n_rows, stream);
+  return sample_batch("hr_sample_train_batch", cameras, n_views, images, HR_PIXEL_RGB8, height, width, c_in, seed, epoch,
+                      batch_index, batch_size, order, coords, rgb, weight, pixel_ids, n_rows, stream);
+}
+
+extern "C" int hr_sample_train_batch_fmt(const hr_camera* cameras, int32_t n_views, const uint8_t* images,
+                                         int32_t pixel_format, int32_t height, int32_t width, int32_t c_in, uint64_t seed,
+                                         int64_t epoch, int64_t batch_index, int64_t batch_size, const int64_t* order,
+                                         float* coords, float* rgb, float* weight, int64_t* pixel_ids, int64_t* n_rows,
+                                         void* stream) {
+  return sample_batch("hr_sample_train_batch_fmt", cameras, n_views, images, pixel_format, height, width, c_in, seed, epoch,
+                      batch_index, batch_size, order, coords, rgb, weight, pixel_ids, n_rows, stream);
 }
 
 extern "C" int hr_sample_train_rows(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height,
@@ -545,12 +605,20 @@ extern "C" int hr_sample_train_rows(const hr_camera* cameras, int32_t n_views, c
                                     int64_t n_table, int32_t mode, uint64_t seed, int64_t epoch, int64_t batch_index,
                                     int64_t batch_size, const int64_t* table_rows, float* coords, float* rgb, float* weight,
                                     int64_t* pixel_ids, int64_t* table_ids, int64_t* n_rows, void* stream) {
-  if (!cameras || !images || !view_start || !view_rule || !coords || !rgb || !weight)
-    return hr_fail("hr_sample_train_rows: null argument");
-  if ((uintptr_t)view_rule % 4) return hr_fail("hr_sample_train_rows: misaligned pointer (view_rule needs 4 bytes)");
-  const hr::TablePlan plan{view_start, view_rule, n_views, n_table};
-  return sample_rows("hr_sample_train_rows", plan, cameras, n_views, images, height, width, c_in, mode, seed, epoch,
-                     batch_index, batch_size, table_rows, coords, rgb, weight, pixel_ids, table_ids, n_rows, stream);
+  return sample_table_rows("hr_sample_train_rows", cameras, n_views, images, HR_PIXEL_RGB8, height, width, c_in, view_start,
+                           view_rule, n_table, mode, seed, epoch, batch_index, batch_size, table_rows, coords, rgb, weight,
+                           pixel_ids, table_ids, n_rows, stream);
+}
+
+extern "C" int hr_sample_train_rows_fmt(const hr_camera* cameras, int32_t n_views, const uint8_t* images,
+                                        int32_t pixel_format, int32_t height, int32_t width, int32_t c_in,
+                                        const int64_t* view_start, const int32_t* view_rule, int64_t n_table, int32_t mode,
+                                        uint64_t seed, int64_t epoch, int64_t batch_index, int64_t batch_size,
+                                        const int64_t* table_rows, float* coords, float* rgb, float* weight,
+                                        int64_t* pixel_ids, int64_t* table_ids, int64_t* n_rows, void* stream) {
+  return sample_table_rows("hr_sample_train_rows_fmt", cameras, n_views, images, pixel_format, height, width, c_in,
+                           view_start, view_rule, n_table, mode, seed, epoch, batch_index, batch_size, table_rows, coords,
+                           rgb, weight, pixel_ids, table_ids, n_rows, stream);
 }
 
 extern "C" int hr_sample_train_mask_rows(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height,

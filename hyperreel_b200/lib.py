@@ -11,7 +11,7 @@ import os
 import subprocess
 import threading
 
-HR_ABI_VERSION = 22
+HR_ABI_VERSION = 23
 HR_MAX_GROUPS = 4
 HR_MAX_LAYERS = 10
 HR_MAX_SAMPLES = 256
@@ -27,6 +27,7 @@ MLP_FP32_SIMT, MLP_BF16X3_TC, MLP_ZERO = 0, 1, 2
 SAMPLE_PERMUTE, SAMPLE_REPLACE = 0, 1  # hr_sample_train_rows modes
 RESIZE_METHODS = {"pil_lanczos": 0, "pil_bicubic": 1, "pil_box": 2, "cv2_linear": 3, "cv2_area": 4}  # HR_RESIZE_*
 RESIZE_BGR = 1
+PIXEL_RGB8, PIXEL_RGBA8 = 0, 1  # HR_PIXEL_*: uint8 RGB, or RGBA composited over white where a colour is consumed
 # extra fields of the colour net (hr_render_fields): key of the reference's dict `x` -> HR_FIELD_* id
 FIELDS = {"points": 0, "distances": 1, "base_times": 2, "time_offset": 3, "times": 4, "viewdirs": 5, "weights": 6,
           "color_scale": 7, "color_shift": 8, "spatial_flow": 9, "sigma": 10, "point_sigma": 11, "point_offset": 12,
@@ -163,6 +164,13 @@ EXPORTS = {
     "hr_sample_train_rows": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                         C.c_int64, C.c_int32, C.c_uint64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
+    "hr_sample_train_batch_fmt": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                             C.c_uint64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
+    "hr_sample_train_rows_fmt": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                            C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_uint64, C.c_int64, C.c_int64,
+                                            C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.POINTER(C.c_int64), C.c_void_p]),
     "hr_importance_workspace_bytes": (C.c_int64, [C.c_int32]),
     "hr_build_importance_table": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                              C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -178,6 +186,8 @@ EXPORTS = {
     "hr_score_views_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]),
     "hr_score_views": (C.c_int, [C.c_void_p, C.POINTER(hr_camera), C.POINTER(C.c_float), C.c_int32, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_int64, C.c_void_p]),
+    "hr_score_views_fmt": (C.c_int, [C.c_void_p, C.POINTER(hr_camera), C.POINTER(C.c_float), C.c_int32, C.c_void_p, C.c_int32,
+                                      C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "hr_encode_rays": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "hr_render_heads": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.POINTER(hr_train_opts), C.c_void_p,
                                    C.c_int64, C.c_void_p]),
@@ -196,6 +206,9 @@ EXPORTS = {
     "hr_resize_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "hr_resize_frames": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int64,
                                     C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]),
+    "hr_resize_workspace_bytes_fmt": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "hr_resize_frames_fmt": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int64,
+                                        C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]),
     "hr_launch_count": (C.c_int64, [C.c_void_p]),
     "hr_timing_enable": (C.c_int, [C.c_void_p, C.c_int]),
     "hr_timing_reset": (C.c_int, [C.c_void_p]),

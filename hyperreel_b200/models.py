@@ -539,12 +539,15 @@ class LightfieldModel(nn.Module):
                                                    stream.cuda_stream))
         return out
 
-    def score_views(self, cameras, images: torch.Tensor, times=None, out: Optional[torch.Tensor] = None, stream=None):
+    def score_views(self, cameras, images: torch.Tensor, times=None, out: Optional[torch.Tensor] = None, stream=None, *,
+                    rgba: bool = False):
         """(mse, ssim) of every held-out view, fp64 [n] device tensors: view i rendered from ``cameras[i]`` at ``times[i]``
         (default each camera's ``time``) in one call that never synchronises (hr_score_views), scored against ``images[i]``
         (uint8 [n, H, W, 3] on the device, contiguous) like ``metrics.image_metrics(pred, images[i] / 255)`` (correctly rounded, as T.ToTensor() converts) of the
         view's eval render, bit for bit.  ``out`` (device fp64 [n, 2], contiguous) receives (mse, ssim) when given; the work
-        goes on ``stream`` (a torch.cuda.Stream; default the current stream)."""
+        goes on ``stream`` (a torch.cuda.Stream; default the current stream).  ``rgba=True``: ``images`` are uint8 RGBA
+        [n, H, W, 4], the DoNeRF and Catacaustics frames, and each view is scored against its composite over white,
+        ``rgb * a + (1 - a)`` of the ``u8 / 255`` values as their ``get_rgb`` computes it on the CPU (hr_score_views_fmt)."""
         if self.training:
             raise RuntimeError("hyperreel_b200.LightfieldModel implements the eval()/render path only; call .eval()")
         cams = list(cameras)
@@ -562,11 +565,12 @@ class LightfieldModel(nn.Module):
                 raise ValueError(f"score_views: camera {i} is {int(c.width)} x {int(c.height)}, camera 0 is {W} x {H}")
         if H < 11 or W < 11:
             raise ValueError(f"score_views: views must be at least 11 x 11 (the SSIM window), got {W} x {H}")
-        shape = (len(cams), H, W, 3)
+        shape = (len(cams), H, W, 4 if rgba else 3)
         if not isinstance(images, torch.Tensor) or images.dtype != torch.uint8 or tuple(images.shape) != shape \
                 or not images.is_contiguous():
             got = f"{images.dtype} {tuple(images.shape)}" if isinstance(images, torch.Tensor) else type(images).__name__
-            raise ValueError(f"score_views: images must be a contiguous uint8 tensor of shape {shape}, got {got}")
+            raise ValueError(f"score_views: images must be a contiguous uint8 tensor of shape {shape}"
+                             f"{' (rgba=True)' if rgba else ''}, got {got}")
         if not images.is_cuda:
             raise RuntimeError("hyperreel_b200 scores views on an H100 only: images must be a CUDA tensor (no CPU fallback)")
         dev = images.device
@@ -588,8 +592,9 @@ class LightfieldModel(nn.Module):
             ws = torch.empty(need, dtype=torch.uint8, device=dev)
             if out is None:
                 out = torch.empty((len(cams), 2), dtype=torch.float64, device=dev)
-            L.check(self._lib.hr_score_views(self._handle, recs, tt, len(cams), images.data_ptr(), out.data_ptr(), ws.data_ptr(),
-                                             need, stream.cuda_stream))
+            fmt = L.PIXEL_RGBA8 if rgba else L.PIXEL_RGB8
+            L.check(self._lib.hr_score_views_fmt(self._handle, recs, tt, len(cams), images.data_ptr(), fmt, out.data_ptr(),
+                                                 ws.data_ptr(), need, stream.cuda_stream))
         return out[:, 0], out[:, 1]
 
     def timing(self, enable: bool = True):

@@ -349,23 +349,24 @@ class INRSystem(nn.Module):
         finally:
             self.train(was_training)
 
-    def score_views(self, cameras, images, times=None, out=None, stream=None):
+    def score_views(self, cameras, images, times=None, out=None, stream=None, *, rgba=False):
         """hyperreel_b200.score_views of this system's model, rendered in eval() (the previous train / eval mode is restored)."""
         was_training = self.training
         self.eval()
         try:
-            return self.render_fn.model.score_views(cameras, images, times, out=out, stream=stream)
+            return self.render_fn.model.score_views(cameras, images, times, out=out, stream=stream, rgba=rgba)
         finally:
             self.train(was_training)
 
-    def validation_views(self, cameras, images, times=None):
+    def validation_views(self, cameras, images, times=None, *, rgba=False):
         """validation_image of every view of a held-out split in one device call (score_views): view i rendered from
         ``cameras[i]`` at ``times[i]`` (default each camera's ``time``) and scored against ``images[i]`` (uint8 [n, H, W, 3]
         on the device).  Returns one dict per view with validation_image's keys and dtypes, 0-d device tensors, so
         validation_epoch_end takes the list as it is: 'val/psnr' and 'val/ssim' equal validation_image's bit for bit (fed the
         view's rays and images[i] / 255, correctly rounded); 'val/loss' is the fp64 MSE rounded to fp32, which differs from
-        validation_image's fp32 mean only in summation order."""
-        mse, ssim = self.score_views(cameras, images, times)
+        validation_image's fp32 mean only in summation order.  ``rgba=True``: ``images`` are uint8 RGBA [n, H, W, 4] and
+        validation_image is fed their composite over white, as the DoNeRF and Catacaustics get_rgb make it."""
+        mse, ssim = self.score_views(cameras, images, times, rgba=rgba)
         return [{"val/loss": mse[i].float(), "val/psnr": 10.0 * torch.log10(1.0 / mse[i]), "val/ssim": ssim[i]}
                 for i in range(mse.shape[0])]
 

@@ -202,13 +202,19 @@ class DeviceRayBatches:
 
     Only the reference's default training mode is provided.  The dataset options of the others (datasets/base.py:85-101)
     are accepted under the reference's names so that they can be refused: ``use_patches``, ``precrop_iters`` > 0 (crop),
-    ``use_full_image`` and ``blur_radius`` > 0 raise ``ValueError``, as do views of different sizes and non-uint8 images."""
+    ``use_full_image`` and ``blur_radius`` > 0 raise ``ValueError``, as do views of different sizes and non-uint8 images.
+
+    ``rgba=True``: the images are uint8 RGBA ``[n, H, W, 4]`` (4 B per pixel held), as the DoNeRF and Catacaustics datasets
+    load them (``dataset_frames`` resizes them), and each row's ``'rgb'`` is the pixel's composite over white that their
+    ``get_rgb`` returns, ``rgb * a + (1 - a)`` of the ``u8 / 255`` values with each operation rounded as torch rounds it on
+    the CPU.  Rays, order, draws and ids are those of the same views given as RGB.  Not combined with ``importance`` (the
+    Immersive dataset, whose frames are RGB)."""
 
     def __init__(self, cameras: Sequence[Camera], images, batch_size: int, seed: int = 0, c_in: int = 8,
                  device: Optional[torch.device] = None, *, use_patches: bool = False, precrop_iters: int = 0,
                  use_full_image: bool = False, blur_radius: int = 0, replacement: bool = False,
                  num_iters: Optional[int] = None, subsample: Optional[Sequence[Tuple[int, int]]] = None,
-                 importance: Optional[Sequence[Optional[Tuple[int, int]]]] = None):
+                 importance: Optional[Sequence[Optional[Tuple[int, int]]]] = None, rgba: bool = False):
         for name, value, default in (("use_patches", use_patches, False), ("precrop_iters", precrop_iters, 0),
                                      ("use_full_image", use_full_image, False), ("blur_radius", blur_radius, 0)):
             if value != default:
@@ -219,8 +225,9 @@ class DeviceRayBatches:
         if int(batch_size) < 1:
             raise ValueError(f"batch_size must be >= 1, got {batch_size}")
         images = _as_image_stack(images)
-        if images.dim() != 4 or images.shape[-1] != 3:
-            raise ValueError(f"images must be [n, H, W, 3], got {tuple(images.shape)}")
+        ch = 4 if rgba else 3
+        if images.dim() != 4 or images.shape[-1] != ch:
+            raise ValueError(f"images must be [n, H, W, {ch}]{' (rgba=True)' if rgba else ''}, got {tuple(images.shape)}")
         cameras = list(cameras)
         n, H, W = int(images.shape[0]), int(images.shape[1]), int(images.shape[2])
         if n < 1 or H < 1 or W < 1:
@@ -238,6 +245,9 @@ class DeviceRayBatches:
             raise ValueError("num_iters sets the epoch length of replacement=True; without replacement an epoch is "
                              "ceil(n_rows / batch_size) batches")
         if importance is not None:
+            if rgba:
+                raise ValueError("importance tables are built from RGB frames (the Immersive dataset): rgba=True is not "
+                                 "supported with importance")
             if subsample is not None:
                 raise ValueError("importance and subsample are two different tables: give one of them")
             importance = self._check_importance(importance, n, H * W)
@@ -272,6 +282,7 @@ class DeviceRayBatches:
         self.num_iters = int(num_iters) if replacement else None
         self.subsample = None if subsample is None else rule
         self.importance = importance
+        self.rgba = bool(rgba)
         if importance is None:
             self._n_rows = int(sum(counts))
             # the table's plan for hr_sample_train_rows: exclusive prefix of the per-view row counts, and (stride, offset) per view
@@ -344,7 +355,9 @@ class DeviceRayBatches:
         """The training batches a reference config trains on: ``cfg.training.batch_size``, ``sample_with_replacement`` and
         ``num_iters``, and for the ``technicolor``, ``neural_3d`` and ``immersive`` datasets the per-frame pixel subsets of
         ``cfg.dataset.{num_frames, load_full_step, subsample_keyframe_step, subsample_keyframe_frac, subsample_frac}``
-        (``importance_subsample_plan`` for immersive, built on the device from the images).
+        (``importance_subsample_plan`` for immersive, built on the device from the images).  For the ``donerf`` and
+        ``catacaustics`` datasets the images may be their RGBA frames ``[n, H, W, 4]`` (``dataset_frames``' output), which
+        are then composited over white as ``rgba=True`` does.
 
         ``cameras`` and ``images`` must be the training views in the reference's training order: frame-major with the
         held-out views removed for technicolor, video-major (each video's frames in order) for neural_3d and immersive.  A
@@ -392,8 +405,10 @@ class DeviceRayBatches:
         elif any(k in dataset for k in keys):
             raise ValueError(f"dataset {name!r} sets {[k for k in keys if k in dataset]}: only technicolor's, neural_3d's "
                              "and immersive's subsets are supported")
+        images = _as_image_stack(images)
+        rgba = name in ("donerf", "catacaustics") and images.dim() == 4 and images.shape[-1] == 4
         return cls(cameras, images, batch_size=int(training["batch_size"]), seed=seed, c_in=c_in, device=device,
-                   replacement=replacement, num_iters=num_iters, subsample=subsample, importance=importance)
+                   replacement=replacement, num_iters=num_iters, subsample=subsample, importance=importance, rgba=rgba)
 
     def __len__(self) -> int:
         if self.replacement:
@@ -446,8 +461,8 @@ class DeviceRayBatches:
     def _launch(self, rows: int, index: int, ids: Optional[torch.Tensor], with_pixel_ids: bool, with_table_ids: bool,
                 ids_are_pixels: bool = False) -> Dict[str, torch.Tensor]:
         """Batch ``index`` of the epoch, or the rows of the explicit ``ids`` (table rows, or pixels with ``ids_are_pixels``).
-        Explicit pixels and the permuted batches without a plan go through ``hr_sample_train_batch``, everything else
-        through the plan's entry (``hr_sample_train_rows`` or ``hr_sample_train_mask_rows``)."""
+        Explicit pixels and the permuted batches without a plan go through ``hr_sample_train_batch(_fmt)``, everything else
+        through the plan's entry (``hr_sample_train_rows(_fmt)`` or ``hr_sample_train_mask_rows``)."""
         dev = self.device
         whole = ids_are_pixels or (ids is None and not self.replacement and self.subsample is None and
                                    self.importance is None)
@@ -459,19 +474,21 @@ class DeviceRayBatches:
         ptr = lambda t: t.data_ptr() if t is not None else None
         n_rows = C.c_int64(0)
         head = (self.cameras.data_ptr(), self.n_views, self.images.data_ptr(), self.height, self.width, self.c_in)
+        fmt = L.PIXEL_RGBA8 if self.rgba else L.PIXEL_RGB8
+        head_fmt = (*head[:3], fmt, *head[3:])
         # an explicit list is the whole batch; otherwise the entry shortens the epoch's last batch
         batch = (index, rows if ids is not None else self.batch_size, ptr(ids), coords.data_ptr(), rgb.data_ptr(),
                  weight.data_ptr(), ptr(pids))
         stream = torch.cuda.current_stream(dev).cuda_stream
         with torch.cuda.device(dev):
             if whole:
-                L.check(self._lib.hr_sample_train_batch(*head, self.seed, self.epoch, *batch, C.byref(n_rows), stream))
+                L.check(self._lib.hr_sample_train_batch_fmt(*head_fmt, self.seed, self.epoch, *batch, C.byref(n_rows), stream))
             else:
                 mode = L.SAMPLE_REPLACE if self.replacement else L.SAMPLE_PERMUTE
                 tail = (self.n_rows, mode, self.seed, self.epoch, *batch, ptr(tids), C.byref(n_rows), stream)
                 if self.importance is None:
-                    L.check(self._lib.hr_sample_train_rows(*head, self._view_start.data_ptr(), self._view_rule.data_ptr(),
-                                                           *tail))
+                    L.check(self._lib.hr_sample_train_rows_fmt(*head_fmt, self._view_start.data_ptr(),
+                                                               self._view_rule.data_ptr(), *tail))
                 else:
                     L.check(self._lib.hr_sample_train_mask_rows(*head, self._view_start.data_ptr(),
                                                                 self._view_slot.data_ptr(), self._block_start.data_ptr(),

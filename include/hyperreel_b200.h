@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define HR_ABI_VERSION 22
+#define HR_ABI_VERSION 23
 
 #define HR_MAX_GROUPS 4   /* ray-parameterisation groups feeding the sample net (ray.py:235-263) */
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
@@ -453,6 +453,28 @@ int hr_sample_train_mask_rows(const hr_camera* cameras, int32_t n_views, const u
                               int64_t batch_index, int64_t batch_size, const int64_t* table_rows, float* coords, float* rgb,
                               float* weight, int64_t* pixel_ids, int64_t* table_ids, int64_t* n_rows, void* stream);
 
+/* Pixel formats of uint8 images (ABI 23).  HR_PIXEL_RGB8: [.., 3] RGB.  HR_PIXEL_RGBA8: [.., 4] RGBA, the frames of the
+ * datasets whose get_rgb loads RGBA (datasets/donerf.py, catacaustics.py); where such an image is consumed as a colour, that
+ * colour is their get_rgb's composite over white, rgb * a + (1 - a) of the u8 / 255 values (T.ToTensor()), each of the
+ * multiply, subtract and add rounded on its own in fp32 (no FMA), as torch computes it on the CPU.  4-byte aligned. */
+#define HR_PIXEL_RGB8 0
+#define HR_PIXEL_RGBA8 1
+
+/* Training batches over images of either pixel format (ABI 23): as hr_sample_train_batch and hr_sample_train_rows, whose
+ * images are HR_PIXEL_RGB8; with HR_PIXEL_RGBA8, images is uint8 [n_views, height, width, 4] and each row's rgb is its
+ * pixel's composite over white.  Rays, order, draws, pixel and table ids are those of the RGB calls.  An unknown
+ * pixel_format, or RGBA images not 4-byte aligned, is refused.  (Keep-mask tables, hr_sample_train_mask_rows, are RGB only:
+ * the Immersive dataset's frames are RGB.) */
+int hr_sample_train_batch_fmt(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t pixel_format,
+                              int32_t height, int32_t width, int32_t c_in, uint64_t seed, int64_t epoch, int64_t batch_index,
+                              int64_t batch_size, const int64_t* order, float* coords, float* rgb, float* weight,
+                              int64_t* pixel_ids, int64_t* n_rows, void* stream);
+int hr_sample_train_rows_fmt(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t pixel_format,
+                             int32_t height, int32_t width, int32_t c_in, const int64_t* view_start, const int32_t* view_rule,
+                             int64_t n_table, int32_t mode, uint64_t seed, int64_t epoch, int64_t batch_index,
+                             int64_t batch_size, const int64_t* table_rows, float* coords, float* rgb, float* weight,
+                             int64_t* pixel_ids, int64_t* table_ids, int64_t* n_rows, void* stream);
+
 /* ---- the step after the path: 8-bit packing (SURVEY.md section 8(f) row f4) ----
  * Replaces: to8b(x) = (255 * clip(x, 0, 1)).astype(uint8) (utils/__init__.py:47) applied to the rendered frame before
  * it is written or displayed (nlf/__init__.py:857-891, utils/gui_utils.py:174-186).  Same as hr_render, but the fused
@@ -504,6 +526,12 @@ int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* ti
 int64_t hr_score_views_workspace_bytes(const hr_handle* h, int32_t n_views, int32_t height, int32_t width);
 int hr_score_views(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views, const uint8_t* gt, double* out,
                    void* workspace, int64_t workspace_bytes, void* stream);
+/* Ground truth of either pixel format (ABI 23): as hr_score_views, whose gt is HR_PIXEL_RGB8.  With HR_PIXEL_RGBA8, gt is
+ * DEVICE uint8 [n_views, height, width, 4] (4-byte aligned) and each view is scored against its composite over white
+ * (HR_PIXEL_RGBA8 above): bit for bit hr_image_metrics against that fp32 composite.  Same workspace.  An unknown
+ * pixel_format or a misaligned RGBA gt is refused. */
+int hr_score_views_fmt(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views, const uint8_t* gt,
+                       int32_t pixel_format, double* out, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- backward pass of the path (SURVEY.md section 8 row f1) ----
  * Replaces: what loss.backward() runs for the render path inside INRSystem.training_step (nlf/__init__.py:634-709): the
@@ -622,6 +650,19 @@ int64_t hr_resize_workspace_bytes(int32_t n, int32_t H0, int32_t W0, int32_t H, 
 int hr_resize_frames(const uint8_t* src, int32_t n, int32_t H0, int32_t W0, uint8_t* dst, int32_t H, int32_t W,
                      int64_t dst_row_stride, int32_t method, int32_t flags, void* workspace, int64_t workspace_bytes,
                      void* stream);
+
+/* RGBA frames (ABI 23): as hr_resize_workspace_bytes / hr_resize_frames for frames of pixel_format (HR_PIXEL_RGB8 gives the
+ * two calls above; HR_PIXEL_RGBA8 is uint8 [n, H0, W0, 4] -> [n, H, W, 4], dst_row_stride >= 4 * W).  RGBA as the datasets
+ * that load RGBA resize it (datasets/donerf.py, catacaustics.py): the Pillow methods resample the premultiplied RGBa image
+ * and convert back, as Image.resize does for an RGBA image on every call (premultiply MULDIV255(c, a); unpremultiply c for
+ * a of 0 or 255, else min(255, 255 * c / a)); cv2_area resamples the four channels independently, as OpenCV does.  The
+ * Pillow intermediate is premultiplied RGBa, 4 bytes per pixel.  HR_RESIZE_BGR reads BGRA.  cv2_linear is refused for RGBA,
+ * and so is an unknown pixel_format (-1 from hr_resize_workspace_bytes_fmt). */
+int64_t hr_resize_workspace_bytes_fmt(int32_t n, int32_t H0, int32_t W0, int32_t H, int32_t W, int32_t method,
+                                      int32_t pixel_format);
+int hr_resize_frames_fmt(const uint8_t* src, int32_t n, int32_t H0, int32_t W0, uint8_t* dst, int32_t H, int32_t W,
+                         int64_t dst_row_stride, int32_t method, int32_t flags, int32_t pixel_format, void* workspace,
+                         int64_t workspace_bytes, void* stream);
 
 /* Number of kernels hr_render launched since creation (bench.py's gpu_launches). */
 int64_t hr_launch_count(const hr_handle* h);
