@@ -142,14 +142,15 @@ __global__ void unpermute_heads(const float* __restrict__ src, float* __restrict
   }
 }
 
-__global__ void permute_heads(const float* __restrict__ src, float* __restrict__ dst, long long n, int S, int stride) {
-  // src [n][s*stride+c] (reference order) -> dst [n][c*S+s] (the kernels' channel-major rows)
-  long long total = n * (long long)S * stride;
+__global__ void permute_heads(const float* __restrict__ src, float* __restrict__ dst, long long n, int S, int stride, int ld) {
+  // src [n][s*stride+c] (reference order) -> dst [n][c*S+s] (the kernels' channel-major rows, ld >= S*stride apart; the
+  // columns past S*stride are zeroed)
+  long long total = n * (long long)ld;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    long long ray = i / (S * stride);
-    int rem = (int)(i % (S * stride));
+    long long ray = i / ld;
+    int rem = (int)(i % ld);
     int c = rem / S, s = rem % S;
-    dst[i] = src[ray * (long long)S * stride + s * stride + c];
+    dst[i] = rem < S * stride ? src[ray * (long long)S * stride + s * stride + c] : 0.0f;
   }
 }
 
@@ -302,6 +303,13 @@ int validate(const hr_config& c) {
   if (has_net && c.mlp_skip != -1 && (c.mlp_skip < 1 || c.mlp_skip > c.mlp_layers - 2)) return hr_fail("bad mlp_skip %d", c.mlp_skip);
   if (c.n_samples < 1 || c.n_samples > HR_MAX_SAMPLES) return hr_fail("unsupported n_samples %d (max %d)", c.n_samples, HR_MAX_SAMPLES);
   if (c.mlp_out != c.n_samples * c.head_stride) return hr_fail("mlp_out %d != S*head_stride %d", c.mlp_out, c.n_samples * c.head_stride);
+  if (c.mlp_mode == HR_MLP_BF16X3_TC) {
+    const int out = c.cascade && c.pre_samples > 0 ? c.mlp_out / c.pre_samples : c.mlp_out;
+    const int passes = c.mlp_layers - 1 + (out + c.mlp_width - 1) / c.mlp_width;
+    if (passes > HR_TC_MAX_PASSES)
+      return hr_fail("tensor-core sample net: %d passes of %d output columns, more than HR_TC_MAX_PASSES = %d", passes, c.mlp_width,
+                     HR_TC_MAX_PASSES);
+  }
   if (c.off_z < 0) return hr_fail("z_vals head is required");
   if ((c.isect_type == HR_ISECT_Z_PLANE || c.isect_type == HR_ISECT_DISTANCE) && c.n_z != 1) return hr_fail("z_plane / euclidean_distance need 1 z channel");
   if ((c.isect_type == HR_ISECT_SPHERE || c.isect_type == HR_ISECT_CYLINDER) && c.n_z != 4) return hr_fail("sphere / cylinder need 4 z channels");
@@ -705,8 +713,9 @@ static int launch_net(hr_handle* h, const SampleNet& net, const float* in, int64
 }
 
 // heads of n rays between the reference's order [n][s*stride+c] and the kernels' channel-major rows [n][c*S+s]
-static cudaError_t permute_heads_async(const hr_config& c, const float* src, float* dst, int64_t n, cudaStream_t st) {
-  permute_heads<<<grid_for(n * (long long)c.mlp_out), 256, 0, st>>>(src, dst, n, c.n_samples, c.head_stride);
+static cudaError_t permute_heads_async(const hr_config& c, const float* src, float* dst, int64_t n, cudaStream_t st, int ld = 0) {
+  if (ld == 0) ld = c.mlp_out;
+  permute_heads<<<grid_for(n * (long long)ld), 256, 0, st>>>(src, dst, n, c.n_samples, c.head_stride, ld);
   return cudaGetLastError();
 }
 
@@ -1603,7 +1612,7 @@ int hr_train_net_backward(hr_handle* h, const float* d_heads, int64_t n, const h
   if (workspace_bytes < (int64_t)t.total) return hr_fail("hr_train_net_backward: workspace too small (hr_train_net_workspace_bytes)");
   if (((uintptr_t)workspace & 255) != 0) return hr_fail("hr_train_net_backward: workspace must be 256-byte aligned");
   uint8_t* ws = (uint8_t*)workspace;
-  cudaError_t e = permute_heads_async(c, d_heads, (float*)(ws + t.dlast), n, st);
+  cudaError_t e = permute_heads_async(c, d_heads, (float*)(ws + t.dlast), n, st, t.ld_dlast);
   if (e == cudaSuccess) e = hr::train_net_backward(c, h->net.simt, n, out->weight, out->bias, ws, h->num_sms, st);
   if (e != cudaSuccess) return hr_fail("hr_train_net_backward: %s", cudaGetErrorString(e));
   h->launches += 1 + 3 * L;

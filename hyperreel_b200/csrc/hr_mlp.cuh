@@ -22,8 +22,7 @@ struct MlpSimtPack {
 
 // wgmma path (HR_MLP_BF16X3_TC): see hr_mlp_tc2.cu.  A "pass" is one accumulator's worth of output columns
 // (W = hidden width: a whole hidden layer, or W columns of the last layer); its weights are stored as n_chunks*2 k-step
-// images.
-#define HR_TC_MAX_PASSES 40  // 9 hidden layers + 28 last-layer parts (W = 128, S = 256 x 14 channels)
+// images.  At most HR_TC_MAX_PASSES passes (hyperreel_b200.h).
 struct TcPass {
   int layer;        // Linear layer index
   int n;            // output columns of this pass (128; a partial last-layer pass is zero padded)
@@ -53,7 +52,7 @@ cudaError_t launch_mlp_simt(const hr_config& cfg, const MlpSimtPack& pk, const f
 cudaError_t launch_mlp_tc2(const hr_config& cfg, const MlpTcPack& pk, const float* rays, float* heads, long long n,
                            int num_sms, cudaStream_t stream, float* rays_copy = nullptr);
 
-// Training net on the tensor cores (hr_mlp_train.cu).  The forward is mlp_tc2_kernel<W, SAVE = true>: it also writes the
+// Training net on the tensor cores (hr_mlp_train.cu).  The forward is mlp_tc2_kernel<W, SAVE = true, false>: it also writes the
 // encoded input enc [n][ld_enc] (zero padded past mlp_in) and hidden layer l's LeakyReLU output at act + l * act_stride,
 // [n][W], all fp32, and stores the heads in the reference's order.
 struct TrainSave {
@@ -66,10 +65,11 @@ cudaError_t launch_mlp_tc2_train(const hr_config& cfg, const MlpTcPack& pk, cons
                                  int num_sms, cudaStream_t stream, const TrainSave& sv);
 
 // Workspace of one training step of the net over n rays (byte offsets, each 256-byte aligned): the forward's saved
-// activations, the channel-major d heads, two [n][W] buffers for the hidden layers' dY, the dW GEMM's split-K partials.
+// activations, the channel-major d heads [n][ld_dlast] (mlp_out rounded up to 4, zero pad columns: the GEMM loaders read
+// float4 rows), two [n][W] buffers for the hidden layers' dY, the dW GEMM's split-K partials.
 struct TrainNetLayout {
   size_t enc, act, act_stride, dlast, dy[2], part, dbpart, total;
-  int ld_enc;
+  int ld_enc, ld_dlast;
 };
 TrainNetLayout train_net_layout(const hr_config& c, long long n, int num_sms);
 // d_heads_cm [n][mlp_out] channel-major (inside the workspace at dlast) -> every layer's dW / db into weight[l] / bias[l]

@@ -25,7 +25,8 @@
 //   * the encoded input X (rows of both warpgroups, read by layer 0 and the skip layer) has the same two kinds of
 //     signal (NB_XW, NB_XR); the next tile is encoded as soon as both warpgroups are past the last pass that reads X.
 // The last layer's columns go from the accumulators (+ bias) straight to the heads scratch in global memory, 4 consecutive
-// columns per 16-byte store; the hidden epilogues write the activation operand with stmatrix.
+// columns per 16-byte store (NARROW: 8- or 4-byte stores, for rows that are not 16-byte aligned); the hidden epilogues write
+// the activation operand with stmatrix.
 //
 // SAVE (the training forward, hr_mlp_train.cu): the same arithmetic, plus every fp32 value the epilogues split goes to global
 // memory as well -- the encoded input (sv.enc) and each hidden layer's LeakyReLU output (sv.act) -- and the heads are stored
@@ -81,7 +82,9 @@ constexpr int NB_XR = 9;   // g's wgmmas that read the encoded input have retire
 
 }  // namespace tc2
 
-template <int W, bool SAVE>
+// NARROW: the heads rows of the render net (SAVE = false) are stored with 8- or 4-byte stores, each column guarded, for an
+// mlp_out that is not a multiple of 4 or a heads pointer that is not 16-byte aligned (launch_mlp_tc2 picks it).
+template <int W, bool SAVE, bool NARROW>
 __global__ void __launch_bounds__(tc2::NTHREADS, 1)
 mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ MlpTcPack pk, const float* __restrict__ rays,
                float* __restrict__ heads, long long n_rays, float* __restrict__ rays_copy, const TrainSave sv) {
@@ -355,19 +358,44 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
 #pragma unroll
               for (int j = 0; j < WH / 8; ++j) {
                 const int c = col0 + 8 * j + q2;
-                if (P.out_col0 + c < cfg.mlp_out) {  // mlp_out is a multiple of 4: the pair is in or out as a whole
+                if (P.out_col0 + c < cfg.mlp_out) {  // each column of the pair is guarded: mlp_out may be odd
                   const float2 b = __ldg(reinterpret_cast<const float2*>(bias + c));
                   // channel-major column c*S+s -> the reference's s*stride+c
                   const int c0 = P.out_col0 + c, c1 = c0 + 1, S = cfg.n_samples;
                   row[(c0 % S) * cfg.head_stride + c0 / S] = acc[m][4 * j + 2 * h] + b.x;
-                  row[(c1 % S) * cfg.head_stride + c1 / S] = acc[m][4 * j + 2 * h + 1] + b.y;
+                  if (c1 < cfg.mlp_out) row[(c1 % S) * cfg.head_stride + c1 / S] = acc[m][4 * j + 2 * h + 1] + b.y;
                 }
               }
             }
+        } else if constexpr (NARROW) {
+          // any mlp_out: a lane's column pair is one 8-byte store when every row starts 8-byte aligned, else two 4-byte
+          // stores; a column past mlp_out is dropped on its own
+          const bool pairs = (cfg.mlp_out % 2) == 0 && (reinterpret_cast<uintptr_t>(heads) & 7) == 0;
+#pragma unroll
+          for (int j = 0; j < WH / 8; ++j) {
+            const int c = col0 + 8 * j + q2, c0 = P.out_col0 + c;
+            const float2 b = __ldg(reinterpret_cast<const float2*>(bias + c));
+#pragma unroll
+            for (int m = 0; m < 2; ++m)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const long long ray = tile * BM + 64 * m + rowq + 8 * h;
+                if (ray >= n_rays || c0 >= cfg.mlp_out) continue;
+                float* dst = heads + ray * cfg.mlp_out + c0;
+                const float v0 = acc[m][4 * j + 2 * h] + b.x, v1 = acc[m][4 * j + 2 * h + 1] + b.y;
+                if (pairs) {
+                  *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+                } else {
+                  dst[0] = v0;
+                  if (c0 + 1 < cfg.mlp_out) dst[1] = v1;
+                }
+              }
+          }
         } else {
           // Lanes 2i and 2i + 1 hold 4 consecutive columns of the same row in column groups j and j + 1: they swap one pair
           // so that each stores 4 consecutive columns with one 16-byte store (the even lane in group j, the odd one in
-          // group j + 1).  mlp_out is a multiple of 4, so the 4 columns are in or out as a whole.
+          // group j + 1).  launch_mlp_tc2 runs this store only when mlp_out is a multiple of 4, so the 4 columns are in or
+          // out as a whole.
           const bool odd = (lane & 1) != 0;
 #pragma unroll
           for (int jp = 0; jp < WH / 16; ++jp) {
@@ -449,8 +477,11 @@ int pack_mlp_tc2(SampleNet& net, const float* const* w_dev, const float* const* 
     np_.wpack = wp; np_.bias = bp;
     alloc_bytes = bytes; alloc_bias = bias_off;
     // opt in to the 224 KB of dynamic shared memory once per (handle, device)
-    e = (W == 256) ? cudaFuncSetAttribute(mlp_tc2_kernel<256, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::SMEM_BYTES)
-                   : cudaFuncSetAttribute(mlp_tc2_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::SMEM_BYTES);
+    for (int narrow = 0; narrow < 2 && e == cudaSuccess; ++narrow) {
+      auto kern = (W == 256) ? (narrow ? mlp_tc2_kernel<256, false, true> : mlp_tc2_kernel<256, false, false>)
+                             : (narrow ? mlp_tc2_kernel<128, false, true> : mlp_tc2_kernel<128, false, false>);
+      e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::SMEM_BYTES);
+    }
     if (e != cudaSuccess) return hr_fail("cudaFuncSetAttribute(mlp_tc2_kernel): %s", cudaGetErrorString(e));
   } else {
     np_.wpack = pk.wpack; np_.bias = pk.bias;
@@ -488,27 +519,24 @@ void free_mlp_tc2(SampleNet& net) {
 
 cudaError_t launch_mlp_tc2(const hr_config& cfg, const MlpTcPack& pk, const float* rays, float* heads, long long n, int num_sms,
                            cudaStream_t stream, float* rays_copy) {
-  // the epilogue stores column pairs and drops a pair past mlp_out as a whole
-  if ((cfg.mlp_out % 4) != 0 || ((uintptr_t)heads % 16) != 0) return cudaErrorInvalidValue;
   long long tiles = (n + tc::BM - 1) / tc::BM;
   int grid = (int)(tiles < num_sms ? tiles : num_sms);
   if (grid < 1) grid = 1;
-  if (cfg.mlp_width == 256)
-    mlp_tc2_kernel<256, false><<<grid, tc2::NTHREADS, tc2::SMEM_BYTES, stream>>>(cfg, pk, rays, heads, n, rays_copy, TrainSave{});
-  else if (cfg.mlp_width == 128)
-    mlp_tc2_kernel<128, false><<<grid, tc2::NTHREADS, tc2::SMEM_BYTES, stream>>>(cfg, pk, rays, heads, n, rays_copy, TrainSave{});
-  else
-    return cudaErrorInvalidValue;
+  // the 16-byte heads stores need every row to start 16-byte aligned; any other row takes the narrow stores
+  const bool narrow = (cfg.mlp_out % 4) != 0 || ((uintptr_t)heads % 16) != 0;
+  auto kern = cfg.mlp_width == 256 ? (narrow ? mlp_tc2_kernel<256, false, true> : mlp_tc2_kernel<256, false, false>)
+                                   : (narrow ? mlp_tc2_kernel<128, false, true> : mlp_tc2_kernel<128, false, false>);
+  if (cfg.mlp_width != 256 && cfg.mlp_width != 128) return cudaErrorInvalidValue;
+  kern<<<grid, tc2::NTHREADS, tc2::SMEM_BYTES, stream>>>(cfg, pk, rays, heads, n, rays_copy, TrainSave{});
   return cudaGetLastError();
 }
 
 cudaError_t launch_mlp_tc2_train(const hr_config& cfg, const MlpTcPack& pk, const float* rays, float* heads, long long n,
                                  int num_sms, cudaStream_t stream, const TrainSave& sv) {
-  if ((cfg.mlp_out % 4) != 0) return cudaErrorInvalidValue;
   long long tiles = (n + tc::BM - 1) / tc::BM;
   int grid = (int)(tiles < num_sms ? tiles : num_sms);
   if (grid < 1) grid = 1;
-  auto kern = cfg.mlp_width == 256 ? mlp_tc2_kernel<256, true> : mlp_tc2_kernel<128, true>;
+  auto kern = cfg.mlp_width == 256 ? mlp_tc2_kernel<256, true, false> : mlp_tc2_kernel<128, true, false>;
   if (cfg.mlp_width != 256 && cfg.mlp_width != 128) return cudaErrorInvalidValue;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::SMEM_BYTES);
   if (e != cudaSuccess) return e;

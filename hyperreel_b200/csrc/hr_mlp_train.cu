@@ -263,7 +263,8 @@ TrainNetLayout train_net_layout(const hr_config& c, long long n, int num_sms) {
   size_t off = 0;
   t.enc = off; off += seg(n * t.ld_enc);
   t.act = off; t.act_stride = seg(n * W) / 4; off += (size_t)(c.mlp_layers - 1) * seg(n * W);
-  t.dlast = off; off += seg(n * c.mlp_out);
+  t.ld_dlast = (c.mlp_out + 3) / 4 * 4;
+  t.dlast = off; off += seg(n * t.ld_dlast);
   t.dy[0] = off; off += seg(n * W);
   t.dy[1] = off; off += seg(n * W);
   // split-K: at most 2 CTAs per SM of 128 x 128 partial tiles (train_net_backward picks the split count)
@@ -284,14 +285,16 @@ cudaError_t train_net_backward(const hr_config& c, const MlpSimtPack& simt, long
   if (e == cudaSuccess) e = cudaFuncSetAttribute(train_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
   if (e != cudaSuccess) return e;
 
-  // dW[rows of dy][col0 .. col0 + n_valid) += dy^T x over all rays, x [n][ldx] with ldx >= n_rows
-  auto dw_gemm = [&](const float* dy, int out_l, const float* x, int ldx, int n_valid, float* dw, int ld_dw, int col0,
+  // dW[rows of dy][col0 .. col0 + n_valid) += dy^T x over all rays, dy [n][ld_dy] (out_l rows of dW, then zero pad columns up
+  // to ld_dy, a multiple of 4: the GEMM computes their rows too, the reduction writes back the out_l real ones), x [n][ldx]
+  // with ldx >= n_rows
+  auto dw_gemm = [&](const float* dy, int out_l, int ld_dy, const float* x, int ldx, int n_valid, float* dw, int ld_dw, int col0,
                      float* db, int perm_S) -> cudaError_t {
     Gemm g{};
-    g.a = dy; g.lda = out_l; g.m_rows = out_l;
+    g.a = dy; g.lda = ld_dy; g.m_rows = ld_dy;
     g.b = x; g.ldb = ldx; g.n_rows = ldx;
     g.k_len = n;
-    const int tm = cdiv(out_l, 128), tn = cdiv(ldx, BN), kbs = cdiv(n, BK);
+    const int tm = cdiv(ld_dy, 128), tn = cdiv(ldx, BN), kbs = cdiv(n, BK);
     int splits = (2 * num_sms) / (tm * tn);
     if (splits < 1) splits = 1;
     if (splits > kbs) splits = kbs > 0 ? kbs : 1;
@@ -307,23 +310,23 @@ cudaError_t train_net_backward(const hr_config& c, const MlpSimtPack& simt, long
 
   for (int l = L - 1; l >= 0; --l) {
     const bool last = (l == L - 1), skip = (l == c.mlp_skip);
-    const int out_l = last ? c.mlp_out : W;
+    const int out_l = last ? c.mlp_out : W, ld_dy = last ? t.ld_dlast : W;
     const float* dy = last ? fp(t.dlast) : fp(t.dy[(L - 2 - l) & 1]);
     const int in_l = l == 0 ? c.mlp_in : (skip ? c.mlp_in + W : W);
     const int perm_S = last ? c.n_samples : 0;
     if (l == 0 || skip) {  // encoded-input columns (and db)
-      e = dw_gemm(dy, out_l, fp(t.enc), t.ld_enc, c.mlp_in, weight[l], in_l, 0, bias[l], perm_S);
+      e = dw_gemm(dy, out_l, ld_dy, fp(t.enc), t.ld_enc, c.mlp_in, weight[l], in_l, 0, bias[l], perm_S);
       if (e != cudaSuccess) return e;
     }
     if (l > 0) {
       const float* a_prev = act + (size_t)(l - 1) * t.act_stride;
-      e = dw_gemm(dy, out_l, a_prev, W, W, weight[l], in_l, skip ? c.mlp_in : 0, skip ? nullptr : bias[l], perm_S);
+      e = dw_gemm(dy, out_l, ld_dy, a_prev, W, W, weight[l], in_l, skip ? c.mlp_in : 0, skip ? nullptr : bias[l], perm_S);
       if (e != cudaSuccess) return e;
       // dY_{l-1} = (dY_l W_l[:, hidden]) * leaky'(a_{l-1})
       Gemm g{};
-      g.a = dy; g.lda = out_l; g.m_rows = n;
+      g.a = dy; g.lda = ld_dy; g.m_rows = n;  // the zero pad columns of d heads meet the zero pad columns of Wt
       g.b = simt.Wt[l] + (size_t)(skip ? simt.in_pad : 0) * simt.Np[l]; g.ldb = simt.Np[l]; g.n_rows = W;
-      g.k_len = out_l;
+      g.k_len = ld_dy;
       g.act = a_prev; g.out = fp(t.dy[(L - 1 - l) & 1]); g.ld_out = W; g.slope = c.leaky_slope;
       train_gemm_kernel<false><<<dim3(cdiv(n, 128), W / BN, 1), NT, SMEM_BYTES, st>>>(g);
       e = cudaGetLastError();

@@ -16,6 +16,7 @@ HR_MAX_GROUPS = 4
 HR_MAX_LAYERS = 10
 HR_MAX_SAMPLES = 256
 HR_MAX_PEERS = 8
+HR_TC_MAX_PASSES = 40
 
 ACT_IDENTITY, ACT_SIGMOID, ACT_TANH = 0, 1, 2
 PARAM_IDENTITY, PARAM_TWO_PLANE, PARAM_PLUECKER = 0, 1, 2

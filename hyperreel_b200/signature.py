@@ -180,6 +180,11 @@ class Signature:
         return self.cfg.n_samples
 
 
+def tc_passes(width: int, depth: int, n_out: int) -> int:
+    """Passes of W output columns the tensor-core sample net runs (hr_mlp_tc2.cu): one per hidden layer, then the last layer's."""
+    return depth - 1 + (n_out + width - 1) // width
+
+
 def lower(model_cfg, dataset: dict, cur_iter: int = RENDER_ITER, iters_per_epoch: Optional[int] = None,
           mlp_mode: int = L.MLP_BF16X3_TC, ease: bool = False) -> Signature:
     """model cfg (reference schema) + dataset facts -> Signature / hr_config.  ``ease``: open EaseValue windows lower to
@@ -398,6 +403,9 @@ def lower(model_cfg, dataset: dict, cur_iter: int = RENDER_ITER, iters_per_epoch
     if zero_net:
         c.mlp_mode = L.MLP_ZERO
     c.mlp_in, c.mlp_width, c.mlp_layers = mlp_in, W, depth
+    if c.mlp_mode == L.MLP_BF16X3_TC and tc_passes(W, depth, shapes[-1][0]) > L.HR_TC_MAX_PASSES:
+        raise UnsupportedPipeline(f"tensor-core sample net of {tc_passes(W, depth, shapes[-1][0])} passes of {W} output columns "
+                                  f"(more than HR_TC_MAX_PASSES = {L.HR_TC_MAX_PASSES}): use mlp_mode 'fp32'")
 
     # ------------------------------------------------------------------ heads (ray.py:331-337)
     offs: Dict[str, int] = {}

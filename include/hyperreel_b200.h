@@ -31,6 +31,10 @@ extern "C" {
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
 #define HR_MAX_SAMPLES 256 /* z_channels S (per-ray sample primitives) */
 #define HR_MAX_PEERS 8    /* destination buffers of hr_render_scatter (GPUs of one NVSwitch domain) */
+/* Passes of an HR_MLP_BF16X3_TC sample net: (mlp_layers - 1) hidden layers + ceil(last layer's outputs / mlp_width).  The
+ * table is a kernel parameter; 40 passes hold every shape at width 256 and, at width 128, depth 10 with S * head_stride up
+ * to 3968 (S = 256 x 15 channels).  hr_create refuses a tensor-core net that needs more (the fp32 net has no such limit). */
+#define HR_TC_MAX_PASSES 40
 
 /* Activation y = f(x*inner_fac + shift) * outer_fac  (nlf/activations.py:53-69,121-137,163-178).
  * EaseValue (activations.py:462-496) wrapped around it: while its window is open (eased != 0) the result is blended with the
@@ -584,7 +588,7 @@ int hr_grad_read(hr_handle* h, const hr_grads* out, void* stream);
  * The weights are those of the last hr_upload.  Needs a handle with mlp_mode HR_MLP_BF16X3_TC; cascaded pipelines and zero
  * nets are refused (hr_last_error).
  * Workspace (hr_train_net_workspace_bytes, 256-byte aligned): fp32 encoded input [n, mlp_in rounded up to 16], fp32
- * activations [mlp_layers - 1][n, mlp_width], d heads [n, mlp_out], two [n, mlp_width] dY buffers and the split-K partials
+ * activations [mlp_layers - 1][n, mlp_width], d heads [n, mlp_out rounded up to 4], two [n, mlp_width] dY buffers and the split-K partials
  * (2 x SMs x 128 x 128 floats) -- 0.62 GB at 65,536 rays on the Technicolor
  * shape (6 layers of width 256, 9 input features, 480 outputs). */
 int64_t hr_train_net_workspace_bytes(const hr_handle* h, int64_t n_rays);

@@ -33,6 +33,7 @@ FACE_ULPS = 4.0  # how far (fp32 ulps) mask_moved moves the AABB faces
 TOL_HEADS = 1e-3  # of max |d heads| (fp64)
 TOL_TABLE = 2e-3  # of max |d table| (fp64)
 MAX_ILL = 0.01  # fraction of rays on which the fp32 reference itself is off by more than TOL_HEADS
+TIE_ULPS = 16.0  # sort keys this close (fp32 ulps of max(|key|, 1)) have no defined order
 TOL_ADD = 2e-4  # additivity over a split of the batch, of max |d table|
 
 
@@ -127,7 +128,8 @@ def oracle_grads(case, heads, d_rgb, white, dtype):
     rgb, leaves = orc.render_with_grad(case.rays.clone(), clamp=False, white_bg=white, heads_leaf=True)
     (rgb * d_rgb.to(dtype)).sum().backward()
     grads = {k: v.grad for k, v in leaves.items() if k != "_mlp_out" and v.grad is not None}
-    return rgb.detach(), leaves["_mlp_out"].grad, grads, {k: stages[k].detach() for k in ("weights", "points", "distances")}
+    return rgb.detach(), leaves["_mlp_out"].grad, grads, {k: stages[k].detach() for k in ("weights", "points", "distances",
+                                                                                          "unsorted_distances") if k in stages}
 
 
 def _oracles(case, heads, d_rgb, white, eased):
@@ -182,10 +184,27 @@ BATCH_CASES = [
 @pytest.mark.parametrize("name,n,white", BATCH_CASES, ids=[f"{c}-{n}-{'white' if w else 'black'}" for c, n, w in BATCH_CASES])
 def test_render_backward_matches_fp64_at_batch_size(name, n, white):
     n = n_multi() if n == "multi" else n
-    eased = name.startswith("ease_")
     if n == n_multi():
         assert n > 32 * _sms()  # every warp of the backward walks several rays
-    case = _case(name, n)
+    check_render_heads(_case(name, n), white, name.startswith("ease_"), f"{name} n={n} white={white}")
+
+
+def tied_rays(keys):
+    """Rays two of whose sort keys lie within TIE_ULPS fp32 ulps of max(|key|, 1) of each other but are not equal: their order
+    is decided by the last bits of the arithmetic, and with it which of the two samples each sorted slot's gradient goes back
+    to.  (Equal keys -- masked samples at t = 0, samples that miss the same primitive -- are the same value on both sides.)"""
+    k = torch.sort(keys, dim=-1).values
+    gap = k[:, 1:] - k[:, :-1]
+    tie = (gap > 0.0) & (gap <= TIE_ULPS * torch.finfo(torch.float32).eps * k[:, 1:].abs().clamp(min=1.0))
+    return tie.any(-1).nonzero().flatten()
+
+
+def check_render_heads(case, white, eased, label, backward=True, few_samples=False, ties_aside=False):
+    """hr_render_heads on the fixed heads against the fp64 oracle and, with `backward`, hr_render_backward against fp64
+    autograd, with the rules below.  `few_samples`: one or two samples per ray, where most rays may be transparent and a
+    density table's gradient may vanish exactly (alpha = 1 whatever the density, on a ray's last sample).  `ties_aside`: rays
+    with tied sort keys (tied_rays) are left out of the backward comparison like the rays that straddle the sample mask."""
+    n = case.rays.shape[0]
     heads = fixed_heads(case)
     d_rgb = torch.randn(n, 3, generator=torch.Generator().manual_seed(n + 17))
     (rgb64, dh64, g64, st64), (rgb32, dh32, g32, _) = _oracles(case, heads, d_rgb, white, eased)
@@ -205,12 +224,19 @@ def test_render_backward_matches_fp64_at_batch_size(name, n, white):
     mismatch = (rgb_err > TOL_RGB).nonzero().flatten()
     for i in mismatch.tolist():
         moved = min(float((rgb[i].cpu().double() - m).abs().max()) for m in mask_moved(case, heads, i, white, eased))
-        print(f"\n[{name} n={n} white={white}] ray {i} straddles the sample mask: {rgb[i].tolist()} vs {rgb64[i].tolist()}, "
+        print(f"\n[{label}] ray {i} straddles the sample mask: {rgb[i].tolist()} vs {rgb64[i].tolist()}, "
               f"{moved:.2e} from the reference with the AABB moved")
         assert moved <= TOL_RGB, f"ray {i} is off the reference by {float(rgb_err[i])}, and not by a sample on an AABB face"
         alone = model._render_heads(rays[i:i + 1].contiguous(), heads[i:i + 1].cuda(), False, white)
         assert torch.equal(alone[0], rgb[i]), f"ray {i} renders differently alone"
     assert len(mismatch) <= n // MISMATCH_RAYS, f"{len(mismatch)} rays off the reference by up to {float(rgb_err.max())}"
+    if not backward:
+        return
+    if ties_aside:
+        tied = tied_rays(st64["unsorted_distances"])
+        print(f"\n[{label}] {len(tied)} rays with tied sort keys left out of the backward comparison")
+        assert len(tied) <= MAX_ILL * n, f"{len(tied)} of {n} rays have tied sort keys"
+        mismatch = torch.cat([mismatch, tied])
     if len(mismatch):
         d_rgb[mismatch] = 0.0
         (rgb64, dh64, g64, st64), (rgb32, dh32, g32, _) = _oracles(case, heads, d_rgb, white, eased)
@@ -218,7 +244,7 @@ def test_render_backward_matches_fp64_at_batch_size(name, n, white):
     d_heads, grads = model._render_backward(rays, heads.cuda(), d_rgb.cuda(), False, white)
     names = grad_names(render)
     assert len(names) == len(grads)
-    assert float((acc > 0.5).float().mean()) >= 0.25, "the case is nearly transparent"
+    assert few_samples or float((acc > 0.5).float().mean()) >= 0.25, "the case is nearly transparent"
 
     # d heads, per ray
     scale = float(dh64.abs().max())
@@ -231,7 +257,7 @@ def test_render_backward_matches_fp64_at_batch_size(name, n, white):
     nw = bwd_warps(n)
     first, later = bad[bad < nw].tolist(), bad[bad >= nw].tolist()
     well_frac = float((err[~ill] / (TOL_HEADS * scale)).max()) if bool((~ill).any()) else 0.0
-    print(f"\n[{name} n={n} white={white}] ill-conditioned rays {int(ill.sum())}/{n}, "
+    print(f"\n[{label}] ill-conditioned rays {int(ill.sum())}/{n}, "
           f"largest well-conditioned d heads error {well_frac:.3f} of the tolerance")
     assert not first and not later, (f"d heads: {len(first)} failing rays of a warp's first round (first {first[:5]}), "
                                      f"{len(later)} of later rounds (first {later[:5]})")
@@ -245,6 +271,9 @@ def test_render_backward_matches_fp64_at_batch_size(name, n, white):
         assert k in g64, k
         ref, ref32 = g64[k], g32[k].double()
         tscale = float(ref.abs().max())
+        if few_samples and tscale == 0.0:
+            assert float(g.abs().max()) == 0.0, k
+            continue
         assert tscale > 0.0, k
         assert float(g.abs().max()) > 0.0, k
         diff = (g.cpu().double() - ref).abs()

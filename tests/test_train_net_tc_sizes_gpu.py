@@ -64,7 +64,12 @@ def _fp64_backward(model, enc_k, acts, d_heads):
 
 
 def _check(name, n):
-    case = _case(name, n)
+    check_case(_case(name, n), f"{name} n={n}")
+
+
+def check_case(case, label):
+    """The training forward and backward of `case`'s net on its rays against the fp64 references (module docstring)."""
+    n = case.rays.shape[0]
     model = _model(case)
     rays = case.rays.cuda()
     model._ensure_uploaded(rays.device)
@@ -89,7 +94,7 @@ def _check(name, n):
         worst = max(worst, float(ratio.max()))
         assert float(ratio.max()) <= 1.0, (f"{what}: {int((ratio > 1).sum())} entries out of tolerance, worst "
                                            f"{float(ratio.max()):.2f} of it")
-    print(f"\n[{name} n={n}] largest error {worst:.3f} of the bound; largest bound per weight, as a fraction of max |ref|: "
+    print(f"\n[{label}] largest error {worst:.3f} of the bound; largest bound per weight, as a fraction of max |ref|: "
           + " ".join(f"{x:.2g}" for x in widths[0::2]))
     # and the reference of tests/test_train_net_tc_gpu.py (activations recomputed in fp64) to its tolerance, which is the
     # tighter one on the largest entries of a large batch
