@@ -68,11 +68,11 @@ def _case(name, n):
     return case
 
 
-def _render(case, eased):
+def _render(case, eased, mlp_mode="fp32"):
     if not eased:
-        return make_render(case).cuda()
+        return make_render(case, mlp_mode=mlp_mode).cuda()
     model = hb.LightfieldModel(case.model_cfg, dataset=case.dataset, iters_per_epoch=ITERS_PER_EPOCH, ease="reference",
-                               mlp_mode="fp32")
+                               mlp_mode=mlp_mode)
     render = hb.RenderLightfield(model, None, case.model_cfg.render, net_chunk=1 << 20)
     render.load_state_dict(case.state_dict, strict=False)
     render.cuda().eval()
