@@ -1118,10 +1118,9 @@ int64_t hr_score_views_workspace_bytes(const hr_handle* h, int32_t n_views, int3
 // one metrics launch on its own stream.  Cross-stream order comes from events: a frame begun by the previous sub-batch (the
 // other stream) is scored after that sub-batch's render, and a ring frame is rendered again only after the launch that
 // scored its previous frame.  Each stream runs its sub-batches in order, so its slot, window and partials are reused safely.
-// gt of pixel_format (HR_PIXEL_*); fn names the entry point in refusals
-static int score_views(const char* fn, hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views,
-                       const uint8_t* gt, int32_t pixel_format, double* out, void* workspace, int64_t workspace_bytes,
-                       void* stream) {
+int hr_score_views(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views, const uint8_t* gt,
+                   int32_t pixel_format, double* out, void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* fn = "hr_score_views";
   if (!h || !cameras || !times || !gt || !out || !workspace) return hr_fail("%s: null argument", fn);
   if (!h->uploaded) return hr_fail("%s: parameters not uploaded", fn);
   if (n_views < 1) return hr_fail("%s: n_views must be >= 1, got %d", fn, n_views);
@@ -1134,9 +1133,8 @@ static int score_views(const char* fn, hr_handle* h, const hr_camera* cameras, c
   if (check_frames(fn, cameras, times, n_views, &mixed)) return 1;
   if (((uintptr_t)out & 7) != 0) return hr_fail("%s: out must be 8-byte aligned", fn);
   if (((uintptr_t)workspace & 15) != 0) return hr_fail("%s: workspace must be 16-byte aligned", fn);
-  if (pixel_format != HR_PIXEL_RGB8 && pixel_format != HR_PIXEL_RGBA8)
-    return hr_fail("%s: unknown pixel format %d", fn, pixel_format);
-  const int gt_px = pixel_format == HR_PIXEL_RGBA8 ? 4 : 3;  // bytes per ground-truth pixel
+  const int gt_px = hr::pixel_bytes(pixel_format);  // bytes per ground-truth pixel
+  if (!gt_px) return hr_fail("%s: unknown pixel format %d", fn, pixel_format);
   if (gt_px == 4 && ((uintptr_t)gt & 3) != 0) return hr_fail("%s: RGBA gt must be 4-byte aligned", fn);
   if (workspace_bytes < lay.total)
     return hr_fail("%s: workspace too small (%lld < %lld)", fn, (long long)workspace_bytes, (long long)lay.total);
@@ -1233,17 +1231,6 @@ static int score_views(const char* fn, hr_handle* h, const hr_camera* cameras, c
   }
   for (cudaEvent_t ev : evs) cudaEventDestroy(ev);
   return rc;
-}
-
-int hr_score_views(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views, const uint8_t* gt, double* out,
-                   void* workspace, int64_t workspace_bytes, void* stream) {
-  return score_views("hr_score_views", h, cameras, times, n_views, gt, HR_PIXEL_RGB8, out, workspace, workspace_bytes, stream);
-}
-
-int hr_score_views_fmt(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views, const uint8_t* gt,
-                       int32_t pixel_format, double* out, void* workspace, int64_t workspace_bytes, void* stream) {
-  return score_views("hr_score_views_fmt", h, cameras, times, n_views, gt, pixel_format, out, workspace, workspace_bytes,
-                     stream);
 }
 
 // the device's view of a pinned (device-addressable) host buffer, or null

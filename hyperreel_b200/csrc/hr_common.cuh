@@ -118,4 +118,23 @@ __device__ __forceinline__ float intersect_axis_plane(float z, float o, float d)
   return __fdiv_rn(__fsub_rn(z, o), dg);
 }
 
+// Bytes per pixel of an HR_PIXEL_* format, 0 for an unknown one
+__host__ __device__ inline int pixel_bytes(int32_t pixel_format) {
+  return pixel_format == HR_PIXEL_RGB8 ? 3 : pixel_format == HR_PIXEL_RGBA8 ? 4 : 0;
+}
+
+// A uint8 channel as a colour, u8 / 255 correctly rounded (T.ToTensor()).  T is the type the byte was loaded as: the
+// conversion instruction follows it.
+template <class T>
+__device__ __forceinline__ float u8_unit(T v) { return __fdiv_rn((float)v, 255.0f); }
+
+// Channel ch (0..2) of the RGBA pixel q (little-endian, alpha in the top byte) composited over white, as the RGBA datasets'
+// get_rgb computes it on the CPU: c * a + (1 - a) of the u8 / 255 values, each operation rounded on its own (no FMA).
+// Training colours and held-out scores both read RGBA ground truth through this, so they agree bit for bit.
+__device__ __forceinline__ float rgba_over_white(uint32_t q, int ch) {
+  const float a = u8_unit(q >> 24);
+  const float c = u8_unit((q >> (8 * ch)) & 0xffu);
+  return __fadd_rn(__fmul_rn(c, a), __fsub_rn(1.0f, a));
+}
+
 }  // namespace hr

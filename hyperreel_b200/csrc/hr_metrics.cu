@@ -69,19 +69,16 @@ __device__ __forceinline__ void block_sum2(double& a, double& b, double (*red)[M
 }
 
 __device__ __forceinline__ float load_gt(const float* p) { return __ldg(p); }
-__device__ __forceinline__ float load_gt(const uint8_t* p) { return __fdiv_rn((float)__ldg(p), 255.0f); }
+__device__ __forceinline__ float load_gt(const uint8_t* p) { return hr::u8_unit(__ldg(p)); }
 
 // One RGBA uint8 pixel, loaded whole
 struct __align__(4) Rgba8 {
   uint8_t v[4];
 };
 
-// Channel ch of an RGBA pixel composited over white, as get_rgb: c * a + (1 - a), c and a u8 / 255
+// Channel ch of an RGBA pixel composited over white
 __device__ __forceinline__ float load_gt(const Rgba8* p, int ch) {
-  const uint32_t q = __ldg(reinterpret_cast<const unsigned int*>(p));
-  const float a = __fdiv_rn((float)(q >> 24), 255.0f);
-  const float c = __fdiv_rn((float)((q >> (8 * ch)) & 0xffu), 255.0f);
-  return __fadd_rn(__fmul_rn(c, a), __fsub_rn(1.0f, a));
+  return hr::rgba_over_white(__ldg(reinterpret_cast<const unsigned int*>(p)), ch);
 }
 
 template <typename GtT>

@@ -385,18 +385,6 @@ bool make_plan(const char* fn, int32_t n, int32_t H0, int32_t W0, int32_t H, int
   return true;
 }
 
-// channels per pixel of an HR_PIXEL_* format, 0 for an unknown one
-int format_channels(int32_t pixel_format) {
-  return pixel_format == HR_PIXEL_RGB8 ? 3 : pixel_format == HR_PIXEL_RGBA8 ? 4 : 0;
-}
-
-int64_t workspace_bytes(const char* fn, int32_t n, int32_t H0, int32_t W0, int32_t H, int32_t W, int32_t method, int kC) {
-  Plan p;
-  char msg[256];
-  if (kC == 0 || !make_plan(fn, n, H0, W0, H, W, method, kC, p, msg, sizeof msg)) return -1;
-  return (int64_t)(p.tab_bytes + p.tmp_bytes);
-}
-
 template <int kC>
 cudaError_t launch_plan(const Plan& p, const uint8_t* src, int32_t n, int32_t H0, int32_t W0, uint8_t* dst, int32_t H,
                         int32_t W, int64_t dst_row_stride, int swap, char* ws, cudaStream_t st) {
@@ -449,12 +437,24 @@ cudaError_t launch_plan(const Plan& p, const uint8_t* src, int32_t n, int32_t H0
   return e;
 }
 
-int resize_frames(const char* fn, const uint8_t* src, int32_t n, int32_t H0, int32_t W0, uint8_t* dst, int32_t H, int32_t W,
-                  int64_t dst_row_stride, int32_t method, int32_t flags, int32_t pixel_format, void* workspace,
-                  int64_t workspace_bytes, void* stream) {
+}  // namespace
+
+extern "C" int64_t hr_resize_workspace_bytes(int32_t n, int32_t H0, int32_t W0, int32_t H, int32_t W, int32_t method,
+                                             int32_t pixel_format) {
+  const int kC = hr::pixel_bytes(pixel_format);
+  Plan p;
+  char msg[256];
+  if (kC == 0 || !make_plan("hr_resize_workspace_bytes", n, H0, W0, H, W, method, kC, p, msg, sizeof msg)) return -1;
+  return (int64_t)(p.tab_bytes + p.tmp_bytes);
+}
+
+extern "C" int hr_resize_frames(const uint8_t* src, int32_t n, int32_t H0, int32_t W0, uint8_t* dst, int32_t H, int32_t W,
+                                int64_t dst_row_stride, int32_t method, int32_t flags, int32_t pixel_format, void* workspace,
+                                int64_t workspace_bytes, void* stream) {
+  const char* fn = "hr_resize_frames";
   if (!src || !dst) return hr_fail("%s: null argument", fn);
   if (flags & ~HR_RESIZE_BGR) return hr_fail("%s: unknown flags 0x%x", fn, (unsigned)flags);
-  const int kC = format_channels(pixel_format);
+  const int kC = hr::pixel_bytes(pixel_format);
   if (kC == 0) return hr_fail("%s: unknown pixel format %d", fn, pixel_format);
   Plan p;
   char msg[256];
@@ -477,29 +477,4 @@ int resize_frames(const char* fn, const uint8_t* src, int32_t n, int32_t H0, int
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) return hr_fail("%s: %s", fn, cudaGetErrorString(e));
   return 0;
-}
-
-}  // namespace
-
-extern "C" int64_t hr_resize_workspace_bytes(int32_t n, int32_t H0, int32_t W0, int32_t H, int32_t W, int32_t method) {
-  return workspace_bytes("hr_resize_workspace_bytes", n, H0, W0, H, W, method, 3);
-}
-
-extern "C" int64_t hr_resize_workspace_bytes_fmt(int32_t n, int32_t H0, int32_t W0, int32_t H, int32_t W, int32_t method,
-                                                 int32_t pixel_format) {
-  return workspace_bytes("hr_resize_workspace_bytes_fmt", n, H0, W0, H, W, method, format_channels(pixel_format));
-}
-
-extern "C" int hr_resize_frames(const uint8_t* src, int32_t n, int32_t H0, int32_t W0, uint8_t* dst, int32_t H, int32_t W,
-                                int64_t dst_row_stride, int32_t method, int32_t flags, void* workspace,
-                                int64_t workspace_bytes, void* stream) {
-  return resize_frames("hr_resize_frames", src, n, H0, W0, dst, H, W, dst_row_stride, method, flags, HR_PIXEL_RGB8,
-                       workspace, workspace_bytes, stream);
-}
-
-extern "C" int hr_resize_frames_fmt(const uint8_t* src, int32_t n, int32_t H0, int32_t W0, uint8_t* dst, int32_t H,
-                                    int32_t W, int64_t dst_row_stride, int32_t method, int32_t flags, int32_t pixel_format,
-                                    void* workspace, int64_t workspace_bytes, void* stream) {
-  return resize_frames("hr_resize_frames_fmt", src, n, H0, W0, dst, H, W, dst_row_stride, method, flags, pixel_format,
-                       workspace, workspace_bytes, stream);
 }

@@ -14,8 +14,8 @@
 // uint64 arithmetic modulo 2^64.  tests/train_order_oracle.py restates it in NumPy.
 //
 // RGBA images (HR_PIXEL_RGBA8, the DoNeRF and Catacaustics datasets): a row's colour is the composite their get_rgb returns,
-// rgb * a + (1 - a) of the u8 / 255 values, each operation rounded on its own as torch rounds it on the CPU (no FMA
-// contraction: __fmul_rn, __fsub_rn, __fadd_rn), from one aligned 4-byte load of the pixel.
+// rgb * a + (1 - a) of the u8 / 255 values (rgba_over_white, hr_common.cuh, which the held-out scores share), from one
+// aligned 4-byte load of the pixel.
 //
 // One thread per row: one 3-byte (or 4-byte) gather and one 48-byte row write (plus 8 B of pixel id when asked).  No float atomics, no
 // host synchronisation; two calls with the same arguments write the same bits.  The camera records live on the device, so
@@ -264,15 +264,14 @@ train_rows_kernel(const hr_camera* __restrict__ cams, const uint8_t* __restrict_
       camera_ray<true, true>(cam, x, y, ndc_scale(cam), row);
       if constexpr (kC == 4) {
         const uint32_t q = *reinterpret_cast<const uint32_t*>(images + 4 * p);  // 4-byte aligned (checked by the host)
-        const float a = __fdiv_rn((float)(q >> 24), 255.0f), ia = __fsub_rn(1.0f, a);
-        c0 = __fadd_rn(__fmul_rn(__fdiv_rn((float)(q & 0xffu), 255.0f), a), ia);
-        c1 = __fadd_rn(__fmul_rn(__fdiv_rn((float)((q >> 8) & 0xffu), 255.0f), a), ia);
-        c2 = __fadd_rn(__fmul_rn(__fdiv_rn((float)((q >> 16) & 0xffu), 255.0f), a), ia);
+        c0 = rgba_over_white(q, 0);
+        c1 = rgba_over_white(q, 1);
+        c2 = rgba_over_white(q, 2);
       } else {
         const uint8_t* px = images + 3 * p;
-        c0 = __fdiv_rn((float)px[0], 255.0f);
-        c1 = __fdiv_rn((float)px[1], 255.0f);
-        c2 = __fdiv_rn((float)px[2], 255.0f);
+        c0 = u8_unit(px[0]);
+        c1 = u8_unit(px[1]);
+        c2 = u8_unit(px[2]);
       }
       w = 1.0f;
     } else {
@@ -315,8 +314,7 @@ struct ImportanceSlot {
 __device__ __forceinline__ uint32_t diff_key(const uint8_t* cur, const uint8_t* prev) {
   float d[3];
 #pragma unroll
-  for (int c = 0; c < 3; ++c)
-    d[c] = fabsf(__fsub_rn(__fdiv_rn((float)cur[c], 255.0f), __fdiv_rn((float)prev[c], 255.0f)));
+  for (int c = 0; c < 3; ++c) d[c] = fabsf(__fsub_rn(u8_unit(cur[c]), u8_unit(prev[c])));
   return __float_as_uint(__fdiv_rn(__fadd_rn(__fadd_rn(d[0], d[1]), d[2]), 3.0f));
 }
 
@@ -541,84 +539,43 @@ size_t importance_workspace(int64_t n_slots) {
 
 }  // namespace
 
-namespace {
-
-int sample_batch(const char* fn, const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t pixel_format,
-                 int32_t height, int32_t width, int32_t c_in, uint64_t seed, int64_t epoch, int64_t batch_index,
-                 int64_t batch_size, const int64_t* order, float* coords, float* rgb, float* weight, int64_t* pixel_ids,
-                 int64_t* n_rows, void* stream) {
+extern "C" int hr_sample_train_batch(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t pixel_format,
+                                     int32_t height, int32_t width, int32_t c_in, uint64_t seed, int64_t epoch,
+                                     int64_t batch_index, int64_t batch_size, const int64_t* order, float* coords, float* rgb,
+                                     float* weight, int64_t* pixel_ids, int64_t* n_rows, void* stream) {
+  const char* fn = "hr_sample_train_batch";
   if (!cameras || !images || !coords || !rgb || !weight) return hr_fail("%s: null argument", fn);
   if (((uintptr_t)coords % 8) || ((uintptr_t)rgb % 4) || ((uintptr_t)weight % 4) || ((uintptr_t)pixel_ids % 8) ||
       ((uintptr_t)order % 8) || ((uintptr_t)cameras % 4))
     return hr_fail("%s: misaligned pointer (coords and pixel_ids / order need 8 bytes, the rest 4)", fn);
-  if (pixel_format != HR_PIXEL_RGB8 && pixel_format != HR_PIXEL_RGBA8)
-    return hr_fail("%s: unknown pixel format %d", fn, pixel_format);
+  const int px = hr::pixel_bytes(pixel_format);
+  if (!px) return hr_fail("%s: unknown pixel format %d", fn, pixel_format);
   // the table is every pixel (sample_rows refuses a bad image stack and more than 2^62 pixels before n_table is used)
   const hr::WholePlan plan{(long long)((uint64_t)n_views * (uint64_t)height * (uint64_t)width)};
-  return pixel_format == HR_PIXEL_RGBA8
-             ? sample_rows<hr::WholePlan, 4>(fn, plan, cameras, n_views, images, height, width, c_in, HR_SAMPLE_PERMUTE,
-                                             seed, epoch, batch_index, batch_size, order, coords, rgb, weight, pixel_ids,
-                                             nullptr, n_rows, stream)
-             : sample_rows(fn, plan, cameras, n_views, images, height, width, c_in, HR_SAMPLE_PERMUTE, seed, epoch,
-                           batch_index, batch_size, order, coords, rgb, weight, pixel_ids, nullptr, n_rows, stream);
+  return px == 4 ? sample_rows<hr::WholePlan, 4>(fn, plan, cameras, n_views, images, height, width, c_in, HR_SAMPLE_PERMUTE,
+                                                 seed, epoch, batch_index, batch_size, order, coords, rgb, weight,
+                                                 pixel_ids, nullptr, n_rows, stream)
+                 : sample_rows(fn, plan, cameras, n_views, images, height, width, c_in, HR_SAMPLE_PERMUTE, seed, epoch,
+                               batch_index, batch_size, order, coords, rgb, weight, pixel_ids, nullptr, n_rows, stream);
 }
 
-int sample_table_rows(const char* fn, const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t pixel_format,
-                      int32_t height, int32_t width, int32_t c_in, const int64_t* view_start, const int32_t* view_rule,
-                      int64_t n_table, int32_t mode, uint64_t seed, int64_t epoch, int64_t batch_index, int64_t batch_size,
-                      const int64_t* table_rows, float* coords, float* rgb, float* weight, int64_t* pixel_ids,
-                      int64_t* table_ids, int64_t* n_rows, void* stream) {
+extern "C" int hr_sample_train_rows(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t pixel_format,
+                                    int32_t height, int32_t width, int32_t c_in, const int64_t* view_start,
+                                    const int32_t* view_rule, int64_t n_table, int32_t mode, uint64_t seed, int64_t epoch,
+                                    int64_t batch_index, int64_t batch_size, const int64_t* table_rows, float* coords,
+                                    float* rgb, float* weight, int64_t* pixel_ids, int64_t* table_ids, int64_t* n_rows,
+                                    void* stream) {
+  const char* fn = "hr_sample_train_rows";
   if (!cameras || !images || !view_start || !view_rule || !coords || !rgb || !weight) return hr_fail("%s: null argument", fn);
   if ((uintptr_t)view_rule % 4) return hr_fail("%s: misaligned pointer (view_rule needs 4 bytes)", fn);
-  if (pixel_format != HR_PIXEL_RGB8 && pixel_format != HR_PIXEL_RGBA8)
-    return hr_fail("%s: unknown pixel format %d", fn, pixel_format);
+  const int px = hr::pixel_bytes(pixel_format);
+  if (!px) return hr_fail("%s: unknown pixel format %d", fn, pixel_format);
   const hr::TablePlan plan{view_start, view_rule, n_views, n_table};
-  return pixel_format == HR_PIXEL_RGBA8
-             ? sample_rows<hr::TablePlan, 4>(fn, plan, cameras, n_views, images, height, width, c_in, mode, seed, epoch,
-                                             batch_index, batch_size, table_rows, coords, rgb, weight, pixel_ids, table_ids,
-                                             n_rows, stream)
-             : sample_rows(fn, plan, cameras, n_views, images, height, width, c_in, mode, seed, epoch, batch_index,
-                           batch_size, table_rows, coords, rgb, weight, pixel_ids, table_ids, n_rows, stream);
-}
-
-}  // namespace
-
-extern "C" int hr_sample_train_batch(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height,
-                                     int32_t width, int32_t c_in, uint64_t seed, int64_t epoch, int64_t batch_index,
-                                     int64_t batch_size, const int64_t* order, float* coords, float* rgb, float* weight,
-                                     int64_t* pixel_ids, int64_t* n_rows, void* stream) {
-  return sample_batch("hr_sample_train_batch", cameras, n_views, images, HR_PIXEL_RGB8, height, width, c_in, seed, epoch,
-                      batch_index, batch_size, order, coords, rgb, weight, pixel_ids, n_rows, stream);
-}
-
-extern "C" int hr_sample_train_batch_fmt(const hr_camera* cameras, int32_t n_views, const uint8_t* images,
-                                         int32_t pixel_format, int32_t height, int32_t width, int32_t c_in, uint64_t seed,
-                                         int64_t epoch, int64_t batch_index, int64_t batch_size, const int64_t* order,
-                                         float* coords, float* rgb, float* weight, int64_t* pixel_ids, int64_t* n_rows,
-                                         void* stream) {
-  return sample_batch("hr_sample_train_batch_fmt", cameras, n_views, images, pixel_format, height, width, c_in, seed, epoch,
-                      batch_index, batch_size, order, coords, rgb, weight, pixel_ids, n_rows, stream);
-}
-
-extern "C" int hr_sample_train_rows(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height,
-                                    int32_t width, int32_t c_in, const int64_t* view_start, const int32_t* view_rule,
-                                    int64_t n_table, int32_t mode, uint64_t seed, int64_t epoch, int64_t batch_index,
-                                    int64_t batch_size, const int64_t* table_rows, float* coords, float* rgb, float* weight,
-                                    int64_t* pixel_ids, int64_t* table_ids, int64_t* n_rows, void* stream) {
-  return sample_table_rows("hr_sample_train_rows", cameras, n_views, images, HR_PIXEL_RGB8, height, width, c_in, view_start,
-                           view_rule, n_table, mode, seed, epoch, batch_index, batch_size, table_rows, coords, rgb, weight,
-                           pixel_ids, table_ids, n_rows, stream);
-}
-
-extern "C" int hr_sample_train_rows_fmt(const hr_camera* cameras, int32_t n_views, const uint8_t* images,
-                                        int32_t pixel_format, int32_t height, int32_t width, int32_t c_in,
-                                        const int64_t* view_start, const int32_t* view_rule, int64_t n_table, int32_t mode,
-                                        uint64_t seed, int64_t epoch, int64_t batch_index, int64_t batch_size,
-                                        const int64_t* table_rows, float* coords, float* rgb, float* weight,
-                                        int64_t* pixel_ids, int64_t* table_ids, int64_t* n_rows, void* stream) {
-  return sample_table_rows("hr_sample_train_rows_fmt", cameras, n_views, images, pixel_format, height, width, c_in,
-                           view_start, view_rule, n_table, mode, seed, epoch, batch_index, batch_size, table_rows, coords,
-                           rgb, weight, pixel_ids, table_ids, n_rows, stream);
+  return px == 4 ? sample_rows<hr::TablePlan, 4>(fn, plan, cameras, n_views, images, height, width, c_in, mode, seed,
+                                                 epoch, batch_index, batch_size, table_rows, coords, rgb, weight,
+                                                 pixel_ids, table_ids, n_rows, stream)
+                 : sample_rows(fn, plan, cameras, n_views, images, height, width, c_in, mode, seed, epoch, batch_index,
+                               batch_size, table_rows, coords, rgb, weight, pixel_ids, table_ids, n_rows, stream);
 }
 
 extern "C" int hr_sample_train_mask_rows(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height,

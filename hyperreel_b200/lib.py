@@ -11,7 +11,7 @@ import os
 import subprocess
 import threading
 
-HR_ABI_VERSION = 23
+HR_ABI_VERSION = 24
 HR_MAX_GROUPS = 4
 HR_MAX_LAYERS = 10
 HR_MAX_SAMPLES = 256
@@ -159,19 +159,13 @@ EXPORTS = {
                                     C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]),
     "hr_render_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]),
     "hr_generate_rays": (C.c_int, [C.POINTER(hr_camera), C.c_int32, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
-    "hr_sample_train_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_uint64, C.c_int64,
-                                         C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                         C.POINTER(C.c_int64), C.c_void_p]),
-    "hr_sample_train_rows": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
-                                        C.c_int64, C.c_int32, C.c_uint64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p,
-                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
-    "hr_sample_train_batch_fmt": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                             C.c_uint64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
-                                             C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
-    "hr_sample_train_rows_fmt": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                            C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_uint64, C.c_int64, C.c_int64,
-                                            C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                            C.POINTER(C.c_int64), C.c_void_p]),
+    "hr_sample_train_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                         C.c_uint64, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
+    "hr_sample_train_rows": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                        C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_uint64, C.c_int64, C.c_int64,
+                                        C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.POINTER(C.c_int64), C.c_void_p]),
     "hr_importance_workspace_bytes": (C.c_int64, [C.c_int32]),
     "hr_build_importance_table": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                              C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -185,10 +179,8 @@ EXPORTS = {
     "hr_render_video_to8b": (C.c_int, [C.c_void_p, C.POINTER(hr_camera), C.POINTER(C.c_float), C.c_int32, C.c_void_p, C.c_void_p,
                                         C.c_int64, C.c_void_p]),
     "hr_score_views_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]),
-    "hr_score_views": (C.c_int, [C.c_void_p, C.POINTER(hr_camera), C.POINTER(C.c_float), C.c_int32, C.c_void_p, C.c_void_p,
-                                  C.c_void_p, C.c_int64, C.c_void_p]),
-    "hr_score_views_fmt": (C.c_int, [C.c_void_p, C.POINTER(hr_camera), C.POINTER(C.c_float), C.c_int32, C.c_void_p, C.c_int32,
-                                      C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "hr_score_views": (C.c_int, [C.c_void_p, C.POINTER(hr_camera), C.POINTER(C.c_float), C.c_int32, C.c_void_p, C.c_int32,
+                                  C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "hr_encode_rays": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "hr_render_heads": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.POINTER(hr_train_opts), C.c_void_p,
                                    C.c_int64, C.c_void_p]),
@@ -204,12 +196,9 @@ EXPORTS = {
     "hr_image_metrics_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32]),
     "hr_image_metrics": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64,
                                     C.c_void_p]),
-    "hr_resize_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "hr_resize_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "hr_resize_frames": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int64,
-                                    C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]),
-    "hr_resize_workspace_bytes_fmt": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
-    "hr_resize_frames_fmt": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int64,
-                                        C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]),
+                                    C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]),
     "hr_launch_count": (C.c_int64, [C.c_void_p]),
     "hr_timing_enable": (C.c_int, [C.c_void_p, C.c_int]),
     "hr_timing_reset": (C.c_int, [C.c_void_p]),

@@ -547,7 +547,7 @@ class LightfieldModel(nn.Module):
         view's eval render, bit for bit.  ``out`` (device fp64 [n, 2], contiguous) receives (mse, ssim) when given; the work
         goes on ``stream`` (a torch.cuda.Stream; default the current stream).  ``rgba=True``: ``images`` are uint8 RGBA
         [n, H, W, 4], the DoNeRF and Catacaustics frames, and each view is scored against its composite over white,
-        ``rgb * a + (1 - a)`` of the ``u8 / 255`` values as their ``get_rgb`` computes it on the CPU (hr_score_views_fmt)."""
+        ``rgb * a + (1 - a)`` of the ``u8 / 255`` values as their ``get_rgb`` computes it on the CPU."""
         if self.training:
             raise RuntimeError("hyperreel_b200.LightfieldModel implements the eval()/render path only; call .eval()")
         cams = list(cameras)
@@ -593,8 +593,8 @@ class LightfieldModel(nn.Module):
             if out is None:
                 out = torch.empty((len(cams), 2), dtype=torch.float64, device=dev)
             fmt = L.PIXEL_RGBA8 if rgba else L.PIXEL_RGB8
-            L.check(self._lib.hr_score_views_fmt(self._handle, recs, tt, len(cams), images.data_ptr(), fmt, out.data_ptr(),
-                                                 ws.data_ptr(), need, stream.cuda_stream))
+            L.check(self._lib.hr_score_views(self._handle, recs, tt, len(cams), images.data_ptr(), fmt, out.data_ptr(),
+                                             ws.data_ptr(), need, stream.cuda_stream))
         return out[:, 0], out[:, 1]
 
     def timing(self, enable: bool = True):

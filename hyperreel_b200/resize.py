@@ -77,7 +77,7 @@ def resize_frames(frames: torch.Tensor, size: Sequence[int], method: str, bgr: b
     lib = L.load_library()
     m = L.RESIZE_METHODS[method]
     fmt = L.PIXEL_RGBA8 if rgba else L.PIXEL_RGB8
-    need = int(lib.hr_resize_workspace_bytes_fmt(n, H0, W0, H, W, m, fmt))
+    need = int(lib.hr_resize_workspace_bytes(n, H0, W0, H, W, m, fmt))
     dev = src.device
     given = out is not None
     if given:
@@ -93,8 +93,8 @@ def resize_frames(frames: torch.Tensor, size: Sequence[int], method: str, bgr: b
         ws = torch.empty(max(need, 0), dtype=torch.uint8, device=dev)
         if out is None:
             out, row = torch.empty((n, H, W, ch), dtype=torch.uint8, device=dev), ch * W
-        L.check(lib.hr_resize_frames_fmt(src.data_ptr(), n, H0, W0, out.data_ptr(), H, W, row, m, L.RESIZE_BGR if bgr else 0,
-                                         fmt, ws.data_ptr() if need > 0 else None, max(need, 0), stream.cuda_stream))
+        L.check(lib.hr_resize_frames(src.data_ptr(), n, H0, W0, out.data_ptr(), H, W, row, m, L.RESIZE_BGR if bgr else 0, fmt,
+                                     ws.data_ptr() if need > 0 else None, max(need, 0), stream.cuda_stream))
     return out[0] if single and not given else out
 
 

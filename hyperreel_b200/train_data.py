@@ -461,8 +461,8 @@ class DeviceRayBatches:
     def _launch(self, rows: int, index: int, ids: Optional[torch.Tensor], with_pixel_ids: bool, with_table_ids: bool,
                 ids_are_pixels: bool = False) -> Dict[str, torch.Tensor]:
         """Batch ``index`` of the epoch, or the rows of the explicit ``ids`` (table rows, or pixels with ``ids_are_pixels``).
-        Explicit pixels and the permuted batches without a plan go through ``hr_sample_train_batch(_fmt)``, everything else
-        through the plan's entry (``hr_sample_train_rows(_fmt)`` or ``hr_sample_train_mask_rows``)."""
+        Explicit pixels and the permuted batches without a plan go through ``hr_sample_train_batch``, everything else
+        through the plan's entry (``hr_sample_train_rows`` or ``hr_sample_train_mask_rows``)."""
         dev = self.device
         whole = ids_are_pixels or (ids is None and not self.replacement and self.subsample is None and
                                    self.importance is None)
@@ -482,13 +482,13 @@ class DeviceRayBatches:
         stream = torch.cuda.current_stream(dev).cuda_stream
         with torch.cuda.device(dev):
             if whole:
-                L.check(self._lib.hr_sample_train_batch_fmt(*head_fmt, self.seed, self.epoch, *batch, C.byref(n_rows), stream))
+                L.check(self._lib.hr_sample_train_batch(*head_fmt, self.seed, self.epoch, *batch, C.byref(n_rows), stream))
             else:
                 mode = L.SAMPLE_REPLACE if self.replacement else L.SAMPLE_PERMUTE
                 tail = (self.n_rows, mode, self.seed, self.epoch, *batch, ptr(tids), C.byref(n_rows), stream)
                 if self.importance is None:
-                    L.check(self._lib.hr_sample_train_rows_fmt(*head_fmt, self._view_start.data_ptr(),
-                                                               self._view_rule.data_ptr(), *tail))
+                    L.check(self._lib.hr_sample_train_rows(*head_fmt, self._view_start.data_ptr(),
+                                                           self._view_rule.data_ptr(), *tail))
                 else:
                     L.check(self._lib.hr_sample_train_mask_rows(*head, self._view_start.data_ptr(),
                                                                 self._view_slot.data_ptr(), self._block_start.data_ptr(),

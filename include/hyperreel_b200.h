@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define HR_ABI_VERSION 23
+#define HR_ABI_VERSION 24
 
 #define HR_MAX_GROUPS 4   /* ray-parameterisation groups feeding the sample net (ray.py:235-263) */
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
@@ -376,13 +376,22 @@ typedef struct hr_camera {
 int hr_generate_rays(const hr_camera* cam, int32_t c_in, int64_t first_pixel, int64_t n_pixels, float* rays_out,
                      void* stream);
 
+/* Pixel formats of uint8 images (ABI 23).  HR_PIXEL_RGB8: [.., 3] RGB.  HR_PIXEL_RGBA8: [.., 4] RGBA, the frames of the
+ * datasets whose get_rgb loads RGBA (datasets/donerf.py, catacaustics.py); where such an image is consumed as a colour, that
+ * colour is their get_rgb's composite over white, rgb * a + (1 - a) of the u8 / 255 values (T.ToTensor()), each of the
+ * multiply, subtract and add rounded on its own in fp32 (no FMA), as torch computes it on the CPU.  4-byte aligned. */
+#define HR_PIXEL_RGB8 0
+#define HR_PIXEL_RGBA8 1
+
 /* ---- training batches from images on the device (SURVEY.md section 2 row 23) ----
  * Replaces: the training split of the reference's datasets in its default mode (datasets/base.py:111-143,202-227,254-289): the
  * host table all_inputs = cat([all_coords, all_rgb, all_weights]) of every training ray, re-permuted every epoch
  * (np.random.permutation) and handed out in consecutive slices that format_batch splits and the loop copies to the GPU.
  * Handle-free.  cameras: device array of n_views records, each of width `width` and height `height`; images: device uint8
- * [n_views, height, width, 3].  Pixel p in [0, N), N = n_views*height*width, is view p / (height*width), then row-major within
- * the view like hr_generate_rays.  Row r of the batch is pixel
+ * [n_views, height, width, 3] for pixel_format HR_PIXEL_RGB8, [n_views, height, width, 4] (4-byte aligned) for HR_PIXEL_RGBA8
+ * (ABI 23), when each row's rgb is its pixel's composite over white; rays, order, draws and ids do not depend on the format.
+ * An unknown pixel_format, or RGBA images not 4-byte aligned, is refused.  Pixel p in [0, N), N = n_views*height*width, is
+ * view p / (height*width), then row-major within the view like hr_generate_rays.  Row r of the batch is pixel
  *   order[r]                                        when order (device int64, batch_size entries) is given;
  *   element batch_index*batch_size + r of epoch's permutation of [0, N), keyed by (seed, epoch)   otherwise
  * (a Feistel network over the next power of two >= N with cycle-walking, so an epoch visits every pixel exactly once;
@@ -395,19 +404,20 @@ int hr_generate_rays(const hr_camera* cam, int32_t c_in, int64_t first_pixel, in
  * Each row takes its view's camera model (ABI 17: a fisheye record's rays as hr_generate_rays writes them; ABI 20: a two-plane
  * record's), so one batch may mix pinhole, fisheye and two-plane views; the records' fisheye coefficients must be finite and
  * their two-plane records well formed as hr_generate_rays requires (the device array is not inspected). */
-int hr_sample_train_batch(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height, int32_t width,
-                          int32_t c_in, uint64_t seed, int64_t epoch, int64_t batch_index, int64_t batch_size,
-                          const int64_t* order, float* coords, float* rgb, float* weight, int64_t* pixel_ids, int64_t* n_rows,
-                          void* stream);
+int hr_sample_train_batch(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t pixel_format,
+                          int32_t height, int32_t width, int32_t c_in, uint64_t seed, int64_t epoch, int64_t batch_index,
+                          int64_t batch_size, const int64_t* order, float* coords, float* rgb, float* weight,
+                          int64_t* pixel_ids, int64_t* n_rows, void* stream);
 
 /* Training batches over a table of per-view pixel subsets, drawn with or without replacement.
  * Replaces: the training split of the video datasets (datasets/technicolor.py:211-269, datasets/neural_3d.py:168-185,217-269),
  * which keep per view only the pixels with (x + y + offset) % stride == 0, sampled as the shipped training configs do
  * (sample_with_replacement: RandomSampler(replacement=True, num_samples=num_iters * batch_size), nlf/__init__.py:222-237).
- * cameras, images, n_views, height, width, c_in: as hr_sample_train_batch.  The table is implicit: view_start (device int64
- * [n_views + 1]) is the exclusive prefix of the per-view row counts and view_rule (device int32 [n_views, 2]) each view's
- * (stride >= 1, offset); table row k is in view v with view_start[v] <= k < view_start[v + 1], at rank k - view_start[v] of that
- * view's kept pixels in row-major order (the reference's all_coords order).  Row r of the batch is table row
+ * cameras, n_views, images, pixel_format, height, width, c_in: as hr_sample_train_batch.  The table is implicit:
+ * view_start (device int64 [n_views + 1]) is the exclusive prefix of the per-view row counts and view_rule (device int32
+ * [n_views, 2]) each view's (stride >= 1, offset); table row k is in view v with view_start[v] <= k < view_start[v + 1], at
+ * rank k - view_start[v] of that view's kept pixels in row-major order (the reference's all_coords order).  Row r of the
+ * batch is table row
  *   table_rows[r]                                       when table_rows (device int64, batch_size entries) is given;
  *   element batch_index*batch_size + r of epoch's permutation of [0, n_table)   when mode == HR_SAMPLE_PERMUTE
  *     (hr_sample_train_batch's permutation; batch_index in [0, ceil(n_table / batch_size)), the last batch short);
@@ -420,20 +430,20 @@ int hr_sample_train_batch(const hr_camera* cameras, int32_t n_views, const uint8
  * float atomics, no host synchronisation: two calls with the same arguments write the same bits. */
 #define HR_SAMPLE_PERMUTE 0
 #define HR_SAMPLE_REPLACE 1
-int hr_sample_train_rows(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height, int32_t width,
-                         int32_t c_in, const int64_t* view_start, const int32_t* view_rule, int64_t n_table, int32_t mode,
-                         uint64_t seed, int64_t epoch, int64_t batch_index, int64_t batch_size, const int64_t* table_rows,
-                         float* coords, float* rgb, float* weight, int64_t* pixel_ids, int64_t* table_ids, int64_t* n_rows,
-                         void* stream);
+int hr_sample_train_rows(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t pixel_format,
+                         int32_t height, int32_t width, int32_t c_in, const int64_t* view_start, const int32_t* view_rule,
+                         int64_t n_table, int32_t mode, uint64_t seed, int64_t epoch, int64_t batch_index,
+                         int64_t batch_size, const int64_t* table_rows, float* coords, float* rgb, float* weight,
+                         int64_t* pixel_ids, int64_t* table_ids, int64_t* n_rows, void* stream);
 
 /* The Immersive dataset's training table: per-view keep masks chosen by image content.
  * Replaces: ImmersiveDataset.prepare_train_data / subsample / importance_subsample (datasets/immersive.py:295-391).  Views are
  * video-major with each video's frames in order; an importance view v keeps the pixels with diff > thr and dz < -0.05 in
  * row-major order, diff = mean over channels of |rgb_v - rgb_{v-1}| (u8 / 255 in fp32, ((d0 + d1) + d2) / 3), thr = diff's value
  * of ascending rank (N - num_take) % N (N = height*width; duplicates counted), dz = channel 5 of hr_generate_rays's row for the
- * pixel.  cameras, images, n_views, height, width: as hr_sample_train_batch (height*width < 2^31).  plan: HOST int64
- * [n_views, 2], per view (num_take, prev): (-1, -1) for a whole view, else num_take in [0, N] and prev == v - 1 (the previous
- * frame of the same video; v >= 1).  At most 65535 importance views per call; n_slots is their number.
+ * pixel.  cameras, n_views, height, width: as hr_sample_train_batch (height*width < 2^31); images HR_PIXEL_RGB8.  plan:
+ * HOST int64 [n_views, 2], per view (num_take, prev): (-1, -1) for a whole view, else num_take in [0, N] and prev == v - 1
+ * (the previous frame of the same video; v >= 1).  At most 65535 importance views per call; n_slots is their number.
  * Outputs (device): view_slot int32 [n_views], the view's slot (its rank among the importance views) or -1;
  *   masks uint32 [n_slots, B, 8], B = ceil(N / 256): bit (p & 31) of word p >> 5 of the slot's mask keeps pixel p;
  *   block_start uint32 [n_slots, B]: exclusive prefix of the kept counts of each 256-pixel block within the view;
@@ -448,36 +458,15 @@ int hr_build_importance_table(const hr_camera* cameras, int32_t n_views, const u
                               uint32_t* block_start, uint32_t* masks, int64_t* view_rows, int64_t* view_start, void* stream);
 
 /* Training batches over a table of per-view keep masks (hr_build_importance_table's outputs): as hr_sample_train_rows, with
- * view_slot, block_start and masks in place of view_rule.  Table row k is in view v with view_start[v] <= k < view_start[v + 1],
- * at rank k - view_start[v] of that view's kept pixels in row-major order (every pixel for slot -1).  n_table is
- * view_start[n_views] for a well-formed table; a row the table does not hold gives a zero row of weight 0 and ids -1. */
+ * view_slot, block_start and masks in place of view_rule, and images HR_PIXEL_RGB8 (the Immersive dataset's frames are
+ * RGB).  Table row k is in view v with view_start[v] <= k < view_start[v + 1], at rank k - view_start[v] of that view's kept
+ * pixels in row-major order (every pixel for slot -1).  n_table is view_start[n_views] for a well-formed table; a row the
+ * table does not hold gives a zero row of weight 0 and ids -1. */
 int hr_sample_train_mask_rows(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t height, int32_t width,
                               int32_t c_in, const int64_t* view_start, const int32_t* view_slot, const uint32_t* block_start,
                               const uint32_t* masks, int64_t n_table, int32_t mode, uint64_t seed, int64_t epoch,
                               int64_t batch_index, int64_t batch_size, const int64_t* table_rows, float* coords, float* rgb,
                               float* weight, int64_t* pixel_ids, int64_t* table_ids, int64_t* n_rows, void* stream);
-
-/* Pixel formats of uint8 images (ABI 23).  HR_PIXEL_RGB8: [.., 3] RGB.  HR_PIXEL_RGBA8: [.., 4] RGBA, the frames of the
- * datasets whose get_rgb loads RGBA (datasets/donerf.py, catacaustics.py); where such an image is consumed as a colour, that
- * colour is their get_rgb's composite over white, rgb * a + (1 - a) of the u8 / 255 values (T.ToTensor()), each of the
- * multiply, subtract and add rounded on its own in fp32 (no FMA), as torch computes it on the CPU.  4-byte aligned. */
-#define HR_PIXEL_RGB8 0
-#define HR_PIXEL_RGBA8 1
-
-/* Training batches over images of either pixel format (ABI 23): as hr_sample_train_batch and hr_sample_train_rows, whose
- * images are HR_PIXEL_RGB8; with HR_PIXEL_RGBA8, images is uint8 [n_views, height, width, 4] and each row's rgb is its
- * pixel's composite over white.  Rays, order, draws, pixel and table ids are those of the RGB calls.  An unknown
- * pixel_format, or RGBA images not 4-byte aligned, is refused.  (Keep-mask tables, hr_sample_train_mask_rows, are RGB only:
- * the Immersive dataset's frames are RGB.) */
-int hr_sample_train_batch_fmt(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t pixel_format,
-                              int32_t height, int32_t width, int32_t c_in, uint64_t seed, int64_t epoch, int64_t batch_index,
-                              int64_t batch_size, const int64_t* order, float* coords, float* rgb, float* weight,
-                              int64_t* pixel_ids, int64_t* n_rows, void* stream);
-int hr_sample_train_rows_fmt(const hr_camera* cameras, int32_t n_views, const uint8_t* images, int32_t pixel_format,
-                             int32_t height, int32_t width, int32_t c_in, const int64_t* view_start, const int32_t* view_rule,
-                             int64_t n_table, int32_t mode, uint64_t seed, int64_t epoch, int64_t batch_index,
-                             int64_t batch_size, const int64_t* table_rows, float* coords, float* rgb, float* weight,
-                             int64_t* pixel_ids, int64_t* table_ids, int64_t* n_rows, void* stream);
 
 /* ---- the step after the path: 8-bit packing (SURVEY.md section 8(f) row f4) ----
  * Replaces: to8b(x) = (255 * clip(x, 0, 1)).astype(uint8) (utils/__init__.py:47) applied to the rendered frame before
@@ -514,9 +503,11 @@ int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* ti
  * Replaces: the reference's evaluation of a validation / test split (nlf/__init__.py:249-265, :895-982, :1015-1030): per
  * view, rays built on the CPU, the view rendered, copied to the host and scored with scikit-image.  cameras / times: HOST
  * arrays of n_views records (one width x height, >= 11 x 11, pinhole, fisheye and two-plane mixed freely) and fp32 times, as
- * hr_render_video_to8b takes them.  gt: DEVICE uint8 [n_views, height, width, 3], the views' ground truth.  out: DEVICE fp64
+ * hr_render_video_to8b takes them.  gt: DEVICE uint8, the views' ground truth: [n_views, height, width, 3] for pixel_format
+ * HR_PIXEL_RGB8, [n_views, height, width, 4] (4-byte aligned) for HR_PIXEL_RGBA8 (ABI 23).  out: DEVICE fp64
  * [n_views][2] = (mse, ssim) of each view, bit for bit hr_image_metrics of the fp32 frame hr_render makes of the view's rays
- * (clamped output, the configured background, no to8b) against gt / 255 correctly rounded in fp32 (T.ToTensor()'s conversion; NumPy's, and torch's on the CPU).
+ * (clamped output, the configured background, no to8b) against gt / 255 correctly rounded in fp32 (T.ToTensor()'s conversion; NumPy's, and torch's on the CPU),
+ * or for RGBA against its fp32 composite over white (HR_PIXEL_RGBA8 above).
  * workspace: device scratch of hr_score_views_workspace_bytes(h, n_views, height, width) bytes (16B aligned, -1 for a size
  * hr_score_views refuses), bounded whatever n_views: two windows of ring-many records and times, a ring of whole fp32
  * frames (enough for two sub-batches and one frame more), two metrics partial buffers and the video path's one or two
@@ -525,17 +516,12 @@ int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* ti
  * scores them with one metrics launch on its own stream, after an event of the other stream for a frame that straddles
  * the two, and a ring frame is reused only after the launch that scored it.  No host synchronisation, no float atomics:
  * two calls write the same bits.  Refused before anything is enqueued (out untouched): null or misaligned pointers
- * (out 8B, workspace 16B), n_views < 1, views of different sizes or smaller than 11 x 11, a size whose bytes overflow int64,
- * a non-finite record field, time or fisheye coefficient, a malformed two-plane record, a workspace too small. */
+ * (out 8B, workspace 16B, RGBA gt 4B), an unknown pixel_format, n_views < 1, views of different sizes or smaller than
+ * 11 x 11, a size whose bytes overflow int64, a non-finite record field, time or fisheye coefficient, a malformed two-plane
+ * record, a workspace too small. */
 int64_t hr_score_views_workspace_bytes(const hr_handle* h, int32_t n_views, int32_t height, int32_t width);
-int hr_score_views(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views, const uint8_t* gt, double* out,
-                   void* workspace, int64_t workspace_bytes, void* stream);
-/* Ground truth of either pixel format (ABI 23): as hr_score_views, whose gt is HR_PIXEL_RGB8.  With HR_PIXEL_RGBA8, gt is
- * DEVICE uint8 [n_views, height, width, 4] (4-byte aligned) and each view is scored against its composite over white
- * (HR_PIXEL_RGBA8 above): bit for bit hr_image_metrics against that fp32 composite.  Same workspace.  An unknown
- * pixel_format or a misaligned RGBA gt is refused. */
-int hr_score_views_fmt(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views, const uint8_t* gt,
-                       int32_t pixel_format, double* out, void* workspace, int64_t workspace_bytes, void* stream);
+int hr_score_views(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views, const uint8_t* gt,
+                   int32_t pixel_format, double* out, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- backward pass of the path (SURVEY.md section 8 row f1) ----
  * Replaces: what loss.backward() runs for the render path inside INRSystem.training_step (nlf/__init__.py:634-709): the
@@ -630,43 +616,36 @@ int hr_image_metrics(const float* pred, const float* gt, int32_t n_images, int32
  * Replaces: the resize in the datasets' get_rgb, run on the host per image: Pillow's Image.resize (datasets/technicolor.py,
  * llff.py, spaces.py, stanford.py: LANCZOS to _img_wh, then BOX to img_wh) and cv2.resize (datasets/neural_3d.py,
  * immersive.py: the flag they pass sits in the dst slot, so both of their steps are OpenCV's default INTER_LINEAR).
- * src: DEVICE uint8 [n, H0, W0, 3] contiguous.  dst: DEVICE uint8, frame f's row y at dst + (f * H + y) * dst_row_stride
- * (dst_row_stride >= 3 * W bytes), so a slice of a larger [N, H, W, 3] tensor can be written in place.  method: one of
- * HR_RESIZE_*; bit for bit the library's result on each frame (Pillow 12's 8-bit convolution resampler with its filter;
- * OpenCV 4's CV_8UC3 INTER_LINEAR, or INTER_AREA for integer factors, with INTER_LINEAR sent to INTER_AREA at exactly 2x).
- * A frame of the same size is copied, as both libraries do.  flags: HR_RESIZE_BGR reads src as BGR (channels 0 and 2
- * swapped), which is what OpenCV decodes; dst is RGB.  workspace: device, 256-byte aligned, at least
- * hr_resize_workspace_bytes(n, H0, W0, H, W, method) bytes (-1 for sizes or a method hr_resize_frames refuses; 0 for the
- * copy and the INTER_AREA paths): the coefficient tables, copied in with the launch, and for the two Pillow passes the uint8
- * intermediate of the rows the vertical pass reads.  Kernels use integer multiply-adds only (INTER_AREA at factors other
- * than 2 x 2 rounds sum * (1.f / area) in fp32, as OpenCV does), no float atomics and no host synchronisation: two calls
- * write the same bits.  Refused before anything is enqueued (dst untouched): null pointers, unknown method or flags, sizes
- * < 1, an enlargement in either direction, cv2_area at a non-integer factor, a Pillow reduction needing more filter
- * coefficients than Pillow allows (outSize > INT_MAX / (ksize * 8), where Pillow raises MemoryError), source, destination
- * or workspace bytes that overflow int64, a short dst_row_stride, a missing, misaligned or short workspace. */
+ * src: DEVICE uint8 [n, H0, W0, C] contiguous, C = 3 for pixel_format HR_PIXEL_RGB8 and 4 for HR_PIXEL_RGBA8 (ABI 23).
+ * dst: DEVICE uint8, frame f's row y at dst + (f * H + y) * dst_row_stride (dst_row_stride >= C * W bytes), so a slice of a
+ * larger [N, H, W, C] tensor can be written in place.  method: one of HR_RESIZE_*; bit for bit the library's result on each
+ * frame (Pillow 12's 8-bit convolution resampler with its filter; OpenCV 4's CV_8UC3 INTER_LINEAR, or INTER_AREA for
+ * integer factors, with INTER_LINEAR sent to INTER_AREA at exactly 2x).  A frame of the same size is copied, as both
+ * libraries do.  flags: HR_RESIZE_BGR reads src as BGR (channels 0 and 2 swapped), which is what OpenCV decodes; dst is
+ * RGB.  For RGBA, HR_RESIZE_BGR reads BGRA and dst is RGBA, resized as the datasets that load RGBA resize it
+ * (datasets/donerf.py, catacaustics.py): the Pillow methods resample the premultiplied RGBa image and convert back, as
+ * Image.resize does for an RGBA image on every call (premultiply MULDIV255(c, a); unpremultiply c for a of 0 or 255, else
+ * min(255, 255 * c / a)); cv2_area resamples the four channels independently, as OpenCV does.  workspace: device, 256-byte
+ * aligned, at least hr_resize_workspace_bytes(n, H0, W0, H, W, method, pixel_format) bytes (-1 for sizes, a method or a
+ * pixel_format hr_resize_frames refuses; 0 for the copy and the INTER_AREA paths): the coefficient tables, copied in with
+ * the launch, and for the two Pillow passes the uint8 intermediate of the rows the vertical pass reads (premultiplied RGBa,
+ * 4 bytes per pixel, for RGBA).  Kernels use integer multiply-adds only (INTER_AREA at factors other than 2 x 2 rounds
+ * sum * (1.f / area) in fp32, as OpenCV does), no float atomics and no host synchronisation: two calls write the same bits.
+ * Refused before anything is enqueued (dst untouched): null pointers, unknown method, flags or pixel_format, cv2_linear for
+ * RGBA, sizes < 1, an enlargement in either direction, cv2_area at a non-integer factor, a Pillow reduction needing more
+ * filter coefficients than Pillow allows (outSize > INT_MAX / (ksize * 8), where Pillow raises MemoryError), source,
+ * destination or workspace bytes that overflow int64, a short dst_row_stride, a missing, misaligned or short workspace. */
 #define HR_RESIZE_PIL_LANCZOS 0
 #define HR_RESIZE_PIL_BICUBIC 1
 #define HR_RESIZE_PIL_BOX 2
 #define HR_RESIZE_CV2_LINEAR 3
 #define HR_RESIZE_CV2_AREA 4
 #define HR_RESIZE_BGR 1
-int64_t hr_resize_workspace_bytes(int32_t n, int32_t H0, int32_t W0, int32_t H, int32_t W, int32_t method);
+int64_t hr_resize_workspace_bytes(int32_t n, int32_t H0, int32_t W0, int32_t H, int32_t W, int32_t method,
+                                  int32_t pixel_format);
 int hr_resize_frames(const uint8_t* src, int32_t n, int32_t H0, int32_t W0, uint8_t* dst, int32_t H, int32_t W,
-                     int64_t dst_row_stride, int32_t method, int32_t flags, void* workspace, int64_t workspace_bytes,
-                     void* stream);
-
-/* RGBA frames (ABI 23): as hr_resize_workspace_bytes / hr_resize_frames for frames of pixel_format (HR_PIXEL_RGB8 gives the
- * two calls above; HR_PIXEL_RGBA8 is uint8 [n, H0, W0, 4] -> [n, H, W, 4], dst_row_stride >= 4 * W).  RGBA as the datasets
- * that load RGBA resize it (datasets/donerf.py, catacaustics.py): the Pillow methods resample the premultiplied RGBa image
- * and convert back, as Image.resize does for an RGBA image on every call (premultiply MULDIV255(c, a); unpremultiply c for
- * a of 0 or 255, else min(255, 255 * c / a)); cv2_area resamples the four channels independently, as OpenCV does.  The
- * Pillow intermediate is premultiplied RGBa, 4 bytes per pixel.  HR_RESIZE_BGR reads BGRA.  cv2_linear is refused for RGBA,
- * and so is an unknown pixel_format (-1 from hr_resize_workspace_bytes_fmt). */
-int64_t hr_resize_workspace_bytes_fmt(int32_t n, int32_t H0, int32_t W0, int32_t H, int32_t W, int32_t method,
-                                      int32_t pixel_format);
-int hr_resize_frames_fmt(const uint8_t* src, int32_t n, int32_t H0, int32_t W0, uint8_t* dst, int32_t H, int32_t W,
-                         int64_t dst_row_stride, int32_t method, int32_t flags, int32_t pixel_format, void* workspace,
-                         int64_t workspace_bytes, void* stream);
+                     int64_t dst_row_stride, int32_t method, int32_t flags, int32_t pixel_format, void* workspace,
+                     int64_t workspace_bytes, void* stream);
 
 /* Number of kernels hr_render launched since creation (bench.py's gpu_launches). */
 int64_t hr_launch_count(const hr_handle* h);

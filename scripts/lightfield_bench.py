@@ -54,6 +54,9 @@ def main():
             fn.restype, fn.argtypes = L.EXPORTS[name]
             if name == "hr_generate_rays":
                 fn.argtypes = [C.c_void_p] + L.EXPORTS[name][1][1:]
+        if lib.hr_abi_version() < 24:  # the sampling entry points take a pixel format from ABI 24
+            for fn in (lib.hr_sample_train_batch, lib.hr_sample_train_rows):
+                fn.argtypes = fn.argtypes[:3] + fn.argtypes[4:]
         return lib
 
     def pinhole(v):
@@ -84,6 +87,7 @@ def main():
     def workloads(lib, host_cam, dev_cams):
         """name -> (kernel names, call)"""
         frame = torch.empty((W * H, 6), dtype=torch.float32, device=dev)
+        fmt = (L.PIXEL_RGB8,) if lib.hr_abi_version() >= 24 else ()
         w = {f"generate_rays {W}x{H}": (("generate_rays_kernel",), lambda: lib.hr_generate_rays(
             C.byref(host_cam), 6, 0, W * H, frame.data_ptr(), stream))}
         for B in (16384, 65536):
@@ -94,13 +98,13 @@ def main():
 
             def batch(B=B, coords=coords, rgb=rgb, weight=weight, state=state):
                 state[0] = (state[0] + 1) % (n_pix // B)
-                return lib.hr_sample_train_batch(dev_cams.data_ptr(), N_VIEWS, images.data_ptr(), H, W, 6, 0, 0, state[0], B,
-                                                 None, coords.data_ptr(), rgb.data_ptr(), weight.data_ptr(), None, None,
-                                                 stream)
+                return lib.hr_sample_train_batch(dev_cams.data_ptr(), N_VIEWS, images.data_ptr(), *fmt, H, W, 6, 0, 0,
+                                                 state[0], B, None, coords.data_ptr(), rgb.data_ptr(), weight.data_ptr(),
+                                                 None, None, stream)
 
             def rows(B=B, coords=coords, rgb=rgb, weight=weight, state=state):
                 state[0] += 1
-                return lib.hr_sample_train_rows(dev_cams.data_ptr(), N_VIEWS, images.data_ptr(), H, W, 6,
+                return lib.hr_sample_train_rows(dev_cams.data_ptr(), N_VIEWS, images.data_ptr(), *fmt, H, W, 6,
                                                 view_start.data_ptr(), view_rule.data_ptr(), n_pix, L.SAMPLE_REPLACE, 0, 0,
                                                 state[0], B, None, coords.data_ptr(), rgb.data_ptr(), weight.data_ptr(),
                                                 None, None, None, stream)

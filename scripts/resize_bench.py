@@ -94,7 +94,7 @@ def run(name, W0, H0, W, H, method, n, reps, rounds, host_reps):
         host_s = t if f == 0 else host_s
         checked.append(bool(np.array_equal(out[f].cpu().numpy(), ref)))
     moved = n * (H0 * W0 * 3 + H * W * 3)
-    ws = int(L.load_library().hr_resize_workspace_bytes(n, H0, W0, H, W, L.RESIZE_METHODS[method]))
+    ws = int(L.load_library().hr_resize_workspace_bytes(n, H0, W0, H, W, L.RESIZE_METHODS[method], L.PIXEL_RGB8))
     if method.startswith("pil"):
         moved += 2 * n * W * 3 * H0  # the intermediate (the rows the vertical pass reads: all of them here), written and read
     rate = moved / n / (ms * 1e-3)

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """RGBA frames against RGB frames on the device, for the three places a DoNeRF or Catacaustics frame is used:
 
-  batches   hr_sample_train_batch_fmt (the whole-image permutation) and hr_sample_train_rows_fmt (draws with replacement)
+  batches   hr_sample_train_batch (the whole-image permutation) and hr_sample_train_rows (draws with replacement)
             over 8 views of 800 x 800, at 16 384 and 65 536 rows per batch: RGBA reads one aligned 4-byte pixel and
             composites it over white, RGB reads three bytes
   score     score_views of a DoNeRF-shaped model (tests/cases.py donerf_s16) on 4 views of 800 x 800, per view
@@ -96,12 +96,12 @@ def bench_batches(timer, reps, warmup):
         rows = C.c_int64(0)
 
         def permute(images, fmt, i=3):
-            return lambda: L.check(lib.hr_sample_train_batch_fmt(
+            return lambda: L.check(lib.hr_sample_train_batch(
                 dcams.data_ptr(), n, images.data_ptr(), fmt, H, W, 6, 0, 0, i, B, None, coords.data_ptr(), col.data_ptr(),
                 w.data_ptr(), None, C.byref(rows), st))
 
         def replace(images, fmt, i=3):
-            return lambda: L.check(lib.hr_sample_train_rows_fmt(
+            return lambda: L.check(lib.hr_sample_train_rows(
                 dcams.data_ptr(), n, images.data_ptr(), fmt, H, W, 6, start.data_ptr(), rule.data_ptr(), n * H * W,
                 L.SAMPLE_REPLACE, 0, 0, i, B, None, coords.data_ptr(), col.data_ptr(), w.data_ptr(), None, None,
                 C.byref(rows), st))
@@ -155,9 +155,9 @@ def bench_resize(timer, reps, warmup):
             if ch == 4:
                 src[..., 3] = 255
             dst = torch.empty((n, H, W, ch), dtype=torch.uint8, device="cuda")
-            need = int(lib.hr_resize_workspace_bytes_fmt(n, H0, W0, H, W, m, fmt))
+            need = int(lib.hr_resize_workspace_bytes(n, H0, W0, H, W, m, fmt))
             ws = torch.empty(max(need, 1), dtype=torch.uint8, device="cuda")
-            calls[ch] = (lambda src=src, dst=dst, ws=ws, need=need, fmt=fmt, ch=ch: L.check(lib.hr_resize_frames_fmt(
+            calls[ch] = (lambda src=src, dst=dst, ws=ws, need=need, fmt=fmt, ch=ch: L.check(lib.hr_resize_frames(
                 src.data_ptr(), n, H0, W0, dst.data_ptr(), H, W, ch * W, m, 0, fmt, ws.data_ptr(), need, st)))
             calls[ch]()
             res.append((src, dst))

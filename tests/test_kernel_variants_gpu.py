@@ -80,12 +80,16 @@ def _template_args(text):
 def kernels_run(fn):
     """Template arguments of every render_kernel and render_bwd_kernel launched by fn(), from the profiler's CUDA events."""
     import re
+    import time
 
-    # the profiler now and then hands back no CUDA activity at all for a window; the call is then profiled again
-    for _ in range(3):
+    # The profiler now and then hands back no CUDA activity at all for a window: the kernel records of a short window can
+    # still be on their way from the device when the window closes.  The window therefore stays open a moment after the
+    # synchronise, and an empty window is profiled again.
+    for attempt in range(8):
         with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
             fn()
             torch.cuda.synchronize()
+            time.sleep(0.02 * (attempt + 1))
         names = {e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA}
         if names:
             break

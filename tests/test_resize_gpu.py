@@ -133,10 +133,10 @@ def test_refused_calls_write_nothing():
     with pytest.raises(ValueError, match="out must be"):
         hb.resize_frames(src, (20, 25), "cv2_linear", out=out.transpose(1, 2))
     lib = L.load_library()
-    need = int(lib.hr_resize_workspace_bytes(2, 30, 40, 20, 25, L.RESIZE_METHODS["pil_lanczos"]))
+    need = int(lib.hr_resize_workspace_bytes(2, 30, 40, 20, 25, L.RESIZE_METHODS["pil_lanczos"], L.PIXEL_RGB8))
     ws = torch.empty(need, dtype=torch.uint8, device="cuda")
     assert lib.hr_resize_frames(src.data_ptr(), 2, 30, 40, out.data_ptr(), 20, 25, 75, L.RESIZE_METHODS["pil_lanczos"], 0,
-                                ws.data_ptr(), need - 1, None) != 0
+                                L.PIXEL_RGB8, ws.data_ptr(), need - 1, None) != 0
     assert b"needed" in lib.hr_last_error()
     torch.cuda.synchronize()
     assert bool((out == 123).all()) and bool((out2 == 123).all())

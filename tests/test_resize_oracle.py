@@ -148,7 +148,7 @@ def test_c_entry_points_refuse_before_touching_the_device():
     """hr_resize_frames validates on the host before anything is enqueued: these calls fail without a GPU and without
     dereferencing their (fake) pointers."""
     lib = L.load_library()
-    ws = lib.hr_resize_workspace_bytes
+    ws = lambda *args: lib.hr_resize_workspace_bytes(*args, L.PIXEL_RGB8)
     assert ws(4, 2028, 2704, 1014, 1352, L.RESIZE_METHODS["cv2_linear"]) == 0  # the 2x INTER_AREA path needs no tables
     assert ws(4, 2028, 2704, 1014, 1352, L.RESIZE_METHODS["cv2_area"]) == 0
     assert ws(1, 30, 40, 30, 40, L.RESIZE_METHODS["pil_lanczos"]) == 0         # the copy
@@ -159,7 +159,7 @@ def test_c_entry_points_refuse_before_touching_the_device():
     assert ws(1, 30, 40, 20, 20, 7) == -1
     fake = 1 << 40
     def call(n=1, H0=30, W0=40, H=15, W=20, row=60, method=4, flags=0, wsp=None, wsb=0, src=fake, dst=fake):
-        return lib.hr_resize_frames(src, n, H0, W0, dst, H, W, row, method, flags, wsp, wsb, None)
+        return lib.hr_resize_frames(src, n, H0, W0, dst, H, W, row, method, flags, L.PIXEL_RGB8, wsp, wsb, None)
     # every call below is refused by the host checks (a valid call would launch; the GPU tests make those)
     cases = [(dict(src=None), "null"), (dict(method=9), "unknown method"), (dict(flags=2), "unknown flags"),
              (dict(n=0), "bad sizes"), (dict(H=31), "enlarges"), (dict(W=30, method=4), "integer factors"),
@@ -177,7 +177,7 @@ def test_size_limits():
     """Sizes whose bytes overflow int64 are refused (-1), and so are Pillow reductions that need more filter coefficients
     than Pillow itself allows (outSize > INT_MAX / (ksize * sizeof(double)): it raises MemoryError)."""
     lib = L.load_library()
-    ws = lib.hr_resize_workspace_bytes
+    ws = lambda *args: lib.hr_resize_workspace_bytes(*args, L.PIXEL_RGB8)
     big = 2 ** 31 - 1
     assert ws(big, big, big, 1, 1, L.RESIZE_METHODS["cv2_area"]) == -1
     assert ws(big, 4096, 4096, 2048, 2047, L.RESIZE_METHODS["pil_lanczos"]) > 2 ** 50  # large, but within int64

@@ -92,10 +92,10 @@ def test_refused_resizes_write_nothing():
     with pytest.raises(ValueError, match="cv2_linear"):
         hb.resize_frames(src, (25, 20), "cv2_linear", out=out, rgba=True)
     lib = L.load_library()
-    need = int(lib.hr_resize_workspace_bytes_fmt(2, 30, 40, 20, 25, L.RESIZE_METHODS["pil_bicubic"], L.PIXEL_RGBA8))
+    need = int(lib.hr_resize_workspace_bytes(2, 30, 40, 20, 25, L.RESIZE_METHODS["pil_bicubic"], L.PIXEL_RGBA8))
     ws = torch.empty(need, dtype=torch.uint8, device="cuda")
-    assert lib.hr_resize_frames_fmt(src.data_ptr(), 2, 30, 40, out.data_ptr(), 20, 25, 100, L.RESIZE_METHODS["pil_bicubic"],
-                                    0, L.PIXEL_RGBA8, ws.data_ptr(), need - 1, None) != 0
+    assert lib.hr_resize_frames(src.data_ptr(), 2, 30, 40, out.data_ptr(), 20, 25, 100, L.RESIZE_METHODS["pil_bicubic"], 0,
+                                L.PIXEL_RGBA8, ws.data_ptr(), need - 1, None) != 0
     assert b"needed" in lib.hr_last_error()
     torch.cuda.synchronize()
     assert bool((out == 123).all())
@@ -186,8 +186,8 @@ def test_refused_batch_calls_write_nothing():
     unaligned = torch.empty(rgba.numel() + 4, dtype=torch.uint8, device="cuda")[1:]
     for images, fmt, msg in ((rgba.data_ptr(), 2, b"unknown pixel format"),
                              (unaligned.data_ptr(), L.PIXEL_RGBA8, b"RGBA images need 4 bytes")):
-        assert lib.hr_sample_train_batch_fmt(dcams.data_ptr(), 3, images, fmt, H, W, 8, 0, 0, 0, 16, None, coords.data_ptr(),
-                                             rgb.data_ptr(), weight.data_ptr(), None, C.byref(n_rows), None) != 0
+        assert lib.hr_sample_train_batch(dcams.data_ptr(), 3, images, fmt, H, W, 8, 0, 0, 0, 16, None, coords.data_ptr(),
+                                         rgb.data_ptr(), weight.data_ptr(), None, C.byref(n_rows), None) != 0
         assert msg in lib.hr_last_error()
     torch.cuda.synchronize()
     assert bool((coords == -3).all()) and bool((rgb == -3).all()) and bool((weight == -3).all())
@@ -292,8 +292,8 @@ def test_refused_scores_leave_the_output_untouched():
     unaligned = torch.empty(images.numel() + 4, dtype=torch.uint8, device="cuda")[2:]
     for gt, fmt, msg in ((images.data_ptr(), 5, b"unknown pixel format"),
                          (unaligned.data_ptr(), L.PIXEL_RGBA8, b"4-byte aligned")):
-        assert lib.hr_score_views_fmt(model._handle, recs, tt, 3, gt, fmt, out.data_ptr(), ws.data_ptr(), need,
-                                      torch.cuda.current_stream().cuda_stream) != 0
+        assert lib.hr_score_views(model._handle, recs, tt, 3, gt, fmt, out.data_ptr(), ws.data_ptr(), need,
+                                  torch.cuda.current_stream().cuda_stream) != 0
         assert msg in lib.hr_last_error()
     torch.cuda.synchronize()
     assert bool((out == -7.0).all())

@@ -170,13 +170,15 @@ def test_score_views_rgba_refusals():
 
 
 def test_c_entry_points_refuse_before_touching_the_device():
-    """The RGBA entry points validate on the host before anything is enqueued: these calls fail without a GPU and without
+    """The entry points validate RGBA calls on the host before anything is enqueued: these calls fail without a GPU and without
     dereferencing their (fake) pointers."""
     lib = L.load_library()
-    ws = lib.hr_resize_workspace_bytes_fmt
+    ws = lib.hr_resize_workspace_bytes
     pil, lin, area = (L.RESIZE_METHODS[m] for m in ("pil_bicubic", "cv2_linear", "cv2_area"))
-    for args in ((2, 3024, 4032, 378, 504, pil), (1, 30, 40, 20, 25, pil), (1, 30, 40, 15, 20, area)):
-        assert ws(*args, L.PIXEL_RGB8) == lib.hr_resize_workspace_bytes(*args)
+    # RGB workspaces as they were before the entry points took a pixel format
+    for args, need in (((2, 3024, 4032, 378, 504, pil), 9268224), ((1, 30, 40, 20, 25, pil), 4352),
+                       ((1, 30, 40, 15, 20, area), 0)):
+        assert ws(*args, L.PIXEL_RGB8) == need, args
     # the tables are the same; the intermediate holds 4 bytes per pixel instead of 3
     n, H0, W0, H, W = 2, 300, 400, 150, 130
     rgb, rgba = ws(n, H0, W0, H, W, pil, L.PIXEL_RGB8), ws(n, H0, W0, H, W, pil, L.PIXEL_RGBA8)
@@ -186,7 +188,7 @@ def test_c_entry_points_refuse_before_touching_the_device():
     fake = 1 << 40
 
     def resize(H=15, W=20, row=80, method=pil, fmt=L.PIXEL_RGBA8):
-        return lib.hr_resize_frames_fmt(fake, 1, 30, 40, fake, H, W, row, method, 0, fmt, None, 0, None)
+        return lib.hr_resize_frames(fake, 1, 30, 40, fake, H, W, row, method, 0, fmt, None, 0, None)
 
     for kw, msg in ((dict(fmt=7), "unknown pixel format"), (dict(method=lin), "cv2_linear is not supported for RGBA"),
                     (dict(row=79), "dst_row_stride"), (dict(), "workspace")):
@@ -195,12 +197,11 @@ def test_c_entry_points_refuse_before_touching_the_device():
     assert resize(method=area, row=79) != 0 and "dst_row_stride 79" in lib.hr_last_error().decode()
 
     def batch(images=fake, fmt=L.PIXEL_RGBA8):
-        return lib.hr_sample_train_batch_fmt(fake, 1, images, fmt, 4, 4, 8, 0, 0, 0, 4, None, fake, fake, fake, None, None,
-                                             None)
+        return lib.hr_sample_train_batch(fake, 1, images, fmt, 4, 4, 8, 0, 0, 0, 4, None, fake, fake, fake, None, None, None)
 
     def rows(images=fake, fmt=L.PIXEL_RGBA8):
-        return lib.hr_sample_train_rows_fmt(fake, 1, images, fmt, 4, 4, 8, fake, fake, 16, L.SAMPLE_PERMUTE, 0, 0, 0, 4,
-                                            None, fake, fake, fake, None, None, None, None)
+        return lib.hr_sample_train_rows(fake, 1, images, fmt, 4, 4, 8, fake, fake, 16, L.SAMPLE_PERMUTE, 0, 0, 0, 4, None,
+                                        fake, fake, fake, None, None, None, None)
 
     for fn in (batch, rows):
         assert fn(fmt=2) != 0 and "unknown pixel format 2" in lib.hr_last_error().decode()

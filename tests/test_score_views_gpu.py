@@ -210,7 +210,7 @@ def test_refusals_leave_the_output_untouched():
     def call(recs, times, n=3, gt=images.data_ptr(), dst=out.data_ptr(), wsp=ws.data_ptr(), ws_bytes=need):
         arr = (L.hr_camera * len(recs))(*recs)
         tt = (C.c_float * len(times))(*times)
-        return lib.hr_score_views(model._handle, arr, tt, n, gt, dst, wsp, ws_bytes, stream)
+        return lib.hr_score_views(model._handle, arr, tt, n, gt, L.PIXEL_RGB8, dst, wsp, ws_bytes, stream)
 
     good = [c.to_c() for c in cams]
     nan_pose = [c.to_c() for c in cams]

@@ -158,8 +158,8 @@ def test_refusals():
 
     def call(batch_index=0, c_in=8, coords=out.data_ptr(), batch_size=1000):
         n = C.c_int64(-1)
-        rc = lib.hr_sample_train_batch(d.cameras.data_ptr(), 3, d.images.data_ptr(), H, W, c_in, 0, 0, batch_index, batch_size,
-                                       None, coords, rgb.data_ptr(), w.data_ptr(), None, C.byref(n), st)
+        rc = lib.hr_sample_train_batch(d.cameras.data_ptr(), 3, d.images.data_ptr(), L.PIXEL_RGB8, H, W, c_in, 0, 0,
+                                       batch_index, batch_size, None, coords, rgb.data_ptr(), w.data_ptr(), None, C.byref(n), st)
         return rc, n.value, lib.hr_last_error().decode()
 
     assert call()[:2] == (0, 1000)

@@ -259,7 +259,7 @@ def test_malformed_plans_and_rows_give_zero_rows_and_the_c_abi_refuses():
              start=d._view_start, rule=d._view_rule, coords_ptr=coords.data_ptr(), start_ptr=None):
         out = C.c_int64(-1)
         rc = lib.hr_sample_train_rows(
-            d.cameras.data_ptr(), n_views, d.images.data_ptr(), height, W, c_in,
+            d.cameras.data_ptr(), n_views, d.images.data_ptr(), L.PIXEL_RGB8, height, W, c_in,
             start.data_ptr() if start_ptr is None else start_ptr, rule.data_ptr(),
             d.n_rows if n_table is None else n_table, mode, 0, 0, batch_index, batch_size,
             rows.data_ptr() if rows is not None else None, coords_ptr, rgb.data_ptr(), w.data_ptr(), pids.data_ptr(),
