@@ -7,7 +7,8 @@ training images: ``DeviceRayBatches`` (train_data.py); decoded frames
 resized to the training resolution as the datasets' ``get_rgb`` resizes them: ``resize_frames`` / ``dataset_frames`` (resize.py).  All compute is in ``libhyperreel_b200.so`` (csrc/, sm_90a CUDA behind the C-ABI of include/hyperreel_b200.h).
 """
 from . import camera, configs, lightfield, metrics, rays, resize, train_data  # noqa: F401
-from .camera import Camera, TwoPlaneCamera, generate_rays, render_video, score_views, spiral_path  # noqa: F401
+from .camera import (Camera, TwoPlaneCamera, VisualRequest, embedding_requests, generate_rays, render_embeddings,  # noqa: F401
+                     render_video, score_views, spiral_path)
 from .lightfield import lightfield_cameras, stanford_file_coords  # noqa: F401
 from .config import Cfg, epochs_to_iters, load_model_yaml, to_cfg  # noqa: F401
 from .models import LightfieldModel, model_dict  # noqa: F401
@@ -17,7 +18,7 @@ from .signature import Signature, UnsupportedPipeline, lower  # noqa: F401
 from .system import INRSystem  # noqa: F401
 from .train_data import DeviceRayBatches, importance_subsample_plan, regular_subsample_plan  # noqa: F401
 
-__all__ = ["camera", "Camera", "TwoPlaneCamera", "generate_rays", "render_video", "score_views", "spiral_path", "lightfield", "lightfield_cameras",
+__all__ = ["camera", "Camera", "TwoPlaneCamera", "generate_rays", "render_video", "score_views", "render_embeddings", "embedding_requests", "VisualRequest", "spiral_path", "lightfield", "lightfield_cameras",
            "stanford_file_coords", "resize", "resize_frames", "dataset_frames", "configs", "metrics", "rays", "train_data", "DeviceRayBatches", "importance_subsample_plan", "regular_subsample_plan", "Cfg", "to_cfg", "load_model_yaml", "epochs_to_iters", "LightfieldModel", "model_dict",
            "RenderLightfield", "render_chunked", "render_fn_dict", "Signature", "UnsupportedPipeline", "lower",
            "INRSystem"]

@@ -303,6 +303,86 @@ def score_views(model_or_system, cameras: Sequence[Camera], images: torch.Tensor
     return target.score_views(cameras, images, times, out=out, stream=stream, rgba=rgba)
 
 
+@dataclass(frozen=True)
+class VisualRequest:
+    """One map of the embedding visualiser: field ``key`` of the colour net reduced in ``mode`` (lib.FIELD_OVER or
+    FIELD_PRED_WEIGHTS) over ``channels`` channels, then visualize_warp's options: ``use_abs``, ``bounds`` (lo, hi) rounded to
+    float32 or None, ``normalize``."""
+    key: str
+    mode: int
+    channels: int
+    use_abs: bool
+    bounds: Optional[Tuple[float, float]]
+    normalize: bool
+
+
+def embedding_requests(visualizer) -> list:
+    """The maps of an embedding-visualiser config (``cfg.visualizers.embedding``, or a loaded
+    conf/experiment/visualizers/embedding/*.yaml) as VisualRequests, in the config's order.  Supported: every field the fused
+    path carries (lib.FIELDS), reduced over the samples (``pred_weights_fields`` selects the predicted weights), with
+    ``use_abs``, scalar ``bounds`` and ``normalize``, and ``sort: False``.  ``data_fields`` (raw dumps) are not maps and are
+    ignored.  Anything else raises UnsupportedPipeline naming the key: another visualiser type, a field the path does not
+    carry, a field in ``no_over_fields`` (per-sample channels), ``sort: True`` (data-dependent channels), or bounds that are
+    not two finite float32 numbers with hi != lo."""
+    from .signature import UnsupportedPipeline
+
+    kind = visualizer.get("type", "embedding")
+    if kind != "embedding":
+        raise UnsupportedPipeline(f"visualiser type '{kind}' is not supported: only 'embedding' maps are rendered")
+    no_over = set(visualizer.get("no_over_fields", None) or [])
+    pred_w = set(visualizer.get("pred_weights_fields", None) or [])
+    out = []
+    for key, opts in (visualizer.get("fields", None) or {}).items():
+        opts = dict(opts or {})
+        if key not in L.FIELDS:
+            raise UnsupportedPipeline(f"embedding visualiser: field '{key}' is not produced by the fused path")
+        if key in no_over:
+            raise UnsupportedPipeline(f"embedding visualiser: field '{key}' is in no_over_fields: per-sample channels are not mapped")
+        if opts.get("sort", False):
+            raise UnsupportedPipeline(f"embedding visualiser: field '{key}' has sort: True, which is not supported")
+        bounds = opts.get("bounds", None)
+        if bounds is not None and len(bounds) > 0:
+            try:
+                with np.errstate(over="ignore"):
+                    lo, hi = (np.float32(float(b)) for b in bounds)
+            except (TypeError, ValueError):
+                raise UnsupportedPipeline(f"embedding visualiser: field '{key}': bounds must be [lo, hi], got {bounds!r}") from None
+            if len(bounds) != 2 or not (np.isfinite(lo) and np.isfinite(hi)) or lo == hi:
+                raise UnsupportedPipeline(f"embedding visualiser: field '{key}': bounds must be two finite float32 numbers "
+                                          f"with hi != lo, got {bounds!r}")
+            bounds = (float(lo), float(hi))
+        else:
+            bounds = None
+        out.append(VisualRequest(key, L.FIELD_PRED_WEIGHTS if key in pred_w else L.FIELD_OVER, L.FIELD_CHANNELS[key],
+                                 bool(opts.get("use_abs", False)), bounds, bool(opts.get("normalize", False))))
+    return out
+
+
+def render_embeddings(model_or_system, cameras: Sequence[Camera], visualizer, times=None, rgb: bool = True, stream=None):
+    """The embedding visualiser's maps of every frame (EmbeddingVisualizer.validation, nlf/visualizers/embedding.py:37-90, with
+    visualize_warp and to8b, utils/visualization.py:24-52, utils/__init__.py:47) of a LightfieldModel, RenderLightfield or
+    INRSystem along ``cameras`` at ``times`` (default each camera's ``time``), on the device in the render pass that makes
+    the RGB frame (hr_render_visuals): one call that never synchronises.  ``visualizer`` is an embedding-visualiser config
+    (see embedding_requests).  Returns a dict of device uint8 stacks keyed as the reference names the maps:
+    'embedding_<key>' [F, H, W] for a 1-channel field (the grayscale image it saves) or [F, H, W, 3], and, with ``rgb``,
+    'rgb' [F, H, W, 3], bit for bit render_video's.  Each map equals visualize_warp + to8b applied to the fp32 field that
+    ``forward(rays, {'fields': [key]})`` returns for the frame's rays."""
+    target = model_or_system if hasattr(model_or_system, "render_visuals") else getattr(model_or_system, "model", None)
+    if target is None or not hasattr(target, "render_visuals"):
+        raise TypeError(f"render_embeddings: expected a LightfieldModel, RenderLightfield or INRSystem, got {type(model_or_system)}")
+    requests = embedding_requests(visualizer)
+    return keyed_maps(requests, *target.render_visuals(cameras, requests, times, rgb=rgb, stream=stream))
+
+
+def keyed_maps(requests, video, maps, prefix: str = "") -> dict:
+    """render_visuals' outputs under the reference's names: prefix + 'rgb' (when rendered) and prefix + 'embedding_<key>',
+    a 1-channel map as [F, H, W]."""
+    out = {} if video is None else {prefix + "rgb": video}
+    for r in requests:
+        out[f"{prefix}embedding_{r.key}"] = maps[r.key][..., 0] if r.channels == 1 else maps[r.key]
+    return out
+
+
 def generate_rays(camera: Camera, c_in: int = 8, device: Optional[torch.device] = None, first_pixel: int = 0,
                   n_pixels: Optional[int] = None) -> torch.Tensor:
     """rays [n, c_in] fp32 on the device for pixels ``first_pixel ... first_pixel + n - 1`` (row-major)."""

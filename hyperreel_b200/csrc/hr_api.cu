@@ -31,6 +31,7 @@ cudaError_t launch_image_metrics_u8(const float* pred, const uint8_t* gt, int32_
                                     double* partial, cudaStream_t st);
 cudaError_t launch_image_metrics_rgba8(const float* pred, const uint8_t* gt, int32_t n, int32_t H, int32_t W, double* out,
                                        double* partial, cudaStream_t st);
+cudaError_t launch_vis_normalize(const float* x, int nf, long long px, int dim, const VisMap& m, float* part, cudaStream_t st);
 }  // namespace hr
 
 static thread_local std::string g_err;
@@ -799,6 +800,7 @@ static int render_impl(hr_handle* h, const float* rays, int64_t n, float* rgb, f
       if (so_off.weights) so_off.weights += off * S;
       if (so_off.rgb_samples) so_off.rgb_samples += off * S * 3;
       for (int f = 0; f < HR_N_FIELDS; ++f) {
+        if (so_off.field_u8[f].out) so_off.field_u8[f].out += off * kFieldWidth[f];
         if (!so_off.field_out[f]) continue;
         so_off.field_out[f] += off * kFieldWidth[f] * (so_off.field_mode[f] == HR_FIELD_NO_OVER ? S : 1);
       }
@@ -852,6 +854,16 @@ int hr_render_stages(hr_handle* h, const float* rays, int64_t n_rays, float* rgb
   return render_impl(h, rays, n_rays, rgb, mlp_out, &so, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
+// Whether the pipeline carries field f (the reference fails with a KeyError on x[key] otherwise): refused with fn's name, or 0
+static int field_refusal(const char* fn, const hr_config& c, int f) {
+  if ((f == HR_FIELD_BASE_TIMES || f == HR_FIELD_TIME_OFFSET) && !(c.dynamic || c.use_flow))
+    return hr_fail("%s: this pipeline has no keyframe times", fn);
+  const int head_off[HR_N_FIELDS] = {0, 0, 0, 0, 0, 0, 0, c.off_cscale, c.off_cshift, c.off_flow, c.off_sigma,
+                                     c.off_point_sigma, c.off_offset, c.off_cscale_global, c.off_cshift_global};
+  if (f >= HR_FIELD_COLOR_SCALE && head_off[f] < 0) return hr_fail("%s: the sample net has no head for field %d", fn, f);
+  return 0;
+}
+
 int hr_render_fields(hr_handle* h, const float* rays, int64_t n_rays, float* rgb, float* render_weights,
                      const hr_field_request* req, int32_t n_req, void* workspace, int64_t workspace_bytes, void* stream) {
   if (!h) return hr_fail("hr_render_fields: null handle");
@@ -866,12 +878,7 @@ int hr_render_fields(hr_handle* h, const float* rays, int64_t n_rays, float* rgb
     if (m != HR_FIELD_OVER && m != HR_FIELD_NO_OVER && m != HR_FIELD_PRED_WEIGHTS) return hr_fail("hr_render_fields: unknown mode %d", m);
     if (!req[i].out) return hr_fail("hr_render_fields: null output for field %d", f);
     if (so.field_out[f]) return hr_fail("hr_render_fields: field %d requested twice", f);
-    // fields the pipeline does not carry (reference: KeyError on x[key])
-    if ((f == HR_FIELD_BASE_TIMES || f == HR_FIELD_TIME_OFFSET) && !(c.dynamic || c.use_flow))
-      return hr_fail("hr_render_fields: this pipeline has no keyframe times");
-    const int head_off[HR_N_FIELDS] = {0, 0, 0, 0, 0, 0, 0, c.off_cscale, c.off_cshift, c.off_flow, c.off_sigma,
-                                       c.off_point_sigma, c.off_offset, c.off_cscale_global, c.off_cshift_global};
-    if (f >= HR_FIELD_COLOR_SCALE && head_off[f] < 0) return hr_fail("hr_render_fields: the sample net has no head for field %d", f);
+    if (field_refusal("hr_render_fields", c, f)) return 1;
     so.field_out[f] = req[i].out;
     so.field_mode[f] = m;
   }
@@ -1213,6 +1220,219 @@ int hr_score_views(hr_handle* h, const hr_camera* cameras, const float* times, i
         break;
       }
       h->launches += 2;
+      next = f_end;
+    }
+    if (lay.n_slots == 2 && (e = cudaEventRecord(done[k], s)) != cudaSuccess) {
+      rc = fail("event record", e);
+      break;
+    }
+    off += m;
+  }
+  if (lay.n_slots == 2) {  // join, also after a failed launch: the caller's stream must not run ahead of enqueued work
+    for (int k = 0; k < 2; ++k) {
+      cudaEvent_t ev;
+      if (new_event(&ev)) break;
+      CK(cudaEventRecord(ev, ss[k]));
+      CK(cudaStreamWaitEvent(st, ev, 0));
+    }
+  }
+  for (cudaEvent_t ev : evs) cudaEventDestroy(ev);
+  return rc;
+}
+
+// ---- embedding maps: every request mapped in the render epilogue, or staged in a ring of whole frames and normalised
+// The requests' checks; *norm_ch: channels of the normalize requests, each of which has a ring of its own.
+static int check_visual_requests(const char* fn, const hr_handle* h, const hr_visual_request* req, int32_t n_req, int* norm_ch) {
+  if (n_req < 0 || (n_req > 0 && !req)) return hr_fail("%s: bad request list", fn);
+  *norm_ch = 0;
+  bool seen[HR_N_FIELDS] = {};
+  for (int i = 0; i < n_req; ++i) {
+    const hr_visual_request& r = req[i];
+    if (r.field < 0 || r.field >= HR_N_FIELDS) return hr_fail("%s: request %d: unknown field %d", fn, i, r.field);
+    if (r.mode != HR_FIELD_OVER && r.mode != HR_FIELD_PRED_WEIGHTS)
+      return hr_fail("%s: request %d: mode %d is not HR_FIELD_OVER or HR_FIELD_PRED_WEIGHTS", fn, i, r.mode);
+    if (seen[r.field]) return hr_fail("%s: field %d requested twice", fn, r.field);
+    seen[r.field] = true;
+    if (r.channels != kFieldWidth[r.field])
+      return hr_fail("%s: request %d: field %d has %d channels, not %d", fn, i, r.field, kFieldWidth[r.field], r.channels);
+    if (!r.out) return hr_fail("%s: request %d: null output", fn, i);
+    if (r.bounded && !(std::isfinite(r.lo) && std::isfinite(r.hi) && r.hi != r.lo))
+      return hr_fail("%s: request %d: bounds [%g, %g] must be finite with hi != lo", fn, i, r.lo, r.hi);
+    if (field_refusal(fn, h->cfg, r.field)) return 1;
+    if (r.normalize) *norm_ch += r.channels;
+  }
+  return 0;
+}
+
+// Workspace layout (each part 256-byte aligned): two record windows (the frames one sub-batch touches), the rings of the
+// normalize requests (ring frames each, in request order), two partial buffers (one per stream), then the video path's one or
+// two slots.  Without a normalize request there is no ring and the sub-batches are not cut.
+struct VisLayout {
+  int64_t sub, win, ring, win_cams, win_times, ring_off, ring_bytes_per_ch, partial_off, partial_bytes, slots_off, slot_bytes, total;
+  int n_slots;
+};
+
+static bool visual_layout(const hr_handle* h, int norm_ch, int32_t n_frames, int32_t height, int32_t width, VisLayout* L) {
+  const int64_t n = video_rays(n_frames, height, width);
+  if (!h || n < 0) return false;
+  const int64_t frame_px = (int64_t)height * width;
+  L->sub = video_sub_rays(h, n);
+  L->win = (L->sub + frame_px - 1) / frame_px + 1;
+  if (L->win > n_frames) L->win = n_frames;
+  L->ring = norm_ch ? score_ring_frames(L->sub, frame_px, n_frames) : 0;
+  if (L->ring < 0) return false;
+  L->n_slots = n > L->sub ? 2 : 1;
+  L->win_cams = align256(L->win * (int64_t)sizeof(hr_camera));
+  L->win_times = align256(L->win * (int64_t)sizeof(float));
+  L->ring_off = 2 * (L->win_cams + L->win_times);
+  int64_t ring_bytes;
+  if (__builtin_mul_overflow(L->ring * frame_px, (int64_t)(norm_ch * sizeof(float)), &ring_bytes)) return false;
+  L->ring_bytes_per_ch = L->ring * frame_px * (int64_t)sizeof(float);
+  L->partial_off = L->ring_off + align256(ring_bytes) + 256 * norm_ch;  // each request's ring starts 256-byte aligned
+  L->partial_bytes = align256(L->ring * hr::kVisBlocks * 6 * (int64_t)sizeof(float));
+  L->slots_off = L->partial_off + 2 * L->partial_bytes;
+  L->slot_bytes = video_slot_bytes(h, L->sub);
+  L->total = L->slots_off + L->n_slots * L->slot_bytes;
+  return true;
+}
+
+int64_t hr_render_visuals_workspace_bytes(const hr_handle* h, const hr_visual_request* req, int32_t n_req, int32_t n_frames,
+                                          int32_t height, int32_t width) {
+  int norm_ch = 0;
+  VisLayout L;
+  if (!h || check_visual_requests("hr_render_visuals_workspace_bytes", h, req, n_req, &norm_ch)) return -1;
+  if (visual_layout(h, norm_ch, n_frames, height, width, &L)) return L.total;
+  hr_fail("hr_render_visuals_workspace_bytes: %d frames of %d x %d pixels: bad size or bytes overflow int64", n_frames, width, height);
+  return -1;
+}
+
+// hr_score_views' walk: one ray sequence in the video path's sub-batches on two streams, each sub-batch also cut where it would
+// wrap the ring.  A sub-batch renders the video's pixels, the epilogue-mapped requests' bytes and the normalize requests' fp32
+// fields (into the ring) in one render launch; when it completes frames it reduces and maps them, per normalize request, on its
+// own stream, after the other stream's last render when a frame straddles the two.  A ring frame is rendered again only after
+// the map launch of the frame it held.
+int hr_render_visuals(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_frames, uint8_t* video,
+                      const hr_visual_request* req, int32_t n_req, void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* fn = "hr_render_visuals";
+  if (!h || !cameras || !times || !workspace) return hr_fail("%s: null argument", fn);
+  if (!h->uploaded) return hr_fail("%s: parameters not uploaded", fn);
+  if (n_frames < 1) return hr_fail("%s: n_frames must be >= 1, got %d", fn, n_frames);
+  int norm_ch = 0;
+  if (check_visual_requests(fn, h, req, n_req, &norm_ch)) return 1;
+  if (!video && n_req == 0) return hr_fail("%s: nothing to write (no video and no request)", fn);
+  const int32_t W = cameras[0].width, H = cameras[0].height;
+  VisLayout lay;
+  if (!visual_layout(h, norm_ch, n_frames, H, W, &lay))
+    return hr_fail("%s: %d frames of %d x %d pixels: bad size or bytes overflow int64", fn, n_frames, W, H);
+  bool mixed = false;
+  if (check_frames(fn, cameras, times, n_frames, &mixed)) return 1;
+  if (((uintptr_t)workspace & 15) != 0) return hr_fail("%s: workspace must be 16-byte aligned", fn);
+  if (workspace_bytes < lay.total)
+    return hr_fail("%s: workspace too small (%lld < %lld)", fn, (long long)workspace_bytes, (long long)lay.total);
+  DeviceGuard guard(h->device);
+  const hr_config& c = h->cfg;
+  cudaStream_t st = (cudaStream_t)stream;
+  char* base = (char*)workspace;
+  const int64_t frame_px = (int64_t)W * H, n = frame_px * n_frames, ring_rays = lay.ring * frame_px;
+  const int64_t rays_bytes = align256(lay.sub * c.c_in * (int64_t)sizeof(float));
+  // the render's outputs for a sub-batch starting at ray 0 of the video and of the ring; render_visuals moves them along
+  hr::ExtraOut so{};
+  std::vector<float*> ring_of(n_req, nullptr);
+  int64_t ring_at = lay.ring_off;
+  for (int i = 0; i < n_req; ++i) {
+    const hr_visual_request& r = req[i];
+    hr::VisMap m{r.out, r.use_abs ? 1 : 0, r.bounded ? 1 : 0, r.lo, r.bounded ? r.hi - r.lo : 1.0f};
+    so.field_mode[r.field] = r.mode;
+    so.field_u8[r.field] = m;
+    if (r.normalize) {
+      ring_of[i] = (float*)(base + ring_at);
+      ring_at += align256(lay.ring_bytes_per_ch * r.channels);
+    }
+  }
+  hr::RgbDst no_rgb{};  // n = 0: the render stores no colour
+  cudaStream_t ss[2] = {st, st};
+  std::vector<cudaEvent_t> evs;  // every event of the call, destroyed at the end (a destroyed event's pending work still runs)
+  auto new_event = [&](cudaEvent_t* ev) -> int {
+    CK(cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
+    evs.push_back(*ev);
+    return 0;
+  };
+  // mapped[k]: recorded after the map launches that read ring frame k last; done[s]: after stream s's last render
+  std::vector<cudaEvent_t> mapped(lay.n_slots == 2 ? lay.ring : 0, nullptr);
+  cudaEvent_t done[2] = {nullptr, nullptr};
+  int rc = 0;
+  if (lay.n_slots == 2) {
+    cudaEvent_t fork;
+    for (int i = 0; i < 2; ++i) {
+      if (pipe_stream(h, i)) return 1;
+      ss[i] = h->pipe.streams[i];
+    }
+    if (new_event(&fork)) return 1;
+    CK(cudaEventRecord(fork, st));
+    CK(cudaStreamWaitEvent(ss[0], fork, 0));
+    CK(cudaStreamWaitEvent(ss[1], fork, 0));
+    for (auto& e : mapped)
+      if ((rc = new_event(&e))) break;
+    for (int i = 0; i < 2 && !rc; ++i) rc = new_event(&done[i]);
+  }
+  int64_t next = 0;  // first frame not yet mapped (normalize requests)
+  int64_t i = 0;
+  for (int64_t off = 0; off < n && !rc; ++i) {
+    const int k = (int)(i % 2);
+    cudaStream_t s = ss[k];
+    const int64_t pos = ring_rays ? off % ring_rays : 0;
+    int64_t m = n - off < lay.sub ? n - off : lay.sub;
+    if (ring_rays && pos + m > ring_rays) m = ring_rays - pos;
+    const int64_t f0 = off / frame_px, f1 = (off + m - 1) / frame_px, f_end = (off + m) / frame_px;
+    auto fail = [&](const char* what, cudaError_t e) { return hr_fail("%s: %s: %s", fn, what, cudaGetErrorString(e)); };
+    cudaError_t e = cudaSuccess;
+    if (ring_rays && lay.n_slots == 2)  // ring frames rendered again: after the map launches of the frames they held
+      for (int64_t f = f0 < lay.ring ? lay.ring : f0; f <= f1 && e == cudaSuccess; ++f)
+        e = cudaStreamWaitEvent(s, mapped[f % lay.ring], 0);
+    hr_camera* win_c = (hr_camera*)(base + k * (lay.win_cams + lay.win_times));
+    float* win_t = (float*)((char*)win_c + lay.win_cams);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(win_c, cameras + f0, (size_t)(f1 - f0 + 1) * sizeof(hr_camera), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(win_t, times + f0, (size_t)(f1 - f0 + 1) * sizeof(float), cudaMemcpyHostToDevice, s);
+    if (e != cudaSuccess) {
+      rc = fail("record copy", e);
+      break;
+    }
+    char* slot = base + lay.slots_off + (i % lay.n_slots) * lay.slot_bytes;
+    e = hr::launch_generate_video_rays(win_c, win_t, mixed, c.c_in, W, frame_px, off - f0 * frame_px, m, (float*)slot, s);
+    if (e != cudaSuccess) {
+      rc = fail("ray generation", e);
+      break;
+    }
+    h->launches += 1;
+    hr::ExtraOut so_b = so;
+    for (int r = 0; r < n_req; ++r) {
+      const int f = req[r].field;
+      if (ring_of[r]) {  // staged in fp32 at its ring position; mapped when the frame completes
+        so_b.field_out[f] = ring_of[r] + pos * req[r].channels;
+        so_b.field_u8[f].out = nullptr;
+      } else {
+        so_b.field_u8[f].out += off * req[r].channels;
+      }
+    }
+    rc = render_impl(h, (const float*)slot, m, nullptr, nullptr, &so_b, slot + rays_bytes, lay.slot_bytes - rays_bytes, s,
+                     video ? video + off * 3 : nullptr, video ? nullptr : &no_rgb);
+    if (rc) break;
+    if (ring_rays && f_end > next) {  // frames next .. f_end - 1 are complete, in consecutive ring frames
+      if (lay.n_slots == 2 && next * frame_px < off) e = cudaStreamWaitEvent(s, done[1 - k], 0);
+      float* part = (float*)(base + lay.partial_off + k * lay.partial_bytes);
+      for (int r = 0; r < n_req && e == cudaSuccess; ++r) {
+        if (!ring_of[r]) continue;
+        hr::VisMap vm = so.field_u8[req[r].field];
+        vm.out += next * frame_px * req[r].channels;
+        e = hr::launch_vis_normalize(ring_of[r] + (next % lay.ring) * frame_px * req[r].channels, (int)(f_end - next), frame_px,
+                                     req[r].channels, vm, part, s);
+        h->launches += 2;
+      }
+      for (int64_t f = next; f < f_end && e == cudaSuccess && lay.n_slots == 2; ++f) e = cudaEventRecord(mapped[f % lay.ring], s);
+      if (e != cudaSuccess) {
+        rc = fail("map launch", e);
+        break;
+      }
       next = f_end;
     }
     if (lay.n_slots == 2 && (e = cudaEventRecord(done[k], s)) != cudaSuccess) {

@@ -61,6 +61,30 @@ struct RgbDst {
   long long row0;
 };
 
+// The elementwise steps of one embedding map (visualize_warp, utils/visualization.py:24-52): |x| when use_abs, then
+// (x - lo) / den when bounded, den = hi - lo rounded once in fp32.  `out` is the map's uint8 [n, dim] when the render
+// epilogue finishes it (no normalize), null otherwise.
+struct VisMap {
+  unsigned char* out;
+  int use_abs, bounded;
+  float lo, den;
+};
+
+// blocks per frame of the normalize reduction (hr_visual.cu): each writes one min / max partial per channel
+constexpr int kVisBlocks = 64;
+
+__device__ __forceinline__ float vis_pre(const VisMap& m, float x) {
+  if (m.use_abs) x = fabsf(x);
+  if (m.bounded) x = __fdiv_rn(__fsub_rn(x, m.lo), m.den);
+  return x;
+}
+
+// clamp(0, 1) then to8b (utils/__init__.py:47): (uint8)(255 * x), truncated.  A NaN clamps to NaN and NumPy casts it to 0;
+// fmaxf(NaN, 0) is 0, which gives the same byte.
+__device__ __forceinline__ unsigned char vis_to8b(float x) {
+  return (unsigned char)(int)__fmul_rn(255.0f, fminf(fmaxf(x, 0.0f), 1.0f));
+}
+
 // Outputs beyond rgb, produced by the EXTRA variant of the render kernel (all pointers may be null):
 //   * per-sample dumps for stage-boundary parity tests (hr_render_stages);
 //   * the extra composited fields of the reference's colour nets (tensorf_dynamic.py:808-837, tensorf_no_sample.py:254-278):
@@ -74,6 +98,7 @@ struct ExtraOut {
   float* rgb_samples;  // [n,S,3] shaded colour of every sample before the colour transform, 0 where w <= rm_weight_mask_thre
   float* field_out[HR_N_FIELDS];
   int field_mode[HR_N_FIELDS];
+  VisMap field_u8[HR_N_FIELDS];  // field_u8[f].out: the reduced field f (HR_FIELD_OVER / PRED_WEIGHTS) as a uint8 map instead
 };
 
 __device__ __forceinline__ float apply_act(const hr_act& a, float x) {

@@ -546,6 +546,8 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
     float carryT = 1.0f;
     float accw = 0.0f, accB[3] = {0.f, 0.f, 0.f};
     float csA[SPL][3];
+    // lane 0's running sums of the extra fields over the rounds before the last (EXTRA with several samples per lane)
+    [[maybe_unused]] float fpart[(EXTRA && SPL > 1) ? HR_N_FIELDS * 3 : 1];
 #pragma unroll
     for (int j = 0; j < SPL; ++j) {
       const int s = sl + 32 * j;
@@ -591,7 +593,8 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
 #pragma unroll 1
         for (int f = 0; f < HR_N_FIELDS; ++f) {
           float* fo = so.field_out[f];
-          if (fo == nullptr) continue;  // warp-uniform
+          unsigned char* fo8 = so.field_u8[f].out;
+          if (fo == nullptr && fo8 == nullptr) continue;  // warp-uniform
           const int mode = so.field_mode[f];
           // per-sample heads are x[name] = activation(raw) (ray.py:333-337); the other keys are built-ins of the pipeline
           int dim = 1, hoff = -1;
@@ -634,10 +637,13 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
               float acc = (s < S) ? __fmul_rn((mode == HR_FIELD_PRED_WEIGHTS) ? pw : w, v) : 0.0f;
 #pragma unroll
               for (int d = 1; d < 32; d <<= 1) acc += __shfl_xor_sync(kFull, acc, d);
-              // SPL registers per lane: partial sums of the rounds are added in round order by lane 0
+              // SPL registers per lane: partial sums of the rounds are added in round order by lane 0, and the last round
+              // stores the field, or its uint8 map
               if (lane == 0) {
-                float* dst = fo + ray * dim + c;
-                *dst = (j == 0) ? acc : (*dst + acc);
+                const float tot = (j == 0) ? acc : (fpart[f * 3 + c] + acc);
+                if (j < SPL - 1) fpart[f * 3 + c] = tot;
+                else if (fo8 != nullptr) fo8[ray * dim + c] = vis_to8b(vis_pre(so.field_u8[f], tot));
+                else fo[ray * dim + c] = tot;
               }
             }
           }

@@ -11,7 +11,7 @@ import os
 import subprocess
 import threading
 
-HR_ABI_VERSION = 24
+HR_ABI_VERSION = 25
 HR_MAX_GROUPS = 4
 HR_MAX_LAYERS = 10
 HR_MAX_SAMPLES = 256
@@ -33,6 +33,8 @@ PIXEL_RGB8, PIXEL_RGBA8 = 0, 1  # HR_PIXEL_*: uint8 RGB, or RGBA composited over
 FIELDS = {"points": 0, "distances": 1, "base_times": 2, "time_offset": 3, "times": 4, "viewdirs": 5, "weights": 6,
           "color_scale": 7, "color_shift": 8, "spatial_flow": 9, "sigma": 10, "point_sigma": 11, "point_offset": 12,
           "color_scale_global": 13, "color_shift_global": 14}
+FIELD_CHANNELS = {k: 3 if k in ("points", "viewdirs", "color_scale", "color_shift", "spatial_flow", "point_offset",
+                                 "color_scale_global", "color_shift_global") else 1 for k in FIELDS}
 FIELD_OVER, FIELD_NO_OVER, FIELD_PRED_WEIGHTS = 0, 1, 2
 PT_NONE, PT_POINT, PT_VIEW, PT_ORIGIN, PT_TIME = -1, 0, 3, 6, 9  # first channel of each source of the point net's input row
 
@@ -117,6 +119,11 @@ class hr_field_request(C.Structure):
     _fields_ = [("field", C.c_int32), ("mode", C.c_int32), ("out", C.c_void_p)]
 
 
+class hr_visual_request(C.Structure):
+    _fields_ = [("field", C.c_int32), ("mode", C.c_int32), ("channels", C.c_int32), ("use_abs", C.c_int32),
+                ("bounded", C.c_int32), ("normalize", C.c_int32), ("lo", C.c_float), ("hi", C.c_float), ("out", C.c_void_p)]
+
+
 class hr_train_opts(C.Structure):
     _fields_ = [("clamp_output", C.c_int32), ("white_bg", C.c_int32)]
 
@@ -181,6 +188,10 @@ EXPORTS = {
     "hr_score_views_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]),
     "hr_score_views": (C.c_int, [C.c_void_p, C.POINTER(hr_camera), C.POINTER(C.c_float), C.c_int32, C.c_void_p, C.c_int32,
                                   C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "hr_render_visuals_workspace_bytes": (C.c_int64, [C.c_void_p, C.POINTER(hr_visual_request), C.c_int32, C.c_int32, C.c_int32,
+                                                       C.c_int32]),
+    "hr_render_visuals": (C.c_int, [C.c_void_p, C.POINTER(hr_camera), C.POINTER(C.c_float), C.c_int32, C.c_void_p,
+                                     C.POINTER(hr_visual_request), C.c_int32, C.c_void_p, C.c_int64, C.c_void_p]),
     "hr_encode_rays": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "hr_render_heads": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.POINTER(hr_train_opts), C.c_void_p,
                                    C.c_int64, C.c_void_p]),

@@ -408,9 +408,7 @@ class LightfieldModel(nn.Module):
             raise UnsupportedPipeline(f"field '{key}' is not produced by the fused path")
         if key not in self._available_fields():
             raise KeyError(key)  # the reference fails the same way on x[key]
-        dims = {"points": 3, "viewdirs": 3, "color_scale": 3, "color_shift": 3, "spatial_flow": 3, "point_offset": 3,
-                "color_scale_global": 3, "color_shift_global": 3}
-        return L.FIELDS[key], dims.get(key, 1)
+        return L.FIELDS[key], L.FIELD_CHANNELS[key]
 
     # ------------------------------------------------------------------ native plumbing
     def render_stages(self, rays: torch.Tensor) -> Dict[str, torch.Tensor]:
@@ -596,6 +594,55 @@ class LightfieldModel(nn.Module):
             L.check(self._lib.hr_score_views(self._handle, recs, tt, len(cams), images.data_ptr(), fmt, out.data_ptr(),
                                              ws.data_ptr(), need, stream.cuda_stream))
         return out[:, 0], out[:, 1]
+
+    def render_visuals(self, cameras, requests, times=None, rgb: bool = True, stream=None):
+        """The uint8 video of ``cameras`` at ``times`` (as render_video makes it, bit for bit) and the embedding maps of
+        ``requests`` (camera.VisualRequest, from camera.embedding_requests) in one render pass per frame and one call that
+        never synchronises (hr_render_visuals).  Returns (video [F, H, W, 3] or None when ``rgb`` is False, {key: uint8
+        [F, H, W, channels]})."""
+        if self.training:
+            raise RuntimeError("hyperreel_b200.LightfieldModel implements the eval()/render path only; call .eval()")
+        from .signature import UnsupportedPipeline
+
+        cams = list(cameras)
+        if not cams:
+            raise ValueError("render_visuals: no cameras")
+        t = [float(c.time) for c in cams] if times is None else times
+        t = torch.as_tensor(t, dtype=torch.float64).reshape(-1).to(torch.float32)
+        if t.numel() != len(cams):
+            raise ValueError(f"render_visuals: {len(cams)} cameras but {t.numel()} times")
+        if not bool(torch.isfinite(t).all()):
+            raise ValueError("render_visuals: times must be finite in float32")
+        H, W = int(cams[0].height), int(cams[0].width)
+        for i, c in enumerate(cams):
+            if (int(c.height), int(c.width)) != (H, W):
+                raise ValueError(f"render_visuals: camera {i} is {int(c.width)} x {int(c.height)}, camera 0 is {W} x {H}")
+        if not rgb and not requests:
+            raise ValueError("render_visuals: nothing to render (rgb=False and no requests)")
+        for r in requests:  # a field this model lacks: the reference's KeyError on x[key], refused before any work
+            try:
+                self._field(r.key)
+            except KeyError:
+                raise UnsupportedPipeline(f"embedding visualiser: field '{r.key}' is not an output of this model") from None
+        dev = torch.device("cuda", self._device_index if self._device_index is not None else torch.cuda.current_device())
+        self._ensure_uploaded(dev)
+        stream = stream if stream is not None else torch.cuda.current_stream(dev)
+        F = len(cams)
+        with torch.cuda.stream(stream):  # the scratch and the outputs belong to the stream the work runs on
+            maps = {r.key: torch.empty((F, H, W, r.channels), dtype=torch.uint8, device=dev) for r in requests}
+            video = torch.empty((F, H, W, 3), dtype=torch.uint8, device=dev) if rgb else None
+            reqs = [L.hr_visual_request(L.FIELDS[r.key], r.mode, r.channels, int(r.use_abs), int(r.bounds is not None),
+                                        int(r.normalize), *(r.bounds or (0.0, 0.0)), maps[r.key].data_ptr()) for r in requests]
+            arr = (L.hr_visual_request * max(len(reqs), 1))(*reqs)
+            need = int(self._lib.hr_render_visuals_workspace_bytes(self._handle, arr, len(reqs), F, H, W))
+            if need < 0:
+                L.check(1)  # the library's reason
+            recs = (L.hr_camera * F)(*[c.to_c() for c in cams])
+            tt = (C.c_float * F)(*t.tolist())
+            ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            L.check(self._lib.hr_render_visuals(self._handle, recs, tt, F, video.data_ptr() if rgb else None, arr, len(reqs),
+                                                ws.data_ptr(), need, stream.cuda_stream))
+        return video, maps
 
     def timing(self, enable: bool = True):
         L.check(self._lib.hr_timing_enable(self._handle, int(enable)))

@@ -9,7 +9,8 @@ one Adam per optimiser group, the TensoRF regulariser (L1 + TV on the tables, nl
 up-sampling / occupancy-pruning schedule with its optimiser reset (tensorf_base.py:379-429,509-553,1151-1232), and, with
 ``schedule="reference"``, the optimisers' own schedule: one learning-rate scheduler per group stepped by
 ``training_epoch_end`` (utils/__init__.py:78-125, nlf/__init__.py:711-725) and the per-group ``reset_opt_list`` restarts
-(nlf/__init__.py:529-578).  Visualisers and datasets are out of scope (SURVEY.md section 2).
+(nlf/__init__.py:529-578).  Of the visualisers, the embedding maps are rendered on the device
+(``validation_video_outputs`` / ``validation_image_embeddings``); datasets are out of scope (SURVEY.md section 2).
 """
 from __future__ import annotations
 
@@ -348,6 +349,53 @@ class INRSystem(nn.Module):
             return self.render_fn.model.render_video(cameras, times, out=out, stream=stream)
         finally:
             self.train(was_training)
+
+    def render_visuals(self, cameras, requests, times=None, rgb=True, stream=None):
+        """LightfieldModel.render_visuals of this system's model, rendered in eval() (the previous train / eval mode is
+        restored)."""
+        was_training = self.training
+        self.eval()
+        try:
+            return self.render_fn.model.render_visuals(cameras, requests, times, rgb=rgb, stream=stream)
+        finally:
+            self.train(was_training)
+
+    def _visual_requests(self, testing: bool = False):
+        """The maps of every visualiser of cfg.visualizers (camera.embedding_requests, which refuses any but 'embedding'),
+        skipping, when ``testing``, those without run_on_test (nlf/__init__.py:929-931)."""
+        from .camera import embedding_requests
+        from .signature import UnsupportedPipeline
+
+        requests = []
+        for vcfg in (self.cfg.get("visualizers", None) or {}).values():
+            if testing and not vcfg.get("run_on_test", False):
+                continue
+            for r in embedding_requests(vcfg):
+                if any(q.key == r.key for q in requests):
+                    raise UnsupportedPipeline(f"embedding visualiser: field '{r.key}' is mapped by two visualisers")
+                requests.append(r)
+        return requests
+
+    def validation_video_outputs(self, cameras, times=None, stream=None):
+        """validation_video's ``all_videos`` of the render path (nlf/__init__.py:809-891) for every frame at once, on the
+        device: 'videos/rgb' uint8 [F, H, W, 3] (bit for bit render_video's) and, for each map of cfg.visualizers,
+        'videos/embedding_<key>' uint8 [F, H, W] or [F, H, W, 3], the frames the reference saves as PNGs (to8b of
+        visualize_warp).  One render pass per frame makes the RGB and the maps."""
+        from .camera import keyed_maps
+
+        requests = self._visual_requests()
+        return keyed_maps(requests, *self.render_visuals(cameras, requests, times, rgb=True, stream=stream), prefix="videos/")
+
+    def validation_image_embeddings(self, cameras, times=None, testing: bool = False, stream=None):
+        """The visualisers' 'images/embedding_<key>' outputs of validation_image (nlf/__init__.py:895-940) for every view
+        of a held-out split, uint8 [n, H, W] or [n, H, W, 3] on the device (to8b of visualize_warp, as the reference saves
+        them).  ``testing``: only visualisers with run_on_test (the shipped embedding configs have none, so {})."""
+        from .camera import keyed_maps
+
+        requests = self._visual_requests(testing)
+        if not requests:
+            return {}
+        return keyed_maps(requests, *self.render_visuals(cameras, requests, times, rgb=False, stream=stream), prefix="images/")
 
     def score_views(self, cameras, images, times=None, out=None, stream=None, *, rgba=False):
         """hyperreel_b200.score_views of this system's model, rendered in eval() (the previous train / eval mode is restored)."""

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define HR_ABI_VERSION 24
+#define HR_ABI_VERSION 25
 
 #define HR_MAX_GROUPS 4   /* ray-parameterisation groups feeding the sample net (ray.py:235-263) */
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
@@ -522,6 +522,42 @@ int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* ti
 int64_t hr_score_views_workspace_bytes(const hr_handle* h, int32_t n_views, int32_t height, int32_t width);
 int hr_score_views(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views, const uint8_t* gt,
                    int32_t pixel_format, double* out, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ---- embedding maps of a video or split (ABI 25) ----
+ * Replaces: the embedding visualiser's second render pass per frame (EmbeddingVisualizer.validation, nlf/visualizers/
+ * embedding.py:37-90, called by validation_video and validation_image, nlf/__init__.py:809-940) and its visualize_warp +
+ * to8b (utils/visualization.py:24-52, utils/__init__.py:47).  One request per map: the field `field` reduced in mode `mode`
+ * (HR_FIELD_OVER or HR_FIELD_PRED_WEIGHTS) as hr_render_fields reduces it, then, each step rounded on its own in fp32:
+ * |x| when use_abs; (x - lo) / (hi - lo) when bounded, hi - lo rounded once; when normalize, (x - min) / (max - min) with
+ * min and max per channel over the frame's pixels (NaN when the frame holds one); clamp to [0, 1] and (uint8)(255 * x),
+ * truncated, a NaN giving 0.  out: DEVICE uint8 [n_frames, height, width, channels]; channels must be the field's (1 or 3). */
+typedef struct hr_visual_request {
+  int32_t field;      /* HR_FIELD_*                              */
+  int32_t mode;       /* HR_FIELD_OVER / HR_FIELD_PRED_WEIGHTS    */
+  int32_t channels;   /* 1 or 3, the field's channel count        */
+  int32_t use_abs;    /* 0 / 1                                    */
+  int32_t bounded;    /* 0 / 1: lo and hi apply                   */
+  int32_t normalize;  /* 0 / 1: per-frame min / max               */
+  float lo, hi;       /* finite, hi != lo, when bounded           */
+  uint8_t* out;
+} hr_visual_request;
+
+/* cameras / times: HOST records and fp32 times as hr_render_video_to8b takes them.  video: DEVICE uint8 [n_frames, height,
+ * width, 3] or NULL; when given, bit for bit what hr_render_video_to8b writes.  Every map comes from the same render pass as
+ * the video.  A request without normalize is mapped to uint8 in the render kernel's epilogue (no fp32 field is written); a
+ * request with normalize stages the field's fp32 values in a ring of whole frames (enough for two sub-batches and one frame
+ * more), and each completed frame gets a min / max reduction (per-block partials, no atomics) and a map launch on the stream
+ * of the sub-batch that completed it, a ring frame being rendered again only after its map launch.  The sub-batches, streams
+ * and events are hr_score_views'; no host synchronisation; two calls write the same bits.  workspace: device scratch of
+ * hr_render_visuals_workspace_bytes(h, req, n_req, n_frames, height, width) bytes (16B aligned, -1 for a call refused),
+ * bounded whatever n_frames.  Refused before anything is enqueued (outputs untouched): null or misaligned pointers
+ * (workspace 16B), n_req < 0 or a null list with n_req > 0, nothing to write, an unknown field or mode, a field requested
+ * twice or not carried by the pipeline, channels other than the field's 1 or 3, non-finite bounds or hi == lo, the checks of
+ * hr_render_video_to8b on the records, times and size, a workspace too small. */
+int64_t hr_render_visuals_workspace_bytes(const hr_handle* h, const hr_visual_request* req, int32_t n_req, int32_t n_frames,
+                                          int32_t height, int32_t width);
+int hr_render_visuals(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_frames, uint8_t* video,
+                      const hr_visual_request* req, int32_t n_req, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- backward pass of the path (SURVEY.md section 8 row f1) ----
  * Replaces: what loss.backward() runs for the render path inside INRSystem.training_step (nlf/__init__.py:634-709): the
