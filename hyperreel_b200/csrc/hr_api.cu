@@ -948,8 +948,8 @@ int hr_render_frame_to8b_host(hr_handle* h, const hr_camera* cam, uint8_t* rgb8_
   return 0;
 }
 
-// ---- videos: many frames per call, rays generated and rendered in sub-batches that span frame boundaries
-// rays of the whole video, or -1 when F * H * W * 3 (the output's bytes) does not fit in int64
+// ---- frame sequences (videos, scored splits, embedding maps): rays generated and rendered in sub-batches across frames
+// rays of the whole sequence, or -1 when F * H * W * 3 (a video's bytes) does not fit in int64
 static int64_t video_rays(int32_t n_frames, int32_t height, int32_t width) {
   if (n_frames < 1 || height < 1 || width < 1) return -1;
   int64_t px, n, bytes;
@@ -959,25 +959,49 @@ static int64_t video_rays(int32_t n_frames, int32_t height, int32_t width) {
   return n;
 }
 
-// Workspace layout: the records [F] and times [F] on the device, then one slot per stream of the pipeline below (two when
-// the video is longer than one sub-batch), each a sub-batch's rays [sub, c_in] and render workspace.  The sub-batch is
-// hr_render's (16 sample-net tile waves unless hr_set_sub_batch says otherwise) whatever the frame size, so the scratch stays
-// bounded for any number of frames; "never split" does not apply here, a video is unbounded.
-static int64_t video_sub_rays(const hr_handle* h, int64_t n_rays) {
-  const int64_t sub = sub_batch_rays(h);
-  return n_rays < sub ? n_rays : sub;
+// Frames of a ring: what two sub-batches cover and one more (so the sub-batch after next is the first that may wait for a
+// frame's finish), at most the sequence; bounded by the sub-batch, whatever n_frames.
+static int64_t ring_frames(int64_t sub, int64_t frame_px, int32_t n_frames) {
+  int64_t r = (2 * sub + frame_px - 1) / frame_px + 1;
+  if (r > n_frames) r = n_frames;
+  return r > 65535 ? 65535 : r;  // frames per metrics launch
 }
 
-static int64_t video_slot_bytes(const hr_handle* h, int64_t sub) {
-  return align256(sub * h->cfg.c_in * (int64_t)sizeof(float)) + align256(ws_bytes_for(h, sub));
+// Workspace of a frame walk, each part 256-byte aligned: the records [F] and times [F] on the device; the caller's middle
+// segment, a ring of whole frames (ring_px_bytes per pixel, 0 for no ring, plus ring_pad bytes for the caller's alignment)
+// and one partial buffer per stream (part_frame_bytes per ring frame); then one slot per stream (two when the sequence is
+// longer than one sub-batch), each a sub-batch's rays [sub, c_in] and render workspace.  The sub-batch is hr_render's (16
+// sample-net tile waves unless hr_set_sub_batch says otherwise) whatever the frame size, so past the records and times the
+// scratch is bounded whatever F; "never split" does not apply here, a sequence is unbounded.  false: a size overflows int64.
+struct WalkLayout {
+  int64_t n, frame_px, sub, ring, ring_off, part_off, part_bytes, slots_off, slot_bytes, total;
+  int n_slots;
+};
+
+static bool walk_layout(const hr_handle* h, int32_t n_frames, int32_t height, int32_t width, int64_t ring_px_bytes,
+                        int64_t ring_pad, int64_t part_frame_bytes, WalkLayout* L) {
+  *L = WalkLayout{};
+  L->n = video_rays(n_frames, height, width);
+  if (!h || L->n < 0) return false;
+  const int64_t sub = sub_batch_rays(h);
+  L->frame_px = (int64_t)height * width;
+  L->sub = L->n < sub ? L->n : sub;
+  L->n_slots = L->n > L->sub ? 2 : 1;
+  L->ring = ring_px_bytes ? ring_frames(L->sub, L->frame_px, n_frames) : 0;
+  int64_t ring_bytes;
+  if (__builtin_mul_overflow(L->ring * L->frame_px, ring_px_bytes, &ring_bytes)) return false;
+  L->ring_off = align256((int64_t)n_frames * (int64_t)sizeof(hr_camera)) + align256((int64_t)n_frames * (int64_t)sizeof(float));
+  L->part_off = L->ring_off + align256(ring_bytes) + ring_pad;
+  L->part_bytes = align256(L->ring * part_frame_bytes);
+  L->slots_off = L->part_off + 2 * L->part_bytes;
+  L->slot_bytes = align256(L->sub * h->cfg.c_in * (int64_t)sizeof(float)) + align256(ws_bytes_for(h, L->sub));
+  L->total = L->slots_off + L->n_slots * L->slot_bytes;
+  return true;
 }
 
 int64_t hr_video_workspace_bytes(const hr_handle* h, int32_t n_frames, int32_t height, int32_t width) {
-  const int64_t n = video_rays(n_frames, height, width);
-  if (!h || n < 0) return -1;
-  const int64_t sub = video_sub_rays(h, n);
-  return align256((int64_t)n_frames * (int64_t)sizeof(hr_camera)) + align256((int64_t)n_frames * (int64_t)sizeof(float)) +
-         (n > sub ? 2 : 1) * video_slot_bytes(h, sub);
+  WalkLayout L;
+  return walk_layout(h, n_frames, height, width, 0, 0, 0, &L) ? L.total : -1;
 }
 
 static bool finite_camera(const hr_camera& c) {
@@ -1004,240 +1028,175 @@ static int check_frames(const char* fn, const hr_camera* cameras, const float* t
   return 0;
 }
 
-// Sub-batch i runs on stream i % 2 of the handle (forked from and joined back to the caller's stream by events) in slot
-// i % 2: its ray generation and sample net overlap the previous sub-batch's render kernel, where one stream would leave the
-// SMs idle between each sub-batch's render tail and the next one's ray generation.  Each stream runs its sub-batches in
-// order, so a slot is reused only after the sub-batch that last held it has finished.
-int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_frames, uint8_t* video,
-                         void* workspace, int64_t workspace_bytes, void* stream) {
-  if (!h || !cameras || !times || !video || !workspace) return hr_fail("hr_render_video_to8b: null argument");
-  if (!h->uploaded) return hr_fail("hr_render_video_to8b: parameters not uploaded");
-  if (n_frames < 1) return hr_fail("hr_render_video_to8b: n_frames must be >= 1, got %d", n_frames);
-  const int32_t W = cameras[0].width, H = cameras[0].height;
-  const int64_t n = video_rays(n_frames, H, W);
-  if (n < 0) return hr_fail("hr_render_video_to8b: %d frames of %d x %d pixels: bad size or output bytes overflow int64", n_frames, W, H);
-  bool mixed = false;
-  if (check_frames("hr_render_video_to8b", cameras, times, n_frames, &mixed)) return 1;
-  const int64_t need = hr_video_workspace_bytes(h, n_frames, H, W);
-  if (workspace_bytes < need) return hr_fail("hr_render_video_to8b: workspace too small (%lld < %lld)", (long long)workspace_bytes, (long long)need);
-  if (((uintptr_t)workspace & 15) != 0) return hr_fail("hr_render_video_to8b: workspace must be 16-byte aligned");
+// The refusals every frame walk makes first: a null argument (null_out: one of the caller's own), parameters not uploaded,
+// a frame count (named `count`) under 1, and check_frames'.
+static int check_walk(const char* fn, const char* count, const hr_handle* h, bool null_out, const hr_camera* cameras,
+                      const float* times, int32_t n_frames, const void* workspace, bool* mixed) {
+  if (null_out || !h || !cameras || !times || !workspace) return hr_fail("%s: null argument", fn);
+  if (!h->uploaded) return hr_fail("%s: parameters not uploaded", fn);
+  if (n_frames < 1) return hr_fail("%s: %s must be >= 1, got %d", fn, count, n_frames);
+  return check_frames(fn, cameras, times, n_frames, mixed);
+}
+
+// The refusals every frame walk makes last, after its own: a size whose bytes overflow int64 (laid_out false), a workspace
+// that is not 16-byte aligned or is too small.
+static int check_workspace(const char* fn, bool laid_out, const WalkLayout& L, const hr_camera* cameras, int32_t n_frames,
+                           const void* workspace, int64_t workspace_bytes) {
+  if (!laid_out)
+    return hr_fail("%s: %d frames of %d x %d pixels: bad size or bytes overflow int64", fn, n_frames, cameras[0].width, cameras[0].height);
+  if (((uintptr_t)workspace & 15) != 0) return hr_fail("%s: workspace must be 16-byte aligned", fn);
+  if (workspace_bytes < L.total)
+    return hr_fail("%s: workspace too small (%lld < %lld)", fn, (long long)workspace_bytes, (long long)L.total);
+  return 0;
+}
+
+// The walk of a frame sequence: its F·H·W rays in sub-batches of L.sub across frame boundaries.  The records and times are
+// copied to the workspace on the caller's stream (stream-ordered: a pageable source is staged before the call returns,
+// without waiting for the device).  Sub-batch i runs on stream i % 2 of the handle (forked from and joined back to the
+// caller's stream by events, also after a failure) in slot i % 2: its ray generation and sample net overlap the previous
+// sub-batch's render kernel, where one stream would leave the SMs idle between each sub-batch's render tail and the next
+// one's ray generation.  render(off, pos, m, rays, ws, ws_bytes, s) enqueues the render of rays [off, off + m) on s, pos
+// being their ring position.  With a ring (L.ring > 0) a sub-batch is also cut where it would wrap it, so its pixels land in
+// consecutive ring positions, and finish(next, f_end, k, s) enqueues the work of the frames next .. f_end - 1 it completes
+// on its own stream k, after the other stream's last render when a frame straddles the two; a ring frame is rendered
+// again only after the finish of the frame it held.  Each stream runs in order, so its slot and partials are reused safely.
+extern "C++" {  // a template, inside the C-ABI block
+template <class Render, class Finish>
+static int walk_frames(hr_handle* h, const char* fn, const WalkLayout& L, const hr_camera* cameras, const float* times,
+                       int32_t n_frames, bool mixed, void* workspace, cudaStream_t st, Render render, Finish finish) {
   DeviceGuard guard(h->device);
-  const hr_config& c = h->cfg;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t sub = video_sub_rays(h, n);
-  const int n_slots = n > sub ? 2 : 1;
-  char* p = (char*)workspace;
-  hr_camera* d_cams = (hr_camera*)p;
-  p += align256((int64_t)n_frames * (int64_t)sizeof(hr_camera));
-  float* d_times = (float*)p;
-  p += align256((int64_t)n_frames * (int64_t)sizeof(float));
-  const int64_t slot_bytes = video_slot_bytes(h, sub), rays_bytes = align256(sub * c.c_in * (int64_t)sizeof(float));
-  // stream-ordered copies: a pageable source is staged before the call returns, without waiting for the device
+  char* base = (char*)workspace;
+  hr_camera* d_cams = (hr_camera*)base;
+  float* d_times = (float*)(base + align256((int64_t)n_frames * (int64_t)sizeof(hr_camera)));
   CK(cudaMemcpyAsync(d_cams, cameras, (size_t)n_frames * sizeof(hr_camera), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_times, times, (size_t)n_frames * sizeof(float), cudaMemcpyHostToDevice, st));
-  cudaStream_t ss[2] = {st, st};
-  cudaEvent_t ev = nullptr;
-  if (n_slots == 2) {
-    for (int i = 0; i < 2; ++i) {
-      if (pipe_stream(h, i)) return 1;
-      ss[i] = h->pipe.streams[i];
-    }
-    CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    CK(cudaEventRecord(ev, st));
-    CK(cudaStreamWaitEvent(ss[0], ev, 0));
-    CK(cudaStreamWaitEvent(ss[1], ev, 0));
-    CK(cudaEventDestroy(ev));
-  }
-  const int64_t frame_px = (int64_t)W * H;
-  int rc = 0;
-  int64_t i = 0;
-  for (int64_t off = 0; off < n && !rc; off += sub, ++i) {
-    const int64_t m = (n - off < sub) ? (n - off) : sub;
-    cudaStream_t s = ss[i % 2];
-    char* slot = p + (i % n_slots) * slot_bytes;
-    float* d_rays = (float*)slot;
-    cudaError_t e = hr::launch_generate_video_rays(d_cams, d_times, mixed, c.c_in, W, frame_px, off, m, d_rays, s);
-    if (e != cudaSuccess) {
-      rc = hr_fail("video ray generation failed: %s", cudaGetErrorString(e));
-      break;
-    }
-    h->launches += 1;
-    rc = render_impl(h, d_rays, m, nullptr, nullptr, nullptr, slot + rays_bytes, slot_bytes - rays_bytes, s, video + off * 3);
-  }
-  if (n_slots == 2) {  // join, also after a failed launch: the caller's stream must not run ahead of enqueued work
-    for (int k = 0; k < 2; ++k) {
-      CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-      CK(cudaEventRecord(ev, ss[k]));
-      CK(cudaStreamWaitEvent(st, ev, 0));
-      CK(cudaEventDestroy(ev));
-    }
-  }
-  return rc;
-}
-
-// ---- held-out splits: every view rendered into a ring of whole fp32 frames and scored against its uint8 ground truth
-// Frames of the ring: what two sub-batches cover and one more (so the sub-batch after next is the first that may wait for a
-// frame's scoring), at most the split; bounded by the sub-batch, whatever n_views.  -1 when the ring's bytes overflow.
-static int64_t score_ring_frames(int64_t sub, int64_t frame_px, int32_t n_views) {
-  int64_t r = (2 * sub + frame_px - 1) / frame_px + 1;
-  if (r > n_views) r = n_views;
-  if (r > 65535) r = 65535;  // frames per metrics launch
-  int64_t bytes;
-  if (__builtin_mul_overflow(r * frame_px, (int64_t)(3 * sizeof(float)), &bytes)) return -1;
-  return r;
-}
-
-// Workspace layout (each part 256-byte aligned): two record windows (ring frames records and times each), the fp32 ring
-// [R][H][W][3], two metrics partial buffers (one per stream, R frames each), then the video path's one or two slots.
-struct ScoreLayout {
-  int64_t sub, ring, win_cams, win_times, ring_off, partial_off, partial_bytes, slots_off, slot_bytes, total;
-  int n_slots;
-};
-
-static bool score_layout(const hr_handle* h, int32_t n_views, int32_t height, int32_t width, ScoreLayout* L) {
-  if (!h || height < 11 || width < 11) return false;
-  const int64_t n = video_rays(n_views, height, width);
-  if (n < 0) return false;
-  const int64_t frame_px = (int64_t)height * width;
-  L->sub = video_sub_rays(h, n);
-  L->ring = score_ring_frames(L->sub, frame_px, n_views);
-  if (L->ring < 1) return false;
-  L->n_slots = n > L->sub ? 2 : 1;
-  L->win_cams = align256(L->ring * (int64_t)sizeof(hr_camera));
-  L->win_times = align256(L->ring * (int64_t)sizeof(float));
-  L->ring_off = 2 * (L->win_cams + L->win_times);
-  L->partial_off = L->ring_off + align256(L->ring * frame_px * 3 * (int64_t)sizeof(float));
-  L->partial_bytes = align256(hr_image_metrics_workspace_bytes((int32_t)L->ring, height, width));
-  L->slots_off = L->partial_off + 2 * L->partial_bytes;
-  L->slot_bytes = video_slot_bytes(h, L->sub);
-  L->total = L->slots_off + L->n_slots * L->slot_bytes;
-  return true;
-}
-
-int64_t hr_score_views_workspace_bytes(const hr_handle* h, int32_t n_views, int32_t height, int32_t width) {
-  ScoreLayout L;
-  return score_layout(h, n_views, height, width, &L) ? L.total : -1;
-}
-
-// The split is one ray sequence walked in the video path's sub-batches on its two streams, each sub-batch also cut where it
-// would wrap the ring, so its pixels land in consecutive ring positions.  A sub-batch copies its frames' records and times
-// into its stream's window, generates their rays, renders them into the ring and, when it completes frames, scores them with
-// one metrics launch on its own stream.  Cross-stream order comes from events: a frame begun by the previous sub-batch (the
-// other stream) is scored after that sub-batch's render, and a ring frame is rendered again only after the launch that
-// scored its previous frame.  Each stream runs its sub-batches in order, so its slot, window and partials are reused safely.
-int hr_score_views(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views, const uint8_t* gt,
-                   int32_t pixel_format, double* out, void* workspace, int64_t workspace_bytes, void* stream) {
-  const char* fn = "hr_score_views";
-  if (!h || !cameras || !times || !gt || !out || !workspace) return hr_fail("%s: null argument", fn);
-  if (!h->uploaded) return hr_fail("%s: parameters not uploaded", fn);
-  if (n_views < 1) return hr_fail("%s: n_views must be >= 1, got %d", fn, n_views);
-  const int32_t W = cameras[0].width, H = cameras[0].height;
-  if (H < 11 || W < 11) return hr_fail("%s: height and width must be >= 11 (the SSIM window), got %d x %d", fn, H, W);
-  ScoreLayout lay;
-  if (!score_layout(h, n_views, H, W, &lay))
-    return hr_fail("%s: %d views of %d x %d pixels: bad size or bytes overflow int64", fn, n_views, W, H);
-  bool mixed = false;
-  if (check_frames(fn, cameras, times, n_views, &mixed)) return 1;
-  if (((uintptr_t)out & 7) != 0) return hr_fail("%s: out must be 8-byte aligned", fn);
-  if (((uintptr_t)workspace & 15) != 0) return hr_fail("%s: workspace must be 16-byte aligned", fn);
-  const int gt_px = hr::pixel_bytes(pixel_format);  // bytes per ground-truth pixel
-  if (!gt_px) return hr_fail("%s: unknown pixel format %d", fn, pixel_format);
-  if (gt_px == 4 && ((uintptr_t)gt & 3) != 0) return hr_fail("%s: RGBA gt must be 4-byte aligned", fn);
-  if (workspace_bytes < lay.total)
-    return hr_fail("%s: workspace too small (%lld < %lld)", fn, (long long)workspace_bytes, (long long)lay.total);
-  DeviceGuard guard(h->device);
-  const hr_config& c = h->cfg;
-  cudaStream_t st = (cudaStream_t)stream;
-  char* base = (char*)workspace;
-  float* ring = (float*)(base + lay.ring_off);
-  const int64_t frame_px = (int64_t)W * H, n = frame_px * n_views, ring_rays = lay.ring * frame_px;
-  const int64_t rays_bytes = align256(lay.sub * c.c_in * (int64_t)sizeof(float));
+  const bool two = L.n_slots == 2, ring_events = two && L.ring > 0;
+  const int64_t ring_rays = L.ring * L.frame_px, rays_bytes = align256(L.sub * h->cfg.c_in * (int64_t)sizeof(float));
   cudaStream_t ss[2] = {st, st};
   std::vector<cudaEvent_t> evs;  // every event of the call, destroyed at the end (a destroyed event's pending work still runs)
-  auto new_event = [&](cudaEvent_t* ev) -> int {
-    CK(cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
-    evs.push_back(*ev);
-    return 0;
+  auto new_event = [&](cudaEvent_t* ev) {
+    const cudaError_t e = cudaEventCreateWithFlags(ev, cudaEventDisableTiming);
+    if (e == cudaSuccess) evs.push_back(*ev);
+    return e;
   };
-  // scored[k]: recorded after the metrics launch that read ring frame k last; done[s]: after stream s's last render
-  std::vector<cudaEvent_t> scored(lay.n_slots == 2 ? lay.ring : 0, nullptr);
+  auto fail = [&](const char* what, cudaError_t e) { return hr_fail("%s: %s: %s", fn, what, cudaGetErrorString(e)); };
+  // freed[f]: recorded after the finish that read ring frame f last; done[k]: after stream k's last render
+  std::vector<cudaEvent_t> freed(ring_events ? L.ring : 0, nullptr);
   cudaEvent_t done[2] = {nullptr, nullptr};
-  int rc = 0;
-  if (lay.n_slots == 2) {
-    cudaEvent_t fork;
-    for (int i = 0; i < 2; ++i) {
-      if (pipe_stream(h, i)) return 1;
-      ss[i] = h->pipe.streams[i];
+  cudaError_t e = cudaSuccess;  // of the event calls: the walk stops at the first failure
+  if (two) {
+    for (int k = 0; k < 2; ++k) {
+      if (pipe_stream(h, k)) return 1;
+      ss[k] = h->pipe.streams[k];
     }
-    if (new_event(&fork)) return 1;
-    CK(cudaEventRecord(fork, st));
-    CK(cudaStreamWaitEvent(ss[0], fork, 0));
-    CK(cudaStreamWaitEvent(ss[1], fork, 0));
-    for (auto& e : scored)
-      if ((rc = new_event(&e))) break;
-    for (int i = 0; i < 2 && !rc; ++i) rc = new_event(&done[i]);
+    cudaEvent_t fork;
+    if ((e = new_event(&fork)) == cudaSuccess) e = cudaEventRecord(fork, st);
+    for (int k = 0; k < 2 && e == cudaSuccess; ++k) e = cudaStreamWaitEvent(ss[k], fork, 0);
+    for (size_t f = 0; f < freed.size() && e == cudaSuccess; ++f) e = new_event(&freed[f]);
+    for (int k = 0; k < 2 && e == cudaSuccess && ring_events; ++k) e = new_event(&done[k]);
   }
-  int64_t next = 0;  // first frame not yet scored
-  int64_t i = 0;
-  for (int64_t off = 0; off < n && !rc; ++i) {
+  int rc = 0;
+  int64_t next = 0;  // first frame not yet finished
+  for (int64_t off = 0, i = 0; off < L.n && !rc && e == cudaSuccess; ++i) {
     const int k = (int)(i % 2);
     cudaStream_t s = ss[k];
-    const int64_t pos = off % ring_rays;
-    int64_t m = n - off < lay.sub ? n - off : lay.sub;
-    if (pos + m > ring_rays) m = ring_rays - pos;
-    const int64_t f0 = off / frame_px, f1 = (off + m - 1) / frame_px, f_end = (off + m) / frame_px;
-    auto fail = [&](const char* what, cudaError_t e) { return hr_fail("%s: %s: %s", fn, what, cudaGetErrorString(e)); };
-    cudaError_t e = cudaSuccess;
-    if (lay.n_slots == 2)  // ring frames rendered again: after the scoring of the frames they held
-      for (int64_t f = f0 < lay.ring ? lay.ring : f0; f <= f1 && e == cudaSuccess; ++f)
-        e = cudaStreamWaitEvent(s, scored[f % lay.ring], 0);
-    hr_camera* win_c = (hr_camera*)(base + k * (lay.win_cams + lay.win_times));
-    float* win_t = (float*)((char*)win_c + lay.win_cams);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(win_c, cameras + f0, (size_t)(f1 - f0 + 1) * sizeof(hr_camera), cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(win_t, times + f0, (size_t)(f1 - f0 + 1) * sizeof(float), cudaMemcpyHostToDevice, s);
-    if (e != cudaSuccess) {
-      rc = fail("record copy", e);
-      break;
-    }
-    char* slot = base + lay.slots_off + (i % lay.n_slots) * lay.slot_bytes;
-    e = hr::launch_generate_video_rays(win_c, win_t, mixed, c.c_in, W, frame_px, off - f0 * frame_px, m, (float*)slot, s);
-    if (e != cudaSuccess) {
-      rc = fail("ray generation", e);
+    const int64_t pos = ring_rays ? off % ring_rays : 0;
+    int64_t m = L.n - off < L.sub ? L.n - off : L.sub;
+    if (ring_rays && pos + m > ring_rays) m = ring_rays - pos;
+    const int64_t f0 = off / L.frame_px, f1 = (off + m - 1) / L.frame_px, f_end = (off + m) / L.frame_px;
+    for (int64_t f = f0 < L.ring ? L.ring : f0; f <= f1 && e == cudaSuccess && ring_events; ++f)  // ring frames rendered again
+      e = cudaStreamWaitEvent(s, freed[f % L.ring], 0);
+    if (e != cudaSuccess) break;
+    char* slot = base + L.slots_off + (i % L.n_slots) * L.slot_bytes;
+    const cudaError_t g = hr::launch_generate_video_rays(d_cams, d_times, mixed, h->cfg.c_in, cameras[0].width, L.frame_px, off, m,
+                                                         (float*)slot, s);
+    if (g != cudaSuccess) {
+      rc = fail("ray generation", g);
       break;
     }
     h->launches += 1;
-    rc = render_impl(h, (const float*)slot, m, ring + pos * 3, nullptr, nullptr, slot + rays_bytes, lay.slot_bytes - rays_bytes, s);
-    if (rc) break;
-    if (f_end > next) {  // frames next .. f_end - 1 are complete, in consecutive ring frames
-      if (lay.n_slots == 2 && next * frame_px < off) e = cudaStreamWaitEvent(s, done[1 - k], 0);
-      if (e == cudaSuccess)
-        e = (gt_px == 4 ? hr::launch_image_metrics_rgba8 : hr::launch_image_metrics_u8)(
-            ring + (next % lay.ring) * frame_px * 3, gt + next * frame_px * gt_px, (int32_t)(f_end - next), H, W, out + 2 * next,
-            (double*)(base + lay.partial_off + k * lay.partial_bytes), s);
-      for (int64_t f = next; f < f_end && e == cudaSuccess && lay.n_slots == 2; ++f) e = cudaEventRecord(scored[f % lay.ring], s);
-      if (e != cudaSuccess) {
-        rc = fail("metrics launch", e);
-        break;
-      }
-      h->launches += 2;
+    if ((rc = render(off, pos, m, (const float*)slot, (void*)(slot + rays_bytes), L.slot_bytes - rays_bytes, s))) break;
+    if (ring_rays && f_end > next) {  // frames next .. f_end - 1 are complete, in consecutive ring frames
+      if (ring_events && next * L.frame_px < off) e = cudaStreamWaitEvent(s, done[1 - k], 0);
+      if (e != cudaSuccess || (rc = finish(next, f_end, k, s))) break;
+      for (int64_t f = next; f < f_end && e == cudaSuccess && ring_events; ++f) e = cudaEventRecord(freed[f % L.ring], s);
       next = f_end;
     }
-    if (lay.n_slots == 2 && (e = cudaEventRecord(done[k], s)) != cudaSuccess) {
-      rc = fail("event record", e);
-      break;
-    }
+    if (e == cudaSuccess && ring_events) e = cudaEventRecord(done[k], s);
     off += m;
   }
-  if (lay.n_slots == 2) {  // join, also after a failed launch: the caller's stream must not run ahead of enqueued work
-    for (int k = 0; k < 2; ++k) {
-      cudaEvent_t ev;
-      if (new_event(&ev)) break;
-      CK(cudaEventRecord(ev, ss[k]));
-      CK(cudaStreamWaitEvent(st, ev, 0));
-    }
+  if (e != cudaSuccess) rc = fail("stream event", e);
+  for (int k = 0; k < 2 && two; ++k) {  // join, also after a failure: the caller's stream must not run ahead of enqueued work
+    cudaEvent_t join;
+    cudaError_t j = new_event(&join);
+    if (j == cudaSuccess) j = cudaEventRecord(join, ss[k]);
+    if (j == cudaSuccess) j = cudaStreamWaitEvent(st, join, 0);
+    if (j != cudaSuccess && !rc) rc = fail("join", j);
   }
   for (cudaEvent_t ev : evs) cudaEventDestroy(ev);
   return rc;
+}
+}  // extern "C++"
+
+int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_frames, uint8_t* video,
+                         void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* fn = "hr_render_video_to8b";
+  bool mixed = false;
+  if (check_walk(fn, "n_frames", h, !video, cameras, times, n_frames, workspace, &mixed)) return 1;
+  WalkLayout L;
+  const bool laid_out = walk_layout(h, n_frames, cameras[0].height, cameras[0].width, 0, 0, 0, &L);
+  if (check_workspace(fn, laid_out, L, cameras, n_frames, workspace, workspace_bytes)) return 1;
+  return walk_frames(
+      h, fn, L, cameras, times, n_frames, mixed, workspace, (cudaStream_t)stream,
+      [&](int64_t off, int64_t, int64_t m, const float* rays, void* ws, int64_t ws_bytes, cudaStream_t s) {
+        return render_impl(h, rays, m, nullptr, nullptr, nullptr, ws, ws_bytes, s, video + off * 3);
+      },
+      [](int64_t, int64_t, int, cudaStream_t) { return 0; });
+}
+
+// ---- held-out splits: every view rendered into a ring of whole fp32 frames and scored against its uint8 ground truth
+// A split's walk layout: the fp32 ring [R][H][W][3], then one metrics partial buffer per stream (R frames each).
+static bool score_layout(const hr_handle* h, int32_t n_views, int32_t height, int32_t width, WalkLayout* L) {
+  return height >= 11 && width >= 11 &&
+         walk_layout(h, n_views, height, width, 3 * sizeof(float), 0, hr_image_metrics_workspace_bytes(1, height, width), L);
+}
+
+int64_t hr_score_views_workspace_bytes(const hr_handle* h, int32_t n_views, int32_t height, int32_t width) {
+  WalkLayout L;
+  return score_layout(h, n_views, height, width, &L) ? L.total : -1;
+}
+
+// The split's walk renders fp32 rgb into the ring; the frames a sub-batch completes are scored by one metrics launch on its
+// stream, with that stream's partial buffer.
+int hr_score_views(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_views, const uint8_t* gt,
+                   int32_t pixel_format, double* out, void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* fn = "hr_score_views";
+  bool mixed = false;
+  if (check_walk(fn, "n_views", h, !gt || !out, cameras, times, n_views, workspace, &mixed)) return 1;
+  const int32_t W = cameras[0].width, H = cameras[0].height;
+  if (H < 11 || W < 11) return hr_fail("%s: height and width must be >= 11 (the SSIM window), got %d x %d", fn, H, W);
+  if (((uintptr_t)out & 7) != 0) return hr_fail("%s: out must be 8-byte aligned", fn);
+  const int gt_px = hr::pixel_bytes(pixel_format);  // bytes per ground-truth pixel
+  if (!gt_px) return hr_fail("%s: unknown pixel format %d", fn, pixel_format);
+  if (gt_px == 4 && ((uintptr_t)gt & 3) != 0) return hr_fail("%s: RGBA gt must be 4-byte aligned", fn);
+  WalkLayout L;
+  const bool laid_out = score_layout(h, n_views, H, W, &L);
+  if (check_workspace(fn, laid_out, L, cameras, n_views, workspace, workspace_bytes)) return 1;
+  float* ring = (float*)((char*)workspace + L.ring_off);
+  const int64_t px = L.frame_px;
+  return walk_frames(
+      h, fn, L, cameras, times, n_views, mixed, workspace, (cudaStream_t)stream,
+      [&](int64_t, int64_t pos, int64_t m, const float* rays, void* ws, int64_t ws_bytes, cudaStream_t s) {
+        return render_impl(h, rays, m, ring + pos * 3, nullptr, nullptr, ws, ws_bytes, s);
+      },
+      [&](int64_t next, int64_t f_end, int k, cudaStream_t s) {
+        const cudaError_t e = (gt_px == 4 ? hr::launch_image_metrics_rgba8 : hr::launch_image_metrics_u8)(
+            ring + (next % L.ring) * px * 3, gt + next * px * gt_px, (int32_t)(f_end - next), H, W, out + 2 * next,
+            (double*)((char*)workspace + L.part_off + k * L.part_bytes), s);
+        if (e != cudaSuccess) return hr_fail("%s: metrics launch: %s", fn, cudaGetErrorString(e));
+        h->launches += 2;
+        return 0;
+      });
 }
 
 // ---- embedding maps: every request mapped in the render epilogue, or staged in a ring of whole frames and normalised
@@ -1264,193 +1223,83 @@ static int check_visual_requests(const char* fn, const hr_handle* h, const hr_vi
   return 0;
 }
 
-// Workspace layout (each part 256-byte aligned): two record windows (the frames one sub-batch touches), the rings of the
-// normalize requests (ring frames each, in request order), two partial buffers (one per stream), then the video path's one or
-// two slots.  Without a normalize request there is no ring and the sub-batches are not cut.
-struct VisLayout {
-  int64_t sub, win, ring, win_cams, win_times, ring_off, ring_bytes_per_ch, partial_off, partial_bytes, slots_off, slot_bytes, total;
-  int n_slots;
-};
-
-static bool visual_layout(const hr_handle* h, int norm_ch, int32_t n_frames, int32_t height, int32_t width, VisLayout* L) {
-  const int64_t n = video_rays(n_frames, height, width);
-  if (!h || n < 0) return false;
-  const int64_t frame_px = (int64_t)height * width;
-  L->sub = video_sub_rays(h, n);
-  L->win = (L->sub + frame_px - 1) / frame_px + 1;
-  if (L->win > n_frames) L->win = n_frames;
-  L->ring = norm_ch ? score_ring_frames(L->sub, frame_px, n_frames) : 0;
-  if (L->ring < 0) return false;
-  L->n_slots = n > L->sub ? 2 : 1;
-  L->win_cams = align256(L->win * (int64_t)sizeof(hr_camera));
-  L->win_times = align256(L->win * (int64_t)sizeof(float));
-  L->ring_off = 2 * (L->win_cams + L->win_times);
-  int64_t ring_bytes;
-  if (__builtin_mul_overflow(L->ring * frame_px, (int64_t)(norm_ch * sizeof(float)), &ring_bytes)) return false;
-  L->ring_bytes_per_ch = L->ring * frame_px * (int64_t)sizeof(float);
-  L->partial_off = L->ring_off + align256(ring_bytes) + 256 * norm_ch;  // each request's ring starts 256-byte aligned
-  L->partial_bytes = align256(L->ring * hr::kVisBlocks * 6 * (int64_t)sizeof(float));
-  L->slots_off = L->partial_off + 2 * L->partial_bytes;
-  L->slot_bytes = video_slot_bytes(h, L->sub);
-  L->total = L->slots_off + L->n_slots * L->slot_bytes;
-  return true;
+// An embedding walk's layout: the normalize requests' rings (norm_ch fp32 channels per pixel in all, each request's ring
+// 256-byte aligned, in request order), then one min / max partial buffer per stream.  Without a normalize request there is
+// no ring, so the walk is the video's.
+static bool visual_layout(const hr_handle* h, int norm_ch, int32_t n_frames, int32_t height, int32_t width, WalkLayout* L) {
+  return walk_layout(h, n_frames, height, width, norm_ch * (int64_t)sizeof(float), 256 * norm_ch,
+                     hr::kVisBlocks * 6 * (int64_t)sizeof(float), L);
 }
 
 int64_t hr_render_visuals_workspace_bytes(const hr_handle* h, const hr_visual_request* req, int32_t n_req, int32_t n_frames,
                                           int32_t height, int32_t width) {
   int norm_ch = 0;
-  VisLayout L;
+  WalkLayout L;
   if (!h || check_visual_requests("hr_render_visuals_workspace_bytes", h, req, n_req, &norm_ch)) return -1;
   if (visual_layout(h, norm_ch, n_frames, height, width, &L)) return L.total;
   hr_fail("hr_render_visuals_workspace_bytes: %d frames of %d x %d pixels: bad size or bytes overflow int64", n_frames, width, height);
   return -1;
 }
 
-// hr_score_views' walk: one ray sequence in the video path's sub-batches on two streams, each sub-batch also cut where it would
-// wrap the ring.  A sub-batch renders the video's pixels, the epilogue-mapped requests' bytes and the normalize requests' fp32
-// fields (into the ring) in one render launch; when it completes frames it reduces and maps them, per normalize request, on its
-// own stream, after the other stream's last render when a frame straddles the two.  A ring frame is rendered again only after
-// the map launch of the frame it held.
+// The walk renders the video's pixels, the epilogue-mapped requests' bytes and the normalize requests' fp32 fields (into
+// their rings) in one render launch per sub-batch; the frames a sub-batch completes are reduced and mapped, per normalize
+// request, on its stream.  Without a request the render is hr_render_video_to8b's, launch for launch.
 int hr_render_visuals(hr_handle* h, const hr_camera* cameras, const float* times, int32_t n_frames, uint8_t* video,
                       const hr_visual_request* req, int32_t n_req, void* workspace, int64_t workspace_bytes, void* stream) {
   const char* fn = "hr_render_visuals";
-  if (!h || !cameras || !times || !workspace) return hr_fail("%s: null argument", fn);
-  if (!h->uploaded) return hr_fail("%s: parameters not uploaded", fn);
-  if (n_frames < 1) return hr_fail("%s: n_frames must be >= 1, got %d", fn, n_frames);
+  bool mixed = false;
+  if (check_walk(fn, "n_frames", h, false, cameras, times, n_frames, workspace, &mixed)) return 1;
   int norm_ch = 0;
   if (check_visual_requests(fn, h, req, n_req, &norm_ch)) return 1;
   if (!video && n_req == 0) return hr_fail("%s: nothing to write (no video and no request)", fn);
-  const int32_t W = cameras[0].width, H = cameras[0].height;
-  VisLayout lay;
-  if (!visual_layout(h, norm_ch, n_frames, H, W, &lay))
-    return hr_fail("%s: %d frames of %d x %d pixels: bad size or bytes overflow int64", fn, n_frames, W, H);
-  bool mixed = false;
-  if (check_frames(fn, cameras, times, n_frames, &mixed)) return 1;
-  if (((uintptr_t)workspace & 15) != 0) return hr_fail("%s: workspace must be 16-byte aligned", fn);
-  if (workspace_bytes < lay.total)
-    return hr_fail("%s: workspace too small (%lld < %lld)", fn, (long long)workspace_bytes, (long long)lay.total);
-  DeviceGuard guard(h->device);
-  const hr_config& c = h->cfg;
-  cudaStream_t st = (cudaStream_t)stream;
-  char* base = (char*)workspace;
-  const int64_t frame_px = (int64_t)W * H, n = frame_px * n_frames, ring_rays = lay.ring * frame_px;
-  const int64_t rays_bytes = align256(lay.sub * c.c_in * (int64_t)sizeof(float));
-  // the render's outputs for a sub-batch starting at ray 0 of the video and of the ring; render_visuals moves them along
+  WalkLayout L;
+  const bool laid_out = visual_layout(h, norm_ch, n_frames, cameras[0].height, cameras[0].width, &L);
+  if (check_workspace(fn, laid_out, L, cameras, n_frames, workspace, workspace_bytes)) return 1;
+  const int64_t px = L.frame_px;
+  // the render's outputs for a sub-batch starting at ray 0 of the video and of the ring; render moves them along
   hr::ExtraOut so{};
   std::vector<float*> ring_of(n_req, nullptr);
-  int64_t ring_at = lay.ring_off;
+  int64_t ring_at = L.ring_off;
   for (int i = 0; i < n_req; ++i) {
     const hr_visual_request& r = req[i];
     hr::VisMap m{r.out, r.use_abs ? 1 : 0, r.bounded ? 1 : 0, r.lo, r.bounded ? r.hi - r.lo : 1.0f};
     so.field_mode[r.field] = r.mode;
     so.field_u8[r.field] = m;
     if (r.normalize) {
-      ring_of[i] = (float*)(base + ring_at);
-      ring_at += align256(lay.ring_bytes_per_ch * r.channels);
+      ring_of[i] = (float*)((char*)workspace + ring_at);
+      ring_at += align256(L.ring * px * (int64_t)sizeof(float) * r.channels);
     }
   }
   hr::RgbDst no_rgb{};  // n = 0: the render stores no colour
-  cudaStream_t ss[2] = {st, st};
-  std::vector<cudaEvent_t> evs;  // every event of the call, destroyed at the end (a destroyed event's pending work still runs)
-  auto new_event = [&](cudaEvent_t* ev) -> int {
-    CK(cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
-    evs.push_back(*ev);
-    return 0;
-  };
-  // mapped[k]: recorded after the map launches that read ring frame k last; done[s]: after stream s's last render
-  std::vector<cudaEvent_t> mapped(lay.n_slots == 2 ? lay.ring : 0, nullptr);
-  cudaEvent_t done[2] = {nullptr, nullptr};
-  int rc = 0;
-  if (lay.n_slots == 2) {
-    cudaEvent_t fork;
-    for (int i = 0; i < 2; ++i) {
-      if (pipe_stream(h, i)) return 1;
-      ss[i] = h->pipe.streams[i];
-    }
-    if (new_event(&fork)) return 1;
-    CK(cudaEventRecord(fork, st));
-    CK(cudaStreamWaitEvent(ss[0], fork, 0));
-    CK(cudaStreamWaitEvent(ss[1], fork, 0));
-    for (auto& e : mapped)
-      if ((rc = new_event(&e))) break;
-    for (int i = 0; i < 2 && !rc; ++i) rc = new_event(&done[i]);
-  }
-  int64_t next = 0;  // first frame not yet mapped (normalize requests)
-  int64_t i = 0;
-  for (int64_t off = 0; off < n && !rc; ++i) {
-    const int k = (int)(i % 2);
-    cudaStream_t s = ss[k];
-    const int64_t pos = ring_rays ? off % ring_rays : 0;
-    int64_t m = n - off < lay.sub ? n - off : lay.sub;
-    if (ring_rays && pos + m > ring_rays) m = ring_rays - pos;
-    const int64_t f0 = off / frame_px, f1 = (off + m - 1) / frame_px, f_end = (off + m) / frame_px;
-    auto fail = [&](const char* what, cudaError_t e) { return hr_fail("%s: %s: %s", fn, what, cudaGetErrorString(e)); };
-    cudaError_t e = cudaSuccess;
-    if (ring_rays && lay.n_slots == 2)  // ring frames rendered again: after the map launches of the frames they held
-      for (int64_t f = f0 < lay.ring ? lay.ring : f0; f <= f1 && e == cudaSuccess; ++f)
-        e = cudaStreamWaitEvent(s, mapped[f % lay.ring], 0);
-    hr_camera* win_c = (hr_camera*)(base + k * (lay.win_cams + lay.win_times));
-    float* win_t = (float*)((char*)win_c + lay.win_cams);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(win_c, cameras + f0, (size_t)(f1 - f0 + 1) * sizeof(hr_camera), cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(win_t, times + f0, (size_t)(f1 - f0 + 1) * sizeof(float), cudaMemcpyHostToDevice, s);
-    if (e != cudaSuccess) {
-      rc = fail("record copy", e);
-      break;
-    }
-    char* slot = base + lay.slots_off + (i % lay.n_slots) * lay.slot_bytes;
-    e = hr::launch_generate_video_rays(win_c, win_t, mixed, c.c_in, W, frame_px, off - f0 * frame_px, m, (float*)slot, s);
-    if (e != cudaSuccess) {
-      rc = fail("ray generation", e);
-      break;
-    }
-    h->launches += 1;
-    hr::ExtraOut so_b = so;
-    for (int r = 0; r < n_req; ++r) {
-      const int f = req[r].field;
-      if (ring_of[r]) {  // staged in fp32 at its ring position; mapped when the frame completes
-        so_b.field_out[f] = ring_of[r] + pos * req[r].channels;
-        so_b.field_u8[f].out = nullptr;
-      } else {
-        so_b.field_u8[f].out += off * req[r].channels;
-      }
-    }
-    rc = render_impl(h, (const float*)slot, m, nullptr, nullptr, &so_b, slot + rays_bytes, lay.slot_bytes - rays_bytes, s,
-                     video ? video + off * 3 : nullptr, video ? nullptr : &no_rgb);
-    if (rc) break;
-    if (ring_rays && f_end > next) {  // frames next .. f_end - 1 are complete, in consecutive ring frames
-      if (lay.n_slots == 2 && next * frame_px < off) e = cudaStreamWaitEvent(s, done[1 - k], 0);
-      float* part = (float*)(base + lay.partial_off + k * lay.partial_bytes);
-      for (int r = 0; r < n_req && e == cudaSuccess; ++r) {
-        if (!ring_of[r]) continue;
-        hr::VisMap vm = so.field_u8[req[r].field];
-        vm.out += next * frame_px * req[r].channels;
-        e = hr::launch_vis_normalize(ring_of[r] + (next % lay.ring) * frame_px * req[r].channels, (int)(f_end - next), frame_px,
-                                     req[r].channels, vm, part, s);
-        h->launches += 2;
-      }
-      for (int64_t f = next; f < f_end && e == cudaSuccess && lay.n_slots == 2; ++f) e = cudaEventRecord(mapped[f % lay.ring], s);
-      if (e != cudaSuccess) {
-        rc = fail("map launch", e);
-        break;
-      }
-      next = f_end;
-    }
-    if (lay.n_slots == 2 && (e = cudaEventRecord(done[k], s)) != cudaSuccess) {
-      rc = fail("event record", e);
-      break;
-    }
-    off += m;
-  }
-  if (lay.n_slots == 2) {  // join, also after a failed launch: the caller's stream must not run ahead of enqueued work
-    for (int k = 0; k < 2; ++k) {
-      cudaEvent_t ev;
-      if (new_event(&ev)) break;
-      CK(cudaEventRecord(ev, ss[k]));
-      CK(cudaStreamWaitEvent(st, ev, 0));
-    }
-  }
-  for (cudaEvent_t ev : evs) cudaEventDestroy(ev);
-  return rc;
+  return walk_frames(
+      h, fn, L, cameras, times, n_frames, mixed, workspace, (cudaStream_t)stream,
+      [&](int64_t off, int64_t pos, int64_t m, const float* rays, void* ws, int64_t ws_bytes, cudaStream_t s) {
+        hr::ExtraOut so_b = so;
+        for (int r = 0; r < n_req; ++r) {
+          const int f = req[r].field;
+          if (ring_of[r]) {  // staged in fp32 at its ring position; mapped when the frame completes
+            so_b.field_out[f] = ring_of[r] + pos * req[r].channels;
+            so_b.field_u8[f].out = nullptr;
+          } else {
+            so_b.field_u8[f].out += off * req[r].channels;
+          }
+        }
+        return render_impl(h, rays, m, nullptr, nullptr, n_req > 0 ? &so_b : nullptr, ws, ws_bytes, s,
+                           video ? video + off * 3 : nullptr, video ? nullptr : &no_rgb);
+      },
+      [&](int64_t next, int64_t f_end, int k, cudaStream_t s) {
+        float* part = (float*)((char*)workspace + L.part_off + k * L.part_bytes);
+        for (int r = 0; r < n_req; ++r) {
+          if (!ring_of[r]) continue;
+          hr::VisMap vm = so.field_u8[req[r].field];
+          vm.out += next * px * req[r].channels;
+          const cudaError_t e = hr::launch_vis_normalize(ring_of[r] + (next % L.ring) * px * req[r].channels, (int)(f_end - next),
+                                                         px, req[r].channels, vm, part, s);
+          if (e != cudaSuccess) return hr_fail("%s: map launch: %s", fn, cudaGetErrorString(e));
+          h->launches += 2;
+        }
+        return 0;
+      });
 }
 
 // the device's view of a pinned (device-addressable) host buffer, or null

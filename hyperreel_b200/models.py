@@ -442,7 +442,7 @@ class LightfieldModel(nn.Module):
         n = rays_host.shape[0]
         if rgb_host is None:
             rgb_host = torch.empty((n, 3), dtype=torch.float32, pin_memory=True)
-        self._ensure_uploaded(torch.device("cuda", self._device_index if self._device_index is not None else torch.cuda.current_device()))
+        self._ensure_uploaded(self._default_device())
         L.check(self._lib.hr_render_host(self._handle, rays_host.data_ptr(), n, rgb_host.data_ptr(), chunk))
         return rgb_host
 
@@ -489,10 +489,35 @@ class LightfieldModel(nn.Module):
             out_host = torch.empty((H, W, 3), dtype=torch.uint8, pin_memory=True)
         if out_host.is_cuda or out_host.dtype != torch.uint8 or out_host.numel() != H * W * 3 or not out_host.is_contiguous():
             raise ValueError("out_host must be a contiguous uint8 host tensor of H*W*3 elements")
-        self._ensure_uploaded(torch.device("cuda", self._device_index if self._device_index is not None else torch.cuda.current_device()))
+        self._ensure_uploaded(self._default_device())
         cam = camera.to_c()
         L.check(self._lib.hr_render_frame_to8b_host(self._handle, C.byref(cam), out_host.data_ptr(), chunk))
         return out_host
+
+    def _default_device(self) -> torch.device:
+        return torch.device("cuda", self._device_index if self._device_index is not None else torch.cuda.current_device())
+
+    def _frame_list(self, fn: str, cameras, times):
+        """The eval check and frame list of render_video, score_views and render_visuals, refused under ``fn``'s name before
+        any work: (F, H, W, the hr_camera records, the float32 times) of ``cameras`` (one size) at ``times`` (one per camera,
+        finite in float32; default each camera's ``time``)."""
+        if self.training:
+            raise RuntimeError("hyperreel_b200.LightfieldModel implements the eval()/render path only; call .eval()")
+        cams = list(cameras)
+        if not cams:
+            raise ValueError(f"{fn}: no cameras")
+        t = [float(c.time) for c in cams] if times is None else times
+        t = torch.as_tensor(t, dtype=torch.float64).reshape(-1).to(torch.float32)
+        if t.numel() != len(cams):
+            raise ValueError(f"{fn}: {len(cams)} cameras but {t.numel()} times")
+        if not bool(torch.isfinite(t).all()):
+            raise ValueError(f"{fn}: times must be finite in float32")
+        H, W = int(cams[0].height), int(cams[0].width)
+        for i, c in enumerate(cams):
+            if (int(c.height), int(c.width)) != (H, W):
+                raise ValueError(f"{fn}: camera {i} is {int(c.width)} x {int(c.height)}, camera 0 is {W} x {H}")
+        recs = (L.hr_camera * len(cams))(*[c.to_c() for c in cams])
+        return len(cams), H, W, recs, (C.c_float * len(cams))(*t.tolist())
 
     def render_video(self, cameras, times=None, out: Optional[torch.Tensor] = None, stream=None) -> torch.Tensor:
         """Frames of ``cameras`` (hyperreel_b200.camera.Camera or TwoPlaneCamera, one size, any mix of models) at ``times`` (one per camera;
@@ -500,40 +525,22 @@ class LightfieldModel(nn.Module):
         (hr_render_video_to8b): frame f is bit for bit the image render_frame_to8b makes of cameras[f] at times[f].  ``out``
         (device uint8 [F, H, W, 3], contiguous) receives it when given; the work goes on ``stream`` (a torch.cuda.Stream;
         default the current stream)."""
-        if self.training:
-            raise RuntimeError("hyperreel_b200.LightfieldModel implements the eval()/render path only; call .eval()")
-        cams = list(cameras)
-        if not cams:
-            raise ValueError("render_video: no cameras")
-        t = [float(c.time) for c in cams] if times is None else times
-        t = torch.as_tensor(t, dtype=torch.float64).reshape(-1).to(torch.float32)
-        if t.numel() != len(cams):
-            raise ValueError(f"render_video: {len(cams)} cameras but {t.numel()} times")
-        if not bool(torch.isfinite(t).all()):
-            raise ValueError("render_video: times must be finite in float32")
-        H, W = int(cams[0].height), int(cams[0].width)
-        for i, c in enumerate(cams):
-            if (int(c.height), int(c.width)) != (H, W):
-                raise ValueError(f"render_video: camera {i} is {int(c.width)} x {int(c.height)}, camera 0 is {W} x {H}")
+        F, H, W, recs, tt = self._frame_list("render_video", cameras, times)
         if out is not None:
-            if not out.is_cuda or out.dtype != torch.uint8 or tuple(out.shape) != (len(cams), H, W, 3) or not out.is_contiguous():
-                raise ValueError(f"render_video: out must be a contiguous CUDA uint8 tensor of shape {(len(cams), H, W, 3)}, got "
+            if not out.is_cuda or out.dtype != torch.uint8 or tuple(out.shape) != (F, H, W, 3) or not out.is_contiguous():
+                raise ValueError(f"render_video: out must be a contiguous CUDA uint8 tensor of shape {(F, H, W, 3)}, got "
                                  f"{out.dtype} {tuple(out.shape)} on {out.device}")
-            dev = out.device
-        else:
-            dev = torch.device("cuda", self._device_index if self._device_index is not None else torch.cuda.current_device())
+        dev = out.device if out is not None else self._default_device()
         self._ensure_uploaded(dev)
-        need = int(self._lib.hr_video_workspace_bytes(self._handle, len(cams), H, W))
+        need = int(self._lib.hr_video_workspace_bytes(self._handle, F, H, W))
         if need < 0:
-            raise ValueError(f"render_video: {len(cams)} frames of {W} x {H} pixels overflow a 64-bit size")
+            raise ValueError(f"render_video: {F} frames of {W} x {H} pixels overflow a 64-bit size")
         stream = stream if stream is not None else torch.cuda.current_stream(dev)
-        recs = (L.hr_camera * len(cams))(*[c.to_c() for c in cams])
-        tt = (C.c_float * len(cams))(*t.tolist())
         with torch.cuda.stream(stream):  # the scratch (and a new out) belong to the stream the work runs on
             ws = torch.empty(need, dtype=torch.uint8, device=dev)
             if out is None:
-                out = torch.empty((len(cams), H, W, 3), dtype=torch.uint8, device=dev)
-            L.check(self._lib.hr_render_video_to8b(self._handle, recs, tt, len(cams), out.data_ptr(), ws.data_ptr(), need,
+                out = torch.empty((F, H, W, 3), dtype=torch.uint8, device=dev)
+            L.check(self._lib.hr_render_video_to8b(self._handle, recs, tt, F, out.data_ptr(), ws.data_ptr(), need,
                                                    stream.cuda_stream))
         return out
 
@@ -546,24 +553,10 @@ class LightfieldModel(nn.Module):
         goes on ``stream`` (a torch.cuda.Stream; default the current stream).  ``rgba=True``: ``images`` are uint8 RGBA
         [n, H, W, 4], the DoNeRF and Catacaustics frames, and each view is scored against its composite over white,
         ``rgb * a + (1 - a)`` of the ``u8 / 255`` values as their ``get_rgb`` computes it on the CPU."""
-        if self.training:
-            raise RuntimeError("hyperreel_b200.LightfieldModel implements the eval()/render path only; call .eval()")
-        cams = list(cameras)
-        if not cams:
-            raise ValueError("score_views: no cameras")
-        t = [float(c.time) for c in cams] if times is None else times
-        t = torch.as_tensor(t, dtype=torch.float64).reshape(-1).to(torch.float32)
-        if t.numel() != len(cams):
-            raise ValueError(f"score_views: {len(cams)} cameras but {t.numel()} times")
-        if not bool(torch.isfinite(t).all()):
-            raise ValueError("score_views: times must be finite in float32")
-        H, W = int(cams[0].height), int(cams[0].width)
-        for i, c in enumerate(cams):
-            if (int(c.height), int(c.width)) != (H, W):
-                raise ValueError(f"score_views: camera {i} is {int(c.width)} x {int(c.height)}, camera 0 is {W} x {H}")
+        F, H, W, recs, tt = self._frame_list("score_views", cameras, times)
         if H < 11 or W < 11:
             raise ValueError(f"score_views: views must be at least 11 x 11 (the SSIM window), got {W} x {H}")
-        shape = (len(cams), H, W, 4 if rgba else 3)
+        shape = (F, H, W, 4 if rgba else 3)
         if not isinstance(images, torch.Tensor) or images.dtype != torch.uint8 or tuple(images.shape) != shape \
                 or not images.is_contiguous():
             got = f"{images.dtype} {tuple(images.shape)}" if isinstance(images, torch.Tensor) else type(images).__name__
@@ -575,23 +568,21 @@ class LightfieldModel(nn.Module):
         p = next(self.parameters(), None)
         if p is not None and p.is_cuda and p.device != dev:
             raise ValueError(f"score_views: images are on {dev}, the model on {p.device}")
-        if out is not None and (not out.is_cuda or out.dtype != torch.float64 or tuple(out.shape) != (len(cams), 2)
+        if out is not None and (not out.is_cuda or out.dtype != torch.float64 or tuple(out.shape) != (F, 2)
                                 or not out.is_contiguous() or out.device != dev):
-            raise ValueError(f"score_views: out must be a contiguous float64 tensor of shape {(len(cams), 2)} on {dev}, got "
+            raise ValueError(f"score_views: out must be a contiguous float64 tensor of shape {(F, 2)} on {dev}, got "
                              f"{out.dtype} {tuple(out.shape)} on {out.device}")
         self._ensure_uploaded(dev)
-        need = int(self._lib.hr_score_views_workspace_bytes(self._handle, len(cams), H, W))
+        need = int(self._lib.hr_score_views_workspace_bytes(self._handle, F, H, W))
         if need < 0:
-            raise ValueError(f"score_views: {len(cams)} views of {W} x {H} pixels overflow a 64-bit size")
+            raise ValueError(f"score_views: {F} views of {W} x {H} pixels overflow a 64-bit size")
         stream = stream if stream is not None else torch.cuda.current_stream(dev)
-        recs = (L.hr_camera * len(cams))(*[c.to_c() for c in cams])
-        tt = (C.c_float * len(cams))(*t.tolist())
         with torch.cuda.stream(stream):  # the scratch (and a new out) belong to the stream the work runs on
             ws = torch.empty(need, dtype=torch.uint8, device=dev)
             if out is None:
-                out = torch.empty((len(cams), 2), dtype=torch.float64, device=dev)
+                out = torch.empty((F, 2), dtype=torch.float64, device=dev)
             fmt = L.PIXEL_RGBA8 if rgba else L.PIXEL_RGB8
-            L.check(self._lib.hr_score_views(self._handle, recs, tt, len(cams), images.data_ptr(), fmt, out.data_ptr(),
+            L.check(self._lib.hr_score_views(self._handle, recs, tt, F, images.data_ptr(), fmt, out.data_ptr(),
                                              ws.data_ptr(), need, stream.cuda_stream))
         return out[:, 0], out[:, 1]
 
@@ -600,23 +591,9 @@ class LightfieldModel(nn.Module):
         ``requests`` (camera.VisualRequest, from camera.embedding_requests) in one render pass per frame and one call that
         never synchronises (hr_render_visuals).  Returns (video [F, H, W, 3] or None when ``rgb`` is False, {key: uint8
         [F, H, W, channels]})."""
-        if self.training:
-            raise RuntimeError("hyperreel_b200.LightfieldModel implements the eval()/render path only; call .eval()")
         from .signature import UnsupportedPipeline
 
-        cams = list(cameras)
-        if not cams:
-            raise ValueError("render_visuals: no cameras")
-        t = [float(c.time) for c in cams] if times is None else times
-        t = torch.as_tensor(t, dtype=torch.float64).reshape(-1).to(torch.float32)
-        if t.numel() != len(cams):
-            raise ValueError(f"render_visuals: {len(cams)} cameras but {t.numel()} times")
-        if not bool(torch.isfinite(t).all()):
-            raise ValueError("render_visuals: times must be finite in float32")
-        H, W = int(cams[0].height), int(cams[0].width)
-        for i, c in enumerate(cams):
-            if (int(c.height), int(c.width)) != (H, W):
-                raise ValueError(f"render_visuals: camera {i} is {int(c.width)} x {int(c.height)}, camera 0 is {W} x {H}")
+        F, H, W, recs, tt = self._frame_list("render_visuals", cameras, times)
         if not rgb and not requests:
             raise ValueError("render_visuals: nothing to render (rgb=False and no requests)")
         for r in requests:  # a field this model lacks: the reference's KeyError on x[key], refused before any work
@@ -624,10 +601,9 @@ class LightfieldModel(nn.Module):
                 self._field(r.key)
             except KeyError:
                 raise UnsupportedPipeline(f"embedding visualiser: field '{r.key}' is not an output of this model") from None
-        dev = torch.device("cuda", self._device_index if self._device_index is not None else torch.cuda.current_device())
+        dev = self._default_device()
         self._ensure_uploaded(dev)
         stream = stream if stream is not None else torch.cuda.current_stream(dev)
-        F = len(cams)
         with torch.cuda.stream(stream):  # the scratch and the outputs belong to the stream the work runs on
             maps = {r.key: torch.empty((F, H, W, r.channels), dtype=torch.uint8, device=dev) for r in requests}
             video = torch.empty((F, H, W, 3), dtype=torch.uint8, device=dev) if rgb else None
@@ -637,8 +613,6 @@ class LightfieldModel(nn.Module):
             need = int(self._lib.hr_render_visuals_workspace_bytes(self._handle, arr, len(reqs), F, H, W))
             if need < 0:
                 L.check(1)  # the library's reason
-            recs = (L.hr_camera * F)(*[c.to_c() for c in cams])
-            tt = (C.c_float * F)(*t.tolist())
             ws = torch.empty(need, dtype=torch.uint8, device=dev)
             L.check(self._lib.hr_render_visuals(self._handle, recs, tt, F, video.data_ptr() if rgb else None, arr, len(reqs),
                                                 ws.data_ptr(), need, stream.cuda_stream))

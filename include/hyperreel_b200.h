@@ -486,8 +486,8 @@ int hr_render_frame_to8b_host(hr_handle* h, const hr_camera* cam, uint8_t* rgb8_
  * cameras: HOST array of n_frames records, all of one width x height, each pinhole, fisheye (ABI 17) or two-plane (ABI 20); times: HOST fp32
  * [n_frames], frame f's time column (channel 7 when c_in == 8; the records' own `time` is not used).  video: DEVICE uint8
  * [n_frames, height, width, 3], frame f's pixels as hr_render_frame_to8b_host renders records[f] with time = times[f], bit for
- * bit.  workspace: device scratch of hr_video_workspace_bytes(h, n_frames, height, width) bytes (16B aligned), bounded
- * whatever n_frames: the records and times, then two slots (one for a video of at most one sub-batch), each one sub-batch
+ * bit.  workspace: device scratch of hr_video_workspace_bytes(h, n_frames, height, width) bytes (16B aligned): the records
+ * and times, then scratch bounded whatever n_frames, two slots (one for a video of at most one sub-batch), each one sub-batch
  * of rays (hr_render's sub-batch, 16 sample-net tile waves) and its render scratch.  The video's rays are generated and
  * rendered sub-batch by sub-batch across frame boundaries, alternating between two streams of the handle that are forked
  * from and joined back to `stream` by events: the call is ordered on `stream` like any other work.  No host
@@ -509,12 +509,13 @@ int hr_render_video_to8b(hr_handle* h, const hr_camera* cameras, const float* ti
  * (clamped output, the configured background, no to8b) against gt / 255 correctly rounded in fp32 (T.ToTensor()'s conversion; NumPy's, and torch's on the CPU),
  * or for RGBA against its fp32 composite over white (HR_PIXEL_RGBA8 above).
  * workspace: device scratch of hr_score_views_workspace_bytes(h, n_views, height, width) bytes (16B aligned, -1 for a size
- * hr_score_views refuses), bounded whatever n_views: two windows of ring-many records and times, a ring of whole fp32
- * frames (enough for two sub-batches and one frame more), two metrics partial buffers and the video path's one or two
- * slots.  The split is one ray sequence rendered in hr_render_video_to8b's sub-batches on its two streams (forked from and
- * joined back to `stream` by events), a sub-batch also cut where it would wrap the ring; a sub-batch that completes frames
- * scores them with one metrics launch on its own stream, after an event of the other stream for a frame that straddles
- * the two, and a ring frame is reused only after the launch that scored it.  No host synchronisation, no float atomics:
+ * hr_score_views refuses): the records and times (sizeof(hr_camera) + 4 = 148 bytes per view, copied once on `stream`),
+ * then scratch bounded whatever n_views, a ring of whole fp32 frames (enough for two sub-batches and one frame more), two
+ * metrics partial buffers and the video path's one or two slots.  The split is one ray sequence rendered in
+ * hr_render_video_to8b's sub-batches on its two streams (forked from and joined back to `stream` by events), a sub-batch
+ * also cut where it would wrap the ring; a sub-batch that completes frames scores them with one metrics launch on its own
+ * stream, after an event of the other stream for a frame that straddles the two, and a ring frame is reused only after the
+ * launch that scored it.  No host synchronisation, no float atomics:
  * two calls write the same bits.  Refused before anything is enqueued (out untouched): null or misaligned pointers
  * (out 8B, workspace 16B, RGBA gt 4B), an unknown pixel_format, n_views < 1, views of different sizes or smaller than
  * 11 x 11, a size whose bytes overflow int64, a non-finite record field, time or fisheye coefficient, a malformed two-plane
@@ -549,10 +550,11 @@ typedef struct hr_visual_request {
  * more), and each completed frame gets a min / max reduction (per-block partials, no atomics) and a map launch on the stream
  * of the sub-batch that completed it, a ring frame being rendered again only after its map launch.  The sub-batches, streams
  * and events are hr_score_views'; no host synchronisation; two calls write the same bits.  workspace: device scratch of
- * hr_render_visuals_workspace_bytes(h, req, n_req, n_frames, height, width) bytes (16B aligned, -1 for a call refused),
- * bounded whatever n_frames.  Refused before anything is enqueued (outputs untouched): null or misaligned pointers
- * (workspace 16B), n_req < 0 or a null list with n_req > 0, nothing to write, an unknown field or mode, a field requested
- * twice or not carried by the pipeline, channels other than the field's 1 or 3, non-finite bounds or hi == lo, the checks of
+ * hr_render_visuals_workspace_bytes(h, req, n_req, n_frames, height, width) bytes (16B aligned, -1 for a call refused): the
+ * records and times (148 bytes per frame), then scratch bounded whatever n_frames; without a request it is
+ * hr_video_workspace_bytes', and the call is hr_render_video_to8b's.  Refused before anything is enqueued (outputs
+ * untouched): null or misaligned pointers (workspace 16B), n_req < 0 or a null list with n_req > 0, nothing to write, an
+ * unknown field or mode, a field requested twice or not carried by the pipeline, channels other than the field's 1 or 3, non-finite bounds or hi == lo, the checks of
  * hr_render_video_to8b on the records, times and size, a workspace too small. */
 int64_t hr_render_visuals_workspace_bytes(const hr_handle* h, const hr_visual_request* req, int32_t n_req, int32_t n_frames,
                                           int32_t height, int32_t width);

@@ -16,6 +16,7 @@ from hyperreel_b200 import lib as L
 from oracle.hyperreel_oracle import HyperReelOracle
 from oracle.visual_oracle import visualize_to8b
 from tests.cases import build_case
+from tests.test_kernel_variants_gpu import kernels_run
 from tests.test_shipped_yaml_golden import SHIPPED, load_fixture
 
 pytestmark = pytest.mark.gpu
@@ -182,6 +183,44 @@ def test_two_calls_write_the_same_bytes_and_a_short_workspace_is_refused():
     assert _raw(model, cams, reqs, short[0].data_ptr(), ws_delta=-1) != 0
     assert "workspace too small" in L.load_library().hr_last_error().decode()
     assert all(bool((t == 77).all()) for t in short)
+
+
+def test_a_call_without_maps_runs_the_video_render_kernel():
+    """render_embeddings without a map is render_video launch for launch: the same render_kernel<...>, without the extra
+    fields' epilogue (EXTRA, the seventh template argument, false); a call with a map runs the EXTRA = true kernel."""
+    render, _, _, _ = _model("technicolor_trained")
+    model = render.model
+    model.set_sub_batch(1000)
+    cams = _cameras(3)
+    model.render_video(cams)  # upload
+    no_maps = hb.to_cfg({"type": "embedding", "fields": {}})
+    one_map = hb.to_cfg({"type": "embedding", "fields": {"distances": {"bounds": [0.0, 5.0]}}})
+    video = kernels_run(lambda: model.render_video(cams))[0]
+    assert len(video) == 1 and not next(iter(video))[6], video
+    assert kernels_run(lambda: hb.render_embeddings(render, cams, no_maps))[0] == video
+    mapped = kernels_run(lambda: hb.render_embeddings(render, cams, one_map))[0]
+    assert len(mapped) == 1 and next(iter(mapped))[6], mapped
+
+
+def test_the_workspaces_share_one_layout():
+    """Without a request the visual workspace is the video's; the video, score and visual workspaces grow with the frame
+    count by the 256-byte aligned record and time tables alone (the ring, partials and slots depend on the sub-batch)."""
+    render, _, _, _ = _model("technicolor_trained")
+    model = render.model
+    model.set_sub_batch(1000)  # a ring of 3 frames of 48 x 30: both frame counts below exceed it
+    model.render_video(_cameras(1))  # upload
+    lib, h = model._lib, model._handle
+    m = torch.empty((40, H, W), dtype=torch.uint8, device="cuda")
+    arr = (L.hr_visual_request * 1)(_req("distances", m.data_ptr(), normalize=1, bounded=0))
+
+    def tables(F):
+        return sum((b + 255) // 256 * 256 for b in (F * C.sizeof(L.hr_camera), F * 4))
+
+    for F in (5, 40):
+        assert lib.hr_video_workspace_bytes(h, F, H, W) == lib.hr_render_visuals_workspace_bytes(h, None, 0, F, H, W) > 0
+    for size in (lambda F: lib.hr_video_workspace_bytes(h, F, H, W), lambda F: lib.hr_score_views_workspace_bytes(h, F, H, W),
+                 lambda F: lib.hr_render_visuals_workspace_bytes(h, arr, 1, F, H, W)):
+        assert size(40) - size(5) == tables(40) - tables(5)
 
 
 def test_refusals_leave_the_outputs_untouched():
