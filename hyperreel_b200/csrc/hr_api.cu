@@ -291,12 +291,16 @@ int stage_in(const float* src, size_t count, int on_device, cudaStream_t st, std
   return 0;
 }
 
+// the net runs on the tensor cores (bf16x3 or fp16): the wgmma kernel, its pass table and its whole-wave launch sizes
+bool tc_net(int mlp_mode) { return mlp_mode == HR_MLP_BF16X3_TC || mlp_mode == HR_MLP_FP16_TC; }
+
 int validate(const hr_config& c) {
   if (c.abi_version != HR_ABI_VERSION) return hr_fail("hr_config.abi_version %d != %d", c.abi_version, HR_ABI_VERSION);
   if (hr::eases_density(c) && c.n_samples > 64) return hr_fail("eased density heads above 64 samples per ray are not supported");
   if (c.c_in != 6 && c.c_in != 8) return hr_fail("unsupported c_in %d (6: static rays, 8: video rays)", c.c_in);
   if (c.n_groups < 1 || c.n_groups > HR_MAX_GROUPS) return hr_fail("unsupported n_groups %d", c.n_groups);
-  if (c.mlp_mode != HR_MLP_FP32_SIMT && c.mlp_mode != HR_MLP_BF16X3_TC && c.mlp_mode != HR_MLP_ZERO) return hr_fail("unsupported mlp_mode");
+  if (c.mlp_mode != HR_MLP_FP32_SIMT && c.mlp_mode != HR_MLP_BF16X3_TC && c.mlp_mode != HR_MLP_ZERO && c.mlp_mode != HR_MLP_FP16_TC)
+    return hr_fail("unsupported mlp_mode");
   const bool has_net = c.mlp_mode != HR_MLP_ZERO;
   if (has_net && (c.mlp_layers < 2 || c.mlp_layers > HR_MAX_LAYERS)) return hr_fail("unsupported mlp_layers %d", c.mlp_layers);
   if (has_net && c.mlp_width != 128 && c.mlp_width != 256) return hr_fail("unsupported mlp_width %d (128 or 256)", c.mlp_width);
@@ -304,7 +308,7 @@ int validate(const hr_config& c) {
   if (has_net && c.mlp_skip != -1 && (c.mlp_skip < 1 || c.mlp_skip > c.mlp_layers - 2)) return hr_fail("bad mlp_skip %d", c.mlp_skip);
   if (c.n_samples < 1 || c.n_samples > HR_MAX_SAMPLES) return hr_fail("unsupported n_samples %d (max %d)", c.n_samples, HR_MAX_SAMPLES);
   if (c.mlp_out != c.n_samples * c.head_stride) return hr_fail("mlp_out %d != S*head_stride %d", c.mlp_out, c.n_samples * c.head_stride);
-  if (c.mlp_mode == HR_MLP_BF16X3_TC) {
+  if (tc_net(c.mlp_mode)) {
     const int out = c.cascade && c.pre_samples > 0 ? c.mlp_out / c.pre_samples : c.mlp_out;
     const int passes = c.mlp_layers - 1 + (out + c.mlp_width - 1) / c.mlp_width;
     if (passes > HR_TC_MAX_PASSES)
@@ -469,7 +473,7 @@ static int pack_net(hr_handle* h, SampleNet& net, const float* const* wsrc, cons
     simt.Kp[l] = Kp;
     simt.Np[l] = Np;
   }
-  if (!r && nc.mlp_mode == HR_MLP_BF16X3_TC) {
+  if (!r && tc_net(nc.mlp_mode)) {
     r = hr::pack_mlp_tc2(net, w_dev, b_dev, st);
     if (!r) net.tc_ready = true;
   }
@@ -702,7 +706,7 @@ static int launch_net(hr_handle* h, const SampleNet& net, const float* in, int64
     if (e != cudaSuccess) return hr_fail("heads memset failed: %s", cudaGetErrorString(e));
     return 0;
   }
-  if (nc.mlp_mode == HR_MLP_BF16X3_TC) {
+  if (tc_net(nc.mlp_mode)) {
     if (!net.tc_ready) return hr_fail("hr_render: tensor-core pack missing");
     e = hr::launch_mlp_tc2(nc, net.tc, in, out, rows, h->num_sms, st);
   } else {
@@ -929,7 +933,7 @@ int hr_render_frame_to8b_host(hr_handle* h, const hr_camera* cam, uint8_t* rgb8_
   DeviceGuard guard(h->device);
   const hr_config& c = h->cfg;
   const int64_t n_rays = (int64_t)cam->width * cam->height;
-  if (chunk <= 0) chunk = (h->cfg.mlp_mode == HR_MLP_BF16X3_TC) ? (int64_t)h->num_sms * 128 * 14 : 262144;  // whole tile waves
+  if (chunk <= 0) chunk = tc_net(h->cfg.mlp_mode) ? (int64_t)h->num_sms * 128 * 14 : 262144;  // whole tile waves
   if (chunk > n_rays) chunk = n_rays;
   HostPipe& P = h->pipe;
   if (ensure_pipe(h, chunk)) return 1;
@@ -1323,12 +1327,12 @@ int hr_render_host(hr_handle* h, const float* rays_host, int64_t n_rays, float* 
   // Default (chunk <= 0), tensor-core net, batches of a few waves: the "wave split" pipeline below.  Otherwise chunks of
   // `chunk` rays (default: whole waves for the tensor-core net, 32 768 rays for the CUDA-core net) on three streams.
   // (a cascaded pipeline runs its nets on point rows: it takes the plain chunked pipeline)
-  const bool whole = chunk <= 0 && c.mlp_mode == HR_MLP_BF16X3_TC && n_rays <= 16 * wave && !c.cascade;  // the batch stays whole on the device
+  const bool whole = chunk <= 0 && tc_net(c.mlp_mode) && n_rays <= 16 * wave && !c.cascade;  // the batch stays whole on the device
   const float* rays_dev_view = (whole && h->net.tc_ready && !h->timing) ? device_view(rays_host) : nullptr;
   const bool zero_copy = rays_dev_view != nullptr;
   float* rgb_dev_view = zero_copy ? device_view(rgb_host) : nullptr;
   const bool split = !zero_copy && whole && n_rays > wave;
-  if (chunk <= 0) chunk = (c.mlp_mode == HR_MLP_BF16X3_TC) ? wave : 32768;
+  if (chunk <= 0) chunk = tc_net(c.mlp_mode) ? wave : 32768;
   if (chunk > n_rays) chunk = n_rays;
   const int64_t alloc = (split || zero_copy) ? n_rays : chunk;  // rays per device slot
   if (ensure_pipe(h, alloc)) return 1;

@@ -20,7 +20,7 @@ struct MlpSimtPack {
   int skip;
 };
 
-// wgmma path (HR_MLP_BF16X3_TC): see hr_mlp_tc2.cu.  A "pass" is one accumulator's worth of output columns
+// wgmma path (HR_MLP_BF16X3_TC, HR_MLP_FP16_TC): see hr_mlp_tc2.cu.  A "pass" is one accumulator's worth of output columns
 // (W = hidden width: a whole hidden layer, or W columns of the last layer); its weights are stored as n_chunks*2 k-step
 // images.  At most HR_TC_MAX_PASSES passes (hyperreel_b200.h).
 struct TcPass {
@@ -34,7 +34,7 @@ struct TcPass {
   int wait_a;       // the issuer must wait for the A chunks (first pass of a layer)
 };
 struct MlpTcPack {
-  const void* wpack;   // bf16 hi/lo weight images, K-major no-swizzle layout, consumption order: columns [0, W/2) of
+  const void* wpack;   // bf16 hi/lo (fp16: fp16) weight images, K-major no-swizzle layout, consumption order: columns [0, W/2) of
                        // every pass, then columns [W/2, W) (wpack_bytes / 2 each)
   const float* bias;   // [bias_count]
   long long wpack_bytes;

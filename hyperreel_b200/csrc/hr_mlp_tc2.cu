@@ -1,4 +1,4 @@
-// Sample-prediction network on the Hopper tensor cores (HR_MLP_BF16X3_TC), wgmma.
+// Sample-prediction network on the Hopper tensor cores (HR_MLP_BF16X3_TC, and HR_MLP_FP16_TC: F16 below), wgmma.
 //
 // Math (reference: nlf/nets/mlp.py:159-172 behind nlf/embedding/ray.py:320-326): every fp32 operand x is split into
 // bf16 hi = rn(x) and lo = rn(x - hi) and each Linear layer is
@@ -28,6 +28,11 @@
 // columns per 16-byte store (NARROW: 8- or 4-byte stores, for rows that are not 16-byte aligned); the hidden epilogues write
 // the activation operand with stmatrix.
 //
+// F16 (HR_MLP_FP16_TC, inference only): what CUDA autocast computes for each F.linear -- the operands rounded to fp16, one
+// wgmma product per k-step (.f32.f16.f16, fp32 accumulation), the fp16 bias added and the sum rounded once to fp16, LeakyReLU
+// on that fp16 value (a negative one rounded again after x * slope).  One operand image (no lo half of A, X or the weights),
+// so the shared-memory map and ring stages differ (tc2::Layout<true>); the last layer's fp16 values go to the heads as fp32.
+//
 // SAVE (the training forward, hr_mlp_train.cu): the same arithmetic, plus every fp32 value the epilogues split goes to global
 // memory as well -- the encoded input (sv.enc) and each hidden layer's LeakyReLU output (sv.act) -- and the heads are stored
 // in the reference's sample-major column order instead of channel-major.
@@ -47,9 +52,7 @@ namespace hr {
 namespace tc2 {
 using namespace tc;
 
-constexpr int NSTAGE = 4;            // depth of each warpgroup's weight ring
-constexpr int STAGE_BYTES = 8192;    // one ring stage: k-step images of W/2 x 16 k x (hi + lo) bf16, 1 (W = 256) or 2 (W = 128)
-constexpr int KSTEP_BYTES = 4096;    // activation k-step image: 128 rays x 16 k bf16
+constexpr int KSTEP_BYTES = 4096;    // activation k-step image: 128 rays x 16 k bf16 (or fp16)
 constexpr int CONSUMERS = 2;         // warpgroups of W/2 output columns
 constexpr int NTHREADS = (CONSUMERS + 1) * 128;  // + the producer warpgroup (lane 0 of its first two warps issues the copies)
 // register split of the 64 K registers (setmaxnreg): the producer warpgroup gives up what the consumers need beside their
@@ -58,21 +61,28 @@ constexpr int PRODUCER_REGS = 40;
 constexpr int CONSUMER_REGS = 232;
 static_assert(128 * PRODUCER_REGS + CONSUMERS * 128 * CONSUMER_REGS <= 65536, "register file");
 
-// shared memory map (bytes)
-constexpr int A_BYTES = 16 * KSTEP_BYTES;                    // 64 KB: one half (hi or lo) of the activation operand
-constexpr int OFF_AHI = 0;
-constexpr int OFF_ALO = OFF_AHI + A_BYTES;
-constexpr int X_BYTES = 4 * KSTEP_BYTES;                     // encoded input: up to 4 k-steps (64 k) hi, then as many lo
-constexpr int OFF_X = OFF_ALO + A_BYTES;                     // 131072
-constexpr int OFF_B = OFF_X + 2 * X_BYTES;                   // 163840: ring of warpgroup 0, then of warpgroup 1
-constexpr int OFF_BAR = OFF_B + CONSUMERS * NSTAGE * STAGE_BYTES;  // 229376
-constexpr int SMEM_BYTES = OFF_BAR + 128;                    // 229504 (of 232448 available)
-static_assert(SMEM_BYTES <= 232448, "shared memory budget");
-
-// barrier slots (8 bytes each) inside OFF_BAR
-constexpr int BAR_FULL = 0;                               // [CONSUMERS][NSTAGE]
-constexpr int BAR_EMPTY = BAR_FULL + CONSUMERS * NSTAGE;  // [CONSUMERS][NSTAGE]
-static_assert((BAR_EMPTY + CONSUMERS * NSTAGE) * 8 <= 128, "barrier block");
+// Shared memory map (bytes) and weight ring.  bf16x3: the activation operand A and the encoded input X as hi then lo images,
+// rings of 4 stages of 8 KB (k-step weight images of W/2 x 16 k x (hi + lo) bf16, 1 at W = 256 or 2 at W = 128 per stage).
+// F16: A and X as one fp16 image each, rings of 8 stages of 4 KB (the same k-steps per stage, each image half the size).
+template <bool F16>
+struct Layout {
+  static constexpr int PARTS = F16 ? 1 : 2;                   // operand images per k-step: hi (+ lo)
+  static constexpr int NSTAGE = F16 ? 8 : 4;                  // depth of each warpgroup's weight ring
+  static constexpr int STAGE_BYTES = F16 ? 4096 : 8192;       // one ring stage
+  static constexpr int A_BYTES = 16 * KSTEP_BYTES;            // 64 KB: one image (hi or lo) of the activation operand
+  static constexpr int OFF_AHI = 0;
+  static constexpr int OFF_ALO = OFF_AHI + A_BYTES;           // bf16x3 only
+  static constexpr int X_BYTES = 4 * KSTEP_BYTES;             // encoded input: up to 4 k-steps (64 k) hi, then as many lo
+  static constexpr int OFF_X = PARTS * A_BYTES;               // 131072 (F16: 65536)
+  static constexpr int OFF_B = OFF_X + PARTS * X_BYTES;       // 163840 (81920): ring of warpgroup 0, then of warpgroup 1
+  static constexpr int OFF_BAR = OFF_B + CONSUMERS * NSTAGE * STAGE_BYTES;  // 229376 (147456)
+  static constexpr int BAR_BYTES = 2 * CONSUMERS * NSTAGE * 8;              // 128 (256)
+  static constexpr int SMEM_BYTES = OFF_BAR + BAR_BYTES;      // 229504 (147712) of 232448 available
+  // barrier slots (8 bytes each) inside OFF_BAR
+  static constexpr int BAR_FULL = 0;                               // [CONSUMERS][NSTAGE]
+  static constexpr int BAR_EMPTY = BAR_FULL + CONSUMERS * NSTAGE;  // [CONSUMERS][NSTAGE]
+  static_assert(SMEM_BYTES <= 232448, "shared memory budget");
+};
 
 // named barriers: 1 + g is warpgroup g's own (wg_sync); id + g below is a signal from warpgroup g to the other one
 constexpr int NB_RET = 3;  // g's wgmmas that read the other warpgroup's half of A have retired: that half may be rewritten
@@ -84,18 +94,23 @@ constexpr int NB_XR = 9;   // g's wgmmas that read the encoded input have retire
 
 // NARROW: the heads rows of the render net (SAVE = false) are stored with 8- or 4-byte stores, each column guarded, for an
 // mlp_out that is not a multiple of 4 or a heads pointer that is not 16-byte aligned (launch_mlp_tc2 picks it).
-template <int W, bool SAVE, bool NARROW>
+template <int W, bool SAVE, bool NARROW, bool F16 = false>
 __global__ void __launch_bounds__(tc2::NTHREADS, 1)
 mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ MlpTcPack pk, const float* __restrict__ rays,
                float* __restrict__ heads, long long n_rays, float* __restrict__ rays_copy, const TrainSave sv) {
   using namespace tc2;
+  static_assert(!(F16 && SAVE), "the training forward is bf16x3 only");
+  using Lay = Layout<F16>;
+  constexpr int NSTAGE = Lay::NSTAGE, STAGE_BYTES = Lay::STAGE_BYTES, OFF_AHI = Lay::OFF_AHI, OFF_ALO = Lay::OFF_ALO;
+  constexpr int X_BYTES = Lay::X_BYTES, OFF_X = Lay::OFF_X, OFF_B = Lay::OFF_B, OFF_BAR = Lay::OFF_BAR;
+  constexpr int BAR_FULL = Lay::BAR_FULL, BAR_EMPTY = Lay::BAR_EMPTY;
   constexpr int WH = W / 2;                          // output columns of one warpgroup
   constexpr int NACC = WH / 2;                       // registers of one m64nWH accumulator
   constexpr int NK = W / 16;                         // k-steps of the hidden activation operand
   constexpr int NKH = NK / 2;                        // k-steps holding one column half
-  constexpr int IMG_BYTES = WH * 64;                 // weight image of one k-step of a column half: WH x 16 k, hi then lo
+  constexpr int IMG_BYTES = WH * 32 * Lay::PARTS;    // weight image of one k-step of a column half: WH x 16 k, hi (then lo)
   constexpr int KPS = STAGE_BYTES / IMG_BYTES;       // k-steps per ring stage
-  static_assert(KPS * IMG_BYTES == STAGE_BYTES && NKH % KPS == 0 && NK * KSTEP_BYTES <= A_BYTES, "pass width");
+  static_assert(KPS * IMG_BYTES == STAGE_BYTES && NKH % KPS == 0 && NK * KSTEP_BYTES <= Lay::A_BYTES, "pass width");
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t sbase = smem_u32(smem);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -110,7 +125,7 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
     for (long long i = (long long)blockIdx.x * NTHREADS + tid; i < lines; i += (long long)gridDim.x * NTHREADS)
       asm volatile("prefetch.global.L2 [%0];" ::"l"(w + i * 128));
   }
-  for (int i = tid; i < (2 * X_BYTES) / 16; i += NTHREADS)  // encoded-input operand: columns >= mlp_in stay zero
+  for (int i = tid; i < (Lay::PARTS * X_BYTES) / 16; i += NTHREADS)  // encoded-input operand: columns >= mlp_in stay zero
     reinterpret_cast<uint4*>(smem + OFF_X)[i] = make_uint4(0u, 0u, 0u, 0u);
   if (tid == 0) {
     for (int s = 0; s < CONSUMERS * NSTAGE; ++s) { mbar_init(bar(BAR_FULL + s), 1); mbar_init(bar(BAR_EMPTY + s), 1); }
@@ -185,17 +200,25 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
     if (++stage == NSTAGE) { stage = 0; phase ^= 1; }
   };
   auto b_img = [&](int sub) -> uint32_t { return ring + stage * STAGE_BYTES + (uint32_t)sub * IMG_BYTES; };
-  // one k-step: the three products for both M halves (a: hi k-step image of all 128 rows, its lo image a_lo bytes later)
+  // one k-step: the three products for both M halves (a: hi k-step image of all 128 rows, its lo image a_lo bytes later);
+  // F16: the one fp16 product
   auto kstep = [&](uint32_t a, uint32_t a_lo, uint32_t b, uint32_t scale) {
-    const uint64_t bh = gmma_desc(b, WH * 16, 128), bl = gmma_desc(b + WH * 32, WH * 16, 128);
-    const uint64_t ah0 = gmma_desc(a, 2048, 128), ah1 = gmma_desc(a + 1024, 2048, 128);
-    const uint64_t al0 = gmma_desc(a + a_lo, 2048, 128), al1 = gmma_desc(a + a_lo + 1024, 2048, 128);
-    wgmma_ss(acc[0], ah0, bh, scale);
-    wgmma_ss(acc[1], ah1, bh, scale);
-    wgmma_ss(acc[0], al0, bh, 1u);
-    wgmma_ss(acc[1], al1, bh, 1u);
-    wgmma_ss(acc[0], ah0, bl, 1u);
-    wgmma_ss(acc[1], ah1, bl, 1u);
+    if constexpr (F16) {
+      const uint64_t bh = gmma_desc(b, WH * 16, 128);
+      const uint64_t ah0 = gmma_desc(a, 2048, 128), ah1 = gmma_desc(a + 1024, 2048, 128);
+      wgmma_ss<true>(acc[0], ah0, bh, scale);
+      wgmma_ss<true>(acc[1], ah1, bh, scale);
+    } else {
+      const uint64_t bh = gmma_desc(b, WH * 16, 128), bl = gmma_desc(b + WH * 32, WH * 16, 128);
+      const uint64_t ah0 = gmma_desc(a, 2048, 128), ah1 = gmma_desc(a + 1024, 2048, 128);
+      const uint64_t al0 = gmma_desc(a + a_lo, 2048, 128), al1 = gmma_desc(a + a_lo + 1024, 2048, 128);
+      wgmma_ss(acc[0], ah0, bh, scale);
+      wgmma_ss(acc[1], ah1, bh, scale);
+      wgmma_ss(acc[0], al0, bh, 1u);
+      wgmma_ss(acc[1], al1, bh, 1u);
+      wgmma_ss(acc[0], ah0, bl, 1u);
+      wgmma_ss(acc[1], ah1, bl, 1u);
+    }
   };
   // One pass: acc = A(chunks of P) * B(P)^T.  fresh: the first pass that reads the A an epilogue just wrote; x_ret /
   // ret: signal NB_XR / NB_RET as soon as the reads of X / of the other warpgroup's half of A have retired (warpgroup 1
@@ -238,7 +261,8 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
     if (pend >= 0 && wt == 0) mbar_arrive(empty0 + pend * 8);
     pend = -1;
   };
-  // hidden epilogue: this warpgroup's columns of A(l+1) = LeakyReLU(acc + bias), split into hi / lo.  The accumulator
+  // hidden epilogue: this warpgroup's columns of A(l+1) = LeakyReLU(acc + bias), split into hi / lo (F16: LeakyReLU of
+  // rn16(acc + bias), rounded to fp16 again).  The accumulator
   // fragment of columns 8 j .. 8 j + 7 and rows 8 h .. 8 h + 7 of the warp is an 8x8 stmatrix fragment, and its
   // destination rows are 16-byte core-matrix rows of A, so one stmatrix.x4 writes a whole 16-wide k-step of the warp's 16
   // rows: matrix i = 2 (j % 2) + h, lane t addresses row t % 8 of matrix t / 8.
@@ -259,9 +283,16 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             float t0 = acc[m][4 * j + 2 * h] + b[jj].x, t1 = acc[m][4 * j + 2 * h + 1] + b[jj].y;
+            if constexpr (F16) {
+              t0 = rn16(t0);
+              t1 = rn16(t1);
+            }
             t0 = fmaxf(t0, t0 * cfg.leaky_slope);  // LeakyReLU, slope in (0,1)
             t1 = fmaxf(t1, t1 * cfg.leaky_slope);
-            split2(t0, t1, hi[2 * jj + h], lo[2 * jj + h]);
+            if constexpr (F16)
+              hi[2 * jj + h] = pack_half2(t0, t1);
+            else
+              split2(t0, t1, hi[2 * jj + h], lo[2 * jj + h]);
             if constexpr (SAVE) {
               const long long ray = tile * BM + 64 * m + rowq + 8 * h;
               if (ray < n_rays) *reinterpret_cast<float2*>(sv.act + layer * sv.act_stride + ray * W + k) = make_float2(t0, t1);
@@ -270,12 +301,13 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
         }
         const uint32_t a = sbase + st_off + (uint32_t)m * 1024u + (uint32_t)(wg * NKH + kk) * KSTEP_BYTES;
         stmatrix_x4(a + OFF_AHI, hi);
-        stmatrix_x4(a + OFF_ALO, lo);
+        if constexpr (!F16) stmatrix_x4(a + OFF_ALO, lo);
       }
     }
   };
   // RayParam + WindowedPE of this warpgroup's 64 rays (tile rows 64 wg ..), two threads per ray, straight into the bf16
-  // hi / lo slots of X; after_x: X still holds the previous tile, wait until the other warpgroup's reads of it retired
+  // hi / lo slots of X (F16: its fp16 slots); after_x: X still holds the previous tile, wait until the other warpgroup's
+  // reads of it retired
   auto encode = [&](long long tile, bool after_x) {
     if (after_x) pair_wait(NB_XR + (wg ^ 1));
     const int r = wg * 64 + (wt & 63), part = wt >> 6;
@@ -284,11 +316,16 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
       if constexpr (SAVE) {
         if (ray < n_rays) sv.enc[ray * sv.ld_enc + k] = val;
       }
-      const __nv_bfloat16 hi = __float2bfloat16_rn(val);
-      const __nv_bfloat16 lo = __float2bfloat16_rn(val - __bfloat162float(hi));
-      const uint32_t off = (uint32_t)(k >> 4) * KSTEP_BYTES + ks_slot(r, (k >> 3) & 1) + (uint32_t)(k & 7) * 2u;
-      *reinterpret_cast<__nv_bfloat16*>(smem + OFF_X + off) = hi;
-      *reinterpret_cast<__nv_bfloat16*>(smem + OFF_X + x_lo_off + off) = lo;
+      if constexpr (F16) {
+        const uint32_t off = (uint32_t)(k >> 4) * KSTEP_BYTES + ks_slot(r, (k >> 3) & 1) + (uint32_t)(k & 7) * 2u;
+        *reinterpret_cast<__half*>(smem + OFF_X + off) = __float2half_rn(val);
+      } else {
+        const __nv_bfloat16 hi = __float2bfloat16_rn(val);
+        const __nv_bfloat16 lo = __float2bfloat16_rn(val - __bfloat162float(hi));
+        const uint32_t off = (uint32_t)(k >> 4) * KSTEP_BYTES + ks_slot(r, (k >> 3) & 1) + (uint32_t)(k & 7) * 2u;
+        *reinterpret_cast<__nv_bfloat16*>(smem + OFF_X + off) = hi;
+        *reinterpret_cast<__nv_bfloat16*>(smem + OFF_X + x_lo_off + off) = lo;
+      }
     };
     if (ray < n_rays) {
       // `rays` may be pinned host memory (zero-copy input of hr_render_host): each ray is read once per thread, with
@@ -347,6 +384,10 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
       } else {
         // ---- last layer: accumulators + bias -> heads scratch (rows past n_rays / columns past mlp_out are dropped) ----
         const float* bias = pk.bias + P.bias_off;
+        auto out = [](float v) -> float {  // F16: the layer's fp16 result, stored as fp32
+          if constexpr (F16) return rn16(v);
+          return v;
+        };
         if constexpr (SAVE) {
 #pragma unroll
           for (int m = 0; m < 2; ++m)
@@ -382,7 +423,7 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
                 const long long ray = tile * BM + 64 * m + rowq + 8 * h;
                 if (ray >= n_rays || c0 >= cfg.mlp_out) continue;
                 float* dst = heads + ray * cfg.mlp_out + c0;
-                const float v0 = acc[m][4 * j + 2 * h] + b.x, v1 = acc[m][4 * j + 2 * h + 1] + b.y;
+                const float v0 = out(acc[m][4 * j + 2 * h] + b.x), v1 = out(acc[m][4 * j + 2 * h + 1] + b.y);
                 if (pairs) {
                   *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
                 } else {
@@ -406,8 +447,8 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
             for (int m = 0; m < 2; ++m)
 #pragma unroll
               for (int h = 0; h < 2; ++h) {
-                const float2 v0 = make_float2(acc[m][4 * j + 2 * h] + b0.x, acc[m][4 * j + 2 * h + 1] + b0.y);
-                const float2 v1 = make_float2(acc[m][4 * j + 4 + 2 * h] + b1.x, acc[m][4 * j + 4 + 2 * h + 1] + b1.y);
+                const float2 v0 = make_float2(out(acc[m][4 * j + 2 * h] + b0.x), out(acc[m][4 * j + 2 * h + 1] + b0.y));
+                const float2 v1 = make_float2(out(acc[m][4 * j + 4 + 2 * h] + b1.x), out(acc[m][4 * j + 4 + 2 * h + 1] + b1.y));
                 const float2 send = odd ? v0 : v1;
                 const float2 recv = make_float2(__shfl_xor_sync(0xffffffffu, send.x, 1), __shfl_xor_sync(0xffffffffu, send.y, 1));
                 const int c4 = odd ? c + 6 : c;  // first of the lane's 4 columns
@@ -424,6 +465,17 @@ mlp_tc2_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Ml
   }
 }
 
+// the inference kernel of a net: width 128 or 256 (anything else is 128: callers check), narrow heads stores, fp16 or bf16x3
+using Tc2Kernel = void (*)(const hr_config, const MlpTcPack, const float*, float*, long long, float*, const TrainSave);
+static Tc2Kernel tc2_kernel(int W, bool narrow, bool f16) {
+  if (f16)
+    return W == 256 ? (narrow ? mlp_tc2_kernel<256, false, true, true> : mlp_tc2_kernel<256, false, false, true>)
+                    : (narrow ? mlp_tc2_kernel<128, false, true, true> : mlp_tc2_kernel<128, false, false, true>);
+  return W == 256 ? (narrow ? mlp_tc2_kernel<256, false, true> : mlp_tc2_kernel<256, false, false>)
+                  : (narrow ? mlp_tc2_kernel<128, false, true> : mlp_tc2_kernel<128, false, false>);
+}
+static int tc2_smem_bytes(bool f16) { return f16 ? tc2::Layout<true>::SMEM_BYTES : tc2::Layout<false>::SMEM_BYTES; }
+
 // Pass table + weight images (format: hr_tc_pack.cu).  Called by hr_upload with the handle's device current.
 int pack_mlp_tc2(SampleNet& net, const float* const* w_dev, const float* const* b_dev, cudaStream_t st) {
   const hr_config& c = net.cfg;
@@ -431,6 +483,8 @@ int pack_mlp_tc2(SampleNet& net, const float* const* w_dev, const float* const* 
   size_t& alloc_bytes = net.tc_alloc_bytes;
   int& alloc_bias = net.tc_alloc_bias;
   const int W = c.mlp_width;
+  const bool f16 = c.mlp_mode == HR_MLP_FP16_TC;
+  const int img_bytes = f16 ? 32 : 64;  // bytes of one k-step image per output column: 16 k of fp16, or bf16 hi + lo
   if (W != 128 && W != 256) return hr_fail("tensor-core sample net: hidden width must be 128 or 256 (got %d)", W);
   if (c.mlp_in > 64) return hr_fail("tensor-core sample net: encoded input wider than 64 features (%d)", c.mlp_in);
   const int in_chunks = (c.mlp_in + 31) / 32;
@@ -458,7 +512,7 @@ int pack_mlp_tc2(SampleNet& net, const float* const* w_dev, const float* const* 
       P.out_col0 = part * W;
       P.wait_a = (part == 0) ? 1 : 0;
       bias_off += P.n;
-      bytes += (size_t)P.n_chunks * 2 * P.n * 64;
+      bytes += (size_t)P.n_chunks * 2 * P.n * img_bytes;
     }
   }
   np_.n_passes = np;
@@ -476,12 +530,9 @@ int pack_mlp_tc2(SampleNet& net, const float* const* w_dev, const float* const* 
     if (e != cudaSuccess) { cudaFree(wp); return hr_fail("cudaMalloc(tc bias): %s", cudaGetErrorString(e)); }
     np_.wpack = wp; np_.bias = bp;
     alloc_bytes = bytes; alloc_bias = bias_off;
-    // opt in to the 224 KB of dynamic shared memory once per (handle, device)
-    for (int narrow = 0; narrow < 2 && e == cudaSuccess; ++narrow) {
-      auto kern = (W == 256) ? (narrow ? mlp_tc2_kernel<256, false, true> : mlp_tc2_kernel<256, false, false>)
-                             : (narrow ? mlp_tc2_kernel<128, false, true> : mlp_tc2_kernel<128, false, false>);
-      e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::SMEM_BYTES);
-    }
+    // opt in to the 224 KB (F16: 144 KB) of dynamic shared memory once per (handle, device)
+    for (int narrow = 0; narrow < 2 && e == cudaSuccess; ++narrow)
+      e = cudaFuncSetAttribute(tc2_kernel(W, narrow != 0, f16), cudaFuncAttributeMaxDynamicSharedMemorySize, tc2_smem_bytes(f16));
     if (e != cudaSuccess) return hr_fail("cudaFuncSetAttribute(mlp_tc2_kernel): %s", cudaGetErrorString(e));
   } else {
     np_.wpack = pk.wpack; np_.bias = pk.bias;
@@ -501,8 +552,8 @@ int pack_mlp_tc2(SampleNet& net, const float* const* w_dev, const float* const* 
       const int in_src = first ? c.mlp_in : (skip ? c.mlp_in + W : W);
       launch_pack_tc_pass(w_dev[l], b_dev[l], wp + off, bp + P.bias_off + half * WH, WH, P.first_chunk, P.n_chunks, in_src,
                           c.mlp_in, skip ? 1 : 0, in_chunks, last ? c.mlp_out : W, last ? c.n_samples : 0, c.head_stride,
-                          P.out_col0 + half * WH, st);
-      off += (size_t)P.n_chunks * 2 * WH * 64;
+                          P.out_col0 + half * WH, f16 ? 1 : 0, st);
+      off += (size_t)P.n_chunks * 2 * WH * img_bytes;
     }
   }
   cudaError_t e = cudaGetLastError();
@@ -524,10 +575,10 @@ cudaError_t launch_mlp_tc2(const hr_config& cfg, const MlpTcPack& pk, const floa
   if (grid < 1) grid = 1;
   // the 16-byte heads stores need every row to start 16-byte aligned; any other row takes the narrow stores
   const bool narrow = (cfg.mlp_out % 4) != 0 || ((uintptr_t)heads % 16) != 0;
-  auto kern = cfg.mlp_width == 256 ? (narrow ? mlp_tc2_kernel<256, false, true> : mlp_tc2_kernel<256, false, false>)
-                                   : (narrow ? mlp_tc2_kernel<128, false, true> : mlp_tc2_kernel<128, false, false>);
+  const bool f16 = cfg.mlp_mode == HR_MLP_FP16_TC;
   if (cfg.mlp_width != 256 && cfg.mlp_width != 128) return cudaErrorInvalidValue;
-  kern<<<grid, tc2::NTHREADS, tc2::SMEM_BYTES, stream>>>(cfg, pk, rays, heads, n, rays_copy, TrainSave{});
+  tc2_kernel(cfg.mlp_width, narrow, f16)<<<grid, tc2::NTHREADS, tc2_smem_bytes(f16), stream>>>(cfg, pk, rays, heads, n, rays_copy,
+                                                                                              TrainSave{});
   return cudaGetLastError();
 }
 
@@ -538,9 +589,10 @@ cudaError_t launch_mlp_tc2_train(const hr_config& cfg, const MlpTcPack& pk, cons
   if (grid < 1) grid = 1;
   auto kern = cfg.mlp_width == 256 ? mlp_tc2_kernel<256, true, false> : mlp_tc2_kernel<128, true, false>;
   if (cfg.mlp_width != 256 && cfg.mlp_width != 128) return cudaErrorInvalidValue;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, tc2::SMEM_BYTES);
+  constexpr int smem = tc2::Layout<false>::SMEM_BYTES;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) return e;
-  kern<<<grid, tc2::NTHREADS, tc2::SMEM_BYTES, stream>>>(cfg, pk, rays, heads, n, nullptr, sv);
+  kern<<<grid, tc2::NTHREADS, smem, stream>>>(cfg, pk, rays, heads, n, nullptr, sv);
   return cudaGetLastError();
 }
 

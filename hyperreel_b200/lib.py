@@ -11,7 +11,7 @@ import os
 import subprocess
 import threading
 
-HR_ABI_VERSION = 25
+HR_ABI_VERSION = 26
 HR_MAX_GROUPS = 4
 HR_MAX_LAYERS = 10
 HR_MAX_SAMPLES = 256
@@ -24,7 +24,7 @@ ISECT_Z_PLANE, ISECT_SPHERE, ISECT_CYLINDER, ISECT_SPHERE_NEW, ISECT_DISTANCE, I
 CONTRACT_NONE, CONTRACT_MIPNERF, CONTRACT_AFFINE = 0, 1, 2
 SHADE_SH, SHADE_RGB = 0, 1
 DENSE_RELU, DENSE_SOFTPLUS, DENSE_RELU_ABS = 0, 1, 2
-MLP_FP32_SIMT, MLP_BF16X3_TC, MLP_ZERO = 0, 1, 2
+MLP_FP32_SIMT, MLP_BF16X3_TC, MLP_ZERO, MLP_FP16_TC = 0, 1, 2, 3
 SAMPLE_PERMUTE, SAMPLE_REPLACE = 0, 1  # hr_sample_train_rows modes
 RESIZE_METHODS = {"pil_lanczos": 0, "pil_bicubic": 1, "pil_box": 2, "cv2_linear": 3, "cv2_area": 4}  # HR_RESIZE_*
 RESIZE_BGR = 1

@@ -45,11 +45,13 @@ def _dataset_facts(system) -> dict:
 
 def resolve_mlp_mode(name: str) -> int:
     """'auto' (default) and 'bf16x3' select the wgmma sample net -- every pipeline the fused path accepts runs on it
-    (hidden width 128 / 256, encoded input <= 64 features); 'fp32' selects the CUDA-core kernel, the parity anchor."""
+    (hidden width 128 / 256, encoded input <= 64 features); 'fp32' selects the CUDA-core kernel, the parity anchor;
+    'fp16' selects the wgmma net at the precision of the reference's interactive viewer (every Linear layer as CUDA autocast
+    computes it: fp16 operands, fp32 accumulation, fp16 results), for rendering."""
     try:
-        return {"auto": L.MLP_BF16X3_TC, "bf16x3": L.MLP_BF16X3_TC, "fp32": L.MLP_FP32_SIMT}[name]
+        return {"auto": L.MLP_BF16X3_TC, "bf16x3": L.MLP_BF16X3_TC, "fp32": L.MLP_FP32_SIMT, "fp16": L.MLP_FP16_TC}[name]
     except KeyError:
-        raise ValueError(f"mlp_mode must be 'auto', 'bf16x3' or 'fp32', got {name!r}") from None
+        raise ValueError(f"mlp_mode must be 'auto', 'bf16x3', 'fp32' or 'fp16', got {name!r}") from None
 
 
 class _RenderHeads(torch.autograd.Function):

@@ -403,7 +403,7 @@ def lower(model_cfg, dataset: dict, cur_iter: int = RENDER_ITER, iters_per_epoch
     if zero_net:
         c.mlp_mode = L.MLP_ZERO
     c.mlp_in, c.mlp_width, c.mlp_layers = mlp_in, W, depth
-    if c.mlp_mode == L.MLP_BF16X3_TC and tc_passes(W, depth, shapes[-1][0]) > L.HR_TC_MAX_PASSES:
+    if c.mlp_mode in (L.MLP_BF16X3_TC, L.MLP_FP16_TC) and tc_passes(W, depth, shapes[-1][0]) > L.HR_TC_MAX_PASSES:
         raise UnsupportedPipeline(f"tensor-core sample net of {tc_passes(W, depth, shapes[-1][0])} passes of {W} output columns "
                                   f"(more than HR_TC_MAX_PASSES = {L.HR_TC_MAX_PASSES}): use mlp_mode 'fp32'")
 

@@ -25,13 +25,13 @@
 extern "C" {
 #endif
 
-#define HR_ABI_VERSION 25
+#define HR_ABI_VERSION 26
 
 #define HR_MAX_GROUPS 4   /* ray-parameterisation groups feeding the sample net (ray.py:235-263) */
 #define HR_MAX_LAYERS 10  /* Linear layers of the sample net (mlp.py:127-154) */
 #define HR_MAX_SAMPLES 256 /* z_channels S (per-ray sample primitives) */
 #define HR_MAX_PEERS 8    /* destination buffers of hr_render_scatter (GPUs of one NVSwitch domain) */
-/* Passes of an HR_MLP_BF16X3_TC sample net: (mlp_layers - 1) hidden layers + ceil(last layer's outputs / mlp_width).  The
+/* Passes of an HR_MLP_BF16X3_TC or HR_MLP_FP16_TC sample net: (mlp_layers - 1) hidden layers + ceil(last layer's outputs / mlp_width).  The
  * table is a kernel parameter; 40 passes hold every shape at width 256 and, at width 128, depth 10 with S * head_stride up
  * to 3968 (S = 256 x 15 channels).  hr_create refuses a tensor-core net that needs more (the fp32 net has no such limit). */
 #define HR_TC_MAX_PASSES 40
@@ -78,9 +78,14 @@ enum { HR_DENSE_RELU = 0, HR_DENSE_SOFTPLUS = 1, HR_DENSE_RELU_ABS = 2 };
 
 /* Sample-net arithmetic.  FP32_SIMT: fp32 FMA on CUDA cores (bit-level closest to the reference's
  * cuBLAS SGEMM).  BF16X3_TC: wgmma tensor cores, every fp32 operand split into bf16 hi+lo and the
- * three leading cross products accumulated in fp32 registers (error ~2^-16 per product, see DESIGN.md). */
+ * three leading cross products accumulated in fp32 registers (error ~2^-16 per product, see DESIGN.md).
+ * FP16_TC: the reference's mixed precision (its interactive viewer runs the net under CUDA autocast): every Linear layer
+ * with fp16 operands and bias, one wgmma product per k-step accumulated in fp32, each layer's result rounded to fp16 and
+ * LeakyReLU applied to it in fp16; the last layer's fp16 outputs are stored as fp32 heads and everything after the net is
+ * the fp32 pipeline.  Rendering only: the training net (hr_train_net_*) is bf16x3. */
 enum { HR_MLP_FP32_SIMT = 0, HR_MLP_BF16X3_TC = 1,
-       HR_MLP_ZERO = 2 /* `net: {type: zero}` (ZeroMLP, nlf/nets/mlp.py:14-33): every head is 0, no network runs */ };
+       HR_MLP_ZERO = 2, /* `net: {type: zero}` (ZeroMLP, nlf/nets/mlp.py:14-33): every head is 0, no network runs */
+       HR_MLP_FP16_TC = 3 };
 
 /* The recognised pipeline signature (SURVEY.md section 8(a)); one struct describes what the
  * reference assembles from conf/experiment/model/<name>.yaml.  Anything the YAML asks for that this
