@@ -101,19 +101,22 @@ struct ExtraOut {
   VisMap field_u8[HR_N_FIELDS];  // field_u8[f].out: the reduced field f (HR_FIELD_OVER / PRED_WEIGHTS) as a uint8 map instead
 };
 
-__device__ __forceinline__ float apply_act(const hr_act& a, float x) {
+// `kind` is a.kind, or the same value known at compile time (a render kernel's fixed head layout, hr_render_kernel.cuh)
+__device__ __forceinline__ float apply_act_kind(int kind, const hr_act& a, float x) {
   // y = f(x*inner + shift) * outer, each op rounded separately like the eager reference.
   float v = __fadd_rn(__fmul_rn(x, a.inner_fac), a.shift);
   // ex2-based forms: relative error ~2e-6, far below the 1e-4 RGB gate and cheaper than expf / tanhf by ~4x
-  if (a.kind == HR_ACT_SIGMOID) {
+  if (kind == HR_ACT_SIGMOID) {
     v = __fdividef(1.0f, 1.0f + __expf(-v));
-  } else if (a.kind == HR_ACT_TANH) {
+  } else if (kind == HR_ACT_TANH) {
     const float av = fminf(fabsf(v), 15.0f);
     const float t = 1.0f - __fdividef(2.0f, 1.0f + __expf(2.0f * av));
     v = copysignf(t, v);
   }
   return __fmul_rn(v, a.outer_fac);
 }
+
+__device__ __forceinline__ float apply_act(const hr_act& a, float x) { return apply_act_kind(a.kind, a, x); }
 
 // apply_act of a density head (act_sigma, act_point_sigma, pre_act_sigma: the only members hr_config may ease), with
 // EaseValue.ease_out (activations.py:482-489): w * out + (1 - w) * start_value while the window is open.  `eased` is uniform

@@ -124,11 +124,16 @@ __device__ __forceinline__ SampleAlpha sample_alpha(const float (&dist)[SPL], in
 }
 
 // feature2density (tensorf_dynamic.py:373-392; static tensorf_no_sample.py:82-88,187: weights == 1)
-__device__ __forceinline__ float feature2density(const hr_config& cfg, float feat) {
-  if (cfg.fea2dense == HR_DENSE_RELU) return fmaxf(feat, 0.0f);
-  if (cfg.fea2dense == HR_DENSE_RELU_ABS) return fabsf(feat);
+// `kind` is cfg.fea2dense, or the same value known at compile time
+__device__ __forceinline__ float feature2density_kind(int kind, const hr_config& cfg, float feat) {
+  if (kind == HR_DENSE_RELU) return fmaxf(feat, 0.0f);
+  if (kind == HR_DENSE_RELU_ABS) return fabsf(feat);
   const float xs = feat + cfg.density_shift;
   return (xs > 20.0f) ? xs : log1pf(expf(xs));
+}
+
+__device__ __forceinline__ float feature2density(const hr_config& cfg, float feat) {
+  return feature2density_kind(cfg.fea2dense, cfg, feat);
 }
 
 // Keyframe snap of a ray's time (utils/flow_utils.py:18-31): the keyframe's time base_t, the ray's offset toff from it, and

@@ -38,3 +38,18 @@ cudaError_t launch_render(const hr_config& cfg, const Derived& dv, const RenderT
 }
 
 }  // namespace hr
+
+#ifdef HR_RENDER_PHASE_CLOCKS
+// Measurement build only: copies the phase cycle sums of the render kernels of this file (and the warp-ray count) to
+// out[0 .. 4] (when `out` is not null), then clears them when `reset`.  Returns 0, or 1 on a CUDA error.
+extern "C" int hr_render_phase_clocks(unsigned long long* out, int reset) {
+  constexpr size_t bytes = (hr::kRenderPhases + 1) * sizeof(unsigned long long);
+  if (cudaDeviceSynchronize() != cudaSuccess) return 1;
+  if (out && cudaMemcpyFromSymbol(out, hr::g_render_phase_clocks, bytes) != cudaSuccess) return 1;
+  if (reset) {
+    const unsigned long long zero[hr::kRenderPhases + 1] = {};
+    if (cudaMemcpyToSymbol(hr::g_render_phase_clocks, zero, bytes) != cudaSuccess) return 1;
+  }
+  return 0;
+}
+#endif

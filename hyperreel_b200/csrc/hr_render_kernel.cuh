@@ -15,6 +15,8 @@
 // lane = sample mapping, and the 32 sample slots of the warp feed the four gather rounds exactly like one 32-sample ray, so
 // no lane idles in either mapping (one ray per warp left half of every warp idle at S = 16, the DoNeRF BASELINE config).
 #pragma once
+#include <type_traits>
+
 #include "hr_common.cuh"
 #include "hr_geom.cuh"
 
@@ -160,12 +162,121 @@ __device__ __forceinline__ float quad_transpose_reduce(const float (&v)[4], int 
   return (alt ? k1 : k0) + z;                // q = 0: v0, 1: v1, 2: v2, 3: v3
 }
 
-template <int SPL, bool DYN, int C0, int C1, int C2, int SHADE, bool EXTRA, int RPW, bool RARE, bool EASE>
-__global__ void __launch_bounds__(kWarpsPerCta * 32, SPL > 2 ? 1 : ((C1 + C2 == 0 || SPL == 1) ? 3 : 2))
-render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Derived dv,
-              const __grid_constant__ RenderTabs tabs, const float* __restrict__ rays,
-              const float* __restrict__ heads, const __grid_constant__ RgbDst dst, long long n_rays, ExtraOut so,
-              unsigned char* __restrict__ rgb8_out) {
+// The head layout of a launch: which heads the sample net writes, the primitive they place, which density scales the point
+// offset and the activation kind of every head.  These are the same for every ray of a launch.  HeadsAny reads them from the
+// config where they are used, for every configuration.  The fixed layouts state them at compile time for the shipped
+// dynamic z-plane configs (technicolor_z_plane, neural_3d_z_plane) and sphere configs (donerf_sphere), so those kernels test
+// none of them per sample; `matches` is the host's check that a config has the layout.  The values the arithmetic uses
+// (head offsets, activation factors, scales, bounds) are read from the config by every layout.
+struct HeadsAny {
+  __device__ static int n_z(const hr_config& c) { return c.n_z; }
+  __device__ static bool flow(const hr_config& c) { return c.use_flow; }
+  __device__ static bool sigma(const hr_config& c) { return c.off_sigma >= 0; }
+  __device__ static bool point_sigma(const hr_config& c) { return c.off_point_sigma >= 0; }
+  __device__ static bool offset(const hr_config& c) { return c.use_offset; }
+  __device__ static bool color_scale_shift(const hr_config& c) { return c.use_color_scale_shift; }
+  __device__ static int isect(const hr_config& c) { return c.isect_type; }
+  __device__ static bool isect_use_sigma(const hr_config& c) { return c.isect_use_sigma; }
+  __device__ static bool sort(const hr_config& c) { return c.isect_sort; }
+  __device__ static int fea2dense(const hr_config& c) { return c.fea2dense; }
+  // the density that scales the intersection distance / the point offset: none, sigma or point sigma
+  __device__ static float isect_density(const hr_config& c, float sg, float sgp) {
+    return (c.isect_density_off < 0) ? 0.0f : ((c.isect_density_off == c.off_sigma) ? sg : sgp);
+  }
+  __device__ static float offset_density(const hr_config& c, float sg, float sgp) {
+    return (c.offset_density_off < 0) ? 0.0f : ((c.offset_density_off == c.off_sigma) ? sg : sgp);
+  }
+  // activation kinds (hr_act::kind)
+  __device__ static int k_z(const hr_config& c) { return c.act_z.kind; }
+  __device__ static int k_isect(const hr_config& c) { return c.isect_act.kind; }
+  __device__ static int k_flow(const hr_config& c) { return c.act_flow.kind; }
+  __device__ static int k_flow_act(const hr_config& c) { return c.flow_act.kind; }
+  __device__ static int k_sigma(const hr_config& c) { return c.act_sigma.kind; }
+  __device__ static int k_point_sigma(const hr_config& c) { return c.act_point_sigma.kind; }
+  __device__ static int k_offset(const hr_config& c) { return c.act_offset.kind; }
+  __device__ static int k_offset_act(const hr_config& c) { return c.offset_act.kind; }
+  __device__ static int k_cscale(const hr_config& c) { return c.act_cscale.kind; }
+  __device__ static int k_cshift(const hr_config& c) { return c.act_cshift.kind; }
+};
+
+// What the shipped configs share: sigma and point-sigma heads (sigmoid), a tanh point offset, identity z / flow / colour
+// scale-shift heads, the intersection scaled by 1 - sigma and sorted, ReLU feature-to-density.
+struct HeadsShipped {
+  __device__ static bool sigma(const hr_config&) { return true; }
+  __device__ static bool point_sigma(const hr_config&) { return true; }
+  __device__ static bool offset(const hr_config&) { return true; }
+  __device__ static bool color_scale_shift(const hr_config&) { return true; }
+  __device__ static bool isect_use_sigma(const hr_config&) { return true; }
+  __device__ static bool sort(const hr_config&) { return true; }
+  __device__ static int fea2dense(const hr_config&) { return HR_DENSE_RELU; }
+  __device__ static float isect_density(const hr_config&, float sg, float) { return sg; }
+  __device__ static int k_z(const hr_config&) { return HR_ACT_IDENTITY; }
+  __device__ static int k_isect(const hr_config&) { return HR_ACT_IDENTITY; }
+  __device__ static int k_flow(const hr_config&) { return HR_ACT_IDENTITY; }
+  __device__ static int k_flow_act(const hr_config&) { return HR_ACT_IDENTITY; }
+  __device__ static int k_sigma(const hr_config&) { return HR_ACT_SIGMOID; }
+  __device__ static int k_point_sigma(const hr_config&) { return HR_ACT_SIGMOID; }
+  __device__ static int k_offset(const hr_config&) { return HR_ACT_TANH; }
+  __device__ static int k_offset_act(const hr_config&) { return HR_ACT_IDENTITY; }
+  __device__ static int k_cscale(const hr_config&) { return HR_ACT_IDENTITY; }
+  __device__ static int k_cshift(const hr_config&) { return HR_ACT_IDENTITY; }
+  static bool matches(const hr_config& c) {
+    return c.off_sigma >= 0 && c.off_point_sigma >= 0 && c.off_point_sigma != c.off_sigma && c.use_offset &&
+           c.use_color_scale_shift && c.isect_use_sigma && c.isect_density_off == c.off_sigma && c.isect_sort &&
+           c.fea2dense == HR_DENSE_RELU && !eases_density(c) && c.act_z.kind == HR_ACT_IDENTITY &&
+           c.isect_act.kind == HR_ACT_IDENTITY && c.act_flow.kind == HR_ACT_IDENTITY && c.flow_act.kind == HR_ACT_IDENTITY &&
+           c.act_sigma.kind == HR_ACT_SIGMOID && c.act_point_sigma.kind == HR_ACT_SIGMOID && c.act_offset.kind == HR_ACT_TANH &&
+           c.offset_act.kind == HR_ACT_IDENTITY && c.act_cscale.kind == HR_ACT_IDENTITY && c.act_cshift.kind == HR_ACT_IDENTITY;
+  }
+};
+
+// dynamic z-plane: one z head, a flow head, the offset scaled by 1 - point sigma
+struct HeadsZPlane : HeadsShipped {
+  __device__ static int n_z(const hr_config&) { return 1; }
+  __device__ static bool flow(const hr_config&) { return true; }
+  __device__ static int isect(const hr_config&) { return HR_ISECT_Z_PLANE; }
+  __device__ static float offset_density(const hr_config&, float, float sgp) { return sgp; }
+  static bool matches(const hr_config& c) {
+    return HeadsShipped::matches(c) && c.n_z == 1 && c.use_flow && c.isect_type == HR_ISECT_Z_PLANE &&
+           c.offset_density_off == c.off_point_sigma;
+  }
+};
+
+// sphere: four z heads (centre scale and radius), no flow, the offset scaled by 1 - sigma
+struct HeadsSphere : HeadsShipped {
+  __device__ static int n_z(const hr_config&) { return 4; }
+  __device__ static bool flow(const hr_config&) { return false; }
+  __device__ static int isect(const hr_config&) { return HR_ISECT_SPHERE; }
+  __device__ static float offset_density(const hr_config&, float sg, float) { return sg; }
+  static bool matches(const hr_config& c) {
+    return HeadsShipped::matches(c) && c.n_z == 4 && !c.use_flow && c.isect_type == HR_ISECT_SPHERE &&
+           c.offset_density_off == c.off_sigma;
+  }
+};
+
+#ifdef HR_RENDER_PHASE_CLOCKS
+// Measurement build only (-DHR_RENDER_PHASE_CLOCKS, scripts/render_split_bench.py): clock64() cycles every warp spends in
+// each phase of its rays, summed over the launches since the last read (hr_render_phase_clocks, hr_render.cu), and the
+// number of warp-rays.  Phases: 0 heads load, 1 keyframe / view matrix / intersect / sort / points / texel coordinates,
+// 2 gather rounds, 3 alpha / transmittance / composite / store.  A load's latency is charged to the phase that first uses it.
+static constexpr int kRenderPhases = 4;
+static __device__ unsigned long long g_render_phase_clocks[kRenderPhases + 1];
+#define HR_PHASE_MARK(p)                              \
+  {                                                   \
+    const long long t_ = clock64();                   \
+    phase_clk[p] += (unsigned long long)(t_ - t_mark); \
+    t_mark = t_;                                      \
+  }
+#else
+#define HR_PHASE_MARK(p)
+#endif
+
+template <int SPL, bool DYN, int C0, int C1, int C2, int SHADE, bool EXTRA, int RPW, bool RARE, bool EASE, class HL>
+__device__ __forceinline__ void render_body(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs,
+                                            const float* __restrict__ rays, const float* __restrict__ heads,
+                                            const RgbDst& dst, long long n_rays, ExtraOut so,
+                                            unsigned char* __restrict__ rgb8_out) {
+  static_assert(std::is_same<HL, HeadsAny>::value || (!EXTRA && !RARE && !EASE), "fixed head layouts: plain lean kernels");
   constexpr int NT = C0 + C1 + C2;
   constexpr int ROWS = (SHADE == HR_SHADE_SH) ? 9 : 1;
   constexpr int ROUNDS = 4 * SPL;
@@ -227,7 +338,15 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
   const float inv_z = __fdiv_rn(2.0f, __fsub_rn(cfg.aabb[5], cfg.aabb[2]));
   const int line_bytes = out_stride * 4;
 
+#ifdef HR_RENDER_PHASE_CLOCKS
+  unsigned long long phase_clk[kRenderPhases] = {}, warp_rays = 0;
+  long long t_mark = 0;
+#endif
   for (long long base = warp0 * RPW; base < n_rays; base += nwarps * RPW) {
+#ifdef HR_RENDER_PHASE_CLOCKS
+    t_mark = clock64();
+    ++warp_rays;
+#endif
     // this lane's ray; the second ray of the last warp may not exist: it is computed on a copy of the last ray (every lane
     // takes part in the shuffles) and never stored
     const bool ray_ok = base + sub < n_rays;
@@ -254,19 +373,20 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
       const int s = sl + 32 * j;
       const float* hp = hrow + ((s < S) ? s : 0);
 #pragma unroll
-      for (int c = 0; c < 4; ++c) hz[j][c] = (c < cfg.n_z) ? __ldg(hp + (cfg.off_z + c) * S) : 0.0f;
+      for (int c = 0; c < 4; ++c) hz[j][c] = (c < HL::n_z(cfg)) ? __ldg(hp + (cfg.off_z + c) * S) : 0.0f;
 #pragma unroll
-      for (int c = 0; c < 3; ++c) hfl[j][c] = cfg.use_flow ? __ldg(hp + (cfg.off_flow + c) * S) : 0.0f;
-      hsg[j] = (cfg.off_sigma >= 0) ? __ldg(hp + cfg.off_sigma * S) : 0.0f;
-      hsp[j] = (cfg.off_point_sigma >= 0) ? __ldg(hp + cfg.off_point_sigma * S) : 0.0f;
+      for (int c = 0; c < 3; ++c) hfl[j][c] = HL::flow(cfg) ? __ldg(hp + (cfg.off_flow + c) * S) : 0.0f;
+      hsg[j] = HL::sigma(cfg) ? __ldg(hp + cfg.off_sigma * S) : 0.0f;
+      hsp[j] = HL::point_sigma(cfg) ? __ldg(hp + cfg.off_point_sigma * S) : 0.0f;
 #pragma unroll
-      for (int c = 0; c < 3; ++c) hof[j][c] = cfg.use_offset ? __ldg(hp + (cfg.off_offset + c) * S) : 0.0f;
+      for (int c = 0; c < 3; ++c) hof[j][c] = HL::offset(cfg) ? __ldg(hp + (cfg.off_offset + c) * S) : 0.0f;
     }
+    HR_PHASE_MARK(0);
 
     // ---- per-ray keyframe snap, time offset and keyframe row ----
     float toff = 0.0f, base_t = 0.0f;
     int krow = 0;
-    if (DYN || cfg.use_flow) {
+    if (DYN || HL::flow(cfg)) {
       const Keyframe kf = keyframe_snap(dv, time);
       base_t = kf.base_t;
       toff = kf.toff;
@@ -328,19 +448,24 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
     for (int j = 0; j < SPL; ++j) {
       const int s = sl + 32 * j;
       const bool act = s < S;
-      const float sg = (cfg.off_sigma >= 0) ? apply_act_head<EASE>(cfg.act_sigma, hsg[j]) : 0.0f;
-      const float sgp = (cfg.off_point_sigma >= 0) ? apply_act_head<EASE>(cfg.act_point_sigma, hsp[j]) : 0.0f;
-      const float dens_i = (cfg.isect_density_off < 0) ? 0.0f : ((cfg.isect_density_off == cfg.off_sigma) ? sg : sgp);
-      const float dens_o = (cfg.offset_density_off < 0) ? 0.0f : ((cfg.offset_density_off == cfg.off_sigma) ? sg : sgp);
-      const float one_m = __fsub_rn(1.0f, cfg.isect_use_sigma ? dens_i : 0.0f);
+      const float sg = HL::sigma(cfg) ? (EASE ? apply_act_head<EASE>(cfg.act_sigma, hsg[j])
+                                              : apply_act_kind(HL::k_sigma(cfg), cfg.act_sigma, hsg[j]))
+                                      : 0.0f;
+      const float sgp = HL::point_sigma(cfg) ? (EASE ? apply_act_head<EASE>(cfg.act_point_sigma, hsp[j])
+                                                     : apply_act_kind(HL::k_point_sigma(cfg), cfg.act_point_sigma, hsp[j]))
+                                             : 0.0f;
+      const float dens_i = HL::isect_density(cfg, sg, sgp);
+      const float dens_o = HL::offset_density(cfg, sg, sgp);
+      const float one_m = __fsub_rn(1.0f, HL::isect_use_sigma(cfg) ? dens_i : 0.0f);
       const float samp = cfg.samples[act ? s : 0];
       float t;
-      if (cfg.isect_type == HR_ISECT_Z_PLANE) {
-        float zr = __fmul_rn(apply_act(cfg.isect_act, apply_act(cfg.act_z, hz[j][0])), one_m);
+      if (HL::isect(cfg) == HR_ISECT_Z_PLANE) {
+        float zr = __fmul_rn(apply_act_kind(HL::k_isect(cfg), cfg.isect_act, apply_act_kind(HL::k_z(cfg), cfg.act_z, hz[j][0])),
+                             one_m);
         float z = __fadd_rn(__fmul_rn(zr, cfg.z_scale), samp);
         if (cfg.contract_samples) z = inv_contract_sample(cfg, dv, z);
         t = intersect_axis_plane(z, oz, dz);
-      } else if (RARE && cfg.isect_type != HR_ISECT_SPHERE && cfg.isect_type != HR_ISECT_CYLINDER) {
+      } else if (RARE && HL::isect(cfg) != HR_ISECT_SPHERE && HL::isect(cfg) != HR_ISECT_CYLINDER) {
         // the less common primitives (sphere_new, euclidean_distance, voxel grids) live in one out-of-line function and are
         // compiled into the RARE variants only: the z-plane / sphere / cylinder kernels keep their instruction stream and
         // register budget (80 registers at three CTAs per SM)
@@ -348,7 +473,9 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
       } else {
         float zc[4];
 #pragma unroll
-        for (int c = 0; c < 4; ++c) zc[c] = __fmul_rn(apply_act(cfg.isect_act, apply_act(cfg.act_z, hz[j][c])), one_m);
+        for (int c = 0; c < 4; ++c)
+          zc[c] = __fmul_rn(apply_act_kind(HL::k_isect(cfg), cfg.isect_act, apply_act_kind(HL::k_z(cfg), cfg.act_z, hz[j][c])),
+                            one_m);
         // primitive.py:410-418
         float gx = __fadd_rn(__fmul_rn(zc[0], cfg.sphere_origin_scale), cfg.sphere_origin_initial[0]);
         float gy = __fadd_rn(__fmul_rn(zc[1], cfg.sphere_origin_scale), cfg.sphere_origin_initial[1]);
@@ -358,7 +485,7 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
         // primitive.py:420-438; IntersectCylinderOld (primitive.py:181-250) for the cylinder
         float sox = __fmul_rn(ox, gx), soy = __fmul_rn(oy, gy), soz = __fmul_rn(oz, gz);
         float sdx = __fmul_rn(dx, gx), sdy = __fmul_rn(dy, gy), sdz = __fmul_rn(dz, gz);
-        t = intersect_quadric(sox, soy, soz, sdx, sdy, sdz, rad, cfg.isect_type == HR_ISECT_CYLINDER).t;
+        t = intersect_quadric(sox, soy, soz, sdx, sdy, sdz, rad, HL::isect(cfg) == HR_ISECT_CYLINDER).t;
       }
       if ((t <= cfg.isect_near) || (t >= cfg.isect_far)) t = 0.0f;
       tkey[j] = act ? t : __int_as_float(0x7f800000);
@@ -366,15 +493,19 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
       // offset * (1 - sigma) (point.py:383-391) -- kept as two addends to preserve the reference's rounding order
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
-        disp[j][c] = cfg.use_flow ? __fmul_rn(apply_act(cfg.flow_act, apply_act(cfg.act_flow, hfl[j][c])), toff) : 0.0f;
-        hof[j][c] = cfg.use_offset
-                        ? __fmul_rn(apply_act(cfg.offset_act, apply_act(cfg.act_offset, hof[j][c])), __fsub_rn(1.0f, dens_o))
-                        : 0.0f;
+        disp[j][c] = HL::flow(cfg) ? __fmul_rn(apply_act_kind(HL::k_flow_act(cfg), cfg.flow_act,
+                                                              apply_act_kind(HL::k_flow(cfg), cfg.act_flow, hfl[j][c])),
+                                               toff)
+                                   : 0.0f;
+        hof[j][c] = HL::offset(cfg) ? __fmul_rn(apply_act_kind(HL::k_offset_act(cfg), cfg.offset_act,
+                                                               apply_act_kind(HL::k_offset(cfg), cfg.act_offset, hof[j][c])),
+                                                __fsub_rn(1.0f, dens_o))
+                                    : 0.0f;
       }
     }
 
     // ---- sort distances only (base.py:206-210) ----
-    if (cfg.isect_sort) {
+    if (HL::sort(cfg)) {
       if (keys_unsorted<SPL>(tkey, sl)) {
         if constexpr (RPW == 1) sort_keys<SPL>(tkey, lane);
         else sort_keys_sub<LW>(tkey[0], sl);
@@ -440,6 +571,7 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
       }
     }
 
+    HR_PHASE_MARK(1);
     // ---- VM gather: 8 samples per round, 4 lanes per sample (matMode [[0,1],[0,2],[1,2]], vecMode [2,1,0]) ----
     float sig_r[ROUNDS];  // density feature of (round, quad): FOLD: in lane q = 3 of the quad, else replicated
     float rgb_r[ROUNDS];  // shaded colour channel q of (round, quad)
@@ -541,6 +673,7 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
       rgb_r[rd] = ok ? col : 0.0f;
     }
 
+    HR_PHASE_MARK(2);
     // ---- back to lane = sample: sigma, alpha, transmittance, weights (tensorf_utils.py:242-253) ----
     float wgt[SPL];
     float carryT = 1.0f;
@@ -553,7 +686,7 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
       const int s = sl + 32 * j;
       const float* hp = hrow + ((s < S) ? s : 0);
       float cs_raw[3] = {0.f, 0.f, 0.f}, csh_raw[3] = {0.f, 0.f, 0.f};
-      if (cfg.use_color_scale_shift) {
+      if (HL::color_scale_shift(cfg)) {
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
           cs_raw[c] = __ldg(hp + (cfg.off_cscale + c) * S);
@@ -566,7 +699,7 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
         float v = __shfl_sync(kFull, sig_r[4 * j + rr], 4 * (lane & 7) + (FOLD ? 3 : 0));
         if ((lane >> 3) == rr) feat = v;
       }
-      float sigma = feature2density(cfg, feat);
+      float sigma = feature2density_kind(HL::fea2dense(cfg), cfg, feat);
       if (!valid[j]) sigma = 0.0f;
       const SampleAlpha sa = sample_alpha<SPL>(dist, j, sigma, cfg.distance_scale, sl, S);
       const float w = sa.alpha * transmittance<LW>(sa.a1, sl, carryT);
@@ -579,8 +712,8 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
       const float m = (w > cfg.weight_thre) ? w : 0.0f;  // app_mask (tensorf_dynamic.py:750)
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
-        const float csv = cfg.use_color_scale_shift ? apply_act(cfg.act_cscale, cs_raw[c]) : 0.0f;
-        const float cshv = cfg.use_color_scale_shift ? apply_act(cfg.act_cshift, csh_raw[c]) : 0.0f;
+        const float csv = HL::color_scale_shift(cfg) ? apply_act_kind(HL::k_cscale(cfg), cfg.act_cscale, cs_raw[c]) : 0.0f;
+        const float cshv = HL::color_scale_shift(cfg) ? apply_act_kind(HL::k_cshift(cfg), cfg.act_cshift, csh_raw[c]) : 0.0f;
         csA[j][c] = (s < S) ? m * (csv + 1.0f) : 0.0f;
         accB[c] += (s < S) ? w * cshv : 0.0f;
       }
@@ -732,8 +865,50 @@ render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Der
       const int d = sl / 3;
       if (d < dst.n && ray_ok) dst.p[d][(dst.row0 + ray) * 3 + (sl % 3)] = vv;
     }
+    HR_PHASE_MARK(3);
   }
+#ifdef HR_RENDER_PHASE_CLOCKS
+  if (lane == 0) {
+#pragma unroll
+    for (int p = 0; p < kRenderPhases; ++p) atomicAdd(&g_render_phase_clocks[p], phase_clk[p]);
+    atomicAdd(&g_render_phase_clocks[kRenderPhases], warp_rays);
+  }
+#endif
 }
+
+// Occupancy target of a render kernel: 3 CTAs per SM for one sample per lane or one VM group, 2 for several groups at two
+// samples per lane, 1 above.
+template <int SPL, int C1, int C2>
+constexpr int render_min_ctas() {
+  return SPL > 2 ? 1 : ((C1 + C2 == 0 || SPL == 1) ? 3 : 2);
+}
+
+// Every configuration: the head layout is read from the config.
+template <int SPL, bool DYN, int C0, int C1, int C2, int SHADE, bool EXTRA, int RPW, bool RARE, bool EASE>
+__global__ void __launch_bounds__(kWarpsPerCta * 32, render_min_ctas<SPL, C1, C2>())
+render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Derived dv,
+              const __grid_constant__ RenderTabs tabs, const float* __restrict__ rays,
+              const float* __restrict__ heads, const __grid_constant__ RgbDst dst, long long n_rays, ExtraOut so,
+              unsigned char* __restrict__ rgb8_out) {
+  render_body<SPL, DYN, C0, C1, C2, SHADE, EXTRA, RPW, RARE, EASE, HeadsAny>(cfg, dv, tabs, rays, heads, dst, n_rays, so,
+                                                                             rgb8_out);
+}
+
+// A fixed head layout (the last parameter's type): the same cell of the template family, the layout's fields compiled in.
+// The layout is not a template argument, so the kernel's template arguments still name the cell.
+#define HR_RENDER_KERNEL_FIXED(Layout)                                                                                      \
+  template <int SPL, bool DYN, int C0, int C1, int C2, int SHADE, bool EXTRA, int RPW, bool RARE, bool EASE>                \
+  __global__ void __launch_bounds__(kWarpsPerCta * 32, render_min_ctas<SPL, C1, C2>())                                    \
+  render_kernel(const __grid_constant__ hr_config cfg, const __grid_constant__ Derived dv,                                 \
+                const __grid_constant__ RenderTabs tabs, const float* __restrict__ rays, const float* __restrict__ heads, \
+                const __grid_constant__ RgbDst dst, long long n_rays, ExtraOut so, unsigned char* __restrict__ rgb8_out,   \
+                Layout) {                                                                                                 \
+    render_body<SPL, DYN, C0, C1, C2, SHADE, EXTRA, RPW, RARE, EASE, Layout>(cfg, dv, tabs, rays, heads, dst, n_rays, so,  \
+                                                                             rgb8_out);                                  \
+  }
+HR_RENDER_KERNEL_FIXED(HeadsZPlane)
+HR_RENDER_KERNEL_FIXED(HeadsSphere)
+#undef HR_RENDER_KERNEL_FIXED
 
 template <int SPL, bool DYN, int C0, int C1, int C2, int SHADE, bool RARE, bool EASE>
 static cudaError_t launch_one(const hr_config& cfg, const Derived& dv, const RenderTabs& tabs, const float* rays,
@@ -754,14 +929,35 @@ static cudaError_t launch_one(const hr_config& cfg, const Derived& dv, const Ren
     return cudaGetLastError();
   }
   ExtraOut none{};
-  if constexpr (SPL == 1) {
-    if (two_rays) {
-      render_kernel<SPL, DYN, C0, C1, C2, SHADE, false, 2, RARE, EASE><<<g, b, smem, stream>>>(cfg, dv, tabs, rays, heads, rgb, n, none, rgb8);
-      return cudaGetLastError();
+  auto plain = [&](auto layout) -> cudaError_t {
+    using HL = decltype(layout);
+    if constexpr (std::is_same<HL, HeadsAny>::value) {
+      if constexpr (SPL == 1) {
+        if (two_rays) {
+          render_kernel<SPL, DYN, C0, C1, C2, SHADE, false, 2, RARE, EASE><<<g, b, smem, stream>>>(cfg, dv, tabs, rays, heads, rgb, n, none, rgb8);
+          return cudaGetLastError();
+        }
+      }
+      render_kernel<SPL, DYN, C0, C1, C2, SHADE, false, 1, RARE, EASE><<<g, b, smem, stream>>>(cfg, dv, tabs, rays, heads, rgb, n, none, rgb8);
+    } else {
+      if constexpr (SPL == 1) {
+        if (two_rays) {
+          render_kernel<SPL, DYN, C0, C1, C2, SHADE, false, 2, RARE, EASE><<<g, b, smem, stream>>>(cfg, dv, tabs, rays, heads, rgb, n, none, rgb8, layout);
+          return cudaGetLastError();
+        }
+      }
+      render_kernel<SPL, DYN, C0, C1, C2, SHADE, false, 1, RARE, EASE><<<g, b, smem, stream>>>(cfg, dv, tabs, rays, heads, rgb, n, none, rgb8, layout);
     }
+    return cudaGetLastError();
+  };
+  // the fixed head layouts of the shipped configs, at the (dynamic, shading) pairs those configs use
+  if constexpr (!RARE && !EASE && DYN && SHADE == HR_SHADE_SH) {
+    if (HeadsZPlane::matches(cfg)) return plain(HeadsZPlane{});
   }
-  render_kernel<SPL, DYN, C0, C1, C2, SHADE, false, 1, RARE, EASE><<<g, b, smem, stream>>>(cfg, dv, tabs, rays, heads, rgb, n, none, rgb8);
-  return cudaGetLastError();
+  if constexpr (!RARE && !EASE && !DYN && SHADE == HR_SHADE_RGB) {
+    if (HeadsSphere::matches(cfg)) return plain(HeadsSphere{});
+  }
+  return plain(HeadsAny{});
 }
 
 template <int SPL, bool DYN, int C0, int C1, int C2, bool RARE, bool EASE>
