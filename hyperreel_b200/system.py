@@ -10,7 +10,8 @@ up-sampling / occupancy-pruning schedule with its optimiser reset (tensorf_base.
 ``schedule="reference"``, the optimisers' own schedule: one learning-rate scheduler per group stepped by
 ``training_epoch_end`` (utils/__init__.py:78-125, nlf/__init__.py:711-725) and the per-group ``reset_opt_list`` restarts
 (nlf/__init__.py:529-578).  Of the visualisers, the embedding maps are rendered on the device
-(``validation_video_outputs`` / ``validation_image_embeddings``); datasets are out of scope (SURVEY.md section 2).
+(``validation_video_outputs`` / ``validation_image_embeddings``).  Of the datasets, the views and facts of a scene
+directory come from ``dataset_cameras`` (datasets.py, ``from_dataset``); decoding their frames stays with the caller.
 """
 from __future__ import annotations
 
@@ -145,6 +146,15 @@ class INRSystem(nn.Module):
             else:
                 raise NotImplementedError(f"regularizer '{rcfg.get('type')}' is outside the fused path's scope")
         self.eval()
+
+    @classmethod
+    def from_dataset(cls, cfg, root: str, **kwargs) -> "INRSystem":
+        """The system of ``cfg`` with the model built from the facts of the scene directory ``root`` (the reference's
+        training dataset's near, far, depth_range, frame counts, ...: ``dataset_cameras(cfg.dataset, root, 'train').facts``);
+        ``kwargs`` as ``INRSystem``."""
+        from .datasets import dataset_cameras
+
+        return cls(cfg, dataset=dataset_cameras(to_cfg(cfg)["dataset"], root, "train").facts, **kwargs)
 
     # ---- nlf/__init__.py:481-502
     def render(self, method_name, coords, **render_kwargs):
@@ -342,7 +352,15 @@ class INRSystem(nn.Module):
 
     def render_video(self, cameras, times=None, out=None, stream=None):
         """The render split's video (validation_video, nlf/__init__.py:809-891) as uint8 [F, H, W, 3] on the device:
-        hyperreel_b200.render_video of this system's model, rendered in eval() (the previous train / eval mode is restored)."""
+        hyperreel_b200.render_video of this system's model, rendered in eval() (the previous train / eval mode is restored).
+        ``cameras`` may be a DatasetViews (``dataset_cameras``' render split): its cameras at their times, each frame cut
+        to its ``crop`` window as the reference renders it."""
+        from .datasets import DatasetViews
+
+        if isinstance(cameras, DatasetViews):
+            crop = cameras.crop
+            video = self.render_video(cameras.cameras, times, out=out, stream=stream)
+            return video if crop is None else video[:, crop[0]:crop[1], crop[2]:crop[3]]
         was_training = self.training
         self.eval()
         try:
@@ -413,7 +431,12 @@ class INRSystem(nn.Module):
         validation_epoch_end takes the list as it is: 'val/psnr' and 'val/ssim' equal validation_image's bit for bit (fed the
         view's rays and images[i] / 255, correctly rounded); 'val/loss' is the fp64 MSE rounded to fp32, which differs from
         validation_image's fp32 mean only in summation order.  ``rgba=True``: ``images`` are uint8 RGBA [n, H, W, 4] and
-        validation_image is fed their composite over white, as the DoNeRF and Catacaustics get_rgb make it."""
+        validation_image is fed their composite over white, as the DoNeRF and Catacaustics get_rgb make it.  ``cameras``
+        may be a DatasetViews (``dataset_cameras``' val or test split), whose ``rgba`` then applies."""
+        from .datasets import DatasetViews
+
+        if isinstance(cameras, DatasetViews):
+            cameras, rgba = cameras.cameras, rgba or cameras.rgba
         mse, ssim = self.score_views(cameras, images, times, rgba=rgba)
         return [{"val/loss": mse[i].float(), "val/psnr": 10.0 * torch.log10(1.0 / mse[i]), "val/ssim": ssim[i]}
                 for i in range(mse.shape[0])]
