@@ -697,10 +697,13 @@ static int ensure_pipe(hr_handle* h, int64_t rays_per_slot) {
   return 0;
 }
 
-// one net (ray net or point net) over `rows` input rows -> out [rows][nc.mlp_out]
-static int launch_net(hr_handle* h, const SampleNet& net, const float* in, int64_t rows, float* out, cudaStream_t st) {
+// one net (ray net or point net) over `rows` input rows -> out [rows][nc.mlp_out].  in_copy (optional, tensor-core net
+// only): `in` may be pinned host memory, and the net leaves a device copy of its rows there.
+static int launch_net(hr_handle* h, const SampleNet& net, const float* in, int64_t rows, float* out, cudaStream_t st,
+                      float* in_copy = nullptr) {
   const hr_config& nc = net.cfg;
   cudaError_t e;
+  if (in_copy && !tc_net(nc.mlp_mode)) return hr_fail("hr_render: only the tensor-core sample net reads host rays");
   if (nc.mlp_mode == HR_MLP_ZERO) {  // ZeroMLP (nlf/nets/mlp.py:29-30): x.new_zeros(N, out_channels)
     e = cudaMemsetAsync(out, 0, (size_t)rows * nc.mlp_out * sizeof(float), st);
     if (e != cudaSuccess) return hr_fail("heads memset failed: %s", cudaGetErrorString(e));
@@ -708,7 +711,7 @@ static int launch_net(hr_handle* h, const SampleNet& net, const float* in, int64
   }
   if (tc_net(nc.mlp_mode)) {
     if (!net.tc_ready) return hr_fail("hr_render: tensor-core pack missing");
-    e = hr::launch_mlp_tc2(nc, net.tc, in, out, rows, h->num_sms, st);
+    e = hr::launch_mlp_tc2(nc, net.tc, in, out, rows, h->num_sms, st, in_copy);
   } else {
     e = hr::launch_mlp_simt(nc, net.simt, in, out, rows, h->num_sms, st);
   }
@@ -730,10 +733,12 @@ static cudaError_t unpermute_heads_async(const hr_config& c, const float* src, f
 }
 
 // rays [n, c_in] -> heads scratch [n, mlp_out] (channel-major per ray).  `scratch` (cascade_layout(c, n).total bytes, only read for a
-// cascaded pipeline) holds the first stage's intermediates.
-static int launch_sample_net(hr_handle* h, const float* rays, int64_t n, float* heads, cudaStream_t st, void* scratch = nullptr) {
+// cascaded pipeline) holds the first stage's intermediates.  rays_copy: as launch_net's in_copy (not for a cascade).
+static int launch_sample_net(hr_handle* h, const float* rays, int64_t n, float* heads, cudaStream_t st, void* scratch = nullptr,
+                             float* rays_copy = nullptr) {
   const hr_config& c = h->cfg;
-  if (!c.cascade) return launch_net(h, h->net, rays, n, heads, st);
+  if (!c.cascade) return launch_net(h, h->net, rays, n, heads, st, rays_copy);
+  if (rays_copy) return hr_fail("hr_render: a cascaded pipeline does not read host rays");
   if (!scratch) return hr_fail("hr_render: cascade scratch missing");
   // PointPredictionEmbedding (nlf/embedding/point.py:142-206): ray net -> S0 z-planes -> one point-net row per point
   const CascadeLayout t = cascade_layout(c, n);
@@ -768,9 +773,11 @@ static hr::RgbDst one_dst(float* rgb) {
 // scales / shifts are 3-vectors
 constexpr int kFieldWidth[HR_N_FIELDS] = {3, 1, 1, 1, 1, 3, 1, 3, 3, 3, 1, 1, 3, 3, 3};
 
+// net_rays (optional): the sample net reads the rays there instead -- a device view of pinned host memory -- and leaves
+// the device copy at `rays`, which the render kernel reads.
 static int render_impl(hr_handle* h, const float* rays, int64_t n, float* rgb, float* mlp_out, const hr::ExtraOut* so,
                        void* workspace, int64_t ws_bytes, cudaStream_t st, unsigned char* rgb8 = nullptr,
-                       const hr::RgbDst* scatter = nullptr) {
+                       const hr::RgbDst* scatter = nullptr, const float* net_rays = nullptr) {
   if (!h) return hr_fail("hr_render: null handle");
   if (!h->uploaded) return hr_fail("hr_render: parameters not uploaded (call hr_upload)");
   if (n == 0) return 0;
@@ -789,7 +796,8 @@ static int render_impl(hr_handle* h, const float* rays, int64_t n, float* rgb, f
       CK(cudaEventCreate(&em.a)); CK(cudaEventCreate(&em.b)); CK(cudaEventCreate(&er.a)); CK(cudaEventCreate(&er.b));
       CK(cudaEventRecord(em.a, st));
     }
-    int rc0 = launch_sample_net(h, r, m, heads, st, (char*)workspace + heads_bytes(h, (n < sub) ? n : sub));
+    int rc0 = launch_sample_net(h, net_rays ? net_rays + off * c.c_in : r, m, heads, st,
+                                (char*)workspace + heads_bytes(h, (n < sub) ? n : sub), net_rays ? const_cast<float*>(r) : nullptr);
     if (rc0) return rc0;
     if (timing) { CK(cudaEventRecord(em.b, st)); CK(cudaEventRecord(er.a, st)); }
     hr::RgbDst d = scatter ? *scatter : one_dst(rgb);
@@ -924,6 +932,53 @@ int hr_generate_rays(const hr_camera* cam, int32_t c_in, int64_t first_pixel, in
   return 0;
 }
 
+// Where the chunks of a host-buffer call take their rays from and put their pixels; one of each is set.
+//   rays: generated from `cam`; read by the sample net from `rays_view`, a device view of pinned host rays, which leaves
+//         the device copy in the slot; or copied in from `rays_host`.
+//   pixels: stored by the render epilogue into `rgb_view`, a device view of pinned host memory; or rendered into the slot
+//           and copied out to `rgb_host` (fp32) or `rgb8_host` (uint8).
+struct HostChunks {
+  const hr_camera* cam = nullptr;
+  const float* rays_view = nullptr;
+  const float* rays_host = nullptr;
+  float* rgb_view = nullptr;
+  float* rgb_host = nullptr;
+  uint8_t* rgb8_host = nullptr;
+};
+
+// n rays in chunks of `chunk` (h->pipe's slots hold that many): chunk i brings its rays in, renders and sends its pixels
+// out on stream and slot i % 3.  Only enqueues; the caller synchronises the streams.
+static int run_host_chunks(hr_handle* h, int64_t n, int64_t chunk, const HostChunks& io) {
+  HostPipe& P = h->pipe;
+  const int c_in = h->cfg.c_in;
+  int slot = 0;
+  for (int64_t off = 0; off < n; off += chunk, slot = (slot + 1) % 3) {
+    const int64_t m = (n - off < chunk) ? (n - off) : chunk;
+    cudaStream_t st = P.streams[slot];
+    if (io.cam) {
+      cudaError_t e = hr::launch_generate_rays(*io.cam, c_in, off, m, P.d_rays[slot], st);
+      if (e != cudaSuccess) return hr_fail("ray generation failed: %s", cudaGetErrorString(e));
+      h->launches += 1;
+    } else if (io.rays_host) {
+      CK(cudaMemcpyAsync(P.d_rays[slot], io.rays_host + off * c_in, (size_t)m * c_in * sizeof(float), cudaMemcpyHostToDevice, st));
+    }
+    float* rgb = io.rgb_view ? io.rgb_view + off * 3 : (io.rgb_host ? P.d_rgb[slot] : nullptr);
+    int rc = render_impl(h, P.d_rays[slot], m, rgb, nullptr, nullptr, P.d_ws[slot], P.ws_bytes, st,
+                         io.rgb8_host ? (unsigned char*)P.d_rgb[slot] : nullptr, nullptr,
+                         io.rays_view ? io.rays_view + off * c_in : nullptr);
+    if (rc) return rc;
+    if (io.rgb_host)
+      CK(cudaMemcpyAsync(io.rgb_host + off * 3, P.d_rgb[slot], (size_t)m * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (io.rgb8_host) CK(cudaMemcpyAsync(io.rgb8_host + off * 3, P.d_rgb[slot], (size_t)m * 3, cudaMemcpyDeviceToHost, st));
+  }
+  return 0;
+}
+
+static int sync_pipe(hr_handle* h) {
+  for (int i = 0; i < 3; ++i) CK(cudaStreamSynchronize(h->pipe.streams[i]));
+  return 0;
+}
+
 int hr_render_frame_to8b_host(hr_handle* h, const hr_camera* cam, uint8_t* rgb8_host, int64_t chunk) {
   if (!h || !cam || !rgb8_host) return hr_fail("hr_render_frame_to8b_host: null argument");
   if (!h->uploaded) return hr_fail("hr_render_frame_to8b_host: parameters not uploaded");
@@ -931,25 +986,16 @@ int hr_render_frame_to8b_host(hr_handle* h, const hr_camera* cam, uint8_t* rgb8_
     return hr_fail("hr_render_frame_to8b_host: fisheye coefficients k1 = %g, k2 = %g are not finite", cam->k1, cam->k2);
   if (const char* why = bad_two_plane(*cam)) return hr_fail("hr_render_frame_to8b_host: %s", why);
   DeviceGuard guard(h->device);
-  const hr_config& c = h->cfg;
   const int64_t n_rays = (int64_t)cam->width * cam->height;
   if (chunk <= 0) chunk = tc_net(h->cfg.mlp_mode) ? (int64_t)h->num_sms * 128 * 14 : 262144;  // whole tile waves
   if (chunk > n_rays) chunk = n_rays;
-  HostPipe& P = h->pipe;
   if (ensure_pipe(h, chunk)) return 1;
-  int slot = 0;
-  for (int64_t off = 0; off < n_rays; off += chunk, slot = (slot + 1) % 3) {
-    const int64_t m = (n_rays - off < chunk) ? (n_rays - off) : chunk;
-    cudaStream_t st = P.streams[slot];
-    cudaError_t e = hr::launch_generate_rays(*cam, c.c_in, off, m, P.d_rays[slot], st);
-    if (e != cudaSuccess) return hr_fail("ray generation failed: %s", cudaGetErrorString(e));
-    h->launches += 1;
-    int rc = render_impl(h, P.d_rays[slot], m, nullptr, nullptr, nullptr, P.d_ws[slot], P.ws_bytes, st, (unsigned char*)P.d_rgb[slot]);
-    if (rc) return rc;
-    CK(cudaMemcpyAsync(rgb8_host + off * 3, P.d_rgb[slot], (size_t)m * 3, cudaMemcpyDeviceToHost, st));
-  }
-  for (int i = 0; i < 3; ++i) CK(cudaStreamSynchronize(P.streams[i]));
-  return 0;
+  // The pixels are copied out: stored straight into pinned memory they would cross PCIe as 3-byte writes per ray.
+  HostChunks io;
+  io.cam = cam;
+  io.rgb8_host = rgb8_host;
+  int rc = run_host_chunks(h, n_rays, chunk, io);
+  return rc ? rc : sync_pipe(h);
 }
 
 // ---- frame sequences (videos, scored splits, embedding maps): rays generated and rendered in sub-batches across frames
@@ -1323,141 +1369,61 @@ int hr_render_host(hr_handle* h, const float* rays_host, int64_t n_rays, float* 
   DeviceGuard guard(h->device);
   const hr_config& c = h->cfg;
   HostPipe& P = h->pipe;
+  // Pinned (device-addressable) buffers are used in place.  The tensor-core sample net reads pinned rays over PCIe -- its
+  // encoder warps work one tile ahead of the tensor pipe, so the transfer hides under the math -- and leaves the device
+  // copy the render kernel reads.  The render epilogue stores into pinned rgb: 12 bytes per ray as posted writes spread over
+  // the kernel's run, made visible by the stream's completion.  A side without a view is copied chunk by chunk.
+  HostChunks io;
+  const bool net_reads_host = tc_net(c.mlp_mode) && h->net.tc_ready && !c.cascade;
+  io.rays_view = net_reads_host ? device_view(rays_host) : nullptr;
+  if (!io.rays_view) io.rays_host = rays_host;
+  io.rgb_view = device_view(rgb_host);
+  if (!io.rgb_view) io.rgb_host = rgb_host;
+  // Default chunk for the tensor-core net: 16 tile waves (hr_render's sub-batch), so that a batch of up to 16 waves stays
+  // whole, since each further chunk costs a sample-net ramp and a render tail.  A larger batch with a copy on either side
+  // goes in one-wave chunks, so that the copies overlap.  The CUDA-core net: 32 768 rays.
   const int64_t wave = (int64_t)h->num_sms * 128;  // one full wave of 128-ray tiles of the tensor-core sample net
-  // Default (chunk <= 0), tensor-core net, batches of a few waves: the "wave split" pipeline below.  Otherwise chunks of
-  // `chunk` rays (default: whole waves for the tensor-core net, 32 768 rays for the CUDA-core net) on three streams.
-  // (a cascaded pipeline runs its nets on point rows: it takes the plain chunked pipeline)
-  const bool whole = chunk <= 0 && tc_net(c.mlp_mode) && n_rays <= 16 * wave && !c.cascade;  // the batch stays whole on the device
-  const float* rays_dev_view = (whole && h->net.tc_ready && !h->timing) ? device_view(rays_host) : nullptr;
-  const bool zero_copy = rays_dev_view != nullptr;
-  float* rgb_dev_view = zero_copy ? device_view(rgb_host) : nullptr;
-  const bool split = !zero_copy && whole && n_rays > wave;
-  if (chunk <= 0) chunk = tc_net(c.mlp_mode) ? wave : 32768;
+  if (chunk <= 0) chunk = !tc_net(c.mlp_mode) ? 32768 : ((io.rays_view && io.rgb_view) || n_rays <= 16 * wave) ? 16 * wave : wave;
   if (chunk > n_rays) chunk = n_rays;
-  const int64_t alloc = (split || zero_copy) ? n_rays : chunk;  // rays per device slot
-  if (ensure_pipe(h, alloc)) return 1;
-  if (!P.fork_ev) {
-    CK(cudaEventCreateWithFlags(&P.fork_ev, cudaEventDisableTiming));
-    for (int i = 0; i < 3; ++i) CK(cudaEventCreateWithFlags(&P.join_ev[i], cudaEventDisableTiming));
-    for (int i = 0; i < 8; ++i) CK(cudaEventCreateWithFlags(&P.dep_ev[i], cudaEventDisableTiming));
-  }
-  // Chunked pipeline: chunk i runs H2D -> sample net -> render -> D2H on stream i % 3.
-  auto enqueue_chunks = [&]() -> int {
-    int slot = 0;
-    for (int64_t off = 0; off < n_rays; off += chunk, slot = (slot + 1) % 3) {
-      int64_t m = (n_rays - off < chunk) ? (n_rays - off) : chunk;
-      cudaStream_t st = P.streams[slot];
-      CK(cudaMemcpyAsync(P.d_rays[slot], rays_host + off * c.c_in, (size_t)m * c.c_in * sizeof(float), cudaMemcpyHostToDevice, st));
-      int rc = render_impl(h, P.d_rays[slot], m, P.d_rgb[slot], nullptr, nullptr, P.d_ws[slot], P.ws_bytes, st);
-      if (rc) return rc;
-      CK(cudaMemcpyAsync(rgb_host + off * 3, P.d_rgb[slot], (size_t)m * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
-    }
-    return 0;
-  };
-  // The whole batch on the device (rays, heads and rgb of slot 0): the render kernel on stream 0 in `pieces` launches
-  // (event Rj after piece j), the rgb of piece j copied out on stream 2 after Rj.
-  auto render_pieces = [&](int pieces) -> int {
-    cudaStream_t s0 = P.streams[0], s2 = P.streams[2];
-    const float* d_rays = P.d_rays[0];
-    float* d_rgb = P.d_rgb[0];
-    const float* heads = (const float*)P.d_ws[0];
-    const int64_t per = ((n_rays + pieces - 1) / pieces + 255) / 256 * 256;
-    int j = 0;
-    for (int64_t off = 0; off < n_rays; off += per, ++j) {
-      const int64_t m = (n_rays - off < per) ? (n_rays - off) : per;
-      cudaError_t e = hr::launch_render(c, h->dv, h->tabs, d_rays + off * c.c_in, heads + off * (int64_t)c.mlp_out, one_dst(d_rgb + off * 3), m,
-                                        nullptr, h->num_sms, s0, nullptr);
-      if (e != cudaSuccess) return hr_fail("render launch failed: %s", cudaGetErrorString(e));
-      h->launches += 1;
-      CK(cudaEventRecord(P.dep_ev[2 + j], s0));
-      CK(cudaStreamWaitEvent(s2, P.dep_ev[2 + j], 0));
-      CK(cudaMemcpyAsync(rgb_host + off * 3, d_rgb + off * 3, (size_t)m * 3 * sizeof(float), cudaMemcpyDeviceToHost, s2));
-    }
-    return 0;
-  };
-  // Wave-split pipeline: splitting a batch into independent chunks costs one cold sample-net launch and one render tail
-  // per chunk, which eats what the copy overlap wins (measured: 0.404 ms unsplit vs 0.410 ms in four chunks).  Instead the
-  // batch stays whole on the device and only the edges are split:
-  //   copy-in  (stream 1): rays of the first tile wave, then the rest          -> events A, B
-  //   compute  (stream 0): sample net on the first wave after A, on the rest after B (together exactly the waves of the
-  //                        unsplit batch), then the render kernel in four pieces -> events R0..R3
-  //   copy-out (stream 2): rgb of piece j after Rj
-  // so only the first wave's H2D and the last piece's D2H are exposed.
-  auto enqueue_split = [&]() -> int {
-    cudaStream_t s0 = P.streams[0], s1 = P.streams[1];
-    float* d_rays = P.d_rays[0];
-    float* heads = (float*)P.d_ws[0];
-    const int64_t nA = wave, nB = n_rays - wave;
-    CK(cudaMemcpyAsync(d_rays, rays_host, (size_t)nA * c.c_in * sizeof(float), cudaMemcpyHostToDevice, s1));
-    CK(cudaEventRecord(P.dep_ev[0], s1));
-    CK(cudaMemcpyAsync(d_rays + nA * c.c_in, rays_host + nA * c.c_in, (size_t)nB * c.c_in * sizeof(float), cudaMemcpyHostToDevice, s1));
-    CK(cudaEventRecord(P.dep_ev[1], s1));
-    CK(cudaStreamWaitEvent(s0, P.dep_ev[0], 0));
-    int rc = launch_sample_net(h, d_rays, nA, heads, s0);
-    if (rc) return rc;
-    CK(cudaStreamWaitEvent(s0, P.dep_ev[1], 0));
-    rc = launch_sample_net(h, d_rays + nA * c.c_in, nB, heads + nA * (int64_t)c.mlp_out, s0);
-    if (rc) return rc;
-    return render_pieces(4);
-  };
-  // Zero-copy input: when the caller's rays are pinned (device-addressable) host memory and the second tensor-core layout
-  // is in use, the sample net reads them straight over PCIe -- its two encoder warps work one tile ahead of the tensor
-  // pipe, so the transfer hides under the math without splitting any launch -- and leaves a device copy for the render
-  // kernel.  The render kernel then runs in two pieces so that half of the D2H overlaps it.
-  auto enqueue_zero_copy = [&]() -> int {
-    cudaStream_t s0 = P.streams[0];
-    float* d_rays = P.d_rays[0];
-    float* heads = (float*)P.d_ws[0];
-    cudaError_t e = hr::launch_mlp_tc2(c, h->net.tc, rays_dev_view, heads, n_rays, h->num_sms, s0, d_rays);
-    if (e != cudaSuccess) return hr_fail("sample-net launch failed: %s", cudaGetErrorString(e));
-    h->launches += 1;
-    if (rgb_dev_view != nullptr) {
-      // Zero-copy output: the caller's rgb buffer is device-addressable pinned memory too -- the render kernel's epilogue
-      // stores the pixels straight into it (12 bytes per ray as posted writes over PCIe, spread over the kernel's whole run),
-      // so there is no D2H copy and no reason to split the launch.  Completion of the stream makes the writes visible.
-      e = hr::launch_render(c, h->dv, h->tabs, d_rays, heads, one_dst(rgb_dev_view), n_rays, nullptr, h->num_sms, s0, nullptr);
-      if (e != cudaSuccess) return hr_fail("render launch failed: %s", cudaGetErrorString(e));
-      h->launches += 1;
-      return 0;
-    }
-    return render_pieces(2);
-  };
-  auto enqueue = [&]() -> int { return zero_copy ? enqueue_zero_copy() : (split ? enqueue_split() : enqueue_chunks()); };
+  if (ensure_pipe(h, chunk)) return 1;
   const int64_t n_chunks = (n_rays + chunk - 1) / chunk;
-  const int64_t key_chunk = zero_copy ? -2 : (split ? -1 : chunk);
-  if (!h->timing && (zero_copy || split || n_chunks > 1)) {
-    // Launch-bound when issued call by call: capture the whole multi-stream pipeline once per (buffers, size) signature
-    // and replay it with a single graph launch.
-    if (!(P.graph && P.g_rays == rays_host && P.g_rgb == rgb_host && P.g_n == n_rays && P.g_chunk == key_chunk)) {
-      drop_host_graph(h);
-      const int64_t launches_before = h->launches;
-      cudaGraph_t g = nullptr;
-      CK(cudaStreamBeginCapture(P.streams[0], cudaStreamCaptureModeRelaxed));
-      CK(cudaEventRecord(P.fork_ev, P.streams[0]));
-      for (int i = 1; i < 3; ++i) CK(cudaStreamWaitEvent(P.streams[i], P.fork_ev, 0));
-      int rc = enqueue();
-      for (int i = 1; i < 3; ++i) {
-        cudaEventRecord(P.join_ev[i], P.streams[i]);
-        cudaStreamWaitEvent(P.streams[0], P.join_ev[i], 0);
-      }
-      cudaError_t ce = cudaStreamEndCapture(P.streams[0], &g);
-      P.g_launches = h->launches - launches_before;
-      h->launches = launches_before;  // capture enqueued nothing; the replay below is what runs
-      if (rc) { if (g) cudaGraphDestroy(g); return rc; }
-      if (ce != cudaSuccess) return hr_fail("hr_render_host: graph capture failed: %s", cudaGetErrorString(ce));
-      ce = cudaGraphInstantiate(&P.graph, g, 0);
-      cudaGraphDestroy(g);
-      if (ce != cudaSuccess) { P.graph = nullptr; return hr_fail("hr_render_host: graph instantiate failed: %s", cudaGetErrorString(ce)); }
-      P.g_rays = rays_host; P.g_rgb = rgb_host; P.g_n = n_rays; P.g_chunk = key_chunk;
-    }
-    CK(cudaGraphLaunch(P.graph, P.streams[0]));
-    h->launches += P.g_launches;
-    CK(cudaStreamSynchronize(P.streams[0]));
-    return 0;
+  // A timed call runs directly: render_impl records its events on the streams.  So does a single chunk that copies its
+  // rays in, a handful of calls on one stream; a zero-copy batch, the pinned buffers' hot path, is replayed.
+  if (h->timing || (n_chunks == 1 && !io.rays_view)) {
+    int rc = run_host_chunks(h, n_rays, chunk, io);
+    return rc ? rc : sync_pipe(h);
   }
-  int rc = enqueue();
-  if (rc) return rc;
-  for (int i = 0; i < 3; ++i) CK(cudaStreamSynchronize(P.streams[i]));
+  // Launch-bound when issued call by call: capture the whole multi-stream pipeline once per (buffers, size, chunk) and
+  // replay it with a single graph launch.
+  if (!(P.graph && P.g_rays == rays_host && P.g_rgb == rgb_host && P.g_n == n_rays && P.g_chunk == chunk)) {
+    drop_host_graph(h);
+    if (!P.fork_ev) {
+      CK(cudaEventCreateWithFlags(&P.fork_ev, cudaEventDisableTiming));
+      for (int i = 0; i < 3; ++i) CK(cudaEventCreateWithFlags(&P.join_ev[i], cudaEventDisableTiming));
+    }
+    const int64_t launches_before = h->launches;
+    cudaGraph_t g = nullptr;
+    CK(cudaStreamBeginCapture(P.streams[0], cudaStreamCaptureModeRelaxed));
+    CK(cudaEventRecord(P.fork_ev, P.streams[0]));
+    for (int i = 1; i < 3; ++i) CK(cudaStreamWaitEvent(P.streams[i], P.fork_ev, 0));
+    int rc = run_host_chunks(h, n_rays, chunk, io);
+    for (int i = 1; i < 3; ++i) {
+      cudaEventRecord(P.join_ev[i], P.streams[i]);
+      cudaStreamWaitEvent(P.streams[0], P.join_ev[i], 0);
+    }
+    cudaError_t ce = cudaStreamEndCapture(P.streams[0], &g);
+    P.g_launches = h->launches - launches_before;
+    h->launches = launches_before;  // capture enqueued nothing; the replay below is what runs
+    if (rc) { if (g) cudaGraphDestroy(g); return rc; }
+    if (ce != cudaSuccess) return hr_fail("hr_render_host: graph capture failed: %s", cudaGetErrorString(ce));
+    ce = cudaGraphInstantiate(&P.graph, g, 0);
+    cudaGraphDestroy(g);
+    if (ce != cudaSuccess) { P.graph = nullptr; return hr_fail("hr_render_host: graph instantiate failed: %s", cudaGetErrorString(ce)); }
+    P.g_rays = rays_host; P.g_rgb = rgb_host; P.g_n = n_rays; P.g_chunk = chunk;
+  }
+  CK(cudaGraphLaunch(P.graph, P.streams[0]));
+  h->launches += P.g_launches;
+  CK(cudaStreamSynchronize(P.streams[0]));
   return 0;
 }
 
@@ -1776,8 +1742,6 @@ int hr_destroy(hr_handle* h) {
   drop_events(h->ev_bwd);
   drop_host_graph(h);
   if (h->pipe.fork_ev) cudaEventDestroy(h->pipe.fork_ev);
-  for (int k = 0; k < 8; ++k)
-    if (h->pipe.dep_ev[k]) cudaEventDestroy(h->pipe.dep_ev[k]);
   for (int i = 0; i < 3; ++i) {
     if (h->pipe.join_ev[i]) cudaEventDestroy(h->pipe.join_ev[i]);
     if (h->pipe.d_rays[i]) cudaFree(h->pipe.d_rays[i]);

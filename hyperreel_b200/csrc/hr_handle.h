@@ -25,7 +25,6 @@ struct HostPipe {
   void* g_rgb = nullptr;
   int64_t g_n = 0, g_chunk = 0, g_launches = 0;
   cudaEvent_t fork_ev = nullptr, join_ev[3] = {nullptr, nullptr, nullptr};
-  cudaEvent_t dep_ev[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // wave-split pipeline edges
 };
 
 // One sample net as hr_upload packs it: its configuration (a copy of the handle's with the net's own shape) and both packs.

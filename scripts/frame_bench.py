@@ -3,7 +3,7 @@
 pinned host memory (hr_render_frame_to8b_host), the reference's validation_video / viewer iteration
 (nlf/__init__.py:828-891) without the per-frame ray upload.  Wall clock per frame, synthetic trained-like parameters.
 
-    python scripts/frame_bench.py --out frames.json
+    python scripts/frame_bench.py --out frames.json [--lib /path/to/libhyperreel_b200.so]
 """
 import argparse, json, os, sys, time
 import torch
@@ -23,7 +23,10 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", required=True)
     ap.add_argument("--frames", type=int, default=20)
+    ap.add_argument("--lib", default="", help="a libhyperreel_b200.so build other than the in-tree one")
     args = ap.parse_args()
+    if args.lib:
+        hb.lib.LIB_PATH = os.path.abspath(args.lib)  # read by load_library() on first use
     rows = []
     for name, (builtin, over, W, H, note) in FRAMES.items():
         cfg, ds = hb.configs.get(builtin, **over)
@@ -49,7 +52,7 @@ def main():
             times.append(time.perf_counter() - t0)
         times = sorted(times[3:])
         ms = 1e3 * times[len(times) // 2]
-        row = {"frame": name, "note": note, "rays": W * H, "samples": sig.n_samples, "ms_per_frame": ms, "fps": 1e3 / ms,
+        row = {"lib": args.lib, "frame": name, "note": note, "rays": W * H, "samples": sig.n_samples, "ms_per_frame": ms, "fps": 1e3 / ms,
                "mrays_s": W * H / ms / 1e3, "mean_pixel": float(out.float().mean())}
         rows.append(row)
         print(json.dumps(row), flush=True)

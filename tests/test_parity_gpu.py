@@ -109,11 +109,12 @@ def test_host_buffer_entry_point_matches_device_path():
 
 
 def test_host_entry_point_whole_batch_pipelines_match_device_path():
-    """Default chunking with the tensor-core net (hr_render_host keeps the batch whole on the device):
-    pinned rays + pinned rgb -> zero-copy input (the sample net's encoder warps read host memory) and zero-copy output (the
-                                render epilogue stores into the host buffer, one render launch, no copies);
-    pinned rays + pageable rgb -> zero-copy input, rgb copied back in two render pieces;
-    pageable rays -> wave split (H2D split at the first 148 x 128-ray wave, sample net in two launches, render in four)."""
+    """hr_render_host with the tensor-core net and the default chunk.  Each side is zero-copy when its buffer is pinned:
+    pinned rays are read by the sample net's encoder warps, which leave the device copy the render kernel reads, and
+    pinned rgb is stored into by the render epilogue; a pageable side is copied per chunk.  A batch of up to 16 tile
+    waves stays whole.  A larger one goes in 16-wave chunks when both sides are zero-copy (the 300 000-ray batch is cut in
+    two), in one-wave chunks otherwise.
+    Timing only turns off the graph replay, so a timed call renders the same pixels."""
     case = build_case("technicolor_trained", n=148 * 128 + 3000)
     render = make_render(case, mlp_mode="bf16x3")
     dev = render(case.rays.cuda())["rgb"].cpu()
@@ -134,6 +135,20 @@ def test_host_entry_point_whole_batch_pipelines_match_device_path():
     # a batch smaller than one wave through the zero-copy path
     small = case.rays[:777].clone().pin_memory()
     assert torch.equal(render.model.render_host(small), dev[:777])
+    render.model.timing(True)
+    try:
+        assert torch.equal(render.model.render_host(case.rays.clone().pin_memory()), dev)
+    finally:
+        render.model.timing(False)
+    # more than 16 waves: zero-copy in and out, in chunks that start at an offset into both host buffers
+    big_case = build_case("technicolor_trained", n=300000)
+    big_dev = render(big_case.rays.cuda())["rgb"].cpu()
+    big = big_case.rays.clone().pin_memory()
+    out = torch.empty((big.shape[0], 3), dtype=torch.float32).pin_memory()
+    for _ in range(2):  # capture, then replay
+        out.zero_()
+        render.model.render_host(big, out)
+        assert torch.equal(out, big_dev)
 
 
 def test_host_entry_point_graph_replay_tracks_buffers_and_reupload():
@@ -158,7 +173,7 @@ def test_host_entry_point_graph_replay_tracks_buffers_and_reupload():
         render.model.mark_dirty()
         render.model.render_host(pinned, out, chunk=1500)  # re-upload drops the graph
         assert torch.equal(out, render(rays_b.cuda())["rgb"].cpu())
-        out2 = render.model.render_host(pinned, chunk=6000)  # single chunk: plain path
+        out2 = render.model.render_host(pinned, chunk=6000)  # single chunk
         assert torch.equal(out2, out)
 
 

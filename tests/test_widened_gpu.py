@@ -63,6 +63,14 @@ def test_ragged_batches_and_chunk_invariance(name, mode):
     out = render(big)["rgb"]
     assert torch.equal(out[: rays.shape[0]], full)
     assert torch.equal(out[rays.shape[0]: 2 * rays.shape[0]], full)
+    # the host-buffer pipeline: zero-copy where the net and the buffers allow it, copies otherwise
+    for pinned in (True, False):
+        rays_host = big.cpu()
+        rgb_host = torch.empty((big.shape[0], 3), dtype=torch.float32)
+        if pinned:
+            rays_host, rgb_host = rays_host.pin_memory(), rgb_host.pin_memory()
+        render.model.render_host(rays_host, rgb_host)
+        assert torch.equal(rgb_host, out.cpu()), (name, mode, pinned)
 
 
 def test_embed_and_extra_fields_of_a_cascaded_pipeline():
