@@ -130,6 +130,8 @@ class LightfieldModel(nn.Module):
         self._version_tensors = None
         self._device_index: Optional[int] = None
         self._ws: Optional[torch.Tensor] = None
+        self._aabb_seen = None  # (aabb buffer, its _version, its values on the host)
+        self._perm_index = {}  # (perm, n, device, inverse) -> _perm_index_on's device index
         self._graph_key = self.sig.graph_key(RENDER_ITER)
 
     # ------------------------------------------------------------------ reference surface
@@ -282,9 +284,7 @@ class LightfieldModel(nn.Module):
             L.check(self._lib.hr_encode_rays(self._handle, rays.data_ptr(), n, enc.data_ptr(), stream))
         perm = list(self.sig.in_perm)
         if perm != list(range(len(perm))):  # BasicPE: reference feature in_perm[k] = kernel feature k
-            inv = torch.empty(len(perm), dtype=torch.long)
-            inv[torch.tensor(perm)] = torch.arange(len(perm))
-            enc = enc.index_select(1, inv.to(rays.device))
+            enc = enc.index_select(1, self._inverse_perm(perm, len(perm), rays.device))
         net = self.embedding_model.embeddings[0].net
         x = enc
         if c.mlp_mode == L.MLP_ZERO:  # ZeroMLP.forward (mlp.py:29-30)
@@ -299,6 +299,23 @@ class LightfieldModel(nn.Module):
             if i < last:
                 x = torch.nn.functional.leaky_relu(x, c.leaky_slope)
         return x
+
+    def _inverse_perm(self, perm, n, dev):
+        """The column index [n] on ``dev`` that takes column perm[k] from column k and keeps the others in place."""
+        return self._perm_index_on(perm, n, dev, inverse=True)
+
+    def _perm_index_on(self, perm, n, dev, inverse):
+        """The column index [n] on ``dev`` of ``perm`` (column k from column perm[k]; the columns past it in place), or of its
+        inverse.  Made once per (perm, n, device), so a training step does not copy it to the device (a pageable copy, which
+        waits for the host)."""
+        key = (tuple(perm), int(n), dev, bool(inverse))
+        if key not in self._perm_index:
+            idx = torch.tensor(list(perm) + list(range(len(perm), n)))
+            if inverse:
+                idx = torch.arange(n)
+                idx[torch.tensor(perm)] = torch.arange(len(perm))
+            self._perm_index[key] = idx.to(dev)
+        return self._perm_index[key]
 
     def _net_params(self):
         """[weight, bias] of every Linear layer of the sample net, in order."""
@@ -331,9 +348,7 @@ class LightfieldModel(nn.Module):
             # column in_perm[k] = uploaded column k; the hidden part of the skip layer keeps its place
             for i in {0, self.sig.cfg.mlp_skip} - {-1}:
                 w = grads[2 * i]
-                src = torch.arange(w.shape[1])
-                src[torch.tensor(perm)] = torch.arange(len(perm))
-                grads[2 * i] = w.index_select(1, src.to(w.device))
+                grads[2 * i] = w.index_select(1, self._inverse_perm(perm, w.shape[1], w.device))
         return grads
 
     def _train_workspace(self, n, dev):
@@ -688,8 +703,12 @@ class LightfieldModel(nn.Module):
         ver = self._param_version()
         if self._handle and self._device_index == idx and self._uploaded_version == ver:
             return
-        # aabb is checkpoint state (it changes when the reference shrinks the grid, tensorf_base.py:1190-1232)
-        aabb = [float(v) for v in self.color_model.net.aabb.detach().cpu().reshape(-1).tolist()]
+        # aabb is checkpoint state (it changes when the reference shrinks the grid, tensorf_base.py:1190-1232); its host
+        # copy is read again only when the buffer was replaced or written, so a training step does not wait on the device
+        t = self.color_model.net.aabb
+        if self._aabb_seen is None or self._aabb_seen[0] is not t or self._aabb_seen[1] != t._version:
+            self._aabb_seen = (t, t._version, [float(v) for v in t.detach().cpu().reshape(-1).tolist()])
+        aabb = self._aabb_seen[2]
         if aabb != [float(self.sig.cfg.aabb[i]) for i in range(6)]:
             for i in range(6):
                 self.sig.cfg.aabb[i] = aabb[i]
@@ -722,8 +741,7 @@ class LightfieldModel(nn.Module):
                 if permuted and (i == 0 or i == skip_layer):
                     # BasicPE column order -> the kernels' per-band order (Signature.in_perm); the hidden part of the skip
                     # layer's input (cat([input, hidden]), mlp.py:167-168) keeps its place
-                    cols = torch.tensor(perm + list(range(len(perm), w.shape[1])), device=w.device)
-                    w = w.detach().index_select(1, cols)
+                    w = w.detach().index_select(1, self._perm_index_on(perm, w.shape[1], w.device, inverse=False))
                 weights[i] = dptr(w)
                 biases[i] = dptr(lin.bias)
 
